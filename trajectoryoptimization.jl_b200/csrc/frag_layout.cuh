@@ -1,5 +1,5 @@
 // frag_layout.cuh -- the per-knot RECORD consumed by the register-resident Riccati kernel (riccati_frag.cu) and written by the
-// error-state expansion kernels (rollout.cu k_expand_lie, riccati_frag.cu k_expansion_rec).
+// error-state expansion kernels (rollout.cu k_expand_lie_rec / k_expand_lie, riccati_frag.cu k_expansion_rec).
 //
 // The backward pass of the error-state Quadrotor (n_e = 12, m = 4, z = [x_e; u] of 16 entries) keeps its whole recursion state in
 // the fragment registers of mma.sync.m8n8k4.f64 (lane L = 4 fr + fc holds A[fr][fc], B[fc][fr], D[fr][2fc], D[fr][2fc+1]).  For
@@ -41,4 +41,8 @@ __host__ __device__ constexpr int ab_index(int e, int j) {
     const int c = phys_z(j);
     return (ks * 32 + 4 * (c & 7) + fc) * 2 + (c >> 3);
 }
+// place of double d of a knot's [A_e B_e] block in the shared-memory image of knot kk of rollout.cu k_expand_lie_rec: bits 1..3 (the 16-byte
+// chunk within the 128-byte line) XOR the line index mod 4 (bits 4..5) and the knot's parity -- a permutation inside each line, so that the
+// column stores of a warp spread over the shared-memory banks while the line stores still read every bank once
+__host__ __device__ constexpr int stage_swz(int d, int kk) { return d ^ ((((d >> 4) & 3) | ((kk & 1) << 2)) << 1); }
 }  // namespace fraglayout

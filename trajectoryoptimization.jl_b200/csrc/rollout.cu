@@ -163,8 +163,9 @@ __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, con
 // Seed pruning.  The position r and the (world-frame) linear velocity v of a RigidBody enter the dynamics only through rdot = v: f does not
 // depend on r, and on v only in rdot.  Their columns of the discrete Jacobian are therefore known in closed form -- d x+/d r = e_r and
 // d x+/d v = h e_r + e_v (the RK4 weights sum to one) -- and need no dual-number sweep: 10 seeds (attitude, angular velocity, controls) are
-// pushed through the RK4 step instead of 16, one thread each; the six trivial columns depend on the time steps only and are written once,
-// when the problem is created (k_trivial_columns).
+// pushed through the RK4 step instead of 16, one thread each; the six trivial columns depend on the time steps only.  The materialised P.ABe
+// (and the record under TO_EXPAND_V1=1) gets them once, when the problem is created (k_trivial_columns); k_expand_lie_rec writes them into
+// every record block it assembles.
 __device__ __forceinline__ int lie_seed(int s) { return (int)((0xFEDCBA9543ULL >> (4 * s)) & 15); }       // 3,4,5,9,10,11,12,13,14,15
 __device__ __forceinline__ int lie_trivial(int s) { return (int)((0x876210ULL >> (4 * s)) & 15); }        // 0,1,2,6,7,8
 
@@ -248,54 +249,81 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
     store_column(j, col);
 }
 
-// k_expand_lie with the knot's fragment block staged in shared memory.  k_expand_lie stores a column as 12 scattered 8-byte words: every one is
-// a partial-sector write for the L2, which has to fill the rest of the sector from DRAM.
-// Here the 10 seed threads of a knot sit in one CTA, drop their columns (and the six closed-form ones) into a 1536-byte image of the
-// record's [A_e B_e] block, and the CTA writes the images out as whole lines.
+// ---- k_expand_lie_rec: the record path's dynamics expansion (the default; TO_EXPAND_V1=1 selects k_expand_lie<QUADROTOR, true>) --------
+// k_expand_lie<.., true> leaves each column as 12 scattered 8-byte stores (one L2 sector operation each) and writes 10 of the 16 columns: in the
+// record's fragment order a 32-byte sector holds columns {c, c + 8} of two rows, and 4 of the 8 column pairs mix a seed column with a closed-form
+// one, so every iteration writes those sectors only partly and the L2 has to fill them from DRAM before it can write them back.
+// Here a CTA owns EXPB_KPB consecutive knots of ONE instance (one thread per (knot, seed), the same expand_lie_column as above: the records are
+// bit-identical).  Each thread drops its column into a shared-memory image of its knot's 1536-byte [A_e B_e] block; the six seed threads
+// sd < 6 of the knot also write one closed-form column each (positions, velocities: 1 on the diagonal, dt[k] at (e, e + 6)), so the image is
+// complete, and the CTA writes the images out as whole 128-byte lines with 16-byte stores: no sector of the block is ever partly written.
+//   mapping   6 knots x 10 seeds = 60 of 64 threads; at N = 101, 17 CTAs per instance and 8 % of the lanes idle.  The instance test of the
+//             overlapped launches (mode 1 / 2) is uniform over the CTA; mode 2 walks the compact late list when there is one (k_linesearch).
+//   CTA size  64 threads like k_expand_lie: a CTA of the late line-search trials that becomes resident beside it displaces 1/8 of an SM.
+//   image     record order (frag_layout.cuh) with the 16-byte chunks of each 128-byte line permuted by fraglayout::stage_swz: the column
+//             stores of a warp spread over the banks, the line stores read every bank once.
+// tests/test_expand_staging.py restates the staging map and the write-out in NumPy.
+#define EXPB_KPB 6
+#define EXPB_T 64
 template <int MODEL>
-__global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 128 / TO_EXPAND_LIE_THREADS) k_expand_lie_staged(const DevProblem P, int mode) {
-    constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, NS = 10, T = TO_EXPAND_LIE_THREADS, KPC = T / NS;
-    static_assert(ne == 12 && m == 4, "record layout of the error-state Quadrotor");
-    __shared__ __align__(16) double st[KPC][TO_REC_G];
-    __shared__ int live[KPC];
+__global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_expand_lie_rec(const DevProblem P, int mode, int nkb) {
+    constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, NS = 10;
+    static_assert(ne == 12 && m == 4 && EXPB_KPB * NS <= EXPB_T, "record layout of the error-state Quadrotor");
+    __shared__ __align__(16) double st[EXPB_KPB][TO_REC_G];
+    const int slot = blockIdx.x / nkb, kb = blockIdx.x - slot * nkb;
+    int b = slot;
+    if (mode == 2 && P.late_list) {                                                    // the instances pass 1 did not accept (acc1[b] == 0)
+        if (slot >= *P.late_count) return;
+        b = P.late_list[slot];
+    } else if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) return;                   // overlapped iterations: the other launch covers this instance
+    const int k0 = kb * EXPB_KPB;
+    const int nk = (P.N - 1 - k0 < EXPB_KPB) ? P.N - 1 - k0 : EXPB_KPB;
     const int tid = threadIdx.x, kk = tid / NS, sd = tid - kk * NS;
-    const long long nknots = (long long)P.B * (P.N - 1);
-    const long long bk0 = (long long)blockIdx.x * KPC;
-    bool work = kk < KPC && bk0 + kk < nknots;
-    int b = 0, k = 0;
-    if (work) {
-        k = (int)((bk0 + kk) % (P.N - 1)); b = (int)((bk0 + kk) / (P.N - 1));
-        if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) work = false;            // overlapped iterations: the other launch covers this instance
-    }
-    if (kk < KPC && sd == 0) live[kk] = work ? 1 : 0;
-    for (int idx = tid; idx < KPC * 72; idx += T) {                                // the closed-form columns (positions, velocities; k_trivial_columns)
-        const int q = idx / 72, r = idx - q * 72, s6 = r / 12, e = r - s6 * 12;
-        if (bk0 + q < nknots) {
-            const int kq = (int)((bk0 + q) % (P.N - 1));
-            const int jt = lie_trivial(s6);
-            st[q][fraglayout::ab_index(e, jt)] = (e == jt) ? 1.0 : ((jt >= 6 && e == jt - 6) ? P.dt[kq] : 0.0);
-        }
-    }
-    if (work) {
-        const int j = lie_seed(sd);
-        const double* X = traj_X(P, P.cur[b], b) + (size_t)k * n;
-        const double* U = traj_U(P, P.cur[b], b) + (size_t)k * m;
-        double col[ne];
-        expand_lie_column<MODEL>(P, k, j, X, U, col);
-        const int c = (int)((0x6420FDB9E7CA8531ULL >> (4 * j)) & 15);               // fraglayout::phys_z(j)
-        double* dst = &st[kk][8 * (c & 7) + (c >> 3)];
+    if (kk < nk) {
+        const int k = k0 + kk;
+        const int buf = P.cur[b];
+        const double* X = traj_X(P, buf, b) + (size_t)k * n;
+        const double* U = traj_U(P, buf, b) + (size_t)k * m;
+        double* img = st[kk];
+        // element (row e, column jj) sits at ab_index(e, 12) | 8 (c & 7) | (c >> 3), c = phys_z(jj) (disjoint bits: ab_index(e, 12) = 64 ks + 2 fc)
+        auto put = [&](int jj, const double (&col)[ne]) {
+            const int c = (int)((0x6420FDB9E7CA8531ULL >> (4 * jj)) & 15);            // fraglayout::phys_z(jj) as a nibble table
+            const int cb = 8 * (c & 7) + (c >> 3);
 #pragma unroll
-        for (int e = 0; e < ne; e++) dst[fraglayout::ab_index(e, 12)] = col[e];
+            for (int e = 0; e < ne; e++) img[fraglayout::stage_swz(fraglayout::ab_index(e, 12) | cb, kk)] = col[e];
+        };
+        double col[ne];
+        expand_lie_column<MODEL>(P, k, lie_seed(sd), X, U, col);
+        put(lie_seed(sd), col);
+        if (sd < 6) {                                                                  // closed-form column jt: d x+/d r = I, d r+/d v = h I, d v+/d v = I
+            const int jt = lie_trivial(sd);
+            const double h = P.dt[k];
+#pragma unroll
+            for (int e = 0; e < ne; e++) col[e] = (e == jt) ? 1.0 : ((jt >= 6 && e == jt - 6) ? h : 0.0);
+            put(jt, col);
+        }
     }
     __syncthreads();
-    for (int idx = tid; idx < KPC * (TO_REC_G / 2); idx += T) {
-        const int q = idx / (TO_REC_G / 2), w = idx - q * (TO_REC_G / 2);
-        if (live[q]) {
-            const int kq = (int)((bk0 + q) % (P.N - 1)), bq = (int)((bk0 + q) / (P.N - 1));
-            double2* rec = reinterpret_cast<double2*>(P.REC + ((size_t)bq * P.N + kq) * TO_REC_LEN);
-            rec[w] = reinterpret_cast<const double2*>(st[q])[w];
+    // write-out: warp w takes knots w, w + 2, w + 4; lane l the 16-byte chunks l, l + 32, l + 64 of the knot's 96 (4 whole lines per store instruction).
+    // Streaming stores: the 629 MB of blocks per iteration (B = 4096, N = 101) cannot stay in the L2 until the Riccati pass reads them; evict-first
+    // keeps the line-search trials' operands there (E beside the late trials 0.409-0.410 -> 0.406-0.407 ms on one H100 80GB HBM3, 700 W).
+    const int warp = tid >> 5, lane = tid & 31;
+    double* recb = P.REC + ((size_t)b * P.N + k0) * TO_REC_LEN;
+    for (int q = warp; q < nk; q += EXPB_T / 32) {
+        double2* dst = reinterpret_cast<double2*>(recb + (size_t)q * TO_REC_LEN);
+        const double2* src = reinterpret_cast<const double2*>(st[q]);
+#pragma unroll
+        for (int r = 0; r < 3; r++) {
+            const int w = lane + 32 * r;
+            __stcs(dst + w, src[fraglayout::stage_swz(2 * w, q) >> 1]);
         }
     }
+}
+
+// TO_EXPAND_V1=1: k_expand_lie<QUADROTOR, true> on the record path (A/B against k_expand_lie_rec; it relies on k_trivial_columns<true> at to_create)
+static bool expand_v1() {
+    static const int v1 = getenv("TO_EXPAND_V1") ? atoi(getenv("TO_EXPAND_V1")) : 0;
+    return v1 != 0;
 }
 
 // the closed-form columns of [A_e B_e] (positions, velocities): thread = (instance, knot, one of the six)
@@ -317,6 +345,7 @@ __global__ void __launch_bounds__(128) k_trivial_columns(const DevProblem P) {
 }
 cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s) {
     const long long total = (long long)P.B * (P.N - 1) * 6;
+    if (P.frag && !expand_v1()) return cudaSuccess;       // k_expand_lie_rec writes the whole block, closed-form columns included, every time
     if (P.frag) k_trivial_columns<true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
     else k_trivial_columns<false><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
     return cudaGetLastError();
@@ -617,12 +646,11 @@ cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
     static_assert(fraglayout::phys_z(0) == 1 && fraglayout::phys_z(5) == 12 && fraglayout::phys_z(11) == 15 && fraglayout::phys_z(12) == 0 && fraglayout::phys_z(15) == 6, "nibble table of k_expand_lie");
     { static bool d1[TO_MAXDEV] = {false}, d2[TO_MAXDEV] = {false}; prefer_common_carveout(k_expand_lie<MODEL_QUADROTOR, true>, d1); prefer_common_carveout(k_expand_lie<MODEL_QUADROTOR, false>, d2); }
     constexpr int T = TO_EXPAND_LIE_THREADS;
-    static const int staged = getenv("TO_EXPAND_STAGE") ? atoi(getenv("TO_EXPAND_STAGE")) : 0;
-    if (P.frag && staged) {
-        constexpr int KPC = T / 10;
-        const long long nknots = (long long)P.B * (P.N - 1);
-        { static bool d3[TO_MAXDEV] = {false}; prefer_common_carveout(k_expand_lie_staged<MODEL_QUADROTOR>, d3); }
-        k_expand_lie_staged<MODEL_QUADROTOR><<<(unsigned)((nknots + KPC - 1) / KPC), T, 0, s>>>(P, mode);
+    if (P.frag && !expand_v1()) {
+        // one CTA per (instance, block of EXPB_KPB knots); mode 2 with the late list: the first *late_count instance slots carry work
+        const int nkb = (P.N - 1 + EXPB_KPB - 1) / EXPB_KPB;
+        { static bool d3[TO_MAXDEV] = {false}; prefer_common_carveout(k_expand_lie_rec<MODEL_QUADROTOR>, d3); }
+        k_expand_lie_rec<MODEL_QUADROTOR><<<(unsigned)((long long)P.B * nkb), EXPB_T, 0, s>>>(P, mode, nkb);
     } else if (P.frag) k_expand_lie<MODEL_QUADROTOR, true><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
     else k_expand_lie<MODEL_QUADROTOR, false><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
     return cudaGetLastError();
