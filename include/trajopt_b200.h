@@ -250,6 +250,12 @@ int to_state_diff(to_handle* h, const double* Xbar, double* dx);
 int to_get_error_dynamics(to_handle* h, double* ABe);
 /* error-state cost + AL expansion of every knot (Altro error_expansion!): grad [B][N][n_e+m], hess [B][N][n_e+m][n_e+m] */
 int to_error_expansion(to_handle* h, double* grad, double* hess);
+/* DIAGNOSTIC (not part of the Julia shim; the hot path does not use it): the cost + AL expansion that the record path's Riccati kernel
+ * (to_backward_algebra = 1) read in the last backward pass, copied from doubles [192, 240) of every knot's record:
+ * out [B][N][48] = g~[16] | hd[16] | Hb[4][4] in the physical order of csrc/frag_layout.cuh.  TO_ESTATE when the handle is not on the
+ * record path or no backward pass has written the records' expansion yet.  to_error_expansion computes the same numbers by another
+ * kernel chain and does not read the records. */
+int to_get_expansion_records(to_handle* h, double* out);
 int to_get_multipliers(to_handle* h, int32_t con, double* lambda /*[B][last-first+1][p]*/);
 int to_set_multipliers(to_handle* h, int32_t con, const double* lambda);
 int to_get_penalty(to_handle* h, int32_t con, double* mu);

@@ -28,7 +28,7 @@ def build_term_table(cons, mus, n=N_X, m=N_U):
     table = [[] for _ in range(nm)]
     for i in range(nm):
         for ci, (c, first, last) in enumerate(cons):
-            kind = type(c).__name__
+            kind = "BoundConstraint" if hasattr(c, "z_max") else type(c).__name__      # (StateBound / ControlBound included)
             mu = mus[ci]
             for side in range(2):
                 row, sign, bound, eq = -1, 1.0, 0.0, False

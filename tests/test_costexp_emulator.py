@@ -4,9 +4,12 @@ oracle's dense error-state expansion (Altro error_expansion! restated in oracle/
 import numpy as np
 import pytest
 
+import record_configs as rc
 import trajopt_b200 as TO
 from costexp_emulator import block_images, build_term_table, image_from_dense
 from oracle_binding import OracleProblem
+
+P = TO.problems
 
 
 def _problem(B, N, state_bounds):
@@ -64,3 +67,62 @@ def test_blocked_cost_expansion_algorithm_matches_the_oracle(N, state_bounds):
             active += int(np.any(np.abs(np.diag(H_ref[b, k])[12:] - R) > 1e-9))
     assert worst < 1e-12, f"max rel difference {worst:.3e}"
     assert active > 0, "no Bound row was active: the test would not see the AL terms"
+
+
+def _emulator_vs_oracle(prob):
+    """the emulator's images of every knot of `prob` (term table and cost table built from its own description, its current penalties and
+    multipliers) against the oracle's dense error-state expansion -> (max relative difference, max |attitude off-diagonal| / block scale)"""
+    cons, cost_of_knot, costs = rc.term_inputs(prob)
+    table, offsets, lam_len = build_term_table(cons, [TO.penalty(prob, i) for i in range(len(cons))])
+    X, U = TO.states(prob), TO.controls(prob)
+    B, N = X.shape[:2]
+    lam = np.zeros((B, lam_len))
+    for ci, (c, first, last) in enumerate(cons):
+        lam[:, offsets[ci]:offsets[ci] + (last - first + 1) * c.p] = TO.multipliers(prob, ci).reshape(B, -1)
+    g_ref, H_ref = TO.error_expansion(prob)
+    worst = offdiag = 0.0
+    for b in range(B):
+        img = block_images(X[b], U[b], lam[b], table, cost_of_knot, costs, N)
+        for k in range(N):
+            ref, rest = image_from_dense(g_ref[b, k], H_ref[b, k])
+            assert rest < 1e-12
+            if k == N - 1:
+                ref[[0, 2, 4, 6, 16, 18, 20, 22]] = 0.0
+            worst = max(worst, float(np.max(np.abs(img[k] - ref))) / max(1.0, float(np.max(np.abs(ref)))))
+            Hb = ref[32:44].reshape(3, 4)[:, :3]
+            offdiag = max(offdiag, float(np.max(np.abs(Hb - np.diag(np.diag(Hb))))) / float(np.max(np.abs(np.diag(Hb)))))
+    return worst, offdiag
+
+
+def _natural_iterate(prob):
+    TO.rollout(prob)
+    TO.ilqr_step(prob, 1); TO.al_update(prob); TO.ilqr_step(prob, 1)
+    for i, mu in enumerate((3.7, 11.0, 0.6, 2.3)[:len(prob.constraints)]):     # a distinct penalty per constraint
+        TO.set_penalty(prob, i, mu)
+
+
+@pytest.mark.parametrize("name", ["quat_weights", "state_bounds", "midblock_ranges", "zigzag"])
+def test_blocked_cost_expansion_algorithm_on_the_record_configurations(name):
+    """the emulated algorithm on the inputs the BASELINE problems never produce (tests/record_configs.py): non-uniform quaternion weights
+    (attitude off-diagonals), inequality rows on every state lane, knot ranges that start / end inside 16-knot blocks, one cost per knot"""
+    prob = P.quadrotor_zigzag(cls=OracleProblem) if name == "zigzag" else getattr(rc, name)(OracleProblem)
+    _natural_iterate(prob)
+    worst, offdiag = _emulator_vs_oracle(prob)
+    assert worst < 1e-12, f"max rel difference {worst:.3e}"
+    if name == "quat_weights":
+        assert offdiag > 1e-3, "the attitude block stayed diagonal"
+    prob.close()
+
+
+def test_blocked_cost_expansion_algorithm_on_a_tracking_objective():
+    """one cost per knot, re-targeted by update_trajectory and moved by shift_trajectory (MPC), on the error state"""
+    prob, Xref, Uref = rc.tracking(OracleProblem)
+    for start in (1, 4):
+        if start > 1:
+            TO.shift_trajectory(prob, 3)
+            TO.update_trajectory(prob, Xref, Uref, start)
+            TO.rollout(prob)
+        _natural_iterate(prob)
+        worst, _ = _emulator_vs_oracle(prob)
+        assert worst < 1e-12, f"start {start}: max rel difference {worst:.3e}"
+    prob.close()

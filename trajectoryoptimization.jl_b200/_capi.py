@@ -181,7 +181,7 @@ def load_library():
         "to_set_phase_timing": [H, C.c_int], "to_get_phase_times": [H, c_double_p, C.POINTER(C.c_int64), C.c_int],
         "to_algorithmic_bytes": [H, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
         "to_backward_algebra": [H, c_int32_p], "to_error_state_dim": [H, c_int32_p], "to_state_diff": [H, c_double_p, c_double_p], "to_get_error_dynamics": [H, c_double_p],
-        "to_error_expansion": [H, c_double_p, c_double_p],
+        "to_error_expansion": [H, c_double_p, c_double_p], "to_get_expansion_records": [H, c_double_p],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)
@@ -205,6 +205,7 @@ EXPORTED_SYMBOLS = [
     "to_set_multipliers", "to_get_penalty", "to_set_penalty", "to_get_solver_state", "to_reduce_merit", "to_reduce_merit_async", "to_merit_device_ptr", "to_update_trajectory", "to_shift_trajectory",
     "to_set_phase_timing", "to_get_phase_times", "to_launch_count", "to_algorithmic_bytes",
     "to_backward_algebra", "to_error_state_dim", "to_state_diff", "to_get_error_dynamics", "to_error_expansion",
+    "to_get_expansion_records",
 ]
 
 

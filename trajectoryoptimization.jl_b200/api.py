@@ -1556,6 +1556,14 @@ def error_expansion(prob):
     return g, np.swapaxes(H, -1, -2)
 
 
+def expansion_records(prob):
+    """Diagnostic, CUDA problems on the record path only (``backward_algebra(prob) == 1``): the cost + AL expansion that the last backward
+    pass read from the per-knot records -> ``[B, N, 48]`` = ``g~[16] | hd[16] | Hb[4, 4]`` in the physical order of csrc/frag_layout.cuh."""
+    out = np.empty((prob.B, prob.N, 48))
+    prob._call("to_get_expansion_records", K._dp(out))
+    return out
+
+
 def errstate_jacobian(prob):
     """``RD.errstate_jacobian!(model, G, z)`` of every knot of the current trajectory -> ``G[B, N, n, n_e]`` (identity blocks around the
     4 x 3 attitude block ``L(q) H``; plain identity without a Lie-group state).  Host-side glue over ``states(prob)``."""

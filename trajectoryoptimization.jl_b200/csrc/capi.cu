@@ -62,6 +62,7 @@ struct to_handle {
     Scratch scratch;
     double t0 = 0;
     bool J_valid = false, expanded = false, backward_done = false;
+    bool rec_costexp = false;     // (record path) a cost + AL expansion has been written into REC[192, 240) (to_get_expansion_records)
     int64_t launches = 0;
     // phase timing
     bool timing = false;
@@ -1055,6 +1056,7 @@ static int do_backward(to_handle* h, bool costexp_done = false) {
             else CU(h, launch_expansion_rec(h->P, h->stream));                          // more than 3 rows on one z entry: descriptor walk
             h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
         }
+        h->rec_costexp = true;     // (costexp_done: to_ilqr_step launched it, split or not)
         PhaseScope ps(h, TO_PHASE_BACKWARD);
         CU(h, launch_backward_frag(h->P, h->d_fragq, h->d_fragpool, h->d_fragerr, h->stream));
     } else if (h->P.dense_riccati) {
@@ -1261,6 +1263,18 @@ int to_error_expansion(to_handle* h, double* grad, double* hess) {
     const size_t nme = h->P.ne + h->P.m, ng = (size_t)h->P.B * h->P.N * nme;
     CU(h, cudaMemcpyAsync(grad, h->P.EG, ng * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     CU(h, cudaMemcpyAsync(hess, h->P.EH, ng * nme * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return TO_OK;
+}
+// diagnostic: the cost + AL expansion as the record path's Riccati kernel reads it, REC[192, 240) of every (instance, knot)
+int to_get_expansion_records(to_handle* h, double* out) {
+    JOIN(h);
+    if (!h || !out) return TO_EINVAL;
+    if (!(h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5)) return fail(h, TO_ESTATE, "to_get_expansion_records: the handle is not on the record path");
+    if (!h->rec_costexp) return fail(h, TO_ESTATE, "to_get_expansion_records before any backward pass wrote the records' expansion");
+    constexpr int W = TO_REC_LEN - TO_REC_G;
+    CU(h, cudaMemcpy2DAsync(out, W * sizeof(double), h->P.REC + TO_REC_G, TO_REC_LEN * sizeof(double), W * sizeof(double), (size_t)h->P.B * h->P.N,
+                            cudaMemcpyDeviceToHost, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
     return TO_OK;
 }
