@@ -41,6 +41,20 @@ def triple(build, opts=None):
     return g, o, t
 
 
+def triple_with_options(build, opts=None):
+    """`triple` with SOLVER options (regularisation, line search, AL schedule) applied to all three problems; `backward_kernel` is a kernel
+    choice of the CUDA problem and goes to it alone (the oracle has one backward pass, in the arithmetic form match_algebra picks)"""
+    opts = dict(opts or {})
+    kernel = opts.pop("backward_kernel", None)
+    g = build(TO.Problem)
+    TO.set_options(g, **opts, **({} if kernel is None else {"backward_kernel": kernel}))
+    o = match_algebra(g, build(OracleProblem))
+    t = match_algebra(g, build(OracleProblem)).set_gain_noise(GAIN_TOL)
+    for p in (o, t):
+        TO.set_options(p, **opts)
+    return g, o, t
+
+
 def check(what, a_gpu, a_orc, a_twin, tight, sel=None, outliers=0.0):
     """every instance (but a fraction `outliers` of them -- after several closed-loop iterations of a chaotic instance one noise draw of the
     twin is a coarse yardstick): err(gpu, oracle) <= max(tight, FACTOR * err(twin, oracle)); returns (worst gpu error, worst twin error)"""

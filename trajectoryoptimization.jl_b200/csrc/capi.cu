@@ -1205,7 +1205,15 @@ int to_ilqr_step(to_handle* h, int32_t iters) {
 int to_al_update(to_handle* h) {
     JOIN(h);
     if (!h) return TO_EINVAL;
-    if (h->P.ncon > 0) { CU(h, launch_al_update(h->P, h->stream)); h->launches++; }
+    if (h->P.ncon > 0) { CU(h, launch_al_update(h->P, h->stream)); h->launches++; }    // (k_al_update also restarts rho / drho)
+    else {
+        // no multipliers to update, but the regularisation restarts at bp_reg_initial all the same: Altro's inner solve resets it at
+        // the start of every AL iteration, constrained or not
+        std::vector<double> r(h->P.B, h->P.opt.bp_reg_initial);
+        CU(h, cudaMemcpyAsync(h->P.rho, r.data(), sizeof(double) * h->P.B, cudaMemcpyHostToDevice, h->stream));
+        CU(h, cudaMemsetAsync(h->P.drho, 0, sizeof(double) * h->P.B, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));     // `r` goes out of scope
+    }
     for (auto& mu : h->h_mu) mu = std::fmin(mu * h->P.opt.penalty_scaling, h->P.opt.penalty_max);
     if (!h->h_mu.empty()) CU(h, cudaMemcpyAsync(h->d_mu, h->h_mu.data(), sizeof(double) * h->h_mu.size(), cudaMemcpyHostToDevice, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
