@@ -46,7 +46,21 @@ int orc_create(const to_spec* s, orc_handle** out) {
         for (int i = 0; i < s->ndyn; i++) {
             const to_dynamics_spec& d = s->dyn[i];
             DynProg dp; dp.n_in = d.n_in; dp.m_in = d.m_in; dp.n_out = d.n_out; dp.discrete = d.discrete != 0;
-            if (!d.prog || d.prog_len < d.n_out || d.n_in > mp.n || d.m_in > mp.m || d.n_out > mp.n) { delete h; return fail(nullptr, TO_EINVAL, "recorded-program model: bad program size or dimensions"); }
+            if (!d.prog || d.prog_len < 1 || d.prog_len > TO_EXPR_MAXLEN || d.nconst < 0 || d.nconst > TO_EXPR_MAXCONST || (d.nconst > 0 && !d.consts) ||
+                d.n_in < 1 || d.n_in > mp.n || d.m_in < 0 || d.m_in > mp.m || d.n_out < 1 || d.n_out > mp.n || d.n_out > d.prog_len) {
+                delete h; return fail(nullptr, TO_EINVAL, "recorded-program model: bad program size or dimensions");
+            }
+            // the instruction checks of to_create: operands of earlier instructions only, constants and inputs in range
+            for (int j = 0; j < d.prog_len; j++) {
+                const int op = d.prog[3 * j], a = d.prog[3 * j + 1], b = d.prog[3 * j + 2];
+                const bool bin = op >= TO_OP_ADD && op <= TO_OP_DIV;
+                bool ok = op >= 0 && op <= TO_OP_RSUBC;
+                if (op == TO_OP_CONST) ok = ok && a >= 0 && a < d.nconst;
+                else if (op == TO_OP_X) ok = ok && a >= 0 && a < d.n_in;
+                else if (op == TO_OP_U) ok = ok && a >= 0 && a < d.m_in;
+                else { ok = ok && a >= 0 && a < j; if (bin) ok = ok && b >= 0 && b < j; if (op == TO_OP_POWC || op >= TO_OP_ADDC) ok = ok && b >= 0 && b < d.nconst; }
+                if (!ok) { delete h; return fail(nullptr, TO_EINVAL, "recorded-program model: invalid instruction"); }
+            }
             dp.prog.assign(d.prog, d.prog + 3 * d.prog_len); dp.consts.assign(d.consts, d.consts + d.nconst);
             P.dyn.push_back(dp);
         }
@@ -54,11 +68,17 @@ int orc_create(const to_spec* s, orc_handle** out) {
             const int di = s->dyn_index[k];
             if (di < 0 || di >= s->ndyn) { delete h; return fail(nullptr, TO_EINVAL, "dyn_index out of range"); }
             const DynProg& d = P.dyn[di];
-            if (d.n_in != s->nx[k] || d.m_in != s->nu[k]) { delete h; return fail(nullptr, TO_EDIM, "Model " + std::to_string(k + 1) + " does not have the dimensions of knot " + std::to_string(k + 1) + "."); }
-            if (d.n_out != s->nx[k + 1]) {    // src/dynamics.jl:23-28
+            if (d.n_in != s->nx[k] || d.m_in != s->nu[k]) {
+                const std::string msg = "Model " + std::to_string(k + 1) + " has state / control dimensions (" + std::to_string(d.n_in) + ", " + std::to_string(d.m_in) +
+                                        ") but knot " + std::to_string(k + 1) + " has (" + std::to_string(s->nx[k]) + ", " + std::to_string(s->nu[k]) + ").";
                 delete h;
-                return fail(nullptr, TO_EDIM, "Model mismatch at time step " + std::to_string(k + 1) + ". Model " + std::to_string(k + 1) + " has an output dimension of " +
-                            std::to_string(d.n_out) + " but model " + std::to_string(k + 2) + " has a state dimension of " + std::to_string(s->nx[k + 1]) + ".");
+                return fail(nullptr, TO_EDIM, msg);
+            }
+            if (d.n_out != s->nx[k + 1]) {    // src/dynamics.jl:23-28
+                const std::string msg = "Model mismatch at time step " + std::to_string(k + 1) + ". Model " + std::to_string(k + 1) + " has an output dimension of " +
+                                        std::to_string(d.n_out) + " but model " + std::to_string(k + 2) + " has a state dimension of " + std::to_string(s->nx[k + 1]) + ".";
+                delete h;     // (d lives in h: the message is built first)
+                return fail(nullptr, TO_EDIM, msg);
             }
             P.dyn_index.push_back(di);
         }

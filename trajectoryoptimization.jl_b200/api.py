@@ -182,7 +182,8 @@ class AutodiffDynamics(_Model):
     model of the path (``RD.DiscretizedDynamics{RD.RK4}``).  ``fun(x, u)`` is called once with recording vectors (see ``Expr``) and returns
     the ``output_dim`` entries of ``xdot``.  ``discrete=True``: ``fun`` is a jump map ``x+ = g(x, u)`` applied as is -- its output dimension
     may differ from its state dimension, which is how the state dimension changes along a hybrid trajectory.  Used through
-    ``Problem([model_1, ..., model_{N-1}], obj, x0, tf)`` (src/problem.jl:36-73)."""
+    ``Problem([model_1, ..., model_{N-1}], obj, x0, tf)`` (src/problem.jl:36-73), or on its own as ``Problem(model, obj, x0, tf)``, which is
+    ``Problem([model] * (N - 1), obj, x0, tf)``."""
     model_id = K.MODEL_EXPR
 
     def __init__(self, n, m, fun, output_dim=None, discrete=False):
@@ -190,7 +191,7 @@ class AutodiffDynamics(_Model):
         self.n_out = self.n if output_dim is None else int(output_dim)
         if self.n_out != self.n and not self.discrete:
             raise ArgumentError("a continuous model integrates its own state: output_dim != state_dim needs discrete=True (a jump map)")
-        tape = _Tape()
+        tape = _Tape("dynamics model")
         x = np.array([tape.emit(K.OP_X, i, 0) for i in range(self.n)], dtype=object)
         u = np.array([tape.emit(K.OP_U, j, 0) for j in range(self.m)], dtype=object)
         out = list(np.atleast_1d(np.asarray(fun(x, u), dtype=object)).ravel())
@@ -440,16 +441,17 @@ class Expr:
     tanh = lambda s: s._un(K.OP_TANH)
 
     def __bool__(self):
-        raise ArgumentError("a recorded cost cannot branch on a state / control value")
+        raise ArgumentError(f"a recorded {self.tape.what} cannot branch on a state / control value")
 
 
 class _Tape:
-    def __init__(self):
+    def __init__(self, what):
+        self.what = what     # what is being recorded ("cost", "dynamics model", "constraint"), for the error messages
         self.prog, self.consts = [], []
 
     def emit(self, op, a, b):
         if len(self.prog) >= K.EXPR_MAXLEN:
-            raise ArgumentError(f"recorded cost exceeds {K.EXPR_MAXLEN} instructions")
+            raise ArgumentError(f"recorded {self.what} exceeds {K.EXPR_MAXLEN} instructions")
         self.prog.append((int(op), int(a), int(b)))
         return Expr(self, len(self.prog) - 1)
 
@@ -459,7 +461,7 @@ class _Tape:
             if c == v and np.signbit(c) == np.signbit(v):
                 return i
         if len(self.consts) >= K.EXPR_MAXCONST:
-            raise ArgumentError(f"recorded cost exceeds {K.EXPR_MAXCONST} constants")
+            raise ArgumentError(f"recorded {self.what} exceeds {K.EXPR_MAXCONST} constants")
         self.consts.append(v)
         return len(self.consts) - 1
 
@@ -488,7 +490,7 @@ class AutodiffCost(CostFunction):
 
     def __init__(self, n, m, fun, terminal=False):
         self.n, self.m, self.fun, self.terminal = int(n), int(m), fun, bool(terminal)
-        tape = _Tape()
+        tape = _Tape("cost")
         x = np.array([tape.emit(K.OP_X, i, 0) for i in range(self.n)], dtype=object)
         u = np.array([tape.emit(K.OP_U, j, 0) for j in range(self.m)], dtype=object)
         out = fun(x, u)
@@ -820,7 +822,7 @@ class AutodiffConstraint(AbstractConstraint):
 
     def __init__(self, n, m, fun, sense, inputs="stage"):
         self.n, self.m, self.fun, self.sense_, self.inputs = int(n), int(m), fun, sense, inputs
-        tape = _Tape()
+        tape = _Tape("constraint")
         x = np.array([tape.emit(K.OP_X, i, 0) for i in range(self.n)], dtype=object)
         u = np.array([tape.emit(K.OP_U, j, 0) for j in range(self.m)], dtype=object)
         out = fun(x, u) if inputs == "stage" else (fun(x) if inputs == "state" else fun(u))
@@ -1040,6 +1042,10 @@ class Problem:
         x0, tf = args
         N = len(obj)
         x0 = np.asarray(x0, dtype=float)
+        if isinstance(model, AutodiffDynamics):
+            # one user model (RD.@autodiff struct M <: ContinuousDynamics + Problem(model, obj, x0, tf)) steps every knot: it is the model
+            # vector [model] * (N - 1), on the padded (4, 2) layout the recorded-program kernels exist for
+            model = [model] * (N - 1)
         self.hybrid = isinstance(model, (list, tuple))
         if self.hybrid:
             # Problem(models::Vector{<:DiscreteDynamics}, obj, x0, tf)  src/problem.jl:36-73: per-knot dimensions from RD.dims(models); the
