@@ -238,6 +238,47 @@ int to_forward(to_handle* h, double* J /*[B] or NULL*/, double* alpha /*[B] or N
 int to_ilqr_step(to_handle* h, int32_t iters);                                /* iters x (expand, backward, forward), no host sync */
 int to_al_update(to_handle* h);                                               /* dual + penalty update */
 int to_get_gains(to_handle* h, double* K /*[B][N-1][n_e][m]: m x n_e col-major (n_e = n unless error_state)*/, double* d /*[B][N-1][m]*/);
+
+/* ---- solve to convergence: Altro's AL-iLQR solve!, per instance ---------------------------------------------------------------------
+ * Altro 0.3 is not under the reference; the semantics are restated in DESIGN.md 5d.  Per instance, independently:
+ *   start   roll out from x0 and the current controls, J = merit, rho = bp_reg_initial, counters zero.  Multipliers and penalties are KEPT
+ *           (a fresh problem has lambda = 0, mu = penalty_initial): to_solve continues from whatever to_al_update / to_set_multipliers left.
+ *   inner   per iteration: expansion, backward pass, line search (to_ilqr_step's iteration), then
+ *             dJ = J_prev - J (AL merit), 0 and dJ_counter + 1 when the line search failed (alpha = 0);
+ *             gradient = mean_k max_i |d_k,i| / (|u_k,i| + 1) with the controls after the step (Altro gradient_todorov);
+ *           the inner loop converges on alpha > 0 && 0 <= dJ < cost_tol && gradient < grad_tol, and ends without converging at
+ *           iterations_inner (constrained problems), iterations (all iterations together) or dJ_counter > dJ_counter_limit.
+ *           A backward pass that fails at bp_reg_max ends the solve of the instance: TO_SOLVE_MAX_REGULARIZATION.
+ *   outer   (constrained problems) c_max = max violation when the inner loop ended: SUCCEEDED when c_max < constraint_tolerance, else
+ *           MAX_ITERATIONS when the iteration cap is reached, else MAX_ITERATIONS_OUTER after iterations_outer outer iterations, else dual
+ *           update + penalty update + rho reset (to_al_update) and the next inner loop.  Inner loops use the *_intermediate tolerances except
+ *           in the last allowed outer iteration (Altro set_tolerances!).
+ *   no constraints: one plain iLQR loop with the final tolerances; SUCCEEDED, MAX_ITERATIONS, or UNSOLVED when it stalled (dJ_counter).
+ * Penalties are per constraint, shared by the batch, so the outer loop is batch-synchronous: an instance whose inner loop has ended waits
+ * (running no kernel) until no instance is in an inner loop; every instance in outer iteration j then sees mu_j = min(mu_0 phi^j, penalty_max),
+ * exactly as when solved alone.  Converged instances are retired from every solver kernel: their X, U, lambda, K, d are those of the iteration
+ * they stopped at, read with the getters above.
+ * Altro's summary after solve! prints these statistics: examples/Cartpole.ipynb:216-223 (ALTRO), :378-382 (iLQR), examples/Quadrotor.ipynb:374-391. */
+enum to_solve_status { TO_SOLVE_UNSOLVED = 0, TO_SOLVE_SUCCEEDED = 1, TO_SOLVE_MAX_ITERATIONS = 2, TO_SOLVE_MAX_ITERATIONS_OUTER = 3,
+                       TO_SOLVE_MAX_REGULARIZATION = 4 };
+/* Altro 0.3 SolverOptions names; defaults (to_default_solve_options) restated from Altro, pinned by the notebooks only where noted */
+typedef struct {
+    double cost_tolerance;                  /* 1e-4 (pinned: the notebook's iLQR run stops at dJ 6.9e-5) */
+    double cost_tolerance_intermediate;     /* 1e-3 (unpinned; the notebook's ALTRO run sets 1e-2) */
+    double gradient_tolerance;              /* 10   (unpinned) */
+    double gradient_tolerance_intermediate; /* 1    (unpinned) */
+    double constraint_tolerance;            /* 1e-6 (unpinned) */
+    int32_t iterations;                     /* 300  (unpinned) all iterations together */
+    int32_t iterations_inner;               /* 300  (unpinned) */
+    int32_t iterations_outer;               /* 30   (unpinned) */
+    int32_t dJ_counter_limit;               /* 10   (unpinned) */
+} to_solve_options;
+int to_default_solve_options(to_solve_options* o);
+/* solve!(prob): outputs [B] each, any may be NULL.  cost = the objective (not the merit) of the final trajectory; dJ, gradient = those of the
+ * last iteration; c_max = the max violation when the last inner loop ended (0 without constraints).  TO_EINVAL for a non-positive
+ * tolerance or cap (dJ_counter_limit may be 0). */
+int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* cost, double* dJ,
+             double* gradient, double* c_max);
 /* ---- Lie-group error state (SURVEY 8 f2) ------------------------------------------------------------------- */
 int to_backward_algebra(const to_handle* h, int32_t* variant);             /* which arithmetic the next to_backward will use: 0 = pivot-by-pivot LDL' solve
                                                                              (riccati.cu, riccati_small.cu, lie.cu), 1 = 2 x 2 block inverse + W'K update

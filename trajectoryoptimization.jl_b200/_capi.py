@@ -27,6 +27,8 @@ COST_DIAGONAL, COST_QUADRATIC, COST_DIAGONAL_QUAT, COST_EXPR = 0, 1, 2, 3
 EXPR_MAXLEN, EXPR_MAXCONST = 128, 64
 CONE_ZERO, CONE_NEGATIVE_ORTHANT, CONE_SECOND_ORDER, CONE_IDENTITY, CONE_POSITIVE_ORTHANT = 0, 1, 2, 3, 4
 CON_GOAL, CON_BOUND, CON_LINEAR, CON_CIRCLE, CON_SPHERE, CON_NORM, CON_COLLISION, CON_QUATVEC, CON_EXPR = 0, 1, 2, 3, 4, 5, 6, 7, 8
+# to_solve_status
+SOLVE_UNSOLVED, SOLVE_SUCCEEDED, SOLVE_MAX_ITERATIONS, SOLVE_MAX_ITERATIONS_OUTER, SOLVE_MAX_REGULARIZATION = 0, 1, 2, 3, 4
 PHASE_EXPAND, PHASE_BACKWARD, PHASE_FORWARD, PHASE_LADDER, PHASE_ACCEPT, PHASE_COSTEXP, PHASE_LATE, PHASE_COUNT = 0, 1, 2, 3, 4, 5, 6, 8
 
 c_double_p = C.POINTER(C.c_double)
@@ -65,6 +67,12 @@ class to_options(C.Structure):
                 ("iterations_linesearch", C.c_int32), ("backward_kernel", C.c_int32),
                 ("max_state_value", C.c_double), ("max_control_value", C.c_double),
                 ("penalty_initial", C.c_double), ("penalty_scaling", C.c_double), ("penalty_max", C.c_double), ("dual_max", C.c_double)]
+
+
+class to_solve_options(C.Structure):
+    _fields_ = [("cost_tolerance", C.c_double), ("cost_tolerance_intermediate", C.c_double), ("gradient_tolerance", C.c_double),
+                ("gradient_tolerance_intermediate", C.c_double), ("constraint_tolerance", C.c_double),
+                ("iterations", C.c_int32), ("iterations_inner", C.c_int32), ("iterations_outer", C.c_int32), ("dJ_counter_limit", C.c_int32)]
 
 
 def _dp(a):
@@ -182,6 +190,8 @@ def load_library():
         "to_algorithmic_bytes": [H, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
         "to_backward_algebra": [H, c_int32_p], "to_error_state_dim": [H, c_int32_p], "to_state_diff": [H, c_double_p, c_double_p], "to_get_error_dynamics": [H, c_double_p],
         "to_error_expansion": [H, c_double_p, c_double_p], "to_get_expansion_records": [H, c_double_p],
+        "to_default_solve_options": [C.POINTER(to_solve_options)],
+        "to_solve": [H, C.POINTER(to_solve_options), c_int32_p, c_int32_p, c_int32_p, c_double_p, c_double_p, c_double_p, c_double_p],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)
@@ -205,7 +215,7 @@ EXPORTED_SYMBOLS = [
     "to_set_multipliers", "to_get_penalty", "to_set_penalty", "to_get_solver_state", "to_reduce_merit", "to_reduce_merit_async", "to_merit_device_ptr", "to_update_trajectory", "to_shift_trajectory",
     "to_set_phase_timing", "to_get_phase_times", "to_launch_count", "to_algorithmic_bytes",
     "to_backward_algebra", "to_error_state_dim", "to_state_diff", "to_get_error_dynamics", "to_error_expansion",
-    "to_get_expansion_records",
+    "to_get_expansion_records", "to_default_solve_options", "to_solve",
 ]
 
 

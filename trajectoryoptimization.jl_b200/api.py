@@ -1654,3 +1654,54 @@ def set_options(prob, **kw):
         setattr(o, k, v)
     prob._options = o
     prob._call("to_set_options", C.byref(o))
+
+
+# ---- solve!(prob): Altro's AL-iLQR solve to convergence, per instance (C ABI to_solve; semantics in include/trajopt_b200.h, DESIGN.md 5d) ----
+SOLVE_STATUS_NAMES = {K.SOLVE_UNSOLVED: "UNSOLVED", K.SOLVE_SUCCEEDED: "SOLVE_SUCCEEDED", K.SOLVE_MAX_ITERATIONS: "MAX_ITERATIONS",
+                      K.SOLVE_MAX_ITERATIONS_OUTER: "MAX_ITERATIONS_OUTER", K.SOLVE_MAX_REGULARIZATION: "MAX_REGULARIZATION"}
+
+
+class SolveStats:
+    """per-instance results of ``solve``, arrays of length B: ``status`` (to_solve_status codes, names in SOLVE_STATUS_NAMES),
+    ``iterations`` (all inner loops together), ``iterations_outer``, ``cost`` (the objective of the final trajectory), ``dJ`` and ``gradient``
+    of the last iteration, ``c_max`` (max violation when the last inner loop ended).  The trajectories, multipliers and gains stay in the
+    problem: ``states(prob)``, ``controls(prob)``, ``multipliers(prob, con)``, ``gains(prob)``."""
+
+    FIELDS = ("status", "iterations", "iterations_outer", "cost", "dJ", "gradient", "c_max")
+
+    def __init__(self, B):
+        self.status = np.zeros(B, dtype=np.int32)
+        self.iterations = np.zeros(B, dtype=np.int32)
+        self.iterations_outer = np.zeros(B, dtype=np.int32)
+        self.cost, self.dJ, self.gradient, self.c_max = np.zeros(B), np.zeros(B), np.zeros(B), np.zeros(B)
+
+    def status_names(self):
+        return [SOLVE_STATUS_NAMES.get(int(s), str(int(s))) for s in self.status]
+
+    def __repr__(self):
+        names, counts = np.unique(self.status_names(), return_counts=True)
+        return (f"SolveStats(B={len(self.status)}, status={dict(zip(names.tolist(), counts.tolist()))}, "
+                f"iterations {int(self.iterations.min())}..{int(self.iterations.max())})")
+
+
+def solve_options(**options):
+    """a ``to_solve_options`` with Altro's defaults (``to_default_solve_options``) and the given overrides; ArgumentError on unknown names"""
+    o = K.to_solve_options()
+    K.load_library().to_default_solve_options(C.byref(o))
+    for k, v in options.items():
+        if k not in dict(K.to_solve_options._fields_):
+            raise ArgumentError(f"unknown solve option {k}")
+        setattr(o, k, v)
+    return o
+
+
+def solve(prob, **options):
+    """solve!(prob): Altro's AL-iLQR solve of every instance to its own stopping point (Altro 0.3 SolverOptions names: cost_tolerance,
+    cost_tolerance_intermediate, gradient_tolerance, gradient_tolerance_intermediate, constraint_tolerance, iterations, iterations_inner,
+    iterations_outer, dJ_counter_limit).  The AL schedule (penalty_initial, penalty_scaling, ...) and the regularisation options are the
+    solver options of ``set_options``.  Returns a ``SolveStats``."""
+    o = solve_options(**options)
+    st = SolveStats(prob.B)
+    prob._call("to_solve", C.byref(o), K._ip(st.status), K._ip(st.iterations), K._ip(st.iterations_outer), K._dp(st.cost), K._dp(st.dJ),
+               K._dp(st.gradient), K._dp(st.c_max))
+    return st

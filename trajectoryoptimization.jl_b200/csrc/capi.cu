@@ -38,6 +38,10 @@ struct to_handle {
     bool partition = false;
     cudaStream_t stream_big = nullptr;
     cudaEvent_t ev_late = nullptr;
+    // to_solve: per-instance solve state on the device; the ACTIVE count of an iteration comes back through pinned memory + an event
+    SolveDev solve{};
+    int* pin_count = nullptr;           // [2] (pinned)
+    cudaEvent_t ev_count[2] = {nullptr, nullptr};
     std::string err;
     std::vector<void*> allocs;
     std::vector<DevCost> h_costs;
@@ -514,7 +518,10 @@ int to_create(const to_spec* s, to_handle** out) {
             cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_merit, cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&h->ev_cons, cudaEventDisableTiming) != cudaSuccess) { h->err = "side stream creation failed"; return bail(TO_ECUDA); }
+            cudaEventCreateWithFlags(&h->ev_cons, cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&h->ev_count[0], cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&h->ev_count[1], cudaEventDisableTiming) != cudaSuccess) { h->err = "side stream creation failed"; return bail(TO_ECUDA); }
+        if (cudaHostAlloc((void**)&h->pin_count, 2 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) { h->err = "cudaHostAlloc failed"; return bail(TO_ENOMEM); }
         // SM partition for the overlapped part of an iteration (A/B switch, off unless TO_PARTITION = SMs of the side stream's partition)
         const int part = getenv("TO_PARTITION") ? atoi(getenv("TO_PARTITION")) : 0;
         GreenPair gp;
@@ -623,6 +630,11 @@ int to_create(const to_spec* s, to_handle** out) {
     }
     ALLOC(h->d_stageX, P.strideX); ALLOC(h->d_stageU, P.strideU); ALLOC(h->d_viol, B); ALLOC(h->d_merit2, 2);
     ALLOC(h->d_work, 1); ALLOC(h->d_err, 1);
+    {   // to_solve state (solve.cu)
+        SolveDev& S = h->solve;
+        ALLOC(S.state, B); ALLOC(S.status, B); ALLOC(S.iter, B); ALLOC(S.outer, B); ALLOC(S.inner, B); ALLOC(S.dj_zero, B);
+        ALLOC(S.J_prev, B); ALLOC(S.dJ, B); ALLOC(S.grad, B); ALLOC(S.cmax, B); ALLOC(S.n_active, 1);
+    }
     if (P.frag) { ALLOC(h->d_fragq, frag_queue_ints(B)); ALLOC(h->d_fragpool, frag_pool_doubles(B, N)); ALLOC(h->d_fragerr, 1); ALLOC(h->d_exptab, 1); }
 #undef ALLOC
     if (rc) return bail(rc);
@@ -683,6 +695,8 @@ int to_destroy(to_handle* h) {
     if (h->ev_join) cudaEventDestroy(h->ev_join);
     if (h->ev_merit) cudaEventDestroy(h->ev_merit);
     if (h->ev_cons) cudaEventDestroy(h->ev_cons);
+    for (auto e : h->ev_count) if (e) cudaEventDestroy(e);
+    if (h->pin_count) cudaFreeHost(h->pin_count);
     if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
     delete h;
     return TO_OK;
@@ -1108,98 +1122,117 @@ int to_forward(to_handle* h, double* J, double* alpha) {
     if (J || alpha) CU(h, cudaStreamSynchronize(h->stream));
     return TO_OK;
 }
+// the ACTIVE count after the iteration's stopping-rule checks -> pinned slot `slot`, event ev_count[slot] (to_solve reads it one iteration later)
+static int record_active_count(to_handle* h, const SolveDev& sv, int slot, cudaStream_t st) {
+    CU(h, cudaMemcpyAsync(h->pin_count + slot, sv.n_active, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(h, cudaEventRecord(h->ev_count[slot], st));
+    return TO_OK;
+}
+// One iteration of to_ilqr_step.  Per iteration: E (expansion) -> R (Riccati) -> F pass 1 (alpha = 1..1/8, ~90% of the instances) -> F pass 2 (the rest).
+// Pass 2 is latency-bound and touches few instances, so it runs on a high-priority side stream followed by the
+// expansion of ITS instances, concurrently with the next iteration's expansion of the instances pass 1 accepted
+// (instances never interact); the Riccati pass joins both. The overlap carries across calls (h->side_pending): any
+// other entry point joins the side stream first.
+// sv (to_solve): the stopping-rule check of every ACTIVE instance right after its line search -- for the two halves of an overlapped iteration
+// on their own streams, before the next iteration's expansion of each -- and the ACTIVE count behind it (record_active_count).
+static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
+    // (error state: only [A_e B_e] is needed by the solver kernels -- k_expand_lie; the full [A B] is produced by to_expand on request)
+    auto expand = [&](cudaStream_t st, int mode) { return h->P.lie ? launch_expand_lie(h->P, st, mode) : launch_expand(h->P, st, mode); };
+    bool costexp_done = false;
+    const bool rec = h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5 && rec_fused(h->P);
+    static const int order = getenv("TO_ITER_ORDER") ? atoi(getenv("TO_ITER_ORDER")) : 0;
+    if (h->side_pending && order == 1) {
+        // TO_ITER_ORDER=1 (A/B): only the latency-bound cost expansion of the instances accepted in pass 1 runs beside the late trials;
+        // the dynamics expansion of EVERY instance and the cost expansion of the late ones follow the join.  An A/B experiment against
+        // the default order below; not the default, and not measured on the H100.
+        if (rec) {
+            { PhaseScope pe(h, TO_PHASE_COSTEXP); CU(h, launch_expansion_rec16(h->P, h->stream, 1)); }
+            h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
+        }
+        JOIN(h);
+        { PhaseScope ps(h, TO_PHASE_EXPAND); CU(h, expand(h->stream, 0)); }
+        h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
+        if (rec) {
+            { PhaseScope pl(h, TO_PHASE_LATE); CU(h, launch_expansion_rec16(h->P, h->stream, 2)); }
+            h->launches++; h->phase_launches[TO_PHASE_LATE]++;
+            costexp_done = true;
+        }
+    } else {
+        if (h->side_pending && h->partition) {
+            // SM partition: the late trials keep their own SMs (stream2); the expansion of the instances accepted in pass 1, then (once the
+            // late trials are through) the expansion of the late instances run on the other partition; the main stream waits for both.
+            cudaStream_t sb = h->stream_big;
+            CU(h, cudaStreamWaitEvent(sb, h->ev_fork, 0));                   // after pass 1 of the line search (and, in to_solve, the check of its instances)
+            if (rec) {
+                { PhaseScope pe(h, TO_PHASE_COSTEXP, sb); CU(h, launch_expansion_rec16(h->P, sb, 1)); }
+                h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
+                costexp_done = true;
+            }
+            { PhaseScope ps(h, TO_PHASE_EXPAND, sb); CU(h, expand(sb, 1)); }
+            h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
+            CU(h, cudaEventRecord(h->ev_late, h->stream2));                  // everything the side stream holds: the late trials (+ a merit reduction)
+            CU(h, cudaStreamWaitEvent(sb, h->ev_late, 0));
+            {
+                PhaseScope pl(h, TO_PHASE_LATE, sb);
+                CU(h, expand(sb, 2)); h->launches++;
+                if (rec) { CU(h, launch_expansion_rec16(h->P, sb, 2)); h->launches++; }
+            }
+            h->phase_launches[TO_PHASE_LATE]++;
+            CU(h, cudaEventRecord(h->ev_join, sb));
+            goto joined;
+        }
+        if (h->side_pending) {
+            {
+                PhaseScope pl(h, TO_PHASE_LATE, h->stream2);
+                CU(h, expand(h->stream2, 2)); h->launches++;
+                if (rec) { CU(h, launch_expansion_rec16(h->P, h->stream2, 2)); h->launches++; }
+            }
+            h->phase_launches[TO_PHASE_LATE]++;
+            if (rec) {
+                { PhaseScope pe(h, TO_PHASE_COSTEXP); CU(h, launch_expansion_rec16(h->P, h->stream, 1)); }
+                h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
+                costexp_done = true;
+            }
+            CU(h, cudaEventRecord(h->ev_join, h->stream2));
+        }
+        { PhaseScope ps(h, TO_PHASE_EXPAND); CU(h, expand(h->stream, h->side_pending ? 1 : 0)); }
+        h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
+    }
+joined:
+    JOIN(h);
+    h->expanded = true;
+    int rc = do_backward(h, costexp_done); if (rc) return rc;
+    { PhaseScope ps(h, TO_PHASE_FORWARD); CU(h, launch_forward(h->P, h->stream)); }
+    h->launches++; h->phase_launches[TO_PHASE_FORWARD]++;
+    if (h->overlap) {
+        // to_solve: the stopping-rule check of the instances pass 1 accepted (final for this iteration) comes before the fork, so that
+        // everything ordered after ev_fork -- the late trials, the side stream's ACTIVE count, the partition's expansions -- sees its decisions
+        if (sv) { CU(h, launch_solve_check(h->P, *sv, 1, h->stream)); h->launches++; }
+        CU(h, cudaEventRecord(h->ev_fork, h->stream));
+        CU(h, cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));
+        { PhaseScope ps(h, TO_PHASE_LADDER, h->stream2); CU(h, launch_ladder(h->P, h->stream2)); }
+        if (sv) { CU(h, launch_solve_check(h->P, *sv, 2, h->stream2)); h->launches++; }      // ... the others, before their expansion on the side stream
+        if (sv) { int rc2 = record_active_count(h, *sv, slot, h->stream2); if (rc2) return rc2; }
+        CU(h, cudaEventRecord(h->ev_join, h->stream2));
+        h->side_pending = true;
+    } else {
+        { PhaseScope ps(h, TO_PHASE_LADDER); CU(h, launch_ladder(h->P, h->stream)); }
+        if (sv) {
+            CU(h, launch_solve_check(h->P, *sv, 0, h->stream)); h->launches++;
+            int rc2 = record_active_count(h, *sv, slot, h->stream); if (rc2) return rc2;
+        }
+    }
+    h->launches++; h->phase_launches[TO_PHASE_LADDER]++;
+    h->expanded = false; h->backward_done = false;   // the trajectory moved
+    return TO_OK;
+}
 int to_ilqr_step(to_handle* h, int32_t iters) {
     if (!h || iters < 0) return TO_EINVAL;
     DeviceGuard device_guard(h);
     int rc = solver_supported(h); if (rc) return rc;
     if (!h->J_valid) { rc = join_side(h); if (rc) return rc; }
     rc = ensure_merit(h); if (rc) return rc;
-    // Per iteration: E (expansion) -> R (Riccati) -> F pass 1 (alpha = 1..1/8, ~90% of the instances) -> F pass 2 (the rest).
-    // Pass 2 is latency-bound and touches few instances, so it runs on a high-priority side stream followed by the
-    // expansion of ITS instances, concurrently with the next iteration's expansion of the instances pass 1 accepted
-    // (instances never interact); the Riccati pass joins both. The overlap carries across calls (h->side_pending): any
-    // other entry point joins the side stream first.
-    for (int it = 0; it < iters; it++) {
-        // (error state: only [A_e B_e] is needed by the solver kernels -- k_expand_lie; the full [A B] is produced by to_expand on request)
-        auto expand = [&](cudaStream_t st, int mode) { return h->P.lie ? launch_expand_lie(h->P, st, mode) : launch_expand(h->P, st, mode); };
-        bool costexp_done = false;
-        const bool rec = h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5 && rec_fused(h->P);
-        static const int order = getenv("TO_ITER_ORDER") ? atoi(getenv("TO_ITER_ORDER")) : 0;
-        if (h->side_pending && order == 1) {
-            // TO_ITER_ORDER=1 (A/B): only the latency-bound cost expansion of the instances accepted in pass 1 runs beside the late trials;
-            // the dynamics expansion of EVERY instance and the cost expansion of the late ones follow the join.  An A/B experiment against
-            // the default order below; not the default, and not measured on the H100.
-            if (rec) {
-                { PhaseScope pe(h, TO_PHASE_COSTEXP); CU(h, launch_expansion_rec16(h->P, h->stream, 1)); }
-                h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
-            }
-            JOIN(h);
-            { PhaseScope ps(h, TO_PHASE_EXPAND); CU(h, expand(h->stream, 0)); }
-            h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
-            if (rec) {
-                { PhaseScope pl(h, TO_PHASE_LATE); CU(h, launch_expansion_rec16(h->P, h->stream, 2)); }
-                h->launches++; h->phase_launches[TO_PHASE_LATE]++;
-                costexp_done = true;
-            }
-        } else {
-            if (h->side_pending && h->partition) {
-                // SM partition: the late trials keep their own SMs (stream2); the expansion of the instances accepted in pass 1, then (once the
-                // late trials are through) the expansion of the late instances run on the other partition; the main stream waits for both.
-                cudaStream_t sb = h->stream_big;
-                CU(h, cudaStreamWaitEvent(sb, h->ev_fork, 0));                   // after pass 1 of the line search (nothing has followed it on the main stream)
-                if (rec) {
-                    { PhaseScope pe(h, TO_PHASE_COSTEXP, sb); CU(h, launch_expansion_rec16(h->P, sb, 1)); }
-                    h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
-                    costexp_done = true;
-                }
-                { PhaseScope ps(h, TO_PHASE_EXPAND, sb); CU(h, expand(sb, 1)); }
-                h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
-                CU(h, cudaEventRecord(h->ev_late, h->stream2));                  // everything the side stream holds: the late trials (+ a merit reduction)
-                CU(h, cudaStreamWaitEvent(sb, h->ev_late, 0));
-                {
-                    PhaseScope pl(h, TO_PHASE_LATE, sb);
-                    CU(h, expand(sb, 2)); h->launches++;
-                    if (rec) { CU(h, launch_expansion_rec16(h->P, sb, 2)); h->launches++; }
-                }
-                h->phase_launches[TO_PHASE_LATE]++;
-                CU(h, cudaEventRecord(h->ev_join, sb));
-                goto joined;
-            }
-            if (h->side_pending) {
-                {
-                    PhaseScope pl(h, TO_PHASE_LATE, h->stream2);
-                    CU(h, expand(h->stream2, 2)); h->launches++;
-                    if (rec) { CU(h, launch_expansion_rec16(h->P, h->stream2, 2)); h->launches++; }
-                }
-                h->phase_launches[TO_PHASE_LATE]++;
-                if (rec) {
-                    { PhaseScope pe(h, TO_PHASE_COSTEXP); CU(h, launch_expansion_rec16(h->P, h->stream, 1)); }
-                    h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
-                    costexp_done = true;
-                }
-                CU(h, cudaEventRecord(h->ev_join, h->stream2));
-            }
-            { PhaseScope ps(h, TO_PHASE_EXPAND); CU(h, expand(h->stream, h->side_pending ? 1 : 0)); }
-            h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
-        }
-    joined:
-        JOIN(h);
-        h->expanded = true;
-        rc = do_backward(h, costexp_done); if (rc) return rc;
-        { PhaseScope ps(h, TO_PHASE_FORWARD); CU(h, launch_forward(h->P, h->stream)); }
-        h->launches++; h->phase_launches[TO_PHASE_FORWARD]++;
-        if (h->overlap) {
-            CU(h, cudaEventRecord(h->ev_fork, h->stream));
-            CU(h, cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));
-            { PhaseScope ps(h, TO_PHASE_LADDER, h->stream2); CU(h, launch_ladder(h->P, h->stream2)); }
-            CU(h, cudaEventRecord(h->ev_join, h->stream2));
-            h->side_pending = true;
-        } else {
-            PhaseScope ps(h, TO_PHASE_LADDER); CU(h, launch_ladder(h->P, h->stream));
-        }
-        h->launches++; h->phase_launches[TO_PHASE_LADDER]++;
-        h->expanded = false; h->backward_done = false;   // the trajectory moved
-    }
+    for (int it = 0; it < iters; it++) { rc = ilqr_iteration(h, nullptr, 0); if (rc) return rc; }
     return TO_OK;
 }
 int to_al_update(to_handle* h) {
@@ -1225,6 +1258,88 @@ int to_get_gains(to_handle* h, double* K, double* d) {
     if (!h) return TO_EINVAL;
     if (K) CU(h, cudaMemcpyAsync(K, h->P.K, sizeof(double) * (size_t)h->P.B * (h->P.N - 1) * h->P.ne * h->P.m, cudaMemcpyDeviceToHost, h->stream));
     if (d) CU(h, cudaMemcpyAsync(d, h->P.d, sizeof(double) * (size_t)h->P.B * (h->P.N - 1) * h->P.m, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return TO_OK;
+}
+// ---- solve to convergence (solve.cu; semantics in include/trajopt_b200.h and DESIGN.md 5d) ----------------------------------------------
+int to_default_solve_options(to_solve_options* o) {
+    if (!o) return TO_EINVAL;
+    o->cost_tolerance = 1e-4; o->cost_tolerance_intermediate = 1e-3;
+    o->gradient_tolerance = 10.0; o->gradient_tolerance_intermediate = 1.0;
+    o->constraint_tolerance = 1e-6;
+    o->iterations = 300; o->iterations_inner = 300; o->iterations_outer = 30; o->dJ_counter_limit = 10;
+    return TO_OK;
+}
+// the solve with P.active set (to_solve clears it on every exit)
+static int solve_run(to_handle* h) {
+    SolveDev& S = h->solve;
+    DevProblem& P = h->P;
+    CU(h, launch_solve_init(P, S, h->stream)); h->launches++;      // every instance ACTIVE, rho = bp_reg_initial, counters zero
+    CU(h, launch_rollout(P, h->stream)); h->launches++;
+    CU(h, launch_merit(P, P.J, h->d_viol, h->stream)); h->launches++;
+    h->J_valid = true;
+    CU(h, launch_solve_begin(P, S, h->stream)); h->launches++;
+    for (;;) {
+        // inner loops: iterations are queued without waiting for each other; the ACTIVE count of iteration i - 1 (ordered after both of its
+        // checks) is read while iteration i is in the queue, so one iteration in which no instance is ACTIVE (every kernel exits at once)
+        // follows the last real one
+        int prev = -1;
+        for (int it = 0;; it++) {
+            const int slot = it & 1;
+            int rc = ilqr_iteration(h, &S, slot); if (rc) return rc;
+            if (prev >= 0) {
+                CU(h, cudaEventSynchronize(h->ev_count[prev]));
+                if (h->pin_count[prev] == 0) break;
+            }
+            prev = slot;
+            if (it > S.opt.iterations + 1) return fail(h, TO_ESTATE, "to_solve: an inner loop outlived the iteration cap");
+        }
+        int rc = join_side(h); if (rc) return rc;
+        if (P.ncon == 0) break;                                       // no constraints: the iLQR loop decided every status
+        // outer step: the WAITING instances are done or go on; the ones that go on get the dual update, the penalties of the next outer
+        // iteration and a fresh merit
+        CU(h, launch_solve_outer(P, S, h->stream)); h->launches++;
+        CU(h, cudaMemcpyAsync(h->pin_count, S.n_active, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+        if (h->pin_count[0] == 0) break;
+        CU(h, launch_al_update(P, h->stream)); h->launches++;        // ACTIVE instances only; also resets their rho / drho
+        for (auto& mu : h->h_mu) mu = std::fmin(mu * P.opt.penalty_scaling, P.opt.penalty_max);
+        CU(h, cudaMemcpyAsync(h->d_mu, h->h_mu.data(), sizeof(double) * h->h_mu.size(), cudaMemcpyHostToDevice, h->stream));
+        CU(h, cudaStreamSynchronize(h->stream));
+        rc = upload_exptab(h); if (rc) return rc;                     // the penalties are part of the table
+        CU(h, launch_merit(P, P.J, h->d_viol, h->stream)); h->launches++;
+        CU(h, launch_solve_begin(P, S, h->stream)); h->launches++;
+    }
+    return TO_OK;
+}
+int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* cost, double* dJ,
+             double* gradient, double* c_max) {
+    JOIN(h);
+    if (!h || !o) return TO_EINVAL;
+    if (!(o->cost_tolerance > 0) || !(o->cost_tolerance_intermediate > 0) || !(o->gradient_tolerance > 0) || !(o->gradient_tolerance_intermediate > 0) ||
+        !(o->constraint_tolerance > 0))
+        return fail(h, TO_EINVAL, "to_solve: tolerances must be positive");
+    if (o->iterations < 1 || o->iterations_inner < 1 || o->iterations_outer < 1 || o->dJ_counter_limit < 0)
+        return fail(h, TO_EINVAL, "to_solve: iterations, iterations_inner and iterations_outer must be positive, dJ_counter_limit non-negative");
+    int rc = solver_supported(h); if (rc) return rc;
+    SolveDev& S = h->solve;
+    S.opt = SolveOpts{o->cost_tolerance, o->cost_tolerance_intermediate, o->gradient_tolerance, o->gradient_tolerance_intermediate, o->constraint_tolerance,
+                      o->iterations, o->iterations_inner, o->iterations_outer, o->dJ_counter_limit};
+    h->P.active = S.state;
+    rc = solve_run(h);
+    const int jrc = join_side(h);
+    h->P.active = nullptr;                 // every other entry point works on every instance again
+    h->J_valid = false; h->expanded = false; h->backward_done = false;   // (the merits of the instances that stopped early belong to older penalties)
+    if (rc) return rc;
+    if (jrc) return jrc;
+    const int B = h->P.B;
+    if (cost) { rc = run_to_host(h, B, cost, [](to_handle* hh, double* d) { return launch_cost(hh->P, d, nullptr, hh->stream); }); if (rc) return rc; }
+    if (status) CU(h, cudaMemcpyAsync(status, S.status, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
+    if (iterations) CU(h, cudaMemcpyAsync(iterations, S.iter, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
+    if (iterations_outer) CU(h, cudaMemcpyAsync(iterations_outer, S.outer, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
+    if (dJ) CU(h, cudaMemcpyAsync(dJ, S.dJ, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
+    if (gradient) CU(h, cudaMemcpyAsync(gradient, S.grad, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
+    if (c_max) CU(h, cudaMemcpyAsync(c_max, S.cmax, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
     return TO_OK;
 }

@@ -153,7 +153,14 @@ struct DevProblem {
     int* late_list;           // [B] the instances pass 1 did not accept, in arrival order (written by pass 1, walked by the later passes)
     int* late_count;          // [1] ... and how many; late_list == nullptr: the later passes scan every instance
     size_t strideX, strideU;  // elements between the two trajectory buffers
+    // to_solve (capi.cu): per-instance solve state, SOLVE_ACTIVE / SOLVE_WAITING / SOLVE_DONE.  The per-instance kernels of an iteration
+    // skip every instance that is not ACTIVE, so a converged instance keeps the X, U, lambda, K, d, rho, J it stopped with.
+    // nullptr outside to_solve: every instance is worked on.
+    const int* active;        // [B]
 };
+
+enum { SOLVE_ACTIVE = 0, SOLVE_WAITING = 1, SOLVE_DONE = 2 };
+__host__ __device__ inline bool retired(const DevProblem& P, int b) { return P.active != nullptr && P.active[b] != SOLVE_ACTIVE; }
 
 __host__ __device__ inline const double* traj_X(const DevProblem& P, int buf, int b) { return P.X + buf * P.strideX + (size_t)b * P.N * P.n; }
 __host__ __device__ inline const double* traj_U(const DevProblem& P, int buf, int b) { return P.U + buf * P.strideU + (size_t)b * (P.N - 1) * P.m; }

@@ -407,7 +407,8 @@ __global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, 
     int b = blockIdx.x * IPB + g;
     if (!first_pass && P.late_list) b = (b < *P.late_count) ? P.late_list[b] : P.B;
     const unsigned gmask = (G == 32) ? 0xffffffffu : (((1u << G) - 1u) << (g * G));
-    const bool valid = b < P.B && threadIdx.x < LANES;
+    // (to_solve: an instance that is not ACTIVE is neither tried, accepted, late-listed nor committed)
+    const bool valid = b < P.B && threadIdx.x < LANES && !retired(P, b);
     const int status = valid ? P.bp_status[b] : -1;
     const int was_accepted = (valid && !first_pass) ? P.accepted[b] : 0;
     const bool work = valid && status >= 0 && !was_accepted && trial0 <= P.opt.ls_iters;

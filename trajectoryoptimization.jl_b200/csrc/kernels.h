@@ -47,3 +47,26 @@ cudaError_t launch_backward_frag(const DevProblem& P, int* queue, double* pool, 
 cudaError_t launch_forward(const DevProblem& P, cudaStream_t s);
 cudaError_t launch_ladder(const DevProblem& P, cudaStream_t s);
 cudaError_t launch_accept(const DevProblem& P, cudaStream_t s);
+// to_solve: per-instance stopping rules (solve.cu).  The options are to_solve_options (include/trajopt_b200.h) field for field.
+struct SolveOpts {
+    double cost_tolerance, cost_tolerance_intermediate, gradient_tolerance, gradient_tolerance_intermediate, constraint_tolerance;
+    int iterations, iterations_inner, iterations_outer, dJ_counter_limit;
+};
+struct SolveDev {
+    SolveOpts opt;
+    int* state;        // [B] SOLVE_ACTIVE / SOLVE_WAITING / SOLVE_DONE (DevProblem::active during to_solve)
+    int* status;       // [B] to_solve_status
+    int* iter;         // [B] iterations, all inner loops together
+    int* outer;        // [B] outer (AL) iteration, 1-based
+    int* inner;        // [B] iterations of the current inner loop
+    int* dj_zero;      // [B] failed line searches in the current inner loop
+    double* J_prev;    // [B] merit before the last step
+    double* dJ;        // [B] last dJ
+    double* grad;      // [B] last gradient (Altro gradient_todorov)
+    double* cmax;      // [B] max violation when the last inner loop ended
+    int* n_active;     // [1] instances ACTIVE
+};
+cudaError_t launch_solve_init(const DevProblem& P, const SolveDev& S, cudaStream_t s);
+cudaError_t launch_solve_begin(const DevProblem& P, const SolveDev& S, cudaStream_t s);
+cudaError_t launch_solve_check(const DevProblem& P, const SolveDev& S, int mode, cudaStream_t s);   // mode as launch_expand
+cudaError_t launch_solve_outer(const DevProblem& P, const SolveDev& S, cudaStream_t s);

@@ -138,6 +138,7 @@ __global__ void __launch_bounds__(128) k_expansion_compact(const DevProblem P) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)P.B * P.N) return;
     const int k = (int)(t % P.N), b = (int)(t / P.N);
+    if (retired(P, b)) return;                                     // to_solve: not ACTIVE
     const bool last = (k == P.N - 1);
     const double* xg = traj_X(P, P.cur[b], b) + (size_t)k * n;
     const double* ug = traj_U(P, P.cur[b], b) + (size_t)k * m;
@@ -203,7 +204,7 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense(const DevProblem P
     __shared__ SM smem[WARPS];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.x * WARPS + warp;
-    if (b >= P.B) return;
+    if (b >= P.B || retired(P, b)) return;       // (to_solve: not ACTIVE)
     SM& sm = smem[warp];
     const int N = P.N;
     const double* ABg = P.ABe + (size_t)b * (N - 1) * NR * NME;
@@ -399,7 +400,7 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
     extern __shared__ __align__(16) unsigned char dense_smem_raw[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int b = blockIdx.x * WARPS + warp;
-    if (b >= P.B) return;
+    if (b >= P.B || retired(P, b)) return;       // (to_solve: not ACTIVE)
     MmaSmem& sm = reinterpret_cast<MmaSmem*>(dense_smem_raw)[warp];
     const int fr = lane >> 2, fc = lane & 3;      // fragment coordinates: A(8x4) row fr col fc ; B(4x8) row fc col fr ; D(8x8) row fr cols 2fc, 2fc+1
     const int N = P.N;

@@ -259,6 +259,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         if (lane == 0) b = atomicAdd(work_counter, 1);
         b = __shfl_sync(0xffffffffu, b, 0);
         if (b >= P.B) break;
+        if (retired(P, b)) continue;            // to_solve: not ACTIVE
 
         const int buf = P.cur[b];
         const double* X = traj_X(P, buf, b);

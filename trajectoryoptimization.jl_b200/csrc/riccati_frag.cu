@@ -124,6 +124,7 @@ __global__ void __launch_bounds__(128) k_expansion_rec(const DevProblem P) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)P.B * P.N) return;
     const int k = (int)(t % P.N), b = (int)(t / P.N);
+    if (retired(P, b)) return;                                     // to_solve: not ACTIVE
     const bool last = (k == P.N - 1);
     const double* xg = traj_X(P, P.cur[b], b) + (size_t)k * n;
     const double* ug = traj_U(P, P.cur[b], b) + (size_t)k * m;
@@ -262,8 +263,13 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_riccati_frag(const DevProb
         if (lane == 0) idx = atomicAdd(q_head, 1);
         idx = __shfl_sync(0xffffffffu, idx, 0);
         int b, cand;
-        if (idx < P.B) { b = idx; cand = 0; }
-        else {
+        if (idx < P.B) {
+            b = idx; cand = 0;
+            if (retired(P, b)) {                    // to_solve: not ACTIVE -- counts as finalised, so the queue still drains at nfinal == B
+                if (lane == 0) atomicAdd(q_nfinal, 1);
+                continue;
+            }
+        } else {
             const int qi = idx - P.B;
             int item = -2;
             if (lane == 0) {

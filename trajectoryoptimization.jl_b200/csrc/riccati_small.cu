@@ -72,7 +72,7 @@ template <int N_, int M_>
 __global__ void __maxnreg__(255) k_riccati_small(const DevProblem P) {
     constexpr int n = N_, m = M_, nm = n + m;
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= P.B) return;
+    if (b >= P.B || retired(P, b)) return;       // (to_solve: not ACTIVE)
     const int N = P.N, ld = P.ldab;
     const int buf = P.cur[b];
     const double* X = traj_X(P, buf, b);

@@ -83,6 +83,7 @@ __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
     const int k = (int)(bk % (P.N - 1));
     const int b = (int)(bk / (P.N - 1));
     if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) return;     // overlapped expansion: this launch covers the other group
+    if (retired(P, b)) return;                                     // to_solve: not ACTIVE
     double* AB = P.AB + ((size_t)b * (P.N - 1) + k) * n * ld;     // pad columns nm..ld-1 stay zero from to_create
     const double* X = traj_X(P, P.cur[b], b) + (size_t)k * n;
     const double* U = traj_U(P, P.cur[b], b) + (size_t)k * m;
@@ -227,6 +228,7 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
     const int k = (int)(bk % (P.N - 1));
     const int b = (int)(bk / (P.N - 1));
     if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) return;
+    if (retired(P, b)) return;                                     // to_solve: not ACTIVE
     const double* X = traj_X(P, P.cur[b], b) + (size_t)k * n;
     const double* U = traj_U(P, P.cur[b], b) + (size_t)k * m;
     const double h = P.dt[k];
@@ -276,6 +278,7 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
         if (slot >= *P.late_count) return;
         b = P.late_list[slot];
     } else if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) return;                   // overlapped iterations: the other launch covers this instance
+    if (retired(P, b)) return;                                                         // to_solve: not ACTIVE (uniform over the CTA)
     const int k0 = kb * EXPB_KPB;
     const int nk = (P.N - 1 - k0 < EXPB_KPB) ? P.N - 1 - k0 : EXPB_KPB;
     const int tid = threadIdx.x, kk = tid / NS, sd = tid - kk * NS;
@@ -398,6 +401,7 @@ __global__ void __launch_bounds__(TO_CEXP_THREADS, TO_CEXP_MINB * 256 / TO_CEXP_
     for (int bk = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 4); bk < total; bk += ngroups) {      // (whole 16-lane groups iterate together)
         const int b = bk / N, k = bk - b * N;
         if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) continue;     // overlapped iterations: this launch covers the other group (see k_expand)
+        if (retired(P, b)) continue;                                    // to_solve: not ACTIVE
         const bool last = (k == N - 1);
         const double* X = traj_X(P, P.cur[b], b) + (size_t)k * n;
         const double* U = traj_U(P, P.cur[b], b) + (size_t)(last ? 0 : k) * P.m;      // (not read at the terminal knot)
@@ -488,6 +492,7 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
     for (int unit = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 4); unit < total; unit += ngroups) {
         const int b = unit / NB, kb = (unit - b * NB) << 4;
         if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) continue;                   // (uniform over the group)
+        if (retired(P, b)) continue;                                                   // to_solve: not ACTIVE
         const int buf = P.cur[b];
         const double* __restrict__ Xb = traj_X(P, buf, b);
         const double* __restrict__ Ub = traj_U(P, buf, b);

@@ -1,0 +1,118 @@
+// solve.cu -- the per-instance stopping rules of to_solve (Altro's AL-iLQR `solve!`, restated in DESIGN.md 5d and include/trajopt_b200.h).
+//
+// The iteration itself is the one to_ilqr_step runs (expansion, backward pass, line search).  These kernels only DECIDE, one thread per
+// instance: after an instance's line search, whether its inner (iLQR) loop goes on; after every inner loop of the batch has ended, whether
+// an instance is done or goes on to another outer (AL) iteration.  An instance whose loop has ended is marked WAITING or DONE in
+// SolveDev::state, which is DevProblem::active while to_solve runs: every per-instance kernel of the iteration then skips it.
+#include "../../include/trajopt_b200.h"
+#include "kernels.h"
+
+namespace {
+
+// Altro gradient_todorov: mean over the knots of max_i |d_k,i| / (|u_k,i| + 1), with the controls after the step
+__device__ double todorov_gradient(const DevProblem& P, int b) {
+    const int m = P.m, N = P.N;
+    const double* U = traj_U(P, P.cur[b], b);
+    const double* d = P.d + (size_t)b * (N - 1) * m;
+    double acc = 0.0;
+    for (int k = 0; k < N - 1; k++) {
+        double g = 0.0;
+        for (int i = 0; i < m; i++) g = fmax(g, fabs(d[(size_t)k * m + i]) / (fabs(U[(size_t)k * m + i]) + 1.0));
+        acc += g;
+    }
+    return acc / (N - 1);
+}
+
+__global__ void k_solve_init(const DevProblem P, SolveDev S) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b == 0) *S.n_active = P.B;
+    if (b >= P.B) return;
+    S.state[b] = SOLVE_ACTIVE; S.status[b] = TO_SOLVE_UNSOLVED;
+    S.iter[b] = 0; S.outer[b] = 1; S.inner[b] = 0; S.dj_zero[b] = 0;
+    S.dJ[b] = 0.0; S.grad[b] = 0.0; S.cmax[b] = 0.0;
+    P.rho[b] = P.opt.bp_reg_initial; P.drho[b] = 0.0;      // Altro initialize!: the regularisation restarts
+}
+
+// start of an inner loop of the ACTIVE instances: J_prev = the merit of the live trajectory (with the current multipliers and penalties)
+__global__ void k_solve_begin(const DevProblem P, SolveDev S) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P.B || S.state[b] != SOLVE_ACTIVE) return;
+    S.J_prev[b] = P.J[b]; S.inner[b] = 0; S.dj_zero[b] = 0;
+}
+
+// after the line search of instance b.  mode 1 / 2: only the instances the first line-search pass accepted / did not accept (the two halves
+// of an overlapped iteration, capi.cu), 0: all.
+__global__ void k_solve_check(const DevProblem P, SolveDev S, int mode) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P.B || S.state[b] != SOLVE_ACTIVE) return;
+    if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) return;
+    const SolveOpts& o = S.opt;
+    const int iter = ++S.iter[b], inner = ++S.inner[b];
+    const bool constrained = P.ncon > 0;
+    // Altro set_tolerances!: the intermediate tolerances except in the last allowed outer iteration; no constraints: the plain iLQR loop
+    const bool final_tol = !constrained || S.outer[b] >= o.iterations_outer;
+    const double ctol = final_tol ? o.cost_tolerance : o.cost_tolerance_intermediate;
+    const double gtol = final_tol ? o.gradient_tolerance : o.gradient_tolerance_intermediate;
+    int next = SOLVE_ACTIVE, status = TO_SOLVE_UNSOLVED;
+    if (P.bp_status[b] < 0) {                      // the backward pass failed at bp_reg_max: terminal
+        S.dJ[b] = 0.0;
+        next = SOLVE_DONE; status = TO_SOLVE_MAX_REGULARIZATION;
+    } else {
+        const double J = P.J[b];
+        const bool stepped = P.alpha[b] > 0.0;
+        const double dJ = stepped ? S.J_prev[b] - J : 0.0;
+        if (!stepped) S.dj_zero[b]++;
+        S.J_prev[b] = J;
+        const double grad = todorov_gradient(P, b);
+        S.dJ[b] = dJ; S.grad[b] = grad;
+        const bool converged = stepped && dJ >= 0.0 && dJ < ctol && grad < gtol;
+        const bool ended = converged || S.dj_zero[b] > o.dJ_counter_limit || iter >= o.iterations || (constrained && inner >= o.iterations_inner);
+        if (ended) {
+            if (constrained) next = SOLVE_WAITING;          // the outer step (k_solve_outer) decides
+            else { next = SOLVE_DONE; status = converged ? TO_SOLVE_SUCCEEDED : iter >= o.iterations ? TO_SOLVE_MAX_ITERATIONS : TO_SOLVE_UNSOLVED; }
+        }
+    }
+    if (next != SOLVE_ACTIVE) {
+        S.cmax[b] = constrained ? P.viol[b] : 0.0;    // max violation of the live trajectory (the line search keeps it current)
+        S.status[b] = status;
+        S.state[b] = next;
+        __threadfence();
+        atomicSub(S.n_active, 1);
+    }
+}
+
+// every inner loop has ended: the WAITING instances are done, or go on to another outer iteration (ACTIVE again)
+__global__ void k_solve_outer(const DevProblem P, SolveDev S) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P.B || S.state[b] != SOLVE_WAITING) return;
+    const SolveOpts& o = S.opt;
+    int status = TO_SOLVE_UNSOLVED;
+    if (S.cmax[b] < o.constraint_tolerance) status = TO_SOLVE_SUCCEEDED;
+    else if (S.iter[b] >= o.iterations) status = TO_SOLVE_MAX_ITERATIONS;
+    else if (S.outer[b] >= o.iterations_outer) status = TO_SOLVE_MAX_ITERATIONS_OUTER;
+    if (status != TO_SOLVE_UNSOLVED) { S.status[b] = status; S.state[b] = SOLVE_DONE; return; }
+    S.outer[b]++;
+    S.state[b] = SOLVE_ACTIVE;
+    atomicAdd(S.n_active, 1);
+}
+
+inline unsigned nblk(int count) { return (unsigned)((count + 127) / 128); }
+
+}  // namespace
+
+cudaError_t launch_solve_init(const DevProblem& P, const SolveDev& S, cudaStream_t s) {
+    k_solve_init<<<nblk(P.B), 128, 0, s>>>(P, S);
+    return cudaGetLastError();
+}
+cudaError_t launch_solve_begin(const DevProblem& P, const SolveDev& S, cudaStream_t s) {
+    k_solve_begin<<<nblk(P.B), 128, 0, s>>>(P, S);
+    return cudaGetLastError();
+}
+cudaError_t launch_solve_check(const DevProblem& P, const SolveDev& S, int mode, cudaStream_t s) {
+    k_solve_check<<<nblk(P.B), 128, 0, s>>>(P, S, mode);
+    return cudaGetLastError();
+}
+cudaError_t launch_solve_outer(const DevProblem& P, const SolveDev& S, cudaStream_t s) {
+    k_solve_outer<<<nblk(P.B), 128, 0, s>>>(P, S);
+    return cudaGetLastError();
+}

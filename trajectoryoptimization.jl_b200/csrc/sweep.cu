@@ -29,6 +29,7 @@ template <bool WITH_AL>
 __global__ void __launch_bounds__(128) k_cost(const DevProblem P, double* __restrict__ J, double* __restrict__ Jk,
                                               double* __restrict__ viol_out) {
     const int b = blockIdx.x;
+    if (retired(P, b)) return;          // to_solve: not ACTIVE (uniform over the CTA)
     const int n = P.n, m = P.m, N = P.N;
     const double* X = traj_X(P, P.cur[b], b);
     const double* U = traj_U(P, P.cur[b], b);
@@ -159,6 +160,7 @@ __global__ void k_hess_projection(int cone, int p, int count, const double* __re
 // dual update: lambda <- clamp(Pi_{K*}(lambda - mu c)); one thread per (instance, constraint, knot)
 __global__ void k_al_update(const DevProblem P) {
     const int b = blockIdx.x;
+    if (retired(P, b)) return;          // to_solve: only the instances that go on to another outer iteration
     double* lam_b = P.lambda + (size_t)b * P.lambda_len;
     const double* X = traj_X(P, P.cur[b], b);
     const double* U = traj_U(P, P.cur[b], b);

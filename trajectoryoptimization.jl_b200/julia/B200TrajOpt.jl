@@ -331,6 +331,39 @@ function max_violation(p::BatchedProblem)
     check(p.h, ccall((:to_max_violation, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}), p.h, v)); v
 end
 
+# Altro's AL-iLQR solve!, per instance, on the device (to_solve; include/trajopt_b200.h, DESIGN.md 5d).  Keywords: Altro 0.3 SolverOptions
+# names (cost_tolerance, cost_tolerance_intermediate, gradient_tolerance, gradient_tolerance_intermediate, constraint_tolerance, iterations,
+# iterations_inner, iterations_outer, dJ_counter_limit).  Returns the per-instance summary Altro prints after solve!
+# (examples/Cartpole.ipynb:216-223, :378-382); the trajectories stay in the problem (states / controls / multipliers getters).
+struct ToSolveOptions
+    cost_tolerance::Float64
+    cost_tolerance_intermediate::Float64
+    gradient_tolerance::Float64
+    gradient_tolerance_intermediate::Float64
+    constraint_tolerance::Float64
+    iterations::Int32
+    iterations_inner::Int32
+    iterations_outer::Int32
+    dJ_counter_limit::Int32
+end
+const SOLVE_STATUS = (:UNSOLVED, :SOLVE_SUCCEEDED, :MAX_ITERATIONS, :MAX_ITERATIONS_OUTER, :MAX_REGULARIZATION)   # to_solve_status 0..4
+function solve!(p::BatchedProblem; kw...)
+    d = Ref{ToSolveOptions}()
+    ccall((:to_default_solve_options, libb200), Cint, (Ref{ToSolveOptions},), d)
+    vals = Dict{Symbol,Any}(f => getfield(d[], f) for f in fieldnames(ToSolveOptions))
+    for (k, v) in kw
+        haskey(vals, k) || throw(ArgumentError("unknown solve option $k"))
+        vals[k] = v
+    end
+    o = Ref(ToSolveOptions((convert(fieldtype(ToSolveOptions, f), vals[f]) for f in fieldnames(ToSolveOptions))...))
+    status, iters, outer = Vector{Int32}(undef, p.B), Vector{Int32}(undef, p.B), Vector{Int32}(undef, p.B)
+    cost, dJ, grad, cmax = (Vector{Float64}(undef, p.B) for _ in 1:4)
+    check(p.h, ccall((:to_solve, libb200), Cint,
+                     (Ptr{Cvoid}, Ref{ToSolveOptions}, Ptr{Int32}, Ptr{Int32}, Ptr{Int32}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                     p.h, o, status, iters, outer, cost, dJ, grad, cmax))
+    (status = [SOLVE_STATUS[s + 1] for s in status], iterations = iters, iterations_outer = outer, cost = cost, dJ = dJ, gradient = grad, c_max = cmax)
+end
+
 # MPC plumbing: update_trajectory!(obj, Z, start) src/objective.jl:198-212 on the batched problem; Xref (n, nref), Uref (m, nref)
 TO.update_trajectory!(p::BatchedProblem, Xref::Matrix{Float64}, Uref::Matrix{Float64}, start::Integer=1) =
     check(p.h, ccall((:to_update_trajectory, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Int32, Int32), p.h, Xref, Uref, size(Xref, 2), start))
