@@ -94,6 +94,21 @@ def four_terms(cls, B=4, N=33, error_state=True):
     return _problem(cls, _lqr(N, Qd), cons, B, N, seed=6, attitude=True, error_state=error_state)
 
 
+def bounded(cls, B=6, N=40):
+    """Bound rows on states AND controls (three AL terms on some entries at the last stage knots) + goal"""
+    obj = TO.LQRObjective(np.full(n, 0.1), np.full(m, 0.01), np.full(n, 100.0), XF, N)
+    cons = TO.ConstraintList(n, m, N)
+    x_max = np.full(n, np.inf); x_min = np.full(n, -np.inf)
+    x_max[:3] = 2.5; x_min[:3] = -0.5; x_max[7:10] = 1.0; x_min[7:10] = -1.0; x_max[12] = 0.3
+    TO.add_constraint(cons, TO.BoundConstraint(n, m, x_min=x_min, x_max=x_max, u_min=np.zeros(4), u_max=np.full(4, 10.0)), (1, N - 1))
+    TO.add_constraint(cons, TO.GoalConstraint(XF), N)
+    r = np.random.default_rng(5)
+    x0 = np.tile(X0, (B, 1)); x0[:, :3] += r.uniform(-1, 1, (B, 3))
+    prob = cls(TO.Quadrotor(), obj, x0, 0.05 * (N - 1), xf=XF, constraints=cons, error_state=True)
+    TO.initial_controls(prob, HOVER[None, None, :] + 0.01 * r.standard_normal((B, N - 1, m)))
+    return prob
+
+
 def long_horizon(cls, N, B=2, error_state=True):
     """the BASELINE constraints over N knots of a 4 s horizon: N = 4094 is the last horizon the 12-bit knot field of the term table takes"""
     return TO.problems.quadrotor(B=B, N=N, dt=4.0 / (N - 1), cls=cls, error_state=error_state)

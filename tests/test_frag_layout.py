@@ -103,6 +103,6 @@ int main() {
             for mi in range(2):
                 assert rec[(ks * 32 + lane) * 2 + mi] == abf[ks, mi, lane]
     assert [int(v) for v in out[3].split()] == [240, 192, 208, 224]
-    # the nibble table of k_expand_lie
+    # the nibble table of k_expand_lie_rec
     tab = 0x6420FDB9E7CA8531
     assert [(tab >> (4 * j)) & 15 for j in range(16)] == FE.PHYS

@@ -246,25 +246,52 @@ def test_twelve_bit_knot_field(N):
 
 
 # ---- split vs unsplit -------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("late_list", ["0", "1"])
-@pytest.mark.parametrize("name", ["baseline", "state_bounds"])
-def test_split_expansion_equals_unsplit(name, late_list, monkeypatch):
-    """iteration 2 of ilqr_step(2) expands the instances accepted by line-search pass 1 (mode 1) and the late ones (mode 2, scanned or
-    through the late list) separately; a fresh expand + backward of the same trajectory must give the same records and gains, bit for bit"""
-    monkeypatch.setenv("TO_LATE_LIST", late_list)          # read by to_create, per handle
-    build = (lambda: P.quadrotor(B=256, N=101, error_state=True)) if name == "baseline" else (lambda: rc.state_bounds(TO.Problem, B=256))
-    a, b = build(), build()
+# the benchmarked problem at the benchmark size and smaller, sizes with partial 6- and 16-knot blocks, and Bound rows on states and controls
+SPLIT = {
+    "baseline": lambda cls: P.quadrotor(B=256, N=101, error_state=True, cls=cls),
+    "state_bounds": lambda cls: rc.state_bounds(cls, B=256),
+    "quadrotor_4096x101": lambda cls: P.quadrotor(B=4096, N=101, error_state=True, cls=cls),
+    "quadrotor_37x101": lambda cls: P.quadrotor(B=37, N=101, error_state=True, cls=cls),
+    "quadrotor_5x23": lambda cls: P.quadrotor(B=5, N=23, error_state=True, cls=cls),
+    "calm_37x101": lambda cls: P.quadrotor(B=37, N=101, error_state=True, u_noise=0.01, cls=cls),
+    "calm_5x33": lambda cls: P.quadrotor(B=5, N=33, error_state=True, u_noise=0.01, cls=cls),
+    "calm_64x16": lambda cls: P.quadrotor(B=64, N=16, error_state=True, u_noise=0.01, cls=cls),
+    "bounded_6x40": lambda cls: rc.bounded(cls, B=6, N=40),
+}
+
+
+@pytest.mark.parametrize("name", list(SPLIT))
+def test_split_expansion_equals_unsplit(name):
+    """an iteration that follows one whose line search needed the later passes expands the instances accepted by pass 1 (mode 1) and the
+    late ones (mode 2, through the late list) separately; a fresh expand + backward of the same trajectory must give the same records and
+    gains, bit for bit.  a and b take the same iterations (an AL update after the third) until b's last one leaves late instances; then a
+    takes one more."""
+    a, b = SPLIT[name](TO.Problem), SPLIT[name](TO.Problem)
     for p in (a, b):
         TO.rollout(p)
-    TO.ilqr_step(a, 2)
-    TO.ilqr_step(b, 1)
-    assert np.any(TO.solver_state(b)["ls_iters"] > 4), "no instance needed the later line-search passes: iteration 2 was not split"
+    for it in range(10):
+        TO.ilqr_step(a, 1); TO.ilqr_step(b, 1)
+        if np.any(TO.solver_state(b)["ls_iters"] > 4):
+            break
+        if it == 2:
+            TO.al_update(a); TO.al_update(b)
+    assert np.any(TO.solver_state(b)["ls_iters"] > 4), "no instance needed the later line-search passes: no iteration was split"
+    TO.ilqr_step(a, 1)
     TO.expand(b); TO.backward(b)
     Ra, Rb = TO.expansion_records(a), TO.expansion_records(b)
     assert np.array_equal(Ra, Rb), f"max |split - unsplit| = {np.max(np.abs(Ra - Rb)):.3e}"
     (Ka, da), (Kb, db) = TO.gains(a), TO.gains(b)
     assert np.array_equal(Ka, Kb) and np.array_equal(da, db)
     a.close(); b.close()
+
+
+@pytest.mark.parametrize("name", [k for k in SPLIT if k not in ("baseline", "state_bounds", "quadrotor_4096x101")])
+def test_split_configurations_against_the_oracle(name):
+    """the records of the configurations above against the oracle's expansion"""
+    g, o = pair(SPLIT[name])
+    worst, _ = records_vs_oracle(g, o)
+    print(f"records vs oracle: max rel err {worst:.2e}")
+    g.close(); o.close()
 
 
 # ---- setters on the record path --------------------------------------------------------------------------------------------------------

@@ -204,15 +204,21 @@ def test_abi_struct_layout_matches_the_binding_tables():
             assert getattr(cls, f).offset == c_layout[(name, f)], (name, f)
 
 
-def test_every_environment_switch_of_the_library_is_documented():
-    """INTEGRATION.md lists every TO_* variable the CUDA sources read with getenv (a switch a maintainer cannot find is a trap)."""
+def test_environment_switches_read_are_exactly_the_documented_ones():
+    """The TO_* variables the CUDA sources read with getenv are exactly the TO_* rows of INTEGRATION.md's switch table (a switch a
+    maintainer cannot find is a trap, a documented one the library ignores misleads), and exactly the three kept for profiling and A/B."""
     import glob
     import re
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     names = set()
     for f in glob.glob(os.path.join(root, "trajectoryoptimization.jl_b200", "csrc", "*.cu*")):
         names |= set(re.findall(r'getenv\("(TO_[A-Z0-9_]+)"\)', open(f).read()))
-    assert len(names) >= 10
     doc = open(os.path.join(root, "INTEGRATION.md")).read()
-    missing = sorted(n for n in names if n not in doc)
-    assert not missing, f"undocumented environment switches: {missing}"
+    section = doc[doc.index("## Environment switches of the library"):]
+    section = section[:section.index("\n## ")] if "\n## " in section else section
+    rows = set()
+    for line in section.splitlines():
+        if line.startswith("| `"):
+            rows |= set(re.findall(r"`(TO_[A-Z0-9_]+)", line.split("|")[1]))
+    assert names == rows, f"read but not documented: {sorted(names - rows)}; documented but not read: {sorted(rows - names)}"
+    assert names == {"TO_NO_OVERLAP", "TO_NO_FRAG", "TO_EXPAND_SEEDS"}, sorted(names)

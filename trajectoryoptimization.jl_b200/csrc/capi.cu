@@ -6,7 +6,6 @@
 #include <cstring>
 #include <string>
 #include <vector>
-#include <cuda.h>      // types of the green-context (SM partition) API only: the entry points are resolved at run time, libcuda is not linked
 
 #include "../../include/trajopt_b200.h"
 #include "frag_layout.cuh"
@@ -32,12 +31,6 @@ struct to_handle {
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_merit = nullptr, ev_cons = nullptr;
     bool overlap = true;                // TO_NO_OVERLAP=1: keep every kernel on the main stream (profiling under ncu, A/B timing)
     bool side_pending = false;          // stream2 still holds the late line-search trials of the last iteration (ev_join follows them)
-    // TO_PARTITION=k (SM partition, CUDA green contexts): stream2 is confined to k SMs of its own for the latency-bound late trials and
-    // stream_big carries the expansion kernels that run beside them on the other SMs (to_ilqr_step); the Riccati and line-search passes
-    // keep the whole device on `stream`.
-    bool partition = false;
-    cudaStream_t stream_big = nullptr;
-    cudaEvent_t ev_late = nullptr;
     // to_solve: per-instance solve state on the device; the ACTIVE count of an iteration comes back through pinned memory + an event
     SolveDev solve{};
     int* pin_count = nullptr;           // [2] (pinned)
@@ -154,56 +147,6 @@ int upload_tables(to_handle* h) {
     return upload_exptab(h);
 }
 
-
-// ---- SM partition (CUDA green contexts) ----------------------------------------------------------------------------------------------------
-// The late line-search trials are a dependent FP64 chain in ~150 one-warp CTAs; beside the FP64-bound expansion kernels every instruction of that
-// chain queues behind 16 expansion warps of its SM and on one H100 the pass takes about twice as long as alone (0.74 vs 0.39 ms).  A green
-// context gives the side stream SMs of its own.  Driver entry points through cudaGetDriverEntryPoint: the library still links cudart only.
-namespace {
-struct GreenApi {
-    CUresult (*DeviceGet)(CUdevice*, int) = nullptr;
-    CUresult (*GetRes)(CUdevice, CUdevResource*, CUdevResourceType) = nullptr;
-    CUresult (*Split)(CUdevResource*, unsigned int*, const CUdevResource*, CUdevResource*, unsigned int, unsigned int) = nullptr;
-    CUresult (*Desc)(CUdevResourceDesc*, CUdevResource*, unsigned int) = nullptr;
-    CUresult (*Create)(CUgreenCtx*, CUdevResourceDesc, CUdevice, unsigned int) = nullptr;
-    CUresult (*Stream)(CUstream*, CUgreenCtx, unsigned int, int) = nullptr;
-    bool ok = false;
-};
-template <class F> bool driver_entry(const char* name, F& fn) {
-    void* p = nullptr; cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint(name, &p, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess || !p) { cudaGetLastError(); return false; }
-    fn = (F)p; return true;
-}
-const GreenApi& green_api() {
-    static GreenApi g = [] {
-        GreenApi a;
-        a.ok = driver_entry("cuDeviceGet", a.DeviceGet) && driver_entry("cuDeviceGetDevResource", a.GetRes) && driver_entry("cuDevSmResourceSplitByCount", a.Split) &&
-               driver_entry("cuDevResourceGenerateDesc", a.Desc) && driver_entry("cuGreenCtxCreate", a.Create) && driver_entry("cuGreenCtxStreamCreate", a.Stream);
-        return a;
-    }();
-    return g;
-}
-// the two partitions of a device, created once per process and shared by its handles (never destroyed: they live as long as the primary context)
-struct GreenPair { CUgreenCtx small = nullptr, big = nullptr; int sms_small = 0, sms_big = 0; int want = -1; };
-bool green_pair(int device, int want, GreenPair& out) {
-    static GreenPair cache[TO_MAXDEV];
-    GreenPair& c = cache[(device >= 0 && device < TO_MAXDEV) ? device : 0];
-    if (c.want == want) { out = c; return c.small != nullptr; }
-    const GreenApi& a = green_api();
-    c = GreenPair(); c.want = want;
-    if (a.ok) {
-        CUdevice dev; CUdevResource all, small, rest; unsigned int nb = 1; CUdevResourceDesc d1, d2;
-        if (a.DeviceGet(&dev, device) == CUDA_SUCCESS && a.GetRes(dev, &all, CU_DEV_RESOURCE_TYPE_SM) == CUDA_SUCCESS &&
-            a.Split(&small, &nb, &all, &rest, 0, (unsigned)want) == CUDA_SUCCESS && nb == 1 && rest.sm.smCount > 0 &&
-            a.Desc(&d1, &small, 1) == CUDA_SUCCESS && a.Desc(&d2, &rest, 1) == CUDA_SUCCESS &&
-            a.Create(&c.small, d1, dev, CU_GREEN_CTX_DEFAULT_STREAM) == CUDA_SUCCESS && a.Create(&c.big, d2, dev, CU_GREEN_CTX_DEFAULT_STREAM) == CUDA_SUCCESS) {
-            c.sms_small = (int)small.sm.smCount; c.sms_big = (int)rest.sm.smCount;
-        } else { c.small = nullptr; c.big = nullptr; }
-    }
-    out = c;
-    return c.small != nullptr;
-}
-}  // namespace
 
 // phase timing helpers
 struct PhaseScope {
@@ -512,7 +455,6 @@ int to_create(const to_spec* s, to_handle** out) {
     {
         int lo = 0, hi = 0;
         cudaDeviceGetStreamPriorityRange(&lo, &hi);
-        if (const char* ev = getenv("TO_SIDE_PRIORITY")) { if (atoi(ev) == 0) hi = lo; }   // A/B switches
         if (const char* ev = getenv("TO_NO_OVERLAP")) h->overlap = atoi(ev) == 0;
         if (cudaStreamCreateWithPriority(&h->stream2, cudaStreamNonBlocking, hi) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming) != cudaSuccess ||
@@ -522,22 +464,6 @@ int to_create(const to_spec* s, to_handle** out) {
             cudaEventCreateWithFlags(&h->ev_count[0], cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_count[1], cudaEventDisableTiming) != cudaSuccess) { h->err = "side stream creation failed"; return bail(TO_ECUDA); }
         if (cudaHostAlloc((void**)&h->pin_count, 2 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) { h->err = "cudaHostAlloc failed"; return bail(TO_ENOMEM); }
-        // SM partition for the overlapped part of an iteration (A/B switch, off unless TO_PARTITION = SMs of the side stream's partition)
-        const int part = getenv("TO_PARTITION") ? atoi(getenv("TO_PARTITION")) : 0;
-        GreenPair gp;
-        if (part > 0 && h->overlap && green_pair(s->device, part, gp)) {
-            CUstream ss = nullptr, sb = nullptr;
-            if (green_api().Stream(&ss, gp.small, CU_STREAM_NON_BLOCKING, hi) == CUDA_SUCCESS && green_api().Stream(&sb, gp.big, CU_STREAM_NON_BLOCKING, lo) == CUDA_SUCCESS &&
-                cudaEventCreateWithFlags(&h->ev_late, cudaEventDisableTiming) == cudaSuccess) {
-                cudaStreamDestroy(h->stream2);
-                h->stream2 = (cudaStream_t)ss; h->stream_big = (cudaStream_t)sb; h->partition = true;
-                if (getenv("TO_VERBOSE")) fprintf(stderr, "[trajopt_b200] SM partition: side stream %d SMs, expansion stream %d SMs\n", gp.sms_small, gp.sms_big);
-            } else {
-                if (ss) cudaStreamDestroy((cudaStream_t)ss);
-                if (sb) cudaStreamDestroy((cudaStream_t)sb);
-                cudaGetLastError();
-            }
-        } else if (part > 0 && getenv("TO_VERBOSE")) fprintf(stderr, "[trajopt_b200] SM partition unavailable, plain streams\n");
     }
     DevProblem& P = h->P;
     P.model = s->model; P.n = mn; P.m = mm; P.N = s->N; P.B = s->B;
@@ -622,12 +548,8 @@ int to_create(const to_spec* s, to_handle** out) {
     // The later line-search passes can walk a compact list of the late instances (the ones pass 1 did not accept) instead of scanning all, in half-warp
     // CTAs of two instances (forward.cu launch_pass): only CTAs with work stay resident next to the expansion kernels of the main stream.  On the record
     // path (error-state Quadrotor: cost + dynamics expansion on the main stream) that balances the two overlapped chains -- 2.10 vs 2.21 ms per step
-    // on one H100 -- and it is the default there; on the other paths the late pass itself is the longer chain and the list makes it
-    // longer, so they keep scanning with full warps.  TO_LATE_LIST = 0 / 1 overrides.
-    {
-        const char* ev = getenv("TO_LATE_LIST");
-        if (ev ? atoi(ev) != 0 : P.frag != 0) { ALLOC(P.late_list, B); ALLOC(P.late_count, 1); }
-    }
+    // on one H100; on the other paths the late pass itself is the longer chain and the list makes it longer, so they keep scanning with full warps.
+    if (P.frag) { ALLOC(P.late_list, B); ALLOC(P.late_count, 1); }
     ALLOC(h->d_stageX, P.strideX); ALLOC(h->d_stageU, P.strideU); ALLOC(h->d_viol, B); ALLOC(h->d_merit2, 2);
     ALLOC(h->d_work, 1); ALLOC(h->d_err, 1);
     {   // to_solve state (solve.cu)
@@ -688,8 +610,6 @@ int to_destroy(to_handle* h) {
     if (h->scratch.ptr) cudaFree(h->scratch.ptr);
     for (auto& e : h->pending) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     for (auto e : h->pool) cudaEventDestroy(e);
-    if (h->stream_big) { cudaStreamSynchronize(h->stream_big); cudaStreamDestroy(h->stream_big); }
-    if (h->ev_late) cudaEventDestroy(h->ev_late);
     if (h->stream2) { cudaStreamSynchronize(h->stream2); cudaStreamDestroy(h->stream2); }
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
     if (h->ev_join) cudaEventDestroy(h->ev_join);
@@ -1132,7 +1052,9 @@ static int record_active_count(to_handle* h, const SolveDev& sv, int slot, cudaS
 // Pass 2 is latency-bound and touches few instances, so it runs on a high-priority side stream followed by the
 // expansion of ITS instances, concurrently with the next iteration's expansion of the instances pass 1 accepted
 // (instances never interact); the Riccati pass joins both. The overlap carries across calls (h->side_pending): any
-// other entry point joins the side stream first.
+// other entry point joins the side stream first.  So with a pass 2 pending, the expansions of the late instances go on the side stream
+// behind it, and the cost expansion (record path) then the dynamics expansion of the pass-1 instances on the main stream; without one,
+// the dynamics expansion of every instance on the main stream.
 // sv (to_solve): the stopping-rule check of every ACTIVE instance right after its line search -- for the two halves of an overlapped iteration
 // on their own streams, before the next iteration's expansion of each -- and the ACTIVE count behind it (record_active_count).
 static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
@@ -1140,65 +1062,22 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
     auto expand = [&](cudaStream_t st, int mode) { return h->P.lie ? launch_expand_lie(h->P, st, mode) : launch_expand(h->P, st, mode); };
     bool costexp_done = false;
     const bool rec = h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5 && rec_fused(h->P);
-    static const int order = getenv("TO_ITER_ORDER") ? atoi(getenv("TO_ITER_ORDER")) : 0;
-    if (h->side_pending && order == 1) {
-        // TO_ITER_ORDER=1 (A/B): only the latency-bound cost expansion of the instances accepted in pass 1 runs beside the late trials;
-        // the dynamics expansion of EVERY instance and the cost expansion of the late ones follow the join.  An A/B experiment against
-        // the default order below; not the default, and not measured on the H100.
+    if (h->side_pending) {
+        {
+            PhaseScope pl(h, TO_PHASE_LATE, h->stream2);
+            CU(h, expand(h->stream2, 2)); h->launches++;
+            if (rec) { CU(h, launch_expansion_rec16(h->P, h->stream2, 2)); h->launches++; }
+        }
+        h->phase_launches[TO_PHASE_LATE]++;
         if (rec) {
             { PhaseScope pe(h, TO_PHASE_COSTEXP); CU(h, launch_expansion_rec16(h->P, h->stream, 1)); }
             h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
-        }
-        JOIN(h);
-        { PhaseScope ps(h, TO_PHASE_EXPAND); CU(h, expand(h->stream, 0)); }
-        h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
-        if (rec) {
-            { PhaseScope pl(h, TO_PHASE_LATE); CU(h, launch_expansion_rec16(h->P, h->stream, 2)); }
-            h->launches++; h->phase_launches[TO_PHASE_LATE]++;
             costexp_done = true;
         }
-    } else {
-        if (h->side_pending && h->partition) {
-            // SM partition: the late trials keep their own SMs (stream2); the expansion of the instances accepted in pass 1, then (once the
-            // late trials are through) the expansion of the late instances run on the other partition; the main stream waits for both.
-            cudaStream_t sb = h->stream_big;
-            CU(h, cudaStreamWaitEvent(sb, h->ev_fork, 0));                   // after pass 1 of the line search (and, in to_solve, the check of its instances)
-            if (rec) {
-                { PhaseScope pe(h, TO_PHASE_COSTEXP, sb); CU(h, launch_expansion_rec16(h->P, sb, 1)); }
-                h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
-                costexp_done = true;
-            }
-            { PhaseScope ps(h, TO_PHASE_EXPAND, sb); CU(h, expand(sb, 1)); }
-            h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
-            CU(h, cudaEventRecord(h->ev_late, h->stream2));                  // everything the side stream holds: the late trials (+ a merit reduction)
-            CU(h, cudaStreamWaitEvent(sb, h->ev_late, 0));
-            {
-                PhaseScope pl(h, TO_PHASE_LATE, sb);
-                CU(h, expand(sb, 2)); h->launches++;
-                if (rec) { CU(h, launch_expansion_rec16(h->P, sb, 2)); h->launches++; }
-            }
-            h->phase_launches[TO_PHASE_LATE]++;
-            CU(h, cudaEventRecord(h->ev_join, sb));
-            goto joined;
-        }
-        if (h->side_pending) {
-            {
-                PhaseScope pl(h, TO_PHASE_LATE, h->stream2);
-                CU(h, expand(h->stream2, 2)); h->launches++;
-                if (rec) { CU(h, launch_expansion_rec16(h->P, h->stream2, 2)); h->launches++; }
-            }
-            h->phase_launches[TO_PHASE_LATE]++;
-            if (rec) {
-                { PhaseScope pe(h, TO_PHASE_COSTEXP); CU(h, launch_expansion_rec16(h->P, h->stream, 1)); }
-                h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
-                costexp_done = true;
-            }
-            CU(h, cudaEventRecord(h->ev_join, h->stream2));
-        }
-        { PhaseScope ps(h, TO_PHASE_EXPAND); CU(h, expand(h->stream, h->side_pending ? 1 : 0)); }
-        h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
+        CU(h, cudaEventRecord(h->ev_join, h->stream2));
     }
-joined:
+    { PhaseScope ps(h, TO_PHASE_EXPAND); CU(h, expand(h->stream, h->side_pending ? 1 : 0)); }
+    h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
     JOIN(h);
     h->expanded = true;
     int rc = do_backward(h, costexp_done); if (rc) return rc;
@@ -1206,7 +1085,7 @@ joined:
     h->launches++; h->phase_launches[TO_PHASE_FORWARD]++;
     if (h->overlap) {
         // to_solve: the stopping-rule check of the instances pass 1 accepted (final for this iteration) comes before the fork, so that
-        // everything ordered after ev_fork -- the late trials, the side stream's ACTIVE count, the partition's expansions -- sees its decisions
+        // everything ordered after ev_fork -- the late trials, the side stream's ACTIVE count -- sees its decisions
         if (sv) { CU(h, launch_solve_check(h->P, *sv, 1, h->stream)); h->launches++; }
         CU(h, cudaEventRecord(h->ev_fork, h->stream));
         CU(h, cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));

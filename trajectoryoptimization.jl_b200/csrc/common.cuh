@@ -172,19 +172,6 @@ __host__ __device__ inline double* traj_Uw(const DevProblem& P, int buf, int b) 
 #define TO_MAXDEV 64
 inline int current_device_slot() { int d = 0; cudaGetDevice(&d); return (d >= 0 && d < TO_MAXDEV) ? d : 0; }
 
-// The kernels of one iteration overlap on two streams (capi.cu to_ilqr_step).  Kernels that prefer different L1 / shared-memory splits cannot
-// share an SM until it drains -- so went the hypothesis; asking every kernel on the iteration path for one carve-out (TO_CARVEOUT = percent of
-// shared memory) measured WORSE than the driver's per-kernel default (-1, the default here).  Kept as an A/B knob.
-template <class Kern>
-inline void prefer_common_carveout(Kern kern, bool (&done)[TO_MAXDEV]) {
-    const int dev = current_device_slot();
-    if (done[dev]) return;
-    done[dev] = true;
-    static int pct = -2;
-    if (pct == -2) { const char* e = getenv("TO_CARVEOUT"); pct = e ? atoi(e) : -1; }
-    if (pct >= 0) cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
-}
-
 // Altro.jl regularization_update! (restated; see oracle/oracle.hpp reg_increase / reg_decrease)
 __host__ __device__ inline void reg_increase(const DevOptions& o, double& rho, double& drho) {
     drho = fmax(drho * o.bp_reg_increase_factor, o.bp_reg_increase_factor);

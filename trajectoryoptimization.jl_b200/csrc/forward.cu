@@ -467,7 +467,6 @@ cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int f
         if (e != cudaSuccess) return e;
     }
     configured[dev] = true;
-    { static bool done[TO_MAXDEV] = {false}; prefer_common_carveout(kern, done); }
     kern<<<blocks, FWD_THREADS, smem, s>>>(P, trial0, first_pass, final_pass);
     return cudaGetLastError();
 }
@@ -475,10 +474,8 @@ cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int f
 template <int MODEL, int G, bool FAST>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     // lanes of each warp that carry groups: 16 for the first pass (half-warp FP64 instructions take one pipe pass); the later passes
-    // use 16 when they walk the compact late list (two-instance CTAs, see to_create) and 32 when they scan all instances.  TO_FWD_LANES_P1 / _P2 override.
-    static int lanes1 = -1, lanes2 = -1;
-    if (lanes1 < 0) { const char* v = getenv("TO_FWD_LANES_P1"); lanes1 = v ? atoi(v) : 16; v = getenv("TO_FWD_LANES_P2"); lanes2 = v ? atoi(v) : 0; }
-    const int lanes = first_pass ? lanes1 : (lanes2 ? lanes2 : (P.late_list ? 16 : 32));
+    // use 16 when they walk the compact late list (two-instance CTAs, see to_create) and 32 when they scan all instances.
+    const int lanes = first_pass ? 16 : (P.late_list ? 16 : 32);
     if constexpr (MODEL == MODEL_QUADROTOR) {   // Lie-group error state: dx = state_diff(xbar, x), gains m x (n - 1)
         if (P.lie) {
             if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, FAST, (G <= 16 ? 16 : 32), true>(P, trial0, first_pass, final_pass, s);

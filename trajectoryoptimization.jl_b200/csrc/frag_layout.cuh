@@ -1,5 +1,5 @@
 // frag_layout.cuh -- the per-knot RECORD consumed by the register-resident Riccati kernel (riccati_frag.cu) and written by the
-// error-state expansion kernels (rollout.cu k_expand_lie_rec / k_expand_lie, riccati_frag.cu k_expansion_rec).
+// error-state expansion kernels (rollout.cu k_expand_lie_rec / k_expansion_rec16b, riccati_frag.cu k_expansion_rec).
 //
 // The backward pass of the error-state Quadrotor (n_e = 12, m = 4, z = [x_e; u] of 16 entries) keeps its whole recursion state in
 // the fragment registers of mma.sync.m8n8k4.f64 (lane L = 4 fr + fc holds A[fr][fc], B[fc][fr], D[fr][2fc], D[fr][2fc+1]).  For

@@ -36,7 +36,7 @@ cudaError_t launch_expansion_compact(const DevProblem& P, cudaStream_t s);      
 cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode = 0);     // [A_e B_e] straight from the dual-number RK4 step (rollout.cu)
 // register-resident Riccati pass of the error-state Quadrotor + its record producers   (riccati_frag.cu)
 cudaError_t launch_expansion_rec(const DevProblem& P, cudaStream_t s);                 // compact expansion -> REC[192..240) of every knot
-cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode);               // ... 16 lanes per knot, from the host-built term table (rollout.cu)
+cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode);               // ... 16-knot blocks per 16-lane group, from the host-built term table (rollout.cu)
 cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s);          // ... of the full-state [A B]
 cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s);               // closed-form position / velocity columns of [A_e B_e], once per problem
 cudaError_t launch_export_abe(const DevProblem& P, cudaStream_t s);                    // REC fragments -> ABe (col-major 12 x 16)

@@ -30,7 +30,6 @@
 //   * Quu + rho I is m x m (m <= 8): LDL' with reciprocal pivots (no fp64 sqrt / division chain) and the triangular
 //     solves are done per right-hand-side column, one lane per column of [Qux Qu], in registers.
 #include <cstddef>
-#include <cstdlib>
 
 #include "costcon.cuh"
 #include "kernels.h"
@@ -984,12 +983,10 @@ cudaError_t launch_riccati_nm(const DevProblem& P, int* work_counter, cudaStream
 
 cudaError_t launch_backward(const DevProblem& P, int* work_counter, cudaStream_t s) {
     if (P.dense_riccati) return launch_backward_dense(P, s);   // lie.cu: error state / quaternion costs (expansion materialised by the caller)
-    // small models: one thread per instance, everything in registers (riccati_small.cu); TO_RICCATI_WARP=1 forces the warp kernel
-    static int force_warp = -1;
-    if (force_warp < 0) { const char* v = getenv("TO_RICCATI_WARP"); force_warp = v ? atoi(v) : 0; }
+    // small models: one thread per instance, everything in registers (riccati_small.cu); backward_kernel = 1 forces the warp kernel
     const int choice = P.opt.pad;   // to_options.backward_kernel: 0 automatic, 1 warp kernel, 2 thread kernel where it applies
     if (choice == 2 && riccati_small_supported(P, true)) return launch_backward_small(P, s);
-    if (choice == 0 && !force_warp && riccati_small_supported(P, false)) return launch_backward_small(P, s);
+    if (choice == 0 && riccati_small_supported(P, false)) return launch_backward_small(P, s);
     if (P.n == 13 && P.m == 4) return launch_riccati_nm<13, 4>(P, work_counter, s);
     if (P.n == 4 && P.m == 1) return launch_riccati_nm<4, 1>(P, work_counter, s);
     if (P.n == 4 && P.m == 2) return launch_riccati_nm<4, 2>(P, work_counter, s);

@@ -28,9 +28,8 @@
 //     positive-definiteness = positive leading minors a, det P, s00, det S (the pivots of LDL' are their ratios).
 //   * the record of knot k (1920 B: fragments of [A_e B_e] + compact expansion) arrives by ONE 1-D bulk TMA copy (cp.async.bulk +
 //     mbarrier, SASS UBLKCP) into a per-warp ring, issued one knot ahead.
-//   * 4-warp CTAs; two builds (TO_FRAG_MINB below): 72 registers x 7 CTAs per SM = 28 resident warps (1.11 waves of
-//     B = 4096 instances on 132 SMs), or 80 registers x 6 CTAs = 24 warps, 1.29 waves of faster sweeps (the default: the faster build on one H100).
-#include <cstdlib>
+//   * 4-warp CTAs; 80 registers x 6 CTAs per SM = 24 resident warps, 1.29 waves of B = 4096 instances on 132 SMs (TO_FRAG_MINB below: the
+//     faster sweeps beat the 1.11 waves of a 72-register x 7-CTA build on one H100).
 #include "costcon.cuh"
 #include "frag_layout.cuh"
 #include "kernels.h"
@@ -49,8 +48,7 @@
 #endif
 // CTAs per SM the register allocation aims at: 7 (72 registers, 28 warps per SM, more spills) or 6 (80 registers, 24 warps, fewer spills: a sweep
 // is faster).  On one H100 (400 W) 6 is the faster build both on the BASELINE inputs (k_riccati_frag 0.55 vs 0.60 ms) and without regularisation
-// restarts (quadrotor_calm 0.46 vs 0.50 ms).
-// Both are compiled; TO_FRAG_MINB (environment, 6 or 7) picks one at run time, the macro is the default.
+// restarts (quadrotor_calm 0.46 vs 0.50 ms).  A build-time knob (-DTO_FRAG_MINB=7) for variant builds.
 #ifndef TO_FRAG_MINB
 #define TO_FRAG_MINB 6
 #endif
@@ -613,11 +611,10 @@ int frag_pool_slots(int B, int N) {
 }
 size_t frag_pool_doubles(int B, int N) { return (size_t)frag_pool_slots(B, N) * ((size_t)(N - 1) * 52 + 2); }
 
-template <int MINB>
-static cudaError_t launch_backward_frag_t(const DevProblem& P, int* queue, double* pool, int* sticky_err, cudaStream_t s) {
+cudaError_t launch_backward_frag(const DevProblem& P, int* queue, double* pool, int* sticky_err, cudaStream_t s) {
     constexpr int STAGES = TO_FRAG_STAGES, WARPS = TO_FRAG_WARPS;
     using SM = FragSmem<STAGES, WARPS>;
-    auto kern = k_riccati_frag<STAGES, WARPS, MINB>;
+    auto kern = k_riccati_frag<STAGES, WARPS, TO_FRAG_MINB>;
     const int smem = (int)sizeof(SM);
     // per-device launch configuration (one process may hold handles on several GPUs)
     static int ctas_per_sm[TO_MAXDEV] = {0}, num_sms[TO_MAXDEV] = {0};
@@ -641,11 +638,6 @@ static cudaError_t launch_backward_frag_t(const DevProblem& P, int* queue, doubl
     int grid = num_sms[dev] * ctas_per_sm[dev];       // persistent: warps pull work from the queue (all CTAs are co-resident: the
     const int need = (P.B + WARPS - 1) / WARPS;       // waiting warps of the speculative ladder cannot starve the running ones)
     if (grid > need) grid = need;
-    { static bool done[TO_MAXDEV] = {false}; prefer_common_carveout(kern, done); }
     kern<<<grid, 32 * WARPS, smem, s>>>(P, queue, pool, pool ? frag_pool_slots(P.B, P.N) : 0, sticky_err);
     return cudaGetLastError();
-}
-cudaError_t launch_backward_frag(const DevProblem& P, int* queue, double* pool, int* sticky_err, cudaStream_t s) {
-    static const int minb = getenv("TO_FRAG_MINB") ? atoi(getenv("TO_FRAG_MINB")) : TO_FRAG_MINB;
-    return minb >= 7 ? launch_backward_frag_t<7>(P, queue, pool, sticky_err, s) : launch_backward_frag_t<6>(P, queue, pool, sticky_err, s);
 }

@@ -165,8 +165,7 @@ __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, con
 // depend on r, and on v only in rdot.  Their columns of the discrete Jacobian are therefore known in closed form -- d x+/d r = e_r and
 // d x+/d v = h e_r + e_v (the RK4 weights sum to one) -- and need no dual-number sweep: 10 seeds (attitude, angular velocity, controls) are
 // pushed through the RK4 step instead of 16, one thread each; the six trivial columns depend on the time steps only.  The materialised P.ABe
-// (and the record under TO_EXPAND_V1=1) gets them once, when the problem is created (k_trivial_columns); k_expand_lie_rec writes them into
-// every record block it assembles.
+// gets them once, when the problem is created (k_trivial_columns); k_expand_lie_rec writes them into every record block it assembles.
 __device__ __forceinline__ int lie_seed(int s) { return (int)((0xFEDCBA9543ULL >> (4 * s)) & 15); }       // 3,4,5,9,10,11,12,13,14,15
 __device__ __forceinline__ int lie_trivial(int s) { return (int)((0x876210ULL >> (4 * s)) & 15); }        // 0,1,2,6,7,8
 
@@ -206,7 +205,6 @@ __device__ __forceinline__ void expand_lie_column(const DevProblem& P, int k, in
     for (int i = qs + 4; i < n; i++) col[i - 1] = xn[i].d[0];
 }
 
-// FRAG: the column goes into the fragment block of the knot's record (frag_layout.cuh) instead of P.ABe.
 #ifndef TO_EXPAND_LIE_MINB
 #define TO_EXPAND_LIE_MINB 4      // CTAs per SM the register allocation aims at: 128 registers, 16 warps per SM
 #endif
@@ -215,10 +213,9 @@ __device__ __forceinline__ void expand_lie_column(const DevProblem& P, int k, in
 #ifndef TO_EXPAND_LIE_THREADS
 #define TO_EXPAND_LIE_THREADS 64
 #endif
-template <int MODEL, bool FRAG>
+template <int MODEL>
 __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 128 / TO_EXPAND_LIE_THREADS) k_expand_lie(const DevProblem P, int mode) {
-    constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, nme = ne + m, qs = 3, NS = 10;
-    using D = Dual<1>;
+    constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, nme = ne + m, NS = 10;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long total = (long long)P.B * (P.N - 1) * NS;
     if (t >= total) return;
@@ -231,32 +228,19 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
     if (retired(P, b)) return;                                     // to_solve: not ACTIVE
     const double* X = traj_X(P, P.cur[b], b) + (size_t)k * n;
     const double* U = traj_U(P, P.cur[b], b) + (size_t)k * m;
-    const double h = P.dt[k];
-    // where column jj of [A_e B_e] goes: the fragment slots of the record, or 12 contiguous doubles of P.ABe
-    auto store_column = [&](int jj, const double (&col)[ne]) {
-        if constexpr (FRAG) {
-            // element (row e, column jj) of the record: (ks(e)*32 + 4*(c & 7) + fc(e))*2 + (c >> 3), c = physical index of column jj
-            const int c = (int)((0x6420FDB9E7CA8531ULL >> (4 * jj)) & 15);       // fraglayout::phys_z(jj) as a nibble table
-            double* rec = P.REC + ((size_t)b * P.N + k) * TO_REC_LEN + 8 * (c & 7) + (c >> 3);
-#pragma unroll
-            for (int e = 0; e < ne; e++) rec[fraglayout::ab_index(e, 12)] = col[e];   // column 12 (u_0, c = 0) has a zero column offset
-        } else {
-            double* out = P.ABe + ((size_t)bk * nme + jj) * ne;
-#pragma unroll
-            for (int e = 0; e < ne; e++) out[e] = col[e];
-        }
-    };
     double col[ne];
     expand_lie_column<MODEL>(P, k, j, X, U, col);
-    store_column(j, col);
+    double* out = P.ABe + ((size_t)bk * nme + j) * ne;                 // column j of [A_e B_e]: 12 contiguous doubles
+#pragma unroll
+    for (int e = 0; e < ne; e++) out[e] = col[e];
 }
 
-// ---- k_expand_lie_rec: the record path's dynamics expansion (the default; TO_EXPAND_V1=1 selects k_expand_lie<QUADROTOR, true>) --------
-// k_expand_lie<.., true> leaves each column as 12 scattered 8-byte stores (one L2 sector operation each) and writes 10 of the 16 columns: in the
-// record's fragment order a 32-byte sector holds columns {c, c + 8} of two rows, and 4 of the 8 column pairs mix a seed column with a closed-form
-// one, so every iteration writes those sectors only partly and the L2 has to fill them from DRAM before it can write them back.
-// Here a CTA owns EXPB_KPB consecutive knots of ONE instance (one thread per (knot, seed), the same expand_lie_column as above: the records are
-// bit-identical).  Each thread drops its column into a shared-memory image of its knot's 1536-byte [A_e B_e] block; the six seed threads
+// ---- k_expand_lie_rec: the record path's dynamics expansion ---------------------------------------------------------------------------------
+// Stored column by column into the record, each column would be 12 scattered 8-byte stores (one L2 sector operation each), and only 10 of the 16
+// columns change: in the record's fragment order a 32-byte sector holds columns {c, c + 8} of two rows, and 4 of the 8 column pairs mix a seed
+// column with a closed-form one, so every iteration would write those sectors only partly and the L2 would fill them from DRAM first.
+// Here a CTA owns EXPB_KPB consecutive knots of ONE instance (one thread per (knot, seed), the same expand_lie_column as k_expand_lie: the
+// blocks are bit-identical to its [A_e B_e]).  Each thread drops its column into a shared-memory image of its knot's 1536-byte [A_e B_e] block; the six seed threads
 // sd < 6 of the knot also write one closed-form column each (positions, velocities: 1 on the diagonal, dt[k] at (e, e + 6)), so the image is
 // complete, and the CTA writes the images out as whole 128-byte lines with 16-byte stores: no sector of the block is ever partly written.
 //   mapping   6 knots x 10 seeds = 60 of 64 threads; at N = 101, 17 CTAs per instance and 8 % of the lanes idle.  The instance test of the
@@ -323,146 +307,41 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
     }
 }
 
-// TO_EXPAND_V1=1: k_expand_lie<QUADROTOR, true> on the record path (A/B against k_expand_lie_rec; it relies on k_trivial_columns<true> at to_create)
-static bool expand_v1() {
-    static const int v1 = getenv("TO_EXPAND_V1") ? atoi(getenv("TO_EXPAND_V1")) : 0;
-    return v1 != 0;
-}
-
 // the closed-form columns of [A_e B_e] (positions, velocities): thread = (instance, knot, one of the six)
-template <bool FRAG>
 __global__ void __launch_bounds__(128) k_trivial_columns(const DevProblem P) {
     constexpr int ne = 12, nme = 16;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)P.B * (P.N - 1) * 6) return;
     const int sd = (int)(t % 6);
     const long long bk = t / 6;
-    const int k = (int)(bk % (P.N - 1)), b = (int)(bk / (P.N - 1));
+    const int k = (int)(bk % (P.N - 1));
     const int jt = lie_trivial(sd);
     const double h = P.dt[k];
-    for (int e = 0; e < ne; e++) {
-        const double v = (e == jt) ? 1.0 : ((jt >= 6 && e == jt - 6) ? h : 0.0);
-        if (FRAG) P.REC[((size_t)b * P.N + k) * TO_REC_LEN + fraglayout::ab_index(e, jt)] = v;
-        else P.ABe[((size_t)bk * nme + jt) * ne + e] = v;
-    }
+    for (int e = 0; e < ne; e++) P.ABe[((size_t)bk * nme + jt) * ne + e] = (e == jt) ? 1.0 : ((jt >= 6 && e == jt - 6) ? h : 0.0);
 }
 cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s) {
     const long long total = (long long)P.B * (P.N - 1) * 6;
-    if (P.frag && !expand_v1()) return cudaSuccess;       // k_expand_lie_rec writes the whole block, closed-form columns included, every time
-    if (P.frag) k_trivial_columns<true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
-    else k_trivial_columns<false><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+    if (P.frag) return cudaSuccess;       // k_expand_lie_rec writes the whole block, closed-form columns included, every time
+    k_trivial_columns<<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }
 
-// Cost + AL expansion part of every record (frag_layout.cuh [192, 240)), the terminal knot included: 16 lanes per knot, lane i = entry i of
-// the full-state z = [x; u] (lane 0 also takes the 17th entry u_3).  Outside the attitude the error-state expansion of a diagonal full-state
-// one is the same entry; the quaternion block is projected by lanes 3..5 from the (g, h, q) of lanes 3..6, fetched by 16-lane shuffles:
-// G'g, G' diag(h) G - (q'g_q) I3 (Altro error_expansion!; lie.cu k_expansion_compact is the one-thread-per-knot version of the same numbers).
-// A light kernel (every load independent, ~40 registers) that runs at full occupancy; fused into the FP64-bound k_expand_lie it doubled that
-// kernel's time.
-#ifndef TO_CEXP_ITERS
-#define TO_CEXP_ITERS 4          // knots per 16-lane group (the grid shrinks accordingly)
-#endif
-#ifndef TO_CEXP_MINB
-#define TO_CEXP_MINB 4          // 64 registers: 32 warps per SM
-#endif
-#ifndef TO_CEXP_THREADS
-#define TO_CEXP_THREADS 128
-#endif
-__global__ void __launch_bounds__(TO_CEXP_THREADS, TO_CEXP_MINB * 256 / TO_CEXP_THREADS) k_expansion_rec16(const DevProblem P, int mode) {
-    constexpr int qs = 3;
-    const int i = threadIdx.x & 15;                                                   // full-state entry of this lane
-    const int n = P.n, N = P.N;
-    const int ngroups = (int)((gridDim.x * blockDim.x) >> 4);
-    const ExpTab& tab = *P.exptab;
-    // the AL rows acting on z_i: loop-invariant, kept in registers (the first version re-read them per knot: 530 instructions per thread)
-    unsigned px[TO_EXP_MAXT], py[TO_EXP_MAXT]; double nms[TO_EXP_MAXT], bnd[TO_EXP_MAXT];
-#pragma unroll
-    for (int t = 0; t < TO_EXP_MAXT; t++) { px[t] = tab.pkx[t][i]; py[t] = tab.pky[t][i]; nms[t] = tab.nms[t][i]; bnd[t] = tab.bound[t][i]; }
-    const int e = (i < qs) ? i : i - 1;                                               // error-state coordinate of entry i (controls: 12 + a = i - 1)
-    const int pme = (int)((0x6420FDB9E7CA8531ULL >> (4 * (e & 15))) & 15);            // its physical slot
-    auto entry = [&](const DevCost& c, int k, int ii, double zi, const double* lam_b, const unsigned (&qx)[TO_EXP_MAXT], const unsigned (&qy)[TO_EXP_MAXT],
-                     const double (&qn)[TO_EXP_MAXT], const double (&qb)[TO_EXP_MAXT], double& g, double& h) {
-        const bool last = (k == N - 1);
-        if (ii < n) { g = fma(c.Qd[ii], zi, c.q[ii]); h = c.Qd[ii]; }
-        else if (last) { g = 0.0; h = 0.0; return; }
-        else { g = fma(c.Rd[ii - n], zi, c.r[ii - n]); h = c.Rd[ii - n]; }
-#pragma unroll
-        for (int t = 0; t < TO_EXP_MAXT; t++) {
-            if ((unsigned)(k + 1) - (qx[t] & 0xfffu) <= ((qx[t] >> 12) & 0xfffu)) {
-                const double lam = lam_b[(int)(qy[t] + (unsigned)(k + 1) * ((qx[t] >> 24) & 0x7fu))];
-                const double lb = fma(qn[t], zi - qb[t], lam);                         // lambda - mu c
-                if ((qx[t] >> 31) || lb <= 0.0) { g += (qn[t] < 0.0) ? -lb : lb; h += fabs(qn[t]); }   // g -= sign lb ; h += mu
-            }
-        }
-    };
-    const int total = P.B * N;
-    const unsigned gm = 0xFFFFu << (threadIdx.x & 16);                                // the two groups of a warp may take different trips
-    for (int bk = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 4); bk < total; bk += ngroups) {      // (whole 16-lane groups iterate together)
-        const int b = bk / N, k = bk - b * N;
-        if (mode != 0 && (P.acc1[b] != 0) != (mode == 1)) continue;     // overlapped iterations: this launch covers the other group (see k_expand)
-        if (retired(P, b)) continue;                                    // to_solve: not ACTIVE
-        const bool last = (k == N - 1);
-        const double* X = traj_X(P, P.cur[b], b) + (size_t)k * n;
-        const double* U = traj_U(P, P.cur[b], b) + (size_t)(last ? 0 : k) * P.m;      // (not read at the terminal knot)
-        const double* lam_b = P.lambda + (size_t)b * P.lambda_len;
-        const DevCost& c = P.costs[P.cost_index[k]];
-        double* rec = P.REC + (size_t)bk * TO_REC_LEN;
-        const double zi = (i < n) ? X[i] : (last ? 0.0 : U[i - n]);
-        double g, h;
-        entry(c, k, i, zi, lam_b, px, py, nms, bnd, g, h);
-        // the quaternion block: (g, h, q) of lanes 3..6 to every lane of the 16-lane group (lanes 3..5 use them)
-        double gq[4], hq[4], q[4];
-#pragma unroll
-        for (int r = 0; r < 4; r++) {
-            gq[r] = __shfl_sync(gm, g, qs + r, 16); hq[r] = __shfl_sync(gm, h, qs + r, 16); q[r] = __shfl_sync(gm, zi, qs + r, 16);
-        }
-        if (i >= qs && i < qs + 3) {
-            const int cc = i - qs;
-            // rows of G' = (L(q) H)': (-x,w,z,-y), (-y,-z,w,x), (-z,y,-x,w)   (kept in registers: no run-time indexed arrays)
-            const double G0[4] = {-q[1], q[0], q[3], -q[2]}, G1[4] = {-q[2], -q[3], q[0], q[1]}, G2[4] = {-q[3], q[2], -q[1], q[0]};
-            double gc[4];
-#pragma unroll
-            for (int r = 0; r < 4; r++) gc[r] = (cc == 0) ? G0[r] : (cc == 1) ? G1[r] : G2[r];
-            double qb = 0.0, ge = 0.0, hb0 = 0.0, hb1 = 0.0, hb2 = 0.0;
-#pragma unroll
-            for (int r = 0; r < 4; r++) {
-                qb += q[r] * gq[r]; ge += gc[r] * gq[r];
-                const double tt = gc[r] * hq[r];
-                hb0 += tt * G0[r]; hb1 += tt * G1[r]; hb2 += tt * G2[r];
-            }
-            const double hd = ((cc == 0) ? hb0 : (cc == 1) ? hb1 : hb2) - qb;
-            const int p = 8 + 2 * cc;                                                 // attitude error e = 3 + c sits on p = 8, 10, 12 (frag_layout.cuh)
-            rec[TO_REC_G + p] = ge; rec[TO_REC_HD + p] = hd;
-            rec[TO_REC_HB + 4 * cc + 0] = (cc == 0) ? hd : hb0;
-            rec[TO_REC_HB + 4 * cc + 1] = (cc == 1) ? hd : hb1;
-            rec[TO_REC_HB + 4 * cc + 2] = (cc == 2) ? hd : hb2;
-            rec[TO_REC_HB + 4 * cc + 3] = 0.0;
-        } else if (i != qs + 3) {                                                      // lane 6 (q_z) has no coordinate of its own
-            rec[TO_REC_G + pme] = g; rec[TO_REC_HD + pme] = h;
-            if (e == 7) { rec[TO_REC_HB + 12] = 0.0; rec[TO_REC_HB + 13] = 0.0; rec[TO_REC_HB + 14] = 0.0; rec[TO_REC_HB + 15] = h; }   // p = 14 is row 3 of Hb
-        }
-        if (i == 0) {                                                                  // the 17th entry: u_3 -> coordinate 15 (physical slot 6)
-            unsigned rx[TO_EXP_MAXT], ry[TO_EXP_MAXT]; double rn[TO_EXP_MAXT], rb[TO_EXP_MAXT];
-#pragma unroll
-            for (int t = 0; t < TO_EXP_MAXT; t++) { rx[t] = __ldg(&tab.pkx[t][n + 3]); ry[t] = __ldg(&tab.pky[t][n + 3]); rn[t] = __ldg(&tab.nms[t][n + 3]); rb[t] = __ldg(&tab.bound[t][n + 3]); }
-            entry(c, k, n + 3, last ? 0.0 : U[3], lam_b, rx, ry, rn, rb, g, h);
-            rec[TO_REC_G + 6] = g; rec[TO_REC_HD + 6] = h;
-        }
-    }
-}
-// ---- k_expansion_rec16b: the same numbers, blocked by 16 knots (the default; TO_CEXP_V1=1 selects the kernel above) -----------------
-// k_expansion_rec16 spends many instructions per lane and knot on 3 outputs, and waits on two-level dependent loads (cur[b] -> X,
-// cost_index[k] -> DevCost): every 16-lane step pays for the
-// attitude projection that 3 of its lanes need (24 shuffles + ~40 FP64), for the 17th entry u_3 that lane 0 takes in a divergent second
-// call, and for the unpacking of the term table.  Here a 16-lane group owns a BLOCK of 16 consecutive knots of one instance:
+// ---- k_expansion_rec16b: the cost + AL expansion part of every record (frag_layout.cuh [192, 240)), the terminal knot included ---------------
+// Outside the attitude the error-state expansion of a diagonal full-state one is the same entry; the quaternion block is projected from the
+// (g, h, q) of q_w..q_z: G'g, G' diag(h) G - (q'g_q) I3 (Altro error_expansion!; lie.cu k_expansion_compact is the one-thread-per-knot version of
+// the same numbers).  A light kernel (every load independent) that runs at full occupancy; fused into the FP64-bound k_expand_lie it doubled
+// that kernel's time.
+// One knot per 16-lane step (lane i = entry i of the full-state z = [x; u]) would spend many instructions per lane and knot on 3 outputs, and wait
+// on two-level dependent loads (cur[b] -> X, cost_index[k] -> DevCost): every step would pay for the attitude projection that 3 of its lanes need
+// (24 shuffles + ~40 FP64), for the 17th entry u_3 that lane 0 would take in a divergent second call, and for the unpacking of the term table.
+// Here a 16-lane group owns a BLOCK of 16 consecutive knots of one instance:
 //   phase A   16 steps, lane i < 13 = state entry x_i of one knot: diagonal cost + AL terms -> (g, h); loads (x_i and the multipliers of
 //             its <= 3 terms) are issued for 4 knots at a time before the arithmetic; the cost coefficients of the lane are cached in
 //             registers while the cost index does not change; lanes 3..6 (the quaternion) leave (g, h, q) in shared memory
 //   phase B   lane j projects the attitude block of knot j (G'g, G' diag(h) G - (q'g_q) I3): once per knot instead of once per step
 //   phase C   lane j takes the four control entries of knot j (their Bound rows are the AL terms that are active at every knot: in
 //             phase A three lanes of sixteen would execute them at every step)
-// ~55 instructions per lane and knot.  Same expressions in the same order as above: the records are bit-identical.
+// ~55 instructions per lane and knot.
 #ifndef TO_CEXP2_MINB
 #define TO_CEXP2_MINB 9
 #endif
@@ -623,41 +502,25 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
 }
 cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode) {
     int dev = 0, sms = 132; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    static const int v1 = getenv("TO_CEXP_V1") ? atoi(getenv("TO_CEXP_V1")) : 0;
-    if (!v1 && P.n == 13 && P.m == 4) {
-        // blocks of 16 knots, one 16-lane group each, TO_CEXP2_UNITS blocks per group (grid-stride)
-        static const int upg = getenv("TO_CEXP2_UNITS") ? atoi(getenv("TO_CEXP2_UNITS")) : 1;   // 2 measured no faster on one H100
-        const long long units = (long long)P.B * ((P.N + 15) / 16);
-        constexpr int GPB = TO_CEXP2_THREADS / 16;                                   // 16-lane groups per CTA
-        long long blocks = ((units + GPB - 1) / GPB + upg - 1) / (upg < 1 ? 1 : upg);
-        if (blocks < sms) blocks = sms;
-        { static bool done[TO_MAXDEV] = {false}; prefer_common_carveout(k_expansion_rec16b, done); }
-        k_expansion_rec16b<<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
-        return cudaGetLastError();
-    }
-    // 16-lane groups, a few knots each (grid-stride): the per-lane term table stays in registers
-    const long long total = (long long)P.B * P.N * 16;
-    constexpr int T = TO_CEXP_THREADS;
-    long long blocks = ((total + T - 1) / T + TO_CEXP_ITERS - 1) / TO_CEXP_ITERS;
+    // blocks of 16 knots, one 16-lane group each
+    const long long units = (long long)P.B * ((P.N + 15) / 16);
+    constexpr int GPB = TO_CEXP2_THREADS / 16;                                       // 16-lane groups per CTA
+    long long blocks = (units + GPB - 1) / GPB;
     if (blocks < sms) blocks = sms;
-    { static bool done[TO_MAXDEV] = {false}; prefer_common_carveout(k_expansion_rec16, done); }
-    k_expansion_rec16<<<(unsigned)blocks, T, 0, s>>>(P, mode);
+    k_expansion_rec16b<<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
 
 cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
     if (P.model != MODEL_QUADROTOR) return cudaErrorNotSupported;
     const long long total = (long long)P.B * (P.N - 1) * 10;      // 10 dual-number seeds per knot (k_expand_lie: seed pruning)
-    static_assert(fraglayout::phys_z(0) == 1 && fraglayout::phys_z(5) == 12 && fraglayout::phys_z(11) == 15 && fraglayout::phys_z(12) == 0 && fraglayout::phys_z(15) == 6, "nibble table of k_expand_lie");
-    { static bool d1[TO_MAXDEV] = {false}, d2[TO_MAXDEV] = {false}; prefer_common_carveout(k_expand_lie<MODEL_QUADROTOR, true>, d1); prefer_common_carveout(k_expand_lie<MODEL_QUADROTOR, false>, d2); }
+    static_assert(fraglayout::phys_z(0) == 1 && fraglayout::phys_z(5) == 12 && fraglayout::phys_z(11) == 15 && fraglayout::phys_z(12) == 0 && fraglayout::phys_z(15) == 6, "nibble table of k_expand_lie_rec and k_expansion_rec16b");
     constexpr int T = TO_EXPAND_LIE_THREADS;
-    if (P.frag && !expand_v1()) {
+    if (P.frag) {
         // one CTA per (instance, block of EXPB_KPB knots); mode 2 with the late list: the first *late_count instance slots carry work
         const int nkb = (P.N - 1 + EXPB_KPB - 1) / EXPB_KPB;
-        { static bool d3[TO_MAXDEV] = {false}; prefer_common_carveout(k_expand_lie_rec<MODEL_QUADROTOR>, d3); }
         k_expand_lie_rec<MODEL_QUADROTOR><<<(unsigned)((long long)P.B * nkb), EXPB_T, 0, s>>>(P, mode, nkb);
-    } else if (P.frag) k_expand_lie<MODEL_QUADROTOR, true><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
-    else k_expand_lie<MODEL_QUADROTOR, false><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
+    } else k_expand_lie<MODEL_QUADROTOR><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
 
@@ -672,7 +535,6 @@ static cudaError_t launch_expand_t(const DevProblem& P, cudaStream_t s, int mode
     constexpr int TPK = (SeedList<MODEL>::count + NP - 1) / NP;
     const long long total = (long long)P.B * (P.N - 1) * TPK;
     const int threads = 128;
-    { static bool done[TO_MAXDEV] = {false}; prefer_common_carveout(k_expand<MODEL, NP>, done); }
     k_expand<MODEL, NP><<<(unsigned)((total + threads - 1) / threads), threads, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
