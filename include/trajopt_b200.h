@@ -3,7 +3,9 @@
  * The reference (/root/reference, v0.7.1) is pure Julia and has no FFI: its "operator API" is the set of
  * Julia functions a solver (Altro.jl) calls on a `Problem`.  Each entry point below replaces one of those
  * calls for a BATCH of B independent problem instances that share model / objective / constraints and
- * differ in x0, X, U, multipliers.  Every function cites the reference interface it stands in for.  The
+ * differ in x0, X, U, multipliers -- and, after a per-instance goal call (to_set_goal_states,
+ * to_update_trajectories, to_set_cost_terms), in the linear cost terms q, r and the Goal constraint values
+ * (goal state / tracking reference per instance).  Every function cites the reference interface it stands in for.  The
  * Julia-side binding (ccall) that a maintainer adds is shown in INTEGRATION.md.
  *
  * Conventions
@@ -207,6 +209,23 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
  * control and state), multipliers move with their knots (the tail keeps its last value), x0 <- X_{1+steps},
  * t0 += the skipped dt. The caller then sets the measured state (to_set_initial_state) and re-rolls out. */
 int to_shift_trajectory(to_handle* h, int32_t steps);
+
+/* ---- per-instance goals / tracking references ---------------------------------------------------------------
+ * The same operations per instance b.  Per instance the handle holds the linear terms q_b, r_b of every distinct cost (cost_index aliasing
+ * kept: a cost shared by several knots tracks the last of them, per instance) and the values of every Goal constraint; Q, R, H, c, the
+ * quaternion cost's w / q_ref, program costs and every other constraint stay shared.  Until the first per-instance call there is no
+ * per-instance data and every kernel runs as before.  The first per-instance call copies the shared values into every instance, then applies
+ * its change; a later shared to_set_goal_state / to_update_trajectory writes through to every instance (the later call wins).
+ * to_shift_trajectory leaves the objective alone: an MPC loop calls to_update_trajectories with the next start.  Multi-GPU: each rank passes
+ * its shard's rows, as for x0.  The quaternion cost's w / q_ref and program costs keep their shared values (program costs have no linear
+ * term); every solver path takes the per-instance values.  Not available (TO_EINVAL) on hybrid problems. */
+int to_set_goal_states(to_handle* h, const double* xf /*[B][n]*/, int objective, int constraint);    /* set_goal_state! per instance */
+int to_update_trajectories(to_handle* h, const double* Xref /*[B][nref][n]*/, const double* Uref /*[B][nref][m]*/,
+                           int32_t nref, int32_t start);                                            /* update_trajectory! per instance (TO_EDIM: nref < start + N - 1) */
+int to_get_cost_terms(to_handle* h, double* q /*[B][ncost][n]*/, double* r /*[B][ncost][m]*/);     /* the shared values broadcast when none are set */
+int to_set_cost_terms(to_handle* h, const double* q, const double* r);                              /* set_LQR_goal!(obj[k], ...) per instance, raw terms */
+int to_get_goal_values(to_handle* h, int32_t con, double* vals /*[B][p]*/);                        /* a Goal constraint's xf[inds] of every instance */
+int to_set_goal_values(to_handle* h, int32_t con, const double* vals);                             /* ... set per instance (TO_EINVAL: not a Goal) */
 
 /* ---- kernel 1: batched RK4 rollout (+ dual-number Jacobians) ---------------------------------------- */
 int to_rollout(to_handle* h);                                                 /* rollout!           src/problem.jl:330-340 */

@@ -1110,6 +1110,7 @@ class Problem:
         self.x0 = np.broadcast_to(x0, (B, n)).copy()
         self.xf = np.full(nf, np.nan) if xf is None else np.asarray(xf, dtype=float).copy()
         self._device = device
+        self._dt = np.array(dtv, dtype=float)        # the time steps as given: a rebuild must not re-derive them from the knot times
         self.spec = self._make_spec(dtv, t0)
         self._open()
         self._sig = self._signature()
@@ -1186,10 +1187,39 @@ class Problem:
         t = np.empty(self.N)
         self._raw_call("to_get_times", K._dp(t))
         opts = getattr(self, "_options", None)
+        # Per-instance state is carried over row by row.  The later change wins: a cost mutated since the handle was built, or a Goal
+        # constraint whose xf changed since the per-instance call, takes its new (shared) value in every instance; a constraint added
+        # since keeps the value it was built with.
+        carry, goal_carry = {}, {}
+        if getattr(self, "_inst", False):
+            q, r = np.empty((self.B, len(self._cost_objs), self.n)), np.empty((self.B, len(self._cost_objs), self.m))
+            self._raw_call("to_get_cost_terms", K._dp(q), K._dp(r))
+            built = self._sig[1]
+            carry = {id(c): (q[:, j].copy(), r[:, j].copy()) for j, c in enumerate(self._cost_objs) if getattr(c, "_version", 0) == built[j]}
+            snap = getattr(self, "_goal_snap", {})
+            live = {id(c): c for c in self.constraints.constraints}
+            for j, cid in enumerate(self._sig[2]):
+                con = live.get(cid)
+                if cid in snap and con is not None and np.array_equal(np.asarray(con.xf), snap[cid]):
+                    vals = np.empty((self.B, con.p))
+                    self._raw_call("to_get_goal_values", j, K._dp(vals))
+                    goal_carry[cid] = vals
         self.close()
-        self.spec = self._make_spec(np.diff(t), float(t[0]))
+        self.spec = self._make_spec(self._dt, float(t[0]))
         self._open()
         self._sig = self._signature()
+        self._inst = bool(carry or goal_carry)
+        if carry:
+            q, r = np.empty((self.B, len(self._cost_objs), self.n)), np.empty((self.B, len(self._cost_objs), self.m))
+            self._raw_call("to_get_cost_terms", K._dp(q), K._dp(r))
+            for j, c in enumerate(self._cost_objs):
+                if id(c) in carry:
+                    q[:, j], r[:, j] = carry[id(c)]
+            self._raw_call("to_set_cost_terms", K._dp(q), K._dp(r))
+        for j, c in enumerate(self.constraints.constraints):
+            if id(c) in goal_carry:
+                self._raw_call("to_set_goal_values", j, K._dp(goal_carry[id(c)]))
+        self._goal_snap = {cid: v for cid, v in getattr(self, "_goal_snap", {}).items() if cid in goal_carry}
         self._raw_call("to_set_initial_state", K._dp(self.x0))
         self._raw_call("to_set_controls", K._dp(U))
         if np.all(np.isfinite(X)):
@@ -1343,7 +1373,18 @@ def setinitialtime(prob, t0):   # RD.setinitialtime!  src/problem.jl:280
 
 
 def set_goal_state(prob, xf, objective=True, constraint=True):   # set_goal_state!  src/problem.jl:294-310
+    """``xf[n]``: the goal of every instance.  ``xf[B, n]``: instance ``b`` goes to ``xf[b]`` (``set_goal_state!`` per instance: its own
+    linear cost terms ``q = -Q xf[b]`` and Goal constraint values; the shared cost / constraint objects are left as they are)."""
     xf = np.ascontiguousarray(np.asarray(xf, dtype=np.float64))
+    if xf.ndim == 2:
+        if xf.shape != (prob.B, prob.n):
+            raise DimensionMismatch(f"set_goal_state!: xf has shape {xf.shape}, expected ({prob.n},) or ({prob.B}, {prob.n})")
+        prob._call("to_set_goal_states", K._dp(xf), int(objective), int(constraint))
+        prob._inst = True
+        if constraint:   # the Goal constraints that now hold per-instance values, with the xf they had (a later change to it wins)
+            prob._goal_snap = {id(c): np.array(c.xf, dtype=float) for c in prob.constraints if isinstance(c, GoalConstraint)}
+        prob.xf = xf.copy()
+        return
     if objective:
         for c in prob._cost_objs:
             if isinstance(c, QuadraticCostFunction):
@@ -1353,13 +1394,28 @@ def set_goal_state(prob, xf, objective=True, constraint=True):   # set_goal_stat
             if isinstance(con, GoalConstraint):
                 con.xf = xf[con.inds - 1].copy() if xf.size != con.xf.size else xf.copy()
     prob.xf = xf.copy()
+    if constraint:
+        prob._goal_snap = {}       # every instance takes the shared Goal values
     prob._call("to_set_goal_state", K._dp(xf), int(objective), int(constraint))
 
 
 def update_trajectory(prob, Xref, Uref, start=1):
     """``update_trajectory!(obj, Z, start)`` (src/objective.jl:198-212): knot ``i`` of the problem's (tracking) objective follows
-    row ``start - 1 + i`` of the reference ``Xref[nref, n]``, ``Uref[nref, m]`` -- ``set_LQR_goal!`` on every knot's cost."""
+    row ``start - 1 + i`` of the reference ``Xref[nref, n]``, ``Uref[nref, m]`` -- ``set_LQR_goal!`` on every knot's cost.
+    ``Xref[B, nref, n]``, ``Uref[B, nref, m]``: instance ``b`` tracks its own reference (same ``start``); the shared cost objects
+    are left as they are."""
     Xref = np.ascontiguousarray(np.asarray(Xref, dtype=np.float64)); Uref = np.ascontiguousarray(np.asarray(Uref, dtype=np.float64))
+    if Xref.ndim == 3 or Uref.ndim == 3:
+        if (Xref.ndim != 3 or Uref.ndim != 3 or Xref.shape[0] != prob.B or Uref.shape[0] != prob.B or Xref.shape[2] != prob.n
+                or Uref.shape[2] != prob.m or Uref.shape[1] != Xref.shape[1]):
+            raise DimensionMismatch("update_trajectory!: per-instance Xref must be [B, nref, n] and Uref [B, nref, m]")
+        if start < 1 or start - 1 + prob.N > Xref.shape[1]:
+            raise DimensionMismatch("update_trajectory!: the reference is shorter than start + N - 1")
+        if not all(isinstance(c, QuadraticCostFunction) for c in prob.obj):
+            raise ArgumentError("update_trajectory! is defined for objectives of QuadraticCostFunctions (src/objective.jl:207)")
+        prob._call("to_update_trajectories", K._dp(Xref), K._dp(Uref), int(Xref.shape[1]), int(start))
+        prob._inst = True
+        return
     if Xref.ndim != 2 or Uref.ndim != 2 or Xref.shape[1] != prob.n or Uref.shape[1] != prob.m or Uref.shape[0] != Xref.shape[0]:
         raise DimensionMismatch("update_trajectory!: Xref must be [nref, n] and Uref [nref, m]")
     if start < 1 or start - 1 + prob.N > Xref.shape[0]:
@@ -1369,6 +1425,28 @@ def update_trajectory(prob, Xref, Uref, start=1):
     for i, k in enumerate(range(start - 1, start - 1 + prob.N)):
         set_LQR_goal(prob.obj[i], Xref[k], Uref[k])
     prob._call("to_update_trajectory", K._dp(Xref), K._dp(Uref), int(Xref.shape[0]), int(start))
+
+
+def cost_terms(prob):
+    """The linear terms of every distinct cost of every instance: ``q[B, ncost, n]``, ``r[B, ncost, m]`` (the shared ones broadcast when no
+    per-instance goal was set).  ``ncost`` counts the distinct cost objects of the objective, in order of first use."""
+    nc = len(prob._cost_objs)
+    q, r = np.empty((prob.B, nc, prob.n)), np.empty((prob.B, nc, prob.m))
+    prob._call("to_get_cost_terms", K._dp(q), K._dp(r))
+    return q, r
+
+
+def set_cost_terms(prob, q, r):
+    """``set_LQR_goal!(obj[k], ...)`` per instance with raw terms: ``q[B, ncost, n]``, ``r[B, ncost, m]`` (layout of ``cost_terms``)."""
+    nc = len(prob._cost_objs)
+    q = np.ascontiguousarray(np.asarray(q, dtype=np.float64)); r = np.ascontiguousarray(np.asarray(r, dtype=np.float64))
+    if q.shape != (prob.B, nc, prob.n) or r.shape != (prob.B, nc, prob.m):
+        raise DimensionMismatch(f"set_cost_terms: expected q [{prob.B}, {nc}, {prob.n}] and r [{prob.B}, {nc}, {prob.m}], got {q.shape} and {r.shape}")
+    prob._ensure_current()
+    if len(prob._cost_objs) != nc:
+        raise DimensionMismatch("set_cost_terms: the objective changed its distinct costs; read cost_terms again")
+    prob._call("to_set_cost_terms", K._dp(q), K._dp(r))
+    prob._inst = True
 
 
 def shift_trajectory(prob, steps=1):

@@ -52,6 +52,9 @@ struct to_handle {
     double* d_merit2 = nullptr;   // {sum J, max viol}
     int* d_work = nullptr;
     ExpTab* d_exptab = nullptr;   // (frag) AL rows per z entry, rebuilt with the constraint tables / penalties
+    // per-instance linear cost terms / Goal values (DevProblem::qr / goal), empty until the first per-instance call; the host copy is the
+    // authoritative one and goes to the device whole after every change
+    std::vector<double> h_qr, h_goal;
     int* d_fragerr = nullptr;     // sticky error word of that kernel (queue overflow / spin limit), read by to_synchronize
     double* d_fragpool = nullptr; // gains of its speculative regularisation candidates
     int* d_fragq = nullptr;       // work queue of the register-resident Riccati kernel (riccati_frag.cu)
@@ -112,7 +115,7 @@ int upload_exptab(to_handle* h) {
     const int nm = h->P.n + h->P.m, n = h->P.n;
     for (int i = 0; i < nm; i++) {
         int nterm = 0;
-        for (int k = 0; k < TO_EXP_MAXT; k++) { t.nms[k][i] = -1.0; t.pkx[k][i] = 4095u; }      // empty knot range
+        for (int k = 0; k < TO_EXP_MAXT; k++) { t.nms[k][i] = -1.0; t.pkx[k][i] = 4095u; t.goal[k][i] = -1; }      // empty knot range
         for (size_t ci = 0; ci < h->h_cons.size(); ci++) {
             const DevCon& con = h->h_cons[ci];
             if (!con.diagonal) continue;
@@ -127,6 +130,7 @@ int upload_exptab(to_handle* h) {
                     t.nms[nterm][i] = -mu * sign; t.bound[nterm][i] = bound;
                     t.pkx[nterm][i] = (unsigned)con.first | ((unsigned)(con.last - con.first) << 12) | ((unsigned)con.p << 24) | (eq ? 0x80000000u : 0u);
                     t.pky[nterm][i] = (unsigned)(con.offset + row - con.first * con.p);
+                    if (eq) t.goal[nterm][i] = con.goff + row;
                 }
                 nterm++;
             }
@@ -134,6 +138,19 @@ int upload_exptab(to_handle* h) {
     }
     CU(h, cudaMemcpyAsync(h->d_exptab, &t, sizeof(t), cudaMemcpyHostToDevice, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));   // `t` goes out of scope
+    return TO_OK;
+}
+
+// set_LQR_goal! (src/cost_functions.jl:245-254): the linear term -M xf of a goal xf (q = -Q xf, r = -R uf), M dim x dim column-major.
+// The one place where a goal becomes a linear term: the shared setters and the per-instance ones produce the same bits for the same xf.
+void lqr_linear_term(const double* M, int dim, const double* xf, double* out) {
+    for (int i = 0; i < dim; i++) { double t = 0; for (int j = 0; j < dim; j++) t += M[j * dim + i] * xf[j]; out[i] = -t; }
+}
+
+int upload_inst(to_handle* h) {
+    CU(h, cudaMemcpyAsync(const_cast<double*>(h->P.qr), h->h_qr.data(), sizeof(double) * h->h_qr.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaMemcpyAsync(const_cast<double*>(h->P.goal), h->h_goal.data(), sizeof(double) * h->h_goal.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));   // the host tables may change right after
     return TO_OK;
 }
 
@@ -506,6 +523,7 @@ int to_create(const to_spec* s, to_handle** out) {
         if (rc) return bail(rc);
         h->h_cons[i].offset = P.lambda_len;
         P.lambda_len += (h->h_cons[i].last - h->h_cons[i].first + 1) * h->h_cons[i].p;
+        if (h->h_cons[i].kind == CON_GOAL) { h->h_cons[i].goff = P.ngoal; P.ngoal += h->h_cons[i].p; }
         if (!h->h_cons[i].diagonal) P.all_diag_con = 0;
     }
     P.ncost = s->ncost; P.ncon = s->ncon;
@@ -759,19 +777,136 @@ int to_set_initial_time(to_handle* h, double t0, double* tf_out) {
     if (tf_out) { double t = t0; for (double d : h->h_dt) t += d; *tf_out = t; }
     return TO_OK;
 }
+// ---- per-instance goals (DevProblem::qr / goal) -------------------------------------------------------------
+// The tables are created by the first per-instance call, filled from the shared values; later shared calls write through to every row.
+static int inst_tables(to_handle* h) {
+    if (h->P.qr) return TO_OK;
+    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance goals are not supported on hybrid problems");
+    const int B = h->P.B, ncost = h->P.ncost, n = h->P.n, m = h->P.m, nm = n + m, ngoal = h->P.ngoal;
+    h->h_qr.assign((size_t)B * ncost * nm, 0.0);
+    h->h_goal.assign((size_t)B * std::max(1, ngoal), 0.0);
+    for (int b = 0; b < B; b++) {
+        for (int ci = 0; ci < ncost; ci++) {
+            double* row = h->h_qr.data() + ((size_t)b * ncost + ci) * nm;
+            std::memcpy(row, h->h_costs[ci].q, sizeof(double) * n);
+            std::memcpy(row + n, h->h_costs[ci].r, sizeof(double) * m);
+        }
+        for (const auto& c : h->h_cons)
+            if (c.kind == CON_GOAL) std::memcpy(h->h_goal.data() + (size_t)b * std::max(1, ngoal) + c.goff, c.a, sizeof(double) * c.p);
+    }
+    double *dq = nullptr, *dg = nullptr;
+    int rc = dalloc(h, &dq, h->h_qr.size()); if (rc) return rc;
+    rc = dalloc(h, &dg, h->h_goal.size()); if (rc) return rc;
+    h->P.ngoal = std::max(1, ngoal);      // row stride of the Goal table (a problem without Goal constraints keeps one unused slot)
+    h->P.qr = dq; h->P.goal = dg;
+    return TO_OK;
+}
+static double* inst_q_row(to_handle* h, int b, int cid) { return h->h_qr.data() + ((size_t)b * h->P.ncost + cid) * (h->P.n + h->P.m); }
+
 // set_goal_state! src/problem.jl:294-310 with set_LQR_goal! (q = -Q xf; c untouched) src/cost_functions.jl:245-248
 int to_set_goal_state(to_handle* h, const double* xf, int objective, int constraint) {
     JOIN(h);
     if (!h || !xf) return TO_EINVAL;
     const int n = h->P.n;
     if (objective)
-        for (auto& c : h->h_costs)
-            for (int i = 0; i < n; i++) { double t = 0; for (int j = 0; j < n; j++) t += c.Q[j * n + i] * xf[j]; c.q[i] = -t; }
+        for (auto& c : h->h_costs) lqr_linear_term(c.Q, n, xf, c.q);
     if (constraint)
         for (auto& c : h->h_cons)
             if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) c.a[i] = xf[c.inds[i]];
     h->J_valid = false;
-    return upload_tables(h);
+    int rc = upload_tables(h); if (rc) return rc;
+    if (!h->P.qr) return TO_OK;
+    for (int b = 0; b < h->P.B; b++) {     // the later call wins: every instance takes the shared goal
+        if (objective)
+            for (int ci = 0; ci < h->P.ncost; ci++) std::memcpy(inst_q_row(h, b, ci), h->h_costs[ci].q, sizeof(double) * n);
+        if (constraint)
+            for (const auto& c : h->h_cons)
+                if (c.kind == CON_GOAL) std::memcpy(h->h_goal.data() + (size_t)b * h->P.ngoal + c.goff, c.a, sizeof(double) * c.p);
+    }
+    return upload_inst(h);
+}
+// set_goal_state! per instance: xf [B][n]
+int to_set_goal_states(to_handle* h, const double* xf, int objective, int constraint) {
+    JOIN(h);
+    if (!h || !xf) return TO_EINVAL;
+    int rc = inst_tables(h); if (rc) return rc;
+    const int n = h->P.n;
+    for (int b = 0; b < h->P.B; b++) {
+        const double* xb = xf + (size_t)b * n;
+        if (objective)
+            for (int ci = 0; ci < h->P.ncost; ci++) lqr_linear_term(h->h_costs[ci].Q, n, xb, inst_q_row(h, b, ci));
+        if (constraint)
+            for (const auto& c : h->h_cons)
+                if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) h->h_goal[(size_t)b * h->P.ngoal + c.goff + i] = xb[c.inds[i]];
+    }
+    h->J_valid = false;
+    return upload_inst(h);
+}
+// update_trajectory! per instance: Xref [B][nref][n], Uref [B][nref][m], one start for the batch
+int to_update_trajectories(to_handle* h, const double* Xref, const double* Uref, int32_t nref, int32_t start) {
+    JOIN(h);
+    if (!h || !Xref || !Uref) return TO_EINVAL;
+    const int n = h->P.n, m = h->P.m, N = h->P.N;
+    if (start < 1 || start - 1 + N > nref) return fail(h, TO_EDIM, "update_trajectory!: the reference is shorter than start + N - 1");
+    int rc = inst_tables(h); if (rc) return rc;
+    for (int b = 0; b < h->P.B; b++)
+        for (int i = 0; i < N; i++) {                   // set_LQR_goal!(obj[i], state(Z[k]), control(Z[k])) of instance b
+            const int cid = h->h_cost_index[i];
+            const DevCost& c = h->h_costs[cid];
+            double* row = inst_q_row(h, b, cid);
+            lqr_linear_term(c.Q, n, Xref + ((size_t)b * nref + start - 1 + i) * n, row);
+            lqr_linear_term(c.R, m, Uref + ((size_t)b * nref + start - 1 + i) * m, row + n);
+        }
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return upload_inst(h);
+}
+// the linear terms of every cost of every instance: q [B][ncost][n], r [B][ncost][m] (the shared ones broadcast when none are set)
+int to_get_cost_terms(to_handle* h, double* q, double* r) {
+    JOIN(h);
+    if (!h || !q || !r) return TO_EINVAL;
+    const int n = h->P.n, m = h->P.m, ncost = h->P.ncost;
+    for (int b = 0; b < h->P.B; b++)
+        for (int ci = 0; ci < ncost; ci++) {
+            const double* sq = h->P.qr ? inst_q_row(h, b, ci) : h->h_costs[ci].q;
+            const double* sr = h->P.qr ? inst_q_row(h, b, ci) + n : h->h_costs[ci].r;
+            std::memcpy(q + ((size_t)b * ncost + ci) * n, sq, sizeof(double) * n);
+            std::memcpy(r + ((size_t)b * ncost + ci) * m, sr, sizeof(double) * m);
+        }
+    return TO_OK;
+}
+// the values of Goal constraint con of every instance: vals [B][p] (the shared ones broadcast when none are set)
+int to_get_goal_values(to_handle* h, int32_t con, double* vals) {
+    JOIN(h);
+    if (!h || !vals) return TO_EINVAL;
+    if (con < 0 || con >= (int)h->h_cons.size() || h->h_cons[con].kind != CON_GOAL) return fail(h, TO_EINVAL, "to_get_goal_values: not a Goal constraint");
+    const DevCon& c = h->h_cons[con];
+    for (int b = 0; b < h->P.B; b++)
+        std::memcpy(vals + (size_t)b * c.p, h->P.goal ? h->h_goal.data() + (size_t)b * h->P.ngoal + c.goff : c.a, sizeof(double) * c.p);
+    return TO_OK;
+}
+int to_set_goal_values(to_handle* h, int32_t con, const double* vals) {
+    JOIN(h);
+    if (!h || !vals) return TO_EINVAL;
+    if (con < 0 || con >= (int)h->h_cons.size() || h->h_cons[con].kind != CON_GOAL) return fail(h, TO_EINVAL, "to_set_goal_values: not a Goal constraint");
+    int rc = inst_tables(h); if (rc) return rc;
+    const DevCon& c = h->h_cons[con];
+    for (int b = 0; b < h->P.B; b++) std::memcpy(h->h_goal.data() + (size_t)b * h->P.ngoal + c.goff, vals + (size_t)b * c.p, sizeof(double) * c.p);
+    h->J_valid = false;
+    return upload_inst(h);
+}
+// set_LQR_goal!(obj[k], ...) per instance with the raw terms: q [B][ncost][n], r [B][ncost][m]
+int to_set_cost_terms(to_handle* h, const double* q, const double* r) {
+    JOIN(h);
+    if (!h || !q || !r) return TO_EINVAL;
+    int rc = inst_tables(h); if (rc) return rc;
+    const int n = h->P.n, m = h->P.m, ncost = h->P.ncost;
+    for (int b = 0; b < h->P.B; b++)
+        for (int ci = 0; ci < ncost; ci++) {
+            std::memcpy(inst_q_row(h, b, ci), q + ((size_t)b * ncost + ci) * n, sizeof(double) * n);
+            std::memcpy(inst_q_row(h, b, ci) + n, r + ((size_t)b * ncost + ci) * m, sizeof(double) * m);
+        }
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return upload_inst(h);
 }
 
 // ---- kernel 1 ---------------------------------------------------------------------------------------------
@@ -782,13 +917,19 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
     if (start < 1 || start - 1 + N > nref) return fail(h, TO_EDIM, "update_trajectory!: the reference is shorter than start + N - 1");
     for (int i = 0; i < N; i++) {                       // set_LQR_goal!(obj[i], state(Z[k]), control(Z[k]))
         DevCost& c = h->h_costs[h->h_cost_index[i]];
-        const double* xf = Xref + (size_t)(start - 1 + i) * n;
-        const double* uf = Uref + (size_t)(start - 1 + i) * m;
-        for (int a = 0; a < n; a++) { double t = 0; for (int j = 0; j < n; j++) t += c.Q[j * n + a] * xf[j]; c.q[a] = -t; }
-        for (int a = 0; a < m; a++) { double t = 0; for (int j = 0; j < m; j++) t += c.R[j * m + a] * uf[j]; c.r[a] = -t; }
+        lqr_linear_term(c.Q, n, Xref + (size_t)(start - 1 + i) * n, c.q);
+        lqr_linear_term(c.R, m, Uref + (size_t)(start - 1 + i) * m, c.r);
     }
     h->J_valid = false; h->expanded = false; h->backward_done = false;
-    return upload_tables(h);
+    int rc = upload_tables(h); if (rc) return rc;
+    if (!h->P.qr) return TO_OK;
+    for (int b = 0; b < h->P.B; b++)                    // the later call wins: every instance takes the shared reference
+        for (int i = 0; i < N; i++) {
+            const int cid = h->h_cost_index[i];
+            std::memcpy(inst_q_row(h, b, cid), h->h_costs[cid].q, sizeof(double) * n);
+            std::memcpy(inst_q_row(h, b, cid) + n, h->h_costs[cid].r, sizeof(double) * m);
+        }
+    return upload_inst(h);
 }
 int to_shift_trajectory(to_handle* h, int32_t steps) {
     JOIN(h);

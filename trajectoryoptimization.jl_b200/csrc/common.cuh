@@ -53,7 +53,8 @@ struct DevCost {
 struct DevCon {
     int kind, first, last, p, sense, offset, ninds, flag;   // first/last: 1-based inclusive knots; offset into lambda
     int diagonal;
-    int n_max, n_min, pad;
+    int n_max, n_min;
+    int goff;                // GOAL: offset of its rows in an instance's row of DevProblem::goal
     int inds[TO_MAXNM];      // GOAL: state index per row (0-based); NORM: indices into z; CIRCLE/SPHERE: xi,yi,zi
     int a_max[TO_MAXNM];     // BOUND: z index of each finite upper bound (row i)        src/constraints.jl:675
     int a_min[TO_MAXNM];     // BOUND: z index of each finite lower bound (row n_max+i)  src/constraints.jl:676
@@ -79,6 +80,7 @@ struct ExpTab {
     double bound[TO_EXP_MAXT][TO_MAXNM];
     unsigned pkx[TO_EXP_MAXT][TO_MAXNM];    // first knot (12 bits) | last - first (12) | rows p of the constraint (7) | equality (1)
     unsigned pky[TO_EXP_MAXT][TO_MAXNM];    // lambda index of the row at knot 0
+    int goal[TO_EXP_MAXT][TO_MAXNM];        // Goal term: index of its bound in an instance's row of DevProblem::goal (-1: other terms)
 };
 
 // one dynamics model of a hybrid problem (to_dynamics_spec): a recorded program, RK4-discretised or a discrete jump map
@@ -157,10 +159,35 @@ struct DevProblem {
     // skip every instance that is not ACTIVE, so a converged instance keeps the X, U, lambda, K, d, rho, J it stopped with.
     // nullptr outside to_solve: every instance is worked on.
     const int* active;        // [B]
+    // Per-instance goals / tracking references (to_set_goal_states, to_update_trajectories, to_set_cost_terms): the linear terms of every
+    // cost and the values of every Goal constraint, per instance.  nullptr until the first per-instance call; every kernel then reads the
+    // shared DevCost::q / r and DevCon::a.
+    const double* qr;         // [B][ncost][n+m]: q | r of cost cid for instance b
+    const double* goal;       // [B][ngoal]: a[row] of Goal constraint ci at DevCon::goff
+    int ngoal, pad_inst;
 };
 
 enum { SOLVE_ACTIVE = 0, SOLVE_WAITING = 1, SOLVE_DONE = 2 };
 __host__ __device__ inline bool retired(const DevProblem& P, int b) { return P.active != nullptr && P.active[b] != SOLVE_ACTIVE; }
+
+// Linear cost terms and Goal values of instance b: the only place that decides between the per-instance tables and the shared descriptors.
+// INST = false is the shared path, compiled without a look at the tables; the hot kernels take INST as a template parameter and are
+// launched with INST = true only when the tables exist.
+template <bool INST>
+__host__ __device__ __forceinline__ const double* inst_q(const DevProblem& P, int b, int cid) {
+    if constexpr (INST) { if (P.qr) return P.qr + ((size_t)b * P.ncost + cid) * (P.n + P.m); }
+    return P.costs[cid].q;
+}
+template <bool INST>
+__host__ __device__ __forceinline__ const double* inst_r(const DevProblem& P, int b, int cid) {
+    if constexpr (INST) { if (P.qr) return P.qr + ((size_t)b * P.ncost + cid) * (P.n + P.m) + P.n; }
+    return P.costs[cid].r;
+}
+template <bool INST>
+__host__ __device__ __forceinline__ const double* goal_values(const DevProblem& P, int b, int ci) {
+    if constexpr (INST) { if (P.goal) return P.goal + (size_t)b * P.ngoal + P.cons[ci].goff; }
+    return P.cons[ci].a;
+}
 
 __host__ __device__ inline const double* traj_X(const DevProblem& P, int buf, int b) { return P.X + buf * P.strideX + (size_t)b * P.N * P.n; }
 __host__ __device__ inline const double* traj_U(const DevProblem& P, int buf, int b) { return P.U + buf * P.strideU + (size_t)b * (P.N - 1) * P.m; }

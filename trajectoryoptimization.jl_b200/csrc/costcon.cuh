@@ -70,16 +70,17 @@ __device__ __forceinline__ double quat_cost_term(const DevCost& c, const double*
     return c.w * fmin(1 + dq, 1 - dq);
 }
 
-__device__ inline double cost_value(const DevCost& c, int n, int m, const double* x, const double* u, bool has_u) {
+// q, r: the linear terms to use (c.q / c.r, or an instance's row of DevProblem::qr, inst_q / inst_r)
+__device__ inline double cost_value(const DevCost& c, const double* q, const double* r, int n, int m, const double* x, const double* u, bool has_u) {
     if (c.expr) return expr_eval(c, n, x, u, has_u, -1, -1).v;
     double J = 0;
     if (c.diag) {
         double a = 0, l = 0;
-        for (int i = 0; i < n; i++) { a = fma(c.Qd[i] * x[i], x[i], a); l = fma(c.q[i], x[i], l); }
+        for (int i = 0; i < n; i++) { a = fma(c.Qd[i] * x[i], x[i], a); l = fma(q[i], x[i], l); }
         J = 0.5 * a + l + c.c;
         if (has_u) {
             double au = 0, lu = 0;
-            for (int i = 0; i < m; i++) { au = fma(c.Rd[i] * u[i], u[i], au); lu = fma(c.r[i], u[i], lu); }
+            for (int i = 0; i < m; i++) { au = fma(c.Rd[i] * u[i], u[i], au); lu = fma(r[i], u[i], lu); }
             J += 0.5 * au + lu;
         }
         if (c.quat) J += quat_cost_term(c, x);
@@ -91,7 +92,7 @@ __device__ inline double cost_value(const DevCost& c, int n, int m, const double
         J = fma(0.5 * qx, x[j], J);
     }
     double lin = 0;
-    for (int i = 0; i < n; i++) lin = fma(c.q[i], x[i], lin);
+    for (int i = 0; i < n; i++) lin = fma(q[i], x[i], lin);
     J += lin + c.c;
     if (has_u) {
         double Ju = 0, linu = 0;
@@ -100,7 +101,7 @@ __device__ inline double cost_value(const DevCost& c, int n, int m, const double
             for (int i = 0; i < m; i++) ru = fma(c.R[j * m + i], u[i], ru);
             Ju = fma(0.5 * ru, u[j], Ju);
         }
-        for (int i = 0; i < m; i++) linu = fma(c.r[i], u[i], linu);
+        for (int i = 0; i < m; i++) linu = fma(r[i], u[i], linu);
         J += Ju + linu;
         if (!c.zeroH) {
             double h = 0;
@@ -111,23 +112,29 @@ __device__ inline double cost_value(const DevCost& c, int n, int m, const double
     }
     return J;
 }
+__device__ inline double cost_value(const DevCost& c, int n, int m, const double* x, const double* u, bool has_u) {
+    return cost_value(c, c.q, c.r, n, m, x, u, has_u);
+}
 
 // grad[n+m]; the u-part is left untouched at the terminal knot (the reference skips it when is_terminal(z))
 template <bool QUAT = true>
-__device__ inline void cost_gradient_quadratic(const DevCost& c, int n, int m, const double* x, const double* u, bool is_terminal, double* grad);
-__device__ inline void cost_gradient(const DevCost& c, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
+__device__ inline void cost_gradient_quadratic(const DevCost& c, const double* q, const double* r, int n, int m, const double* x, const double* u, bool is_terminal, double* grad);
+__device__ inline void cost_gradient(const DevCost& c, const double* q, const double* r, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
     if (c.expr) {   // RD.gradient!(ForwardAD) of a user cost
         const int lim = is_terminal ? n : n + m;
         for (int i = 0; i < lim; i++) grad[i] = expr_eval(c, n, x, u, !is_terminal, i, -1).d1;
         return;
     }
-    cost_gradient_quadratic(c, n, m, x, u, is_terminal, grad);
+    cost_gradient_quadratic(c, q, r, n, m, x, u, is_terminal, grad);
+}
+__device__ inline void cost_gradient(const DevCost& c, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
+    cost_gradient(c, c.q, c.r, n, m, x, u, is_terminal, grad);
 }
 // QuadraticCostFunction only (the register-resident kernels call this directly with QUAT = false: no dynamically indexed stores)
 template <bool QUAT>
-__device__ inline void cost_gradient_quadratic(const DevCost& c, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
+__device__ inline void cost_gradient_quadratic(const DevCost& c, const double* q, const double* r, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
     for (int i = 0; i < n; i++) {
-        double g = c.q[i];
+        double g = q[i];
         if (c.diag) g = fma(c.Qd[i], x[i], g);
         else for (int j = 0; j < n; j++) g = fma(c.Q[j * n + i], x[j], g);
         grad[i] = g;
@@ -140,7 +147,7 @@ __device__ inline void cost_gradient_quadratic(const DevCost& c, int n, int m, c
     }
     if (!is_terminal) {
         for (int i = 0; i < m; i++) {
-            double g = c.r[i];
+            double g = r[i];
             if (c.diag) g = fma(c.Rd[i], u[i], g);
             else for (int j = 0; j < m; j++) g = fma(c.R[j * m + i], u[j], g);
             grad[n + i] = g;
@@ -184,10 +191,11 @@ __device__ inline void cost_hessian_quadratic(const DevCost& c, int n, int m, bo
 
 __device__ __forceinline__ double zget(int n, const double* x, const double* u, int j) { return j < n ? x[j] : u[j - n]; }
 
-__device__ inline void con_evaluate(const DevCon& con, int n, int m, const double* x, const double* u, double* c) {
+// goal: the Goal values to use (con.a, or an instance's row of DevProblem::goal, goal_values); read for CON_GOAL only
+__device__ inline void con_evaluate(const DevCon& con, const double* goal, int n, int m, const double* x, const double* u, double* c) {
     switch (con.kind) {
         case CON_GOAL:
-            for (int i = 0; i < con.p; i++) c[i] = x[con.inds[i]] - con.a[i];
+            for (int i = 0; i < con.p; i++) c[i] = x[con.inds[i]] - goal[i];
             break;
         case CON_BOUND: {   // upper block first, then the lower block
             int i = 0;
@@ -250,6 +258,9 @@ __device__ inline void con_evaluate(const DevCon& con, int n, int m, const doubl
             break;
         }
     }
+}
+__device__ inline void con_evaluate(const DevCon& con, int n, int m, const double* x, const double* u, double* c) {
+    con_evaluate(con, con.a, n, m, x, u, c);
 }
 
 // jac: p x (n+m) col-major, fully written
@@ -464,9 +475,10 @@ __device__ inline int cone_hess_projection(int cone, const double* x, const doub
 }
 
 // AL penalty of one knot (conic form): sum_c (|Pi_{K*}(lambda - mu c)|^2 - |lambda|^2) / (2 mu); also the
-// knot's constraint violation |c - Pi_K(c)|_inf.  k1 = 1-based knot.  x/u may be registers, local or global.
+// knot's constraint violation |c - Pi_K(c)|_inf.  k1 = 1-based knot, b = instance (its Goal values when INST).  x/u may be registers, local or global.
+template <bool INST = false>
 __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const double* x, const double* u,
-                                         const double* lam_b, double& viol) {
+                                         const double* lam_b, double& viol, int b = 0) {
     double pen = 0;
     for (int ci = 0; ci < P.ncon; ci++) {
         const DevCon& con = P.cons[ci];
@@ -474,7 +486,7 @@ __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const doub
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k1 - con.first) * con.p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
-        con_evaluate(con, P.n, P.m, x, u, c);
+        con_evaluate(con, goal_values<INST>(P, b, ci), P.n, P.m, x, u, c);
         for (int i = 0; i < con.p; i++) lbar[i] = lam[i] - mu * c[i];
         cone_projection(dualcone(con.sense), lbar, con.p, lp);
         double a = 0, l2 = 0;
@@ -488,14 +500,16 @@ __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const doub
 
 // Cost expansion of one knot with the AL terms (Gauss-Newton):
 //   grad += -cz' D' lp ; hess += mu cz' D'D cz,  D = grad Pi_{K*}(lambda - mu c), lp = Pi_{K*}(lambda - mu c)
-// k0 = 0-based knot.  grad[n+m], hess[(n+m)^2] col-major symmetric.
+// k0 = 0-based knot, b = instance (its linear cost terms and Goal values when INST).  grad[n+m], hess[(n+m)^2] col-major symmetric.
+template <bool INST = false>
 __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const double* x, const double* u, const double* lam_b,
-                                         double* grad, double* hess) {
+                                         double* grad, double* hess, int b = 0) {
     const int n = P.n, m = P.m, nm = n + m;
     const bool last = (k0 == P.N - 1);
-    const DevCost& cost = P.costs[P.cost_index[k0]];
+    const int cid = P.cost_index[k0];
+    const DevCost& cost = P.costs[cid];
     for (int i = 0; i < nm; i++) grad[i] = 0;
-    cost_gradient(cost, n, m, x, u, last, grad);
+    cost_gradient(cost, inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, last, grad);
     cost_hessian(cost, n, m, x, u, last, hess);
     const int lim = last ? n : nm;
     for (int ci = 0; ci < P.ncon; ci++) {
@@ -505,7 +519,7 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k0 + 1 - con.first) * p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
-        con_evaluate(con, n, m, x, u, c);
+        con_evaluate(con, goal_values<INST>(P, b, ci), n, m, x, u, c);
         if (con.diagonal) {   // Goal / Bound: +-1 selector rows (src/constraints.jl:62-68, :757-765) -- row by row, no dense products
             const bool eq = (con.kind == CON_GOAL);
             const int nrow = eq ? p : con.n_max + con.n_min;

@@ -165,7 +165,8 @@ __device__ __forceinline__ void prefetch_knot(double* base, int g, int l, int k,
 
 // closed-loop rollout of instance b (group g of the CTA) with step size alpha, diagonal costs, Goal/Bound constraints.
 // The candidate trajectory goes to buffer `cbuf`.  Returns the merit; `ok` = no blow-up.
-template <int MODEL, int IPB, int G, bool LIE>
+// INST: the instance's own linear cost terms and Goal values (DevProblem::qr / goal, read from global memory instead of the CTA's table).
+template <int MODEL, int IPB, int G, bool LIE, bool INST>
 __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab& tab, double* stage, int b, int g, int l, unsigned gmask,
                                                double alpha, int cbuf, bool& ok, double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
@@ -245,20 +246,23 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
             double a2 = 0.0, l1 = 0.0, cc;
             if (tab.ncost_cached) {
                 const FwdCost& c = tab.cost[cid];
+                const double* cq = c.q; const double* cr = c.r;
+                if constexpr (INST) { cq = inst_q<true>(P, b, cid); cr = inst_r<true>(P, b, cid); }
 #pragma unroll
-                for (int i = 0; i < n; i++) { a2 = fma(c.Qd[i] * x[i], x[i], a2); l1 = fma(c.q[i], x[i], l1); }
+                for (int i = 0; i < n; i++) { a2 = fma(c.Qd[i] * x[i], x[i], a2); l1 = fma(cq[i], x[i], l1); }
                 if (!last) {
 #pragma unroll
-                    for (int i = 0; i < m; i++) { a2 = fma(c.Rd[i] * u[i], u[i], a2); l1 = fma(c.r[i], u[i], l1); }
+                    for (int i = 0; i < m; i++) { a2 = fma(c.Rd[i] * u[i], u[i], a2); l1 = fma(cr[i], u[i], l1); }
                 }
                 cc = c.c;
             } else {
                 const DevCost& c = P.costs[cid];
+                const double* cq = inst_q<INST>(P, b, cid); const double* cr = inst_r<INST>(P, b, cid);
 #pragma unroll
-                for (int i = 0; i < n; i++) { a2 = fma(c.Qd[i] * x[i], x[i], a2); l1 = fma(c.q[i], x[i], l1); }
+                for (int i = 0; i < n; i++) { a2 = fma(c.Qd[i] * x[i], x[i], a2); l1 = fma(cq[i], x[i], l1); }
                 if (!last) {
 #pragma unroll
-                    for (int i = 0; i < m; i++) { a2 = fma(c.Rd[i] * u[i], u[i], a2); l1 = fma(c.r[i], u[i], l1); }
+                    for (int i = 0; i < m; i++) { a2 = fma(c.Rd[i] * u[i], u[i], a2); l1 = fma(cr[i], u[i], l1); }
                 }
                 cc = c.c;
             }
@@ -275,12 +279,14 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
                 double a = 0.0, l2 = 0.0;
                 if (c.kind == CON_GOAL) {
                     const unsigned mk = c.mask_max;
+                    const double* ga = c.a;
+                    if constexpr (INST) ga = goal_values<true>(P, b, ci);
 #pragma unroll
                     for (int i = 0; i < n; i++) {
                         if (mk & (1u << i)) {
                             const int row = c.row_max[i];
                             const double lm = st[S::sidx(lo + row, g)];
-                            const double cv = x[i] - c.a[row];
+                            const double cv = x[i] - ga[row];
                             const double lp = fma(-mu, cv, lm);
                             a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, fabs(cv));
                         }
@@ -326,7 +332,7 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
 }
 
 // generic path (dense costs or general constraints): pointer-based evaluation, operands read directly from global
-template <int MODEL, bool LIE>
+template <int MODEL, bool LIE, bool INST>
 __device__ __forceinline__ double rollout_generic(const DevProblem& P, int b, double alpha, int cbuf, bool& ok, double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     const int N = P.N, buf = P.cur[b];
@@ -369,8 +375,9 @@ __device__ __forceinline__ double rollout_generic(const DevProblem& P, int b, do
 #pragma unroll
             for (int a = 0; a < m; a++) Uc[(size_t)k * m + a] = u[a];
         }
-        J += cost_value(P.costs[P.cost_index[k]], n, m, x, u, !last);
-        J += al_knot_penalty(P, k + 1, x, u, lam_b, viol);
+        const int cid = P.cost_index[k];
+        J += cost_value(P.costs[cid], inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, !last);
+        J += al_knot_penalty<INST>(P, k + 1, x, u, lam_b, viol, b);
         if (!last) {
             rk4_step<MODEL, double>(model_params<MODEL>(P, k), x, u, P.dt[k], xn);
 #pragma unroll
@@ -392,7 +399,7 @@ extern __shared__ __align__(16) unsigned char fwd_smem[];
 
 // One line-search pass: lane l of group g evaluates trial (trial0 + l) of instance b.
 //   first_pass : ignore / reset accepted[b];   final_pass : commit failures (no acceptable step size).
-template <int MODEL, int G, bool FAST, int LANES, bool LIE>
+template <int MODEL, int G, bool FAST, int LANES, bool LIE, bool INST>
 __global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, int trial0, int first_pass, int final_pass) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     // LANES = 16: only half of the warp carries groups.  The pass is a latency-bound FP64 chain at ~4 warps per SM, and
@@ -423,8 +430,8 @@ __global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, 
         const int cbuf = (P.cur[b] + 1 + l) % TO_NBUF;
         bool ok = false;
         double J, viol = 0.0;
-        if (FAST) J = rollout_fast<MODEL, IPB, G, LIE>(P, *tab, stage, b, g, l, gmask, alpha, cbuf, ok, viol);
-        else J = rollout_generic<MODEL, LIE>(P, b, alpha, cbuf, ok, viol);
+        if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST>(P, *tab, stage, b, g, l, gmask, alpha, cbuf, ok, viol);
+        else J = rollout_generic<MODEL, LIE, INST>(P, b, alpha, cbuf, ok, viol);
         const bool good = (trial <= P.opt.ls_iters) && ls_accept(P, J, P.J[b], alpha, P.dV[2 * b], P.dV[2 * b + 1], ok);
         const unsigned votes = __ballot_sync(gmask, good) & gmask;
         if (votes) {
@@ -453,13 +460,13 @@ __global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, 
     (void)sizeof(S);
 }
 
-template <int MODEL, int G, bool FAST, int LANES, bool LIE = false>
+template <int MODEL, int G, bool FAST, int LANES, bool LIE = false, bool INST = false>
 cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     constexpr int IPB = LANES / G;
     const int blocks = (P.B + IPB - 1) / IPB;
     const size_t smem = FAST ? sizeof(FwdTab) + (size_t)FWD_STAGES * Stage<n, m, IPB, NE>::DOUBLES * sizeof(double) : 0;
-    auto kern = k_linesearch<MODEL, G, FAST, LANES, LIE>;
+    auto kern = k_linesearch<MODEL, G, FAST, LANES, LIE, INST>;
     static bool configured[TO_MAXDEV] = {false};
     const int dev = current_device_slot();
     if (!configured[dev] && smem > 48 * 1024) {
@@ -471,19 +478,26 @@ cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int f
     return cudaGetLastError();
 }
 
-template <int MODEL, int G, bool FAST>
-cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
+template <int MODEL, int G, bool FAST, bool INST>
+cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     // lanes of each warp that carry groups: 16 for the first pass (half-warp FP64 instructions take one pipe pass); the later passes
     // use 16 when they walk the compact late list (two-instance CTAs, see to_create) and 32 when they scan all instances.
     const int lanes = first_pass ? 16 : (P.late_list ? 16 : 32);
     if constexpr (MODEL == MODEL_QUADROTOR) {   // Lie-group error state: dx = state_diff(xbar, x), gains m x (n - 1)
         if (P.lie) {
-            if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, FAST, (G <= 16 ? 16 : 32), true>(P, trial0, first_pass, final_pass, s);
-            return launch_pass_l<MODEL, G, FAST, 32, true>(P, trial0, first_pass, final_pass, s);
+            if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, FAST, (G <= 16 ? 16 : 32), true, INST>(P, trial0, first_pass, final_pass, s);
+            return launch_pass_l<MODEL, G, FAST, 32, true, INST>(P, trial0, first_pass, final_pass, s);
         }
     }
-    if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, FAST, (G <= 16 ? 16 : 32)>(P, trial0, first_pass, final_pass, s);
-    return launch_pass_l<MODEL, G, FAST, 32>(P, trial0, first_pass, final_pass, s);
+    if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, FAST, (G <= 16 ? 16 : 32), false, INST>(P, trial0, first_pass, final_pass, s);
+    return launch_pass_l<MODEL, G, FAST, 32, false, INST>(P, trial0, first_pass, final_pass, s);
+}
+
+// per-instance linear cost terms / Goal values: a kernel variant of its own, so that the shared one is the code it has always been
+template <int MODEL, int G, bool FAST>
+cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
+    if (P.qr) return launch_pass_i<MODEL, G, FAST, true>(P, trial0, first_pass, final_pass, s);
+    return launch_pass_i<MODEL, G, FAST, false>(P, trial0, first_pass, final_pass, s);
 }
 
 bool fast_path(const DevProblem& P) {

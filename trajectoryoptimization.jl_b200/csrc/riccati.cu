@@ -168,7 +168,7 @@ __device__ __forceinline__ uint2 pack_term(int first, int last, int base, int p,
     return make_uint2((unsigned)f | ((unsigned)span << 12) | ((unsigned)p << 24) | (eq ? 0x80000000u : 0u), (unsigned)(base - f * p));
 }
 
-template <int N_, int M_, int STAGES, bool FASTAL, bool MMA, int MINB, int NSLOT>
+template <int N_, int M_, int STAGES, bool FASTAL, bool MMA, int MINB, int NSLOT, bool INST>
 __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __restrict__ work_counter) {
     using SM = RiccatiSmem<N_, M_, STAGES, MMA>;
     constexpr int n = N_, m = M_, NM = SM::NM, LDAB = SM::LDAB, LDT = SM::LDT, NP = SM::NP, LDK = SM::LDK;
@@ -220,6 +220,9 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
     }
 
     // ---- lane-resident AL terms of z_lane (Goal / Bound constraints) ----------------------------------------
+    int tgoal[MAXT];   // (INST) index of a Goal term's value in an instance's row of P.goal, -1 for the other terms
+#pragma unroll
+    for (int t = 0; t < MAXT; t++) tgoal[t] = -1;
     if (FASTAL) {
         if (lane < SM::NMT) {
 #pragma unroll
@@ -237,6 +240,10 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     else { row = con.row_min[lane]; bound = con.b[lane]; sign = -1.0; }
                     if (row < 0) continue;
                     if (nterm < MAXT) { sm.tnms[nterm][lane] = -mu * sign; sm.tbound[nterm][lane] = bound; sm.tpk[nterm][lane] = pack_term(con.first, con.last, con.offset + row, con.p, eq); }
+                    if (INST && eq && nterm < MAXT) {
+#pragma unroll
+                        for (int t = 0; t < MAXT; t++) if (t == nterm) tgoal[t] = con.goff + row;
+                    }
                     nterm++;
                 }
             }
@@ -259,6 +266,12 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         b = __shfl_sync(0xffffffffu, b, 0);
         if (b >= P.B) break;
         if (retired(P, b)) continue;            // to_solve: not ACTIVE
+        if constexpr (INST && FASTAL) {         // this instance's Goal values into the lane-resident terms (read back by this lane only)
+            if (P.goal && lane < NM) {
+#pragma unroll
+                for (int t = 0; t < MAXT; t++) if (tgoal[t] >= 0) sm.tbound[t][lane] = P.goal[(size_t)b * P.ngoal + tgoal[t]];
+            }
+        }
 
         const int buf = P.cur[b];
         const double* X = traj_X(P, buf, b);
@@ -282,6 +295,11 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         static_assert(offsetof(DevCost, r) - offsetof(DevCost, Rd) == offsetof(DevCost, q) - offsetof(DevCost, Qd), "DevCost layout");
         auto cost_coeff_ptr = [&](int cid, bool hess) -> const double* {
             return reinterpret_cast<const double*>(reinterpret_cast<const char*>(P.costs) + (size_t)cid * sizeof(DevCost) + coff + (hess ? 0 : GOFF));
+        };
+        // cG of cost cid: the instance's own q | r row when INST (same lane -> entry mapping: q_i | r_a sit at i | n + a)
+        auto cost_g_ptr = [&](int cid) -> const double* {
+            if constexpr (INST) { if (P.qr) return inst_q<true>(P, b, cid) + (lane < NM ? lane : n); }
+            return cost_coeff_ptr(cid, false);
         };
         // act: bit t = term slot t is active at the knot, bit 4 + t = it is an equality (computed by load_lams one knot ahead)
         auto expand_fast = [&](double zi, const double (&lam)[MAXT], int act, double cH, double cG, double& gi, double& hi) {
@@ -378,7 +396,9 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
             __syncwarp();
             double s_reg = 0.0;   // lane i < n holds s_i
             {
-                const DevCost& cost = P.costs[P.cost_index[N - 1]];
+                const int cidN = P.cost_index[N - 1];
+                const DevCost& cost = P.costs[cidN];
+                const double* cq = inst_q<INST>(P, b, cidN);
                 if (lane < n) {
                     const int i = lane;
                     const double xi = X[(size_t)(N - 1) * n + i];
@@ -386,10 +406,10 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     if (FASTAL && cost.diag) {
                         double lam[MAXT];
                         int act; load_lams(N - 1, lam, act);
-                        expand_fast(xi, lam, act, cost.Qd[lane], cost.q[lane], gi, hi);
+                        expand_fast(xi, lam, act, cost.Qd[lane], cq[lane], gi, hi);
                         sm.S[i * LDS_ + i] = hi;
                     } else {
-                        gi = cost.q[i]; hi = 0.0;
+                        gi = cq[i]; hi = 0.0;
                         if (cost.diag) { gi = fma(cost.Qd[i], xi, gi); hi = cost.Qd[i]; }
                         else {
                             for (int j = 0; j < n; j++) { gi = fma(cost.Q[j * n + i], X[(size_t)(N - 1) * n + j], gi); sm.S[j * LDS_ + i] = cost.Q[j * n + i]; }
@@ -401,7 +421,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                             const double* lam = lam_b + con.offset + (size_t)(N - con.first) * con.p;
                             if (con.kind == CON_GOAL) {
                                 const int row = con.row_max[i];
-                                if (row >= 0) { const double lp = lam[row] - mu * (xi - con.a[row]); gi -= lp; hi += mu; }
+                                if (row >= 0) { const double lp = lam[row] - mu * (xi - goal_values<INST>(P, b, ci)[row]); gi -= lp; hi += mu; }
                             } else if (con.kind == CON_BOUND) {
                                 int row = con.row_max[i];
                                 if (row >= 0) { const double lb = lam[row] - mu * (xi - con.a[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
@@ -424,7 +444,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
             // software pipeline of the cost coefficients: (cH,cG) of knot k are loaded during knot k+1, its index during knot k+2
             double cH_cur = 0.0, cG_cur = 0.0;
             int cid_next = (N >= 3) ? P.cost_index[N - 3] : 0;
-            if (FASTAL && P.all_diag_cost) { const int c0 = P.cost_index[N - 2]; cH_cur = *cost_coeff_ptr(c0, true); cG_cur = *cost_coeff_ptr(c0, false); }
+            if (FASTAL && P.all_diag_cost) { const int c0 = P.cost_index[N - 2]; cH_cur = *cost_coeff_ptr(c0, true); cG_cur = *cost_g_ptr(c0); }
             __syncwarp();
 
             double dV1 = 0.0, dV2 = 0.0;   // accumulated by lane n
@@ -442,7 +462,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                 double cH_nxt = 0.0, cG_nxt = 0.0;
                 int cid_next2 = 0;
                 if (FASTAL && P.all_diag_cost && k > 0) {
-                    cH_nxt = ldg_pinned(cost_coeff_ptr(cid_next, true)); cG_nxt = ldg_pinned(cost_coeff_ptr(cid_next, false));
+                    cH_nxt = ldg_pinned(cost_coeff_ptr(cid_next, true)); cG_nxt = ldg_pinned(cost_g_ptr(cid_next));
                     if (k > 1) cid_next2 = ldg_pinned(P.cost_index + (k - 2));
                 }
                 // ---- cost + AL expansion of knot k: lane i < NM handles z_i (diagonal terms) ------------
@@ -452,23 +472,26 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     if (FASTAL && P.all_diag_cost) {
                         if (lane < NM) expand_fast(z_cur, lam_cur, act_cur, cH_cur, cG_cur, gi, hi);
                     } else if (lane < NM) {
-                        const DevCost& cost = P.costs[P.cost_index[k]];
+                        const int cidk = P.cost_index[k];
+                        const DevCost& cost = P.costs[cidk];
+                        const double* cq = inst_q<INST>(P, b, cidk);
+                        const double* cr = inst_r<INST>(P, b, cidk);
                         const int i = lane;
                         const double zi = z_cur;
                         if (FASTAL && cost.diag) {
-                            expand_fast(zi, lam_cur, act_cur, (i < n) ? cost.Qd[i] : cost.Rd[i - n], (i < n) ? cost.q[i] : cost.r[i - n], gi, hi);
+                            expand_fast(zi, lam_cur, act_cur, (i < n) ? cost.Qd[i] : cost.Rd[i - n], (i < n) ? cq[i] : cr[i - n], gi, hi);
                         } else {
                             if (cost.diag) {
-                                if (i < n) { gi = fma(cost.Qd[i], zi, cost.q[i]); hi = cost.Qd[i]; }
-                                else { gi = fma(cost.Rd[i - n], zi, cost.r[i - n]); hi = cost.Rd[i - n]; }
+                                if (i < n) { gi = fma(cost.Qd[i], zi, cq[i]); hi = cost.Qd[i]; }
+                                else { gi = fma(cost.Rd[i - n], zi, cr[i - n]); hi = cost.Rd[i - n]; }
                             } else {
                                 if (i < n) {
-                                    gi = cost.q[i];
+                                    gi = cq[i];
                                     for (int j = 0; j < n; j++) gi = fma(cost.Q[j * n + i], X[(size_t)k * n + j], gi);
                                     if (!cost.zeroH) for (int a = 0; a < m; a++) gi = fma(cost.H[i * m + a], U[(size_t)k * m + a], gi);
                                 } else {
                                     const int a = i - n;
-                                    gi = cost.r[a];
+                                    gi = cr[a];
                                     for (int j = 0; j < m; j++) gi = fma(cost.R[j * m + a], U[(size_t)k * m + j], gi);
                                     if (!cost.zeroH) for (int j = 0; j < n; j++) gi = fma(cost.H[j * m + a], X[(size_t)k * n + j], gi);
                                 }
@@ -480,7 +503,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                                 const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
                                 if (con.kind == CON_GOAL) {
                                     const int row = (i < n) ? con.row_max[i] : -1;
-                                    if (row >= 0) { const double lp = lam[row] - mu * (zi - con.a[row]); gi -= lp; hi += mu; }
+                                    if (row >= 0) { const double lp = lam[row] - mu * (zi - goal_values<INST>(P, b, ci)[row]); gi -= lp; hi += mu; }
                                 } else if (con.kind == CON_BOUND) {
                                     int row = con.row_max[i];
                                     if (row >= 0) { const double lb = lam[row] - mu * (zi - con.a[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
@@ -934,10 +957,10 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
     }
 }
 
-template <int N_, int M_, bool FASTAL, int STAGES, int MINB, bool MMA, int NSLOT = MAXT>
+template <int N_, int M_, bool FASTAL, int STAGES, int MINB, bool MMA, int NSLOT, bool INST>
 cudaError_t launch_riccati_v(const DevProblem& P, int* work_counter, cudaStream_t s) {
     using SM = RiccatiSmem<N_, M_, STAGES, MMA>;
-    auto kern = k_riccati<N_, M_, STAGES, FASTAL, MMA, MINB, NSLOT>;
+    auto kern = k_riccati<N_, M_, STAGES, FASTAL, MMA, MINB, NSLOT, INST>;
     static int ctas_cfg[TO_MAXDEV] = {0}, sms_cfg[TO_MAXDEV] = {0};      // per device (0 = not configured yet)
     const int smem = (int)sizeof(SM);
     const int dev = current_device_slot();
@@ -959,24 +982,26 @@ cudaError_t launch_riccati_v(const DevProblem& P, int* work_counter, cudaStream_
     return cudaGetLastError();
 }
 
-template <int N_, int M_, bool FASTAL>
+// INST: per-instance linear cost terms / Goal values (P.qr), a kernel variant of its own so that the shared one stays as it is
+template <int N_, int M_, bool FASTAL, bool INST>
 cudaError_t launch_riccati_t(const DevProblem& P, int* work_counter, cudaStream_t s) {
     if constexpr (N_ >= 8 && M_ <= 4) {
         if (P.all_diag_cost && P.all_diag_con) {   // tensor-MMA kernel: diagonal lzz (DiagonalCost + Goal/Bound)
             // 2-stage ring, 16 one-warp CTAs per SM.  NSLOT stays MAXT (the loop bound of the slot loop).
-            return launch_riccati_v<N_, M_, FASTAL, TO_RICCATI_STAGES, TO_RICCATI_MINB, true, MAXT>(P, work_counter, s);
+            return launch_riccati_v<N_, M_, FASTAL, TO_RICCATI_STAGES, TO_RICCATI_MINB, true, MAXT, INST>(P, work_counter, s);
         }
-        return launch_riccati_v<N_, M_, FASTAL, 2, 12, false>(P, work_counter, s);   // dense costs: DFMA micro-block kernel
+        return launch_riccati_v<N_, M_, FASTAL, 2, 12, false, MAXT, INST>(P, work_counter, s);   // dense costs: DFMA micro-block kernel
     } else {
-        return launch_riccati_v<N_, M_, FASTAL, 3, 16, false>(P, work_counter, s);
+        return launch_riccati_v<N_, M_, FASTAL, 3, 16, false, MAXT, INST>(P, work_counter, s);
     }
 }
 
 template <int N_, int M_>
 cudaError_t launch_riccati_nm(const DevProblem& P, int* work_counter, cudaStream_t s) {
     // the lane-resident AL terms hold at most MAXT rows per z entry (upper + lower bound + goal)
-    if (P.max_terms_per_z <= MAXT && P.N < 4095 && P.max_p_knot < 128) return launch_riccati_t<N_, M_, true>(P, work_counter, s);
-    return launch_riccati_t<N_, M_, false>(P, work_counter, s);
+    const bool fastal = P.max_terms_per_z <= MAXT && P.N < 4095 && P.max_p_knot < 128;
+    if (P.qr) return fastal ? launch_riccati_t<N_, M_, true, true>(P, work_counter, s) : launch_riccati_t<N_, M_, false, true>(P, work_counter, s);
+    return fastal ? launch_riccati_t<N_, M_, true, false>(P, work_counter, s) : launch_riccati_t<N_, M_, false, false>(P, work_counter, s);
 }
 
 }  // namespace

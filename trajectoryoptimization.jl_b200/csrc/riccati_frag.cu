@@ -117,6 +117,7 @@ __device__ __forceinline__ double rcp_pos(double x) {
 // One thread per (instance, knot).  Full-state expansion of a DiagonalCost + Goal / Bound AL rows is a gradient g and a DIAGONAL h;
 // on the error state it is G'g, the same diagonal outside the attitude, and the 3 x 3 block G_q' diag(h_q) G_q - (q'g_q) I3
 // (Altro error_expansion!; lie.cu k_expansion_compact computes the same numbers in logical order for the shared-memory kernel).
+template <bool INST>   // INST: the linear cost terms and Goal values of each instance
 __global__ void __launch_bounds__(128) k_expansion_rec(const DevProblem P) {
     const int n = P.n, m = P.m, nm = n + m, qs = P.qs;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -130,9 +131,11 @@ __global__ void __launch_bounds__(128) k_expansion_rec(const DevProblem P) {
     double z[TO_MAXNM], g[TO_MAXNM], h[TO_MAXNM];
     for (int i = 0; i < n; i++) z[i] = xg[i];
     for (int a = 0; a < m; a++) z[n + a] = last ? 0.0 : ug[a];
-    const DevCost& c = P.costs[P.cost_index[k]];
-    for (int i = 0; i < n; i++) { g[i] = fma(c.Qd[i], z[i], c.q[i]); h[i] = c.Qd[i]; }
-    for (int a = 0; a < m; a++) { g[n + a] = last ? 0.0 : fma(c.Rd[a], z[n + a], c.r[a]); h[n + a] = last ? 0.0 : c.Rd[a]; }
+    const int cid = P.cost_index[k];
+    const DevCost& c = P.costs[cid];
+    const double* cq = inst_q<INST>(P, b, cid); const double* cr = inst_r<INST>(P, b, cid);
+    for (int i = 0; i < n; i++) { g[i] = fma(c.Qd[i], z[i], cq[i]); h[i] = c.Qd[i]; }
+    for (int a = 0; a < m; a++) { g[n + a] = last ? 0.0 : fma(c.Rd[a], z[n + a], cr[a]); h[n + a] = last ? 0.0 : c.Rd[a]; }
     const int lim = last ? n : nm;
     for (int ci = 0; ci < P.ncon; ci++) {
         const DevCon& con = P.cons[ci];
@@ -140,11 +143,12 @@ __global__ void __launch_bounds__(128) k_expansion_rec(const DevProblem P) {
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
         const bool eq = (con.kind == CON_GOAL);
+        const double* ga = goal_values<INST>(P, b, ci);
         const int nrow = eq ? con.p : con.n_max + con.n_min;
         for (int r = 0; r < nrow; r++) {
             const int j = eq ? con.inds[r] : (r < con.n_max ? con.a_max[r] : con.a_min[r - con.n_max]);
             const bool lower = !eq && r >= con.n_max;
-            const double cv = eq ? z[j] - con.a[r] : (lower ? con.b[j] - z[j] : z[j] - con.a[j]);
+            const double cv = eq ? z[j] - ga[r] : (lower ? con.b[j] - z[j] : z[j] - con.a[j]);
             const double lb = lam[r] - mu * cv;
             if ((eq || lb <= 0.0) && j < lim) { g[j] -= lower ? -lb : lb; h[j] += mu; }
         }
@@ -593,7 +597,8 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_riccati_frag(const DevProb
 }  // namespace
 
 cudaError_t launch_expansion_rec(const DevProblem& P, cudaStream_t s) {
-    k_expansion_rec<<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
+    if (P.qr) k_expansion_rec<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
+    else k_expansion_rec<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }
 cudaError_t launch_export_abe(const DevProblem& P, cudaStream_t s) {

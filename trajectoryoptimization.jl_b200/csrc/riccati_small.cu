@@ -24,15 +24,17 @@ namespace {
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 
 // cost + AL expansion of knot k0 (0-based) for Goal / Bound constraints: g[nm], H[nm*nm] col-major symmetric
-template <int n, int m>
-__device__ __forceinline__ void expand_knot(const DevProblem& P, int k0, const double* x, const double* u, const double* lam_b,
+// (INST: with the linear cost terms and Goal values of instance b)
+template <int n, int m, bool INST>
+__device__ __forceinline__ void expand_knot(const DevProblem& P, int b, int k0, const double* x, const double* u, const double* lam_b,
                                             double (&g)[n + m], double (&H)[(n + m) * (n + m)]) {
     constexpr int nm = n + m;
     const bool last = (k0 == P.N - 1);
-    const DevCost& cost = P.costs[P.cost_index[k0]];
+    const int cid = P.cost_index[k0];
+    const DevCost& cost = P.costs[cid];
 #pragma unroll
     for (int i = 0; i < nm; i++) g[i] = 0.0;
-    cost_gradient_quadratic<false>(cost, n, m, x, u, last, g);      // this kernel never sees user (program) costs: launch_backward routes them to lie.cu
+    cost_gradient_quadratic<false>(cost, inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, last, g);      // this kernel never sees user (program) costs: launch_backward routes them to lie.cu
     cost_hessian_quadratic(cost, n, m, last, H);
     double z[nm];
 #pragma unroll
@@ -46,10 +48,11 @@ __device__ __forceinline__ void expand_knot(const DevProblem& P, int k0, const d
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k0 + 1 - con.first) * con.p;
         if (con.kind == CON_GOAL) {
+            const double* ga = goal_values<INST>(P, b, ci);
             for (int r = 0; r < con.p; r++) {
                 const int j = con.inds[r];
 #pragma unroll
-                for (int i = 0; i < n; i++) if (i == j) { const double lb = lam[r] - mu * (x[i] - con.a[r]); g[i] -= lb; H[i * nm + i] += mu; }
+                for (int i = 0; i < n; i++) if (i == j) { const double lb = lam[r] - mu * (x[i] - ga[r]); g[i] -= lb; H[i * nm + i] += mu; }
             }
         } else {   // CON_BOUND: upper block, then lower block
             for (int r = 0; r < con.n_max; r++) {
@@ -68,7 +71,7 @@ __device__ __forceinline__ void expand_knot(const DevProblem& P, int k0, const d
     }
 }
 
-template <int N_, int M_>
+template <int N_, int M_, bool INST>
 __global__ void __maxnreg__(255) k_riccati_small(const DevProblem P) {
     constexpr int n = N_, m = M_, nm = n + m;
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -92,7 +95,7 @@ __global__ void __maxnreg__(255) k_riccati_small(const DevProblem P) {
             double xk[n];
 #pragma unroll
             for (int i = 0; i < n; i++) xk[i] = X[(size_t)(N - 1) * n + i];
-            expand_knot<n, m>(P, N - 1, xk, xk, lam_b, g, H);   // u is not read at the terminal knot
+            expand_knot<n, m, INST>(P, b, N - 1, xk, xk, lam_b, g, H);   // u is not read at the terminal knot
 #pragma unroll
             for (int j = 0; j < n; j++) {
                 s[j] = g[j];
@@ -131,7 +134,7 @@ __global__ void __maxnreg__(255) k_riccati_small(const DevProblem P) {
                 for (int i = 0; i < n; i++) xk[i] = X[(size_t)k * n + i];
 #pragma unroll
                 for (int i = 0; i < m; i++) uk[i] = U[(size_t)k * m + i];
-                expand_knot<n, m>(P, k, xk, uk, lam_b, g, H);
+                expand_knot<n, m, INST>(P, b, k, xk, uk, lam_b, g, H);
             }
             // T = S [A B] (n x nm), ts = s
             double T[n * nm];
@@ -242,7 +245,8 @@ __global__ void __maxnreg__(255) k_riccati_small(const DevProblem P) {
 
 template <int N_, int M_>
 cudaError_t launch_small(const DevProblem& P, cudaStream_t s) {
-    k_riccati_small<N_, M_><<<(P.B + 31) / 32, 32, 0, s>>>(P);
+    if (P.qr) k_riccati_small<N_, M_, true><<<(P.B + 31) / 32, 32, 0, s>>>(P);
+    else k_riccati_small<N_, M_, false><<<(P.B + 31) / 32, 32, 0, s>>>(P);
     return cudaGetLastError();
 }
 

@@ -142,20 +142,25 @@ cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s) {
 // + the AL terms of the Goal / Bound rows acting on z_i (src/constraints.jl:55-68, :738-765; projection on the dual cone src/cones.jl:96-145).
 // The compact problem class only (P.compact): every cost diagonal, every constraint Goal or Bound, at most TO_EXP_MAXT rows per entry
 // (the host-built table P.exptab; walking the constraint descriptors per thread instead adds work comparable to the RK4 itself).
-__device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, const ExpTab& tab, int k, int i, double zi, const double* __restrict__ lam_b, double& g, double& h) {
+// (INST: the linear cost terms and Goal bounds of instance b)
+template <bool INST>
+__device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, const ExpTab& tab, int b, int k, int i, double zi, const double* __restrict__ lam_b, double& g, double& h) {
     const int n = P.n;
     const bool last = (k == P.N - 1);
-    const DevCost& c = P.costs[P.cost_index[k]];
-    if (i < n) { g = fma(c.Qd[i], zi, c.q[i]); h = c.Qd[i]; }
+    const int cid = P.cost_index[k];
+    const DevCost& c = P.costs[cid];
+    if (i < n) { g = fma(c.Qd[i], zi, inst_q<INST>(P, b, cid)[i]); h = c.Qd[i]; }
     else if (last) { g = 0.0; h = 0.0; return; }
-    else { g = fma(c.Rd[i - n], zi, c.r[i - n]); h = c.Rd[i - n]; }
+    else { g = fma(c.Rd[i - n], zi, inst_r<INST>(P, b, cid)[i - n]); h = c.Rd[i - n]; }
 #pragma unroll
     for (int t = 0; t < TO_EXP_MAXT; t++) {
         const unsigned px = __ldg(&tab.pkx[t][i]);
         if ((unsigned)(k + 1) - (px & 0xfffu) <= ((px >> 12) & 0xfffu)) {
             const double nms = __ldg(&tab.nms[t][i]);
             const double lam = lam_b[(int)(__ldg(&tab.pky[t][i]) + (unsigned)(k + 1) * ((px >> 24) & 0x7fu))];
-            const double lb = fma(nms, zi - __ldg(&tab.bound[t][i]), lam);          // lambda - mu c
+            double bound = __ldg(&tab.bound[t][i]);
+            if constexpr (INST) { const int gi = tab.goal[t][i]; if (P.goal && gi >= 0) bound = P.goal[(size_t)b * P.ngoal + gi]; }
+            const double lb = fma(nms, zi - bound, lam);          // lambda - mu c
             if ((px >> 31) || lb <= 0.0) { g += (nms < 0.0) ? -lb : lb; h += fabs(nms); }   // g -= sign lb ; h += mu
         }
     }
@@ -348,6 +353,8 @@ cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s) {
 #ifndef TO_CEXP2_THREADS
 #define TO_CEXP2_THREADS 64
 #endif
+// INST: the linear cost terms and Goal bounds of each instance (DevProblem::qr / goal), a variant of its own so that the shared one stays as it is
+template <bool INST>
 __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_rec16b(const DevProblem P, int mode) {
     constexpr int qs = 3, n = 13, m = 4;
     constexpr int ROW = 49;                                                          // 48 doubles of expansion per knot, padded: lane j works on row j (stride 98 words: conflict-free)
@@ -377,6 +384,12 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
         const double* __restrict__ Ub = traj_U(P, buf, b);
         const double* __restrict__ lam_b = P.lambda + (size_t)b * P.lambda_len;
         double* __restrict__ recb = P.REC + ((size_t)b * N + kb) * TO_REC_LEN + TO_REC_G;
+        if constexpr (INST) {                                                         // this instance's Goal bounds into the lane's terms
+            if (P.goal) {
+#pragma unroll
+                for (int t = 0; t < TO_EXP_MAXT; t++) { const int gi = tab.goal[t][i]; if (gi >= 0) bnd[t] = P.goal[(size_t)b * P.ngoal + gi]; }
+            }
+        }
         const int nk = (N - kb < 16) ? N - kb : 16;
         const int mycid = (i < nk) ? P.cost_index[kb + i] : 0;                        // lane j <-> knot kb + j (phases B, C; broadcast in phase A)
         int ccid = -1; double ca = 0.0, cb = 0.0;                                     // this lane's coefficients (Qd_i, q_i) of cost ccid
@@ -410,7 +423,7 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
                 if (k0 + u >= nk) break;                                               // (uniform over the group)
                 const int cid = __shfl_sync(gm, mycid, k0 + u, 16);
                 if (i < n) {
-                    if (cid != ccid) { const DevCost& c = P.costs[cid]; ca = c.Qd[i]; cb = c.q[i]; ccid = cid; }
+                    if (cid != ccid) { const DevCost& c = P.costs[cid]; ca = c.Qd[i]; cb = inst_q<INST>(P, b, cid)[i]; ccid = cid; }
                     double g = fma(ca, zi[u], cb), h = ca;
 #pragma unroll
                     for (int t = 0; t < TO_EXP_MAXT; t++) {
@@ -460,6 +473,7 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
             // ---- phase C: the control entries of knot kb + i (coordinate 12 + a, physical slot 2a) ----------------------------------
             const int k = kb + i;
             const DevCost& c = P.costs[mycid];
+            const double* cr = inst_r<INST>(P, b, mycid);
             double zu[m], lu[m][TO_EXP_MAXT];
 #pragma unroll
             for (int a = 0; a < m; a++) {                                             // every load of the phase first
@@ -475,7 +489,7 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
             for (int a = 0; a < m; a++) {
                 double g = 0.0, h = 0.0;
                 if (k != N - 1) {
-                    g = fma(c.Rd[a], zu[a], c.r[a]); h = c.Rd[a];
+                    g = fma(c.Rd[a], zu[a], cr[a]); h = c.Rd[a];
 #pragma unroll
                     for (int t = 0; t < TO_EXP_MAXT; t++) {
                         const unsigned rx = __ldg(&tab.pkx[t][n + a]);
@@ -507,7 +521,8 @@ cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode
     constexpr int GPB = TO_CEXP2_THREADS / 16;                                       // 16-lane groups per CTA
     long long blocks = (units + GPB - 1) / GPB;
     if (blocks < sms) blocks = sms;
-    k_expansion_rec16b<<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
+    if (P.qr) k_expansion_rec16b<true><<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
+    else k_expansion_rec16b<false><<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
 

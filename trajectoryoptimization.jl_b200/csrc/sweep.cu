@@ -25,7 +25,8 @@ __device__ __forceinline__ double warp_max(double v) {
     return v;
 }
 
-template <bool WITH_AL>
+// INST (here and below): per-instance linear cost terms / Goal values, a variant of its own so that the shared one stays as it is
+template <bool WITH_AL, bool INST>
 __global__ void __launch_bounds__(128) k_cost(const DevProblem P, double* __restrict__ J, double* __restrict__ Jk,
                                               double* __restrict__ viol_out) {
     const int b = blockIdx.x;
@@ -40,9 +41,10 @@ __global__ void __launch_bounds__(128) k_cost(const DevProblem P, double* __rest
         double zero_u[TO_MAXM];
         for (int i = 0; i < m; i++) zero_u[i] = 0.0;
         const double* u = last ? zero_u : U + (size_t)k * m;
-        double v = cost_value(P.costs[P.cost_index[k]], n, m, X + (size_t)k * n, u, !last);
+        const int cid = P.cost_index[k];
+        double v = cost_value(P.costs[cid], inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, X + (size_t)k * n, u, !last);
         if (Jk) Jk[(size_t)b * N + k] = v;
-        if (WITH_AL) v += al_knot_penalty(P, k + 1, X + (size_t)k * n, u, lam, viol);
+        if (WITH_AL) v += al_knot_penalty<INST>(P, k + 1, X + (size_t)k * n, u, lam, viol, b);
         acc += v;
     }
     __shared__ double s_sum[4], s_max[4];
@@ -58,6 +60,7 @@ __global__ void __launch_bounds__(128) k_cost(const DevProblem P, double* __rest
     }
 }
 
+template <bool INST>
 __global__ void k_cost_gradient(const DevProblem P, double* __restrict__ grad) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)P.B * P.N) return;
@@ -69,7 +72,8 @@ __global__ void k_cost_gradient(const DevProblem P, double* __restrict__ grad) {
     const double* u = last ? zero_u : traj_U(P, P.cur[b], b) + (size_t)k * m;
     double g[TO_MAXNM];
     for (int i = 0; i < nm; i++) g[i] = 0;
-    cost_gradient(P.costs[P.cost_index[k]], n, m, x, u, last, g);
+    const int cid = P.cost_index[k];
+    cost_gradient(P.costs[cid], inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, last, g);
     for (int i = 0; i < nm; i++) grad[t * nm + i] = g[i];
 }
 
@@ -85,6 +89,7 @@ __global__ void k_cost_hessian(const DevProblem P, double* __restrict__ hess) {
     cost_hessian(P.costs[P.cost_index[k]], P.n, P.m, x, u, last, hess + t * nm * nm);
 }
 
+template <bool INST>
 __global__ void k_al_expansion(const DevProblem P, double* __restrict__ grad, double* __restrict__ hess) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)P.B * P.N) return;
@@ -94,9 +99,10 @@ __global__ void k_al_expansion(const DevProblem P, double* __restrict__ grad, do
     double zero_u[TO_MAXM] = {0};
     const double* x = traj_X(P, P.cur[b], b) + (size_t)k * n;
     const double* u = last ? zero_u : traj_U(P, P.cur[b], b) + (size_t)k * m;
-    al_knot_expansion(P, k, x, u, P.lambda + (size_t)b * P.lambda_len, grad + t * nm, hess + t * nm * nm);
+    al_knot_expansion<INST>(P, k, x, u, P.lambda + (size_t)b * P.lambda_len, grad + t * nm, hess + t * nm * nm, b);
 }
 
+template <bool INST>
 __global__ void k_eval_constraints(const DevProblem P, int ci, double* __restrict__ vals) {
     const DevCon& con = P.cons[ci];
     const int len = con.last - con.first + 1;
@@ -108,7 +114,7 @@ __global__ void k_eval_constraints(const DevProblem P, int ci, double* __restric
     const double* x = traj_X(P, P.cur[b], b) + (size_t)(k1 - 1) * P.n;
     const double* u = (k1 == P.N) ? zero_u : traj_U(P, P.cur[b], b) + (size_t)(k1 - 1) * P.m;
     double c[TO_MAXPV];
-    con_evaluate(con, P.n, P.m, x, u, c);
+    con_evaluate(con, goal_values<INST>(P, b, ci), P.n, P.m, x, u, c);
     for (int i = 0; i < con.p; i++) vals[t * con.p + i] = c[i];
 }
 
@@ -158,6 +164,7 @@ __global__ void k_hess_projection(int cone, int p, int count, const double* __re
 }
 
 // dual update: lambda <- clamp(Pi_{K*}(lambda - mu c)); one thread per (instance, constraint, knot)
+template <bool INST>
 __global__ void k_al_update(const DevProblem P) {
     const int b = blockIdx.x;
     if (retired(P, b)) return;          // to_solve: only the instances that go on to another outer iteration
@@ -173,7 +180,7 @@ __global__ void k_al_update(const DevProblem P) {
             const double* u = (k1 == P.N) ? zero_u : U + (size_t)(k1 - 1) * P.m;
             double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
             double* lam = lam_b + con.offset + (size_t)(k1 - con.first) * con.p;
-            con_evaluate(con, P.n, P.m, x, u, c);
+            con_evaluate(con, goal_values<INST>(P, b, ci), P.n, P.m, x, u, c);
             for (int i = 0; i < con.p; i++) lbar[i] = lam[i] - mu * c[i];
             cone_projection(dualcone(con.sense), lbar, con.p, lp);
             for (int i = 0; i < con.p; i++) lam[i] = fmax(-P.opt.dual_max, fmin(P.opt.dual_max, lp[i]));
@@ -230,15 +237,18 @@ __global__ void k_export_ab(const DevProblem P, double* __restrict__ out) {
 static inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
 cudaError_t launch_cost(const DevProblem& P, double* J, double* Jk, cudaStream_t s) {
-    k_cost<false><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
+    if (P.qr) k_cost<false, true><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
+    else k_cost<false, false><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
     return cudaGetLastError();
 }
 cudaError_t launch_merit(const DevProblem& P, double* J, double* viol, cudaStream_t s) {
-    k_cost<true><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
+    if (P.qr) k_cost<true, true><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
+    else k_cost<true, false><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
     return cudaGetLastError();
 }
 cudaError_t launch_cost_gradient(const DevProblem& P, double* grad, cudaStream_t s) {
-    k_cost_gradient<<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
+    if (P.qr) k_cost_gradient<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
+    else k_cost_gradient<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
     return cudaGetLastError();
 }
 cudaError_t launch_cost_hessian(const DevProblem& P, double* hess, cudaStream_t s) {
@@ -246,12 +256,14 @@ cudaError_t launch_cost_hessian(const DevProblem& P, double* hess, cudaStream_t 
     return cudaGetLastError();
 }
 cudaError_t launch_al_expansion(const DevProblem& P, double* grad, double* hess, cudaStream_t s) {
-    k_al_expansion<<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
+    if (P.qr) k_al_expansion<true><<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
+    else k_al_expansion<false><<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
     return cudaGetLastError();
 }
 cudaError_t launch_eval_constraints(const DevProblem& P, int con, double* vals, cudaStream_t s) {
     // the knot-range length is read on the device; size the grid for the worst case N
-    k_eval_constraints<<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
+    if (P.qr) k_eval_constraints<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
+    else k_eval_constraints<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
     return cudaGetLastError();
 }
 cudaError_t launch_constraint_hessians(const DevProblem& P, int con, int len, const double* lam, double* H, cudaStream_t s) {
@@ -276,7 +288,8 @@ cudaError_t launch_hess_projection(int cone, int p, int count, const double* x, 
     return cudaGetLastError();
 }
 cudaError_t launch_al_update(const DevProblem& P, cudaStream_t s) {
-    k_al_update<<<P.B, 128, 0, s>>>(P);
+    if (P.qr) k_al_update<true><<<P.B, 128, 0, s>>>(P);
+    else k_al_update<false><<<P.B, 128, 0, s>>>(P);
     return cudaGetLastError();
 }
 cudaError_t launch_reduce_merit(const DevProblem& P, const double* viol, double* out2, cudaStream_t s) {

@@ -319,6 +319,11 @@ TO.∇²projection!(p::BatchedProblem, cone::TO.ConstraintSense, H::Array{Float6
 
 TO.set_goal_state!(p::BatchedProblem, xf::Vector{Float64}; objective=true, constraint=true) =      # src/problem.jl:294-310
     check(p.h, ccall((:to_set_goal_state, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Cint, Cint), p.h, xf, objective, constraint))
+# per instance: column b of xf (n, B) is instance b's goal (its own q = -Q xf_b and Goal values; Q, R, c and the rest stay shared)
+function TO.set_goal_state!(p::BatchedProblem, xf::AbstractMatrix{Float64}; objective=true, constraint=true)
+    size(xf, 2) == p.B || throw(DimensionMismatch("xf must be (n, B)"))
+    check(p.h, ccall((:to_set_goal_states, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Cint, Cint), p.h, Matrix{Float64}(xf), objective, constraint))
+end
 
 # ---- what Altro.jl's iLQR / AL loop does with the API above, fused on the device ------------------------------
 expand!(p::BatchedProblem) = check(p.h, ccall((:to_expand, libb200), Cint, (Ptr{Cvoid},), p.h))
@@ -367,6 +372,11 @@ end
 # MPC plumbing: update_trajectory!(obj, Z, start) src/objective.jl:198-212 on the batched problem; Xref (n, nref), Uref (m, nref)
 TO.update_trajectory!(p::BatchedProblem, Xref::Matrix{Float64}, Uref::Matrix{Float64}, start::Integer=1) =
     check(p.h, ccall((:to_update_trajectory, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Int32, Int32), p.h, Xref, Uref, size(Xref, 2), start))
+# per instance: Xref (n, nref, B), Uref (m, nref, B), one start for the batch
+function TO.update_trajectory!(p::BatchedProblem, Xref::Array{Float64,3}, Uref::Array{Float64,3}, start::Integer=1)
+    (size(Xref, 3) == p.B && size(Uref, 3) == p.B && size(Uref, 2) == size(Xref, 2)) || throw(DimensionMismatch("Xref (n, nref, B), Uref (m, nref, B)"))
+    check(p.h, ccall((:to_update_trajectories, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Int32, Int32), p.h, Xref, Uref, size(Xref, 2), start))
+end
 shift_trajectory!(p::BatchedProblem, steps::Integer=1) = check(p.h, ccall((:to_shift_trajectory, libb200), Cint, (Ptr{Cvoid}, Int32), p.h, steps))
 
 # multi-GPU (one process per GPU, e.g. under MPI.jl + NCCL.jl): the only collective is the {sum J, max violation} all-reduce.
