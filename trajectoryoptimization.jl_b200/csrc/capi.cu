@@ -540,6 +540,21 @@ int to_create(const to_spec* s, to_handle** out) {
         P.max_p_knot = std::max(P.max_p_knot, pk);
         P.max_cons_knot = std::max(P.max_cons_knot, nk);
     }
+    {   // DevProblem::fwd_compact
+        bool cls = N >= 2 && P.all_diag_cost && P.all_diag_con;
+        for (int k = 1; k < N - 1; k++) if (h->h_cost_index[k] != h->h_cost_index[0]) cls = false;
+        int nbox = 0, ngc = 0;
+        for (const auto& c : h->h_cons) {
+            if (c.kind == CON_BOUND) {
+                bool ubox = c.first == 1 && c.last == N - 1 && c.p == 2 * m;
+                for (int j = 0; j < n + m; j++) if ((c.row_max[j] >= 0) != (j >= n) || (c.row_min[j] >= 0) != (j >= n)) ubox = false;
+                cls = cls && ubox; nbox++;
+            } else if (c.kind == CON_GOAL) {
+                cls = cls && c.first == N && c.last == N; ngc++;
+            } else cls = false;
+        }
+        P.fwd_compact = (cls && nbox <= 1 && ngc <= 1) ? 1 : 0;
+    }
     h->h_mu.assign(s->ncon, P.opt.penalty_initial);
     h->h_dt.assign(s->dt, s->dt + (N - 1));
     h->h_dyn = dyn_tab; h->h_dyn_index = dyn_idx;

@@ -164,7 +164,11 @@ struct DevProblem {
     // shared DevCost::q / r and DevCon::a.
     const double* qr;         // [B][ncost][n+m]: q | r of cost cid for instance b
     const double* goal;       // [B][ngoal]: a[row] of Goal constraint ci at DevCon::goff
-    int ngoal, pad_inst;
+    int ngoal;
+    // The line search's compact problem class (forward.cu rollout_compact): one cost on every stage knot and another on the terminal
+    // knot, at most one Bound with finite limits on every control and none on the state, on every stage knot, and at most one Goal, on the
+    // terminal knot only.  Set at to_create (the structure of the costs and constraints never changes afterwards).
+    int fwd_compact;
 };
 
 enum { SOLVE_ACTIVE = 0, SOLVE_WAITING = 1, SOLVE_DONE = 2 };

@@ -1,4 +1,5 @@
 #include <cstdlib>
+#include <type_traits>
 // forward.cu -- the forward pass of iLQR: closed-loop RK4 rollout fused with the cost + constraint + AL-penalty
 // sweep (kernel 1 without partials + kernel 2), and the per-instance backtracking line search.
 //
@@ -95,6 +96,52 @@ __device__ inline void load_tables(const DevProblem& P, FwdTab& tab) {
     __syncthreads();
 }
 
+// The compact problem class (DevProblem::fwd_compact): the stage cost, the control box and the terminal Goal, laid out for the
+// straight-line knot loop of rollout_compact.  {coefficient, linear term} pairs are read with one 16-byte load each.
+struct alignas(16) FwdCompactTab {
+    double2 sx[TO_MAXN];             // stage cost {Qd_i, q_i}
+    double2 su[TO_MAXM];             // stage cost {Rd_i, r_i}
+    double2 box[TO_MAXM];            // control box {u_max_i, u_min_i}
+    double sc, mu, inv2mu, pad0;     // stage cost c; the box's penalty
+    int cid, tcid, box_off, box_p;   // stage / terminal cost; the box's multipliers of knot 1 and rows per knot (0: no box)
+    int goal_ci, goal_off, goal_p, pad1;   // the Goal (-1: none) and its multipliers
+    FwdCost term;                    // terminal cost (Qd, q, c)
+    FwdCon goal;                     // the Goal's mu, inv2mu, mask_max, row_max, a
+    double dt[FWD_MAX_N];
+};
+
+__device__ inline void load_compact_tables(const DevProblem& P, FwdCompactTab& tab) {
+    const int t = threadIdx.x, T = blockDim.x;
+    const int cid = P.cost_index[0], tcid = P.cost_index[P.N - 1];
+    const DevCost& c = P.costs[cid];
+    const DevCost& ct = P.costs[tcid];
+    for (int j = t; j < TO_MAXN; j += T) { tab.sx[j] = make_double2(c.Qd[j], c.q[j]); tab.term.Qd[j] = ct.Qd[j]; tab.term.q[j] = ct.q[j]; }
+    for (int j = t; j < TO_MAXM; j += T) tab.su[j] = make_double2(c.Rd[j], c.r[j]);
+    if (t == 0) {
+        tab.sc = c.c; tab.term.c = ct.c; tab.cid = cid; tab.tcid = tcid;
+        tab.box_off = tab.box_p = 0; tab.goal_ci = -1; tab.goal_off = tab.goal_p = 0;
+    }
+    for (int ci = 0; ci < P.ncon; ci++) {
+        const DevCon& k = P.cons[ci];
+        if (k.kind == CON_BOUND) {   // knots 1..N-1, rows 0..m-1 = upper, m..2m-1 = lower
+            for (int j = t; j < P.m; j += T) tab.box[j] = make_double2(k.a[P.n + j], k.b[P.n + j]);
+            if (t == 0) { tab.box_off = k.offset; tab.box_p = k.p; tab.mu = P.mu[ci]; tab.inv2mu = 1.0 / (2.0 * P.mu[ci]); }
+        } else {                     // the Goal, knot N
+            FwdCon& f = tab.goal;
+            if (t == 0) {
+                tab.goal_ci = ci; tab.goal_off = k.offset; tab.goal_p = k.p;
+                f.mu = P.mu[ci]; f.inv2mu = 1.0 / (2.0 * P.mu[ci]);
+                unsigned mx = 0;
+                for (int j = 0; j < TO_MAXNM; j++) if (k.row_max[j] >= 0) mx |= 1u << j;
+                f.mask_max = mx;
+            }
+            for (int j = t; j < TO_MAXNM; j += T) { f.row_max[j] = k.row_max[j]; f.a[j] = k.a[j]; }
+        }
+    }
+    for (int k = t; k < P.N - 1; k += T) tab.dt[k] = P.dt[k];
+    __syncthreads();
+}
+
 __device__ __forceinline__ void cp_async8(double* smem_dst, const double* gsrc) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
@@ -108,6 +155,8 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 #define TO_FWD_STAGES 2
 #endif
 constexpr int FWD_STAGES = TO_FWD_STAGES;
+// knots of candidate trajectory staged in shared memory per lane before the group writes them out (rollout_compact)
+constexpr int FWD_OKNOTS = 4;
 template <int NPEND> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(NPEND) : "memory"); }
 
 // shared-memory stage of one knot's operands for the IPB instances of a CTA.
@@ -124,10 +173,10 @@ struct Stage {
     __device__ static __forceinline__ int sidx(int slot, int g) { return slot * IPB + g; }
 };
 
-// lanes of a group cooperatively issue the async copies of knot k's operands of instance g
+// lanes of a group cooperatively issue the async copies of knot k's K_k, d_k, u_k, x_k of instance g (none on the terminal knot)
 template <int n, int m, int IPB, int G, int NE>
-__device__ __forceinline__ void prefetch_knot(double* base, int g, int l, int k, const double* Kg, const double* dg, const double* X,
-                                              const double* U, const double* lam_b, const FwdTab& tab, int N) {
+__device__ __forceinline__ void prefetch_operands(double* base, int g, int l, int k, const double* Kg, const double* dg, const double* X,
+                                                  const double* U, int N) {
     using S = Stage<n, m, IPB, NE>;
     if (k < N - 1) {
         const double* Kk = Kg + (size_t)k * NE * m;
@@ -153,6 +202,14 @@ __device__ __forceinline__ void prefetch_knot(double* base, int g, int l, int k,
             else if (s < 2 * m + n) cp_async8(base + S::sidx(S::OFF_X + s - 2 * m, g), X + (size_t)k * n + (s - 2 * m));
         }
     }
+}
+
+// ... and the multipliers of knot k+1 (prefetch_operands + multipliers = one knot of the operand ring)
+template <int n, int m, int IPB, int G, int NE>
+__device__ __forceinline__ void prefetch_knot(double* base, int g, int l, int k, const double* Kg, const double* dg, const double* X,
+                                              const double* U, const double* lam_b, const FwdTab& tab, int N) {
+    using S = Stage<n, m, IPB, NE>;
+    prefetch_operands<n, m, IPB, G, NE>(base, g, l, k, Kg, dg, X, U, N);
     // multipliers of the (at most two) constraints active at knot k+1, packed in constraint order
     {
         const int c0 = tab.lam_cnt[k][0], c1 = tab.lam_cnt[k][1];
@@ -331,6 +388,195 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
     return J;
 }
 
+// rollout_fast for the compact class, the same FP64 operations on the same operands in the same order, with less work around them:
+//   * the terminal knot (no control, no feedback, the Goal) is peeled off, so the knot loop has no `last` tests and no constraint loop:
+//     the box is the only constraint of a stage knot, its multipliers of knot k+1 sit at box_off + k p;
+//   * the stage cost is a {Qd_i, q_i} pair per 16-byte load instead of two 8-byte loads;
+//   * the AL clamp and the violation max are compare-and-select (proofs at the box below);
+//   * the candidate trajectory leaves through shared memory: each lane stages FWD_OKNOTS knots of its x and u, then the lanes of the group
+//     write each lane's runs together, G consecutive doubles per store instruction.  One lane storing its own 8-byte words sent one L2 write
+//     request per word from every lane, and those requests, not the arithmetic, set the pace of the pass (a timing-only build without the
+//     candidate stores ran pass 1 in about half the time);
+//   * RK4 writes the next state over the current one (rk4_step reads x_i for the last time where it writes xn_i), so the loop carries
+//     no x <- xn copies.  (Unrolled by two with x / xn swapping roles instead, the loop took 40 more registers and spilled.)
+template <int MODEL, int IPB, int G, bool LIE, bool INST>
+__device__ __forceinline__ double rollout_compact(const DevProblem& P, const FwdCompactTab& tab, double* stage, double* ost, int b, int g,
+                                                  int l, unsigned gmask, double alpha, int cbuf, bool& ok, double& viol) {
+    constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
+    using S = Stage<n, m, IPB, NE>;
+    const int N = P.N, buf = P.cur[b];
+    const double* X = traj_X(P, buf, b);
+    const double* U = traj_U(P, buf, b);
+    double* Xc = traj_Xw(P, cbuf, b);
+    const double* Kg = P.K + (size_t)b * (N - 1) * NE * m;
+    const double* dg = P.d + (size_t)b * (N - 1) * m;
+    const double* lam_b = P.lambda + (size_t)b * P.lambda_len;
+    // ost: the group's output staging, FWD_OKNOTS knots of x then u per lane; lane j's candidate goes to buffer (buf + 1 + j) % TO_NBUF
+    constexpr int OX = FWD_OKNOTS * n, OL = FWD_OKNOTS * (n + m);
+    double* myx = ost + l * OL;
+    double* myu = myx + OX;
+    const double* cq = INST ? inst_q<true>(P, b, tab.cid) : nullptr;   // INST: the instance's linear terms, read as rollout_fast does
+    const double* cr = INST ? inst_r<true>(P, b, tab.cid) : nullptr;
+    const bool box = tab.box_p != 0;
+    double x[n], u[m];
+    double J = 0.0;
+    ok = true; viol = 0.0;
+#pragma unroll
+    for (int i = 0; i < n; i++) x[i] = P.x0[(size_t)b * n + i];
+    constexpr int D = FWD_STAGES - 1;
+    // knot k of the operand ring: K, d, u, x of knot k and the multipliers of knot k+1 (the box's, or the Goal's on the terminal knot)
+    auto prefetch = [&](double* base, int k) {
+        prefetch_operands<n, m, IPB, G, NE>(base, g, l, k, Kg, dg, X, U, N);
+        const bool stg = k < N - 1;
+        const int cnt = stg ? tab.box_p : tab.goal_p;
+        const double* src = lam_b + (stg ? tab.box_off + k * tab.box_p : tab.goal_off);
+        for (int i = l; i < cnt; i += G) cp_async8(base + S::sidx(S::OFF_L + i, g), src + i);
+    };
+#pragma unroll
+    for (int j = 0; j < D; j++) {
+        if (j < N) prefetch(stage + j * S::DOUBLES, j);
+        cp_async_commit();
+    }
+    int sb = 0, sp = D;
+    auto next_stage = [&](int k) -> const double* {
+        __syncwarp(gmask);                      // every lane of the group is done reading the stage of knot k-1
+        if (k + D < N) prefetch(stage + sp * S::DOUBLES, k + D);
+        cp_async_commit();
+        cp_async_wait<D>();                     // this lane's copies for knot k have landed ...
+        __syncwarp(gmask);                      // ... and so have the other lanes'
+        const double* st = stage + sb * S::DOUBLES;
+        sb = (sb + 1 == FWD_STAGES) ? 0 : sb + 1; sp = (sp + 1 == FWD_STAGES) ? 0 : sp + 1;
+        return st;
+    };
+    // stage knot k < N - 1: x_k -> x_{k+1} in place
+    auto knot = [&](int k, double* x) {
+        const double* st = next_stage(k);
+#pragma unroll
+        for (int a = 0; a < m; a++) u[a] = fma(alpha, st[S::sidx(S::OFF_D + a, g)], st[S::sidx(S::OFF_U + a, g)]);
+        double dxe[NE];
+        if constexpr (LIE) {
+            double xr[n];
+#pragma unroll
+            for (int i = 0; i < n; i++) xr[i] = st[S::sidx(S::OFF_X + i, g)];
+            state_diff(true, n, 3, x, xr, dxe);
+        } else {
+#pragma unroll
+            for (int i = 0; i < n; i++) dxe[i] = x[i] - st[S::sidx(S::OFF_X + i, g)];
+        }
+#pragma unroll
+        for (int i = 0; i < NE; i++) {
+            const double dx = dxe[i];
+            if (S::K16 && (m % 2 == 0)) {
+#pragma unroll
+                for (int a = 0; a < m; a += 2) {
+                    const double2 kv = *reinterpret_cast<const double2*>(&st[S::kidx(i * m + a, g)]);
+                    u[a] = fma(kv.x, dx, u[a]);
+                    u[a + 1] = fma(kv.y, dx, u[a + 1]);
+                }
+            } else {
+#pragma unroll
+                for (int a = 0; a < m; a++) u[a] = fma(st[S::kidx(i * m + a, g)], dx, u[a]);
+            }
+        }
+#pragma unroll
+        for (int a = 0; a < m; a++) if (!(fabs(u[a]) <= P.opt.max_control_value)) ok = false;
+        const int kk = k % FWD_OKNOTS;
+#pragma unroll
+        for (int i = 0; i < n; i++) myx[kk * n + i] = x[i];
+#pragma unroll
+        for (int a = 0; a < m; a++) myu[kk * m + a] = u[a];
+        if (kk == FWD_OKNOTS - 1 || k == N - 2) {   // group-uniform: write the staged knots k0..k of every lane of the group
+            __syncwarp(gmask);
+            const int k0 = k - kk, nx = (kk + 1) * n, nu = (kk + 1) * m;
+            for (int j = 0; j < G; j++) {
+                const int cb = (buf + 1 + j) % TO_NBUF;
+                double* xd = traj_Xw(P, cb, b) + (size_t)k0 * n;
+                double* ud = traj_Uw(P, cb, b) + (size_t)k0 * m;
+                const double* xs = ost + j * OL;
+                for (int e = l; e < nx; e += G) xd[e] = xs[e];
+                for (int e = l; e < nu; e += G) ud[e] = xs[OX + e];
+            }
+            // the next knot overwrites the staging only after next_stage's __syncwarp
+        }
+        {   // stage cost
+            double a2 = 0.0, l1 = 0.0;
+#pragma unroll
+            for (int i = 0; i < n; i++) { const double2 c = tab.sx[i]; a2 = fma(c.x * x[i], x[i], a2); l1 = fma(INST ? cq[i] : c.y, x[i], l1); }
+#pragma unroll
+            for (int i = 0; i < m; i++) { const double2 c = tab.su[i]; a2 = fma(c.x * u[i], u[i], a2); l1 = fma(INST ? cr[i] : c.y, u[i], l1); }
+            J += fma(0.5, a2, l1) + tab.sc;
+        }
+        if (box) {
+            // AL penalty of the control box, rollout_fast's ubox branch with two replacements:
+            //   pu = fmin(0, v)  ->  v < 0 ? v : 0.  They differ only at v = -0 (fmin gives -0, the select +0; NaN gives 0 in both), and pu
+            //     is only used squared in fma(pu, pu, a), whose exact product is +0 either way, so a gets the same bits.
+            //   viol = fmax(viol, fmax(cu, cl))  ->  t = cu > cl ? cu : cl ; viol = t > viol ? t : viol.  CUDA's fmax returns the
+            //     non-NaN operand and orders -0 below +0 (measured on sm_90a).  viol starts at +0 and so is never NaN or -0.  The bounds
+            //     are finite, so cu and cl are both NaN (u is) or neither: both NaN -> t = NaN, and both forms keep viol.  Otherwise t is
+            //     fmax(cu, cl) except for cu = +0, cl = -0, where t = -0: then fmax(viol, +0) = viol = the select, as viol >= +0.  For
+            //     t != NaN, fmax(viol, t) and the select agree except at viol = +0, t = -0, where both give viol.
+            const double mu = tab.mu;
+            double a = 0.0, l2 = 0.0;
+#pragma unroll
+            for (int i = 0; i < m; i++) {
+                const double lu = st[S::sidx(S::OFF_L + i, g)], ll = st[S::sidx(S::OFF_L + m + i, g)];
+                const double2 bx = tab.box[i];
+                const double cu = u[i] - bx.x, cl = bx.y - u[i];
+                const double vu = fma(-mu, cu, lu), vl = fma(-mu, cl, ll);
+                const double pu = vu < 0.0 ? vu : 0.0, pl = vl < 0.0 ? vl : 0.0;
+                a = fma(pu, pu, a); a = fma(pl, pl, a); l2 = fma(lu, lu, l2); l2 = fma(ll, ll, l2);
+                const double t = cu > cl ? cu : cl;
+                viol = t > viol ? t : viol;
+            }
+            J = fma(a - l2, tab.inv2mu, J);
+        }
+        if constexpr (MODEL == MODEL_EXPR_42) {   // a discrete jump map writes its outputs while it reads its inputs
+            double xn[n];
+            rk4_step<MODEL, double>(model_params<MODEL>(P, k), x, u, tab.dt[k], xn);
+#pragma unroll
+            for (int i = 0; i < n; i++) x[i] = xn[i];
+        } else {
+            rk4_step<MODEL, double>(model_params<MODEL>(P, k), x, u, tab.dt[k], x);
+        }
+#pragma unroll
+        for (int i = 0; i < n; i++) if (!(fabs(x[i]) <= P.opt.max_state_value)) ok = false;
+        // a blown-up trial keeps integrating (the group stays in lock step); its result is rejected through `ok`
+    };
+#pragma unroll 1
+    for (int k = 0; k < N - 1; k++) knot(k, x);
+    {   // terminal knot N - 1: terminal cost and the Goal, as rollout_fast evaluates them on its last knot
+        const double* st = next_stage(N - 1);
+#pragma unroll
+        for (int i = 0; i < n; i++) Xc[(size_t)(N - 1) * n + i] = x[i];
+        const double* tq = INST ? inst_q<true>(P, b, tab.tcid) : tab.term.q;
+        double a2 = 0.0, l1 = 0.0;
+#pragma unroll
+        for (int i = 0; i < n; i++) { a2 = fma(tab.term.Qd[i] * x[i], x[i], a2); l1 = fma(tq[i], x[i], l1); }
+        J += fma(0.5, a2, l1) + tab.term.c;
+        if (tab.goal_ci >= 0) {
+            const FwdCon& c = tab.goal;
+            const double mu = c.mu;
+            double a = 0.0, l2 = 0.0;
+            const unsigned mk = c.mask_max;
+            const double* ga = c.a;
+            if constexpr (INST) ga = goal_values<true>(P, b, tab.goal_ci);
+#pragma unroll
+            for (int i = 0; i < n; i++) {
+                if (mk & (1u << i)) {
+                    const int row = c.row_max[i];
+                    const double lm = st[S::sidx(S::OFF_L + row, g)];
+                    const double cv = x[i] - ga[row];
+                    const double lp = fma(-mu, cv, lm);
+                    a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, fabs(cv));
+                }
+            }
+            J = fma(a - l2, c.inv2mu, J);
+        }
+    }
+    cp_async_wait<0>();
+    return J;
+}
+
 // generic path (dense costs or general constraints): pointer-based evaluation, operands read directly from global
 template <int MODEL, bool LIE, bool INST>
 __device__ __forceinline__ double rollout_generic(const DevProblem& P, int b, double alpha, int cbuf, bool& ok, double& viol) {
@@ -397,17 +643,26 @@ __device__ __forceinline__ bool ls_accept(const DevProblem& P, double J, double 
 
 extern __shared__ __align__(16) unsigned char fwd_smem[];
 
+// rollout of a trial: rollout_generic, rollout_fast or rollout_compact
+enum { FWD_GENERIC = 0, FWD_FAST = 1, FWD_COMPACT = 2 };
+// the knot loop of the compact class: 1 = rollout_compact; 0 = rollout_fast for it as for every other fast-path problem (A/B builds)
+#ifndef TO_FWD_COMPACT
+#define TO_FWD_COMPACT 1
+#endif
+
 // One line-search pass: lane l of group g evaluates trial (trial0 + l) of instance b.
 //   first_pass : ignore / reset accepted[b];   final_pass : commit failures (no acceptable step size).
-template <int MODEL, int G, bool FAST, int LANES, bool LIE, bool INST>
-__global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, int trial0, int first_pass, int final_pass) {
+template <int MODEL, int G, int PATH, int LANES, bool LIE, bool INST>
+__device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
+    constexpr bool FAST = PATH != FWD_GENERIC;
     // LANES = 16: only half of the warp carries groups.  The pass is a latency-bound FP64 chain at ~4 warps per SM, and
     // an FP64 instruction of a half-empty warp takes one pipe pass instead of two.
     constexpr int IPB = LANES / G;
     using S = Stage<n, m, IPB, NE>;
-    FwdTab* tab = reinterpret_cast<FwdTab*>(fwd_smem);
-    double* stage = reinterpret_cast<double*>(fwd_smem + sizeof(FwdTab));
+    using Tab = std::conditional_t<PATH == FWD_COMPACT, FwdCompactTab, FwdTab>;
+    Tab* tab = reinterpret_cast<Tab*>(fwd_smem);
+    double* stage = reinterpret_cast<double*>(fwd_smem + sizeof(Tab));
     const int g = (threadIdx.x % LANES) / G, l = threadIdx.x % G;
     // pass 1 walks every instance; the later passes walk the list pass 1 left of the instances it did not accept, so that only CTAs with work
     // stay resident next to the kernels of the main stream (a CTA with one late instance of four used to hold its registers for the whole pass)
@@ -421,7 +676,8 @@ __global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, 
     const bool work = valid && status >= 0 && !was_accepted && trial0 <= P.opt.ls_iters;
     // CTA-uniform: skip the table load when no group of this CTA has work
     const unsigned any = __ballot_sync(0xffffffffu, work);
-    if (FAST && any) load_tables(P, *tab);
+    if constexpr (PATH == FWD_COMPACT) { if (any) load_compact_tables(P, *tab); }
+    else if (FAST && any) load_tables(P, *tab);
     if (!valid) return;
     bool accepted = was_accepted != 0;
     if (work) {
@@ -430,7 +686,11 @@ __global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, 
         const int cbuf = (P.cur[b] + 1 + l) % TO_NBUF;
         bool ok = false;
         double J, viol = 0.0;
-        if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST>(P, *tab, stage, b, g, l, gmask, alpha, cbuf, ok, viol);
+        if constexpr (PATH == FWD_COMPACT) {
+            double* ost = stage + FWD_STAGES * S::DOUBLES + (size_t)g * G * FWD_OKNOTS * (n + m);
+            J = rollout_compact<MODEL, IPB, G, LIE, INST>(P, *tab, stage, ost, b, g, l, gmask, alpha, cbuf, ok, viol);
+        }
+        else if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST>(P, *tab, stage, b, g, l, gmask, alpha, cbuf, ok, viol);
         else J = rollout_generic<MODEL, LIE, INST>(P, b, alpha, cbuf, ok, viol);
         const bool good = (trial <= P.opt.ls_iters) && ls_accept(P, J, P.J[b], alpha, P.dV[2 * b], P.dV[2 * b + 1], ok);
         const unsigned votes = __ballot_sync(gmask, good) & gmask;
@@ -460,13 +720,28 @@ __global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, 
     (void)sizeof(S);
 }
 
-template <int MODEL, int G, bool FAST, int LANES, bool LIE = false, bool INST = false>
+template <int MODEL, int G, bool FAST, int LANES, bool LIE, bool INST>
+__global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, int trial0, int first_pass, int final_pass) {
+    linesearch_pass<MODEL, G, FAST ? FWD_FAST : FWD_GENERIC, LANES, LIE, INST>(P, trial0, first_pass, final_pass);
+}
+
+template <int MODEL, int G, int LANES, bool LIE, bool INST>
+__global__ void __launch_bounds__(FWD_THREADS) k_linesearch_compact(const DevProblem P, int trial0, int first_pass, int final_pass) {
+    linesearch_pass<MODEL, G, FWD_COMPACT, LANES, LIE, INST>(P, trial0, first_pass, final_pass);
+}
+
+template <int MODEL, int G, int PATH, int LANES, bool LIE = false, bool INST = false>
 cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     constexpr int IPB = LANES / G;
     const int blocks = (P.B + IPB - 1) / IPB;
-    const size_t smem = FAST ? sizeof(FwdTab) + (size_t)FWD_STAGES * Stage<n, m, IPB, NE>::DOUBLES * sizeof(double) : 0;
-    auto kern = k_linesearch<MODEL, G, FAST, LANES, LIE, INST>;
+    const size_t tab = PATH == FWD_COMPACT ? sizeof(FwdCompactTab) : sizeof(FwdTab);
+    const size_t ost = PATH == FWD_COMPACT ? (size_t)LANES * FWD_OKNOTS * (n + m) * sizeof(double) : 0;   // rollout_compact's output staging
+    const size_t smem = PATH != FWD_GENERIC ? tab + (size_t)FWD_STAGES * Stage<n, m, IPB, NE>::DOUBLES * sizeof(double) + ost : 0;
+    auto kern = [] {
+        if constexpr (PATH == FWD_COMPACT) return k_linesearch_compact<MODEL, G, LANES, LIE, INST>;
+        else return k_linesearch<MODEL, G, PATH == FWD_FAST, LANES, LIE, INST>;
+    }();
     static bool configured[TO_MAXDEV] = {false};
     const int dev = current_device_slot();
     if (!configured[dev] && smem > 48 * 1024) {
@@ -478,30 +753,40 @@ cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int f
     return cudaGetLastError();
 }
 
-template <int MODEL, int G, bool FAST, bool INST>
+template <int MODEL, int G, int PATH, bool INST>
 cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     // lanes of each warp that carry groups: 16 for the first pass (half-warp FP64 instructions take one pipe pass); the later passes
     // use 16 when they walk the compact late list (two-instance CTAs, see to_create) and 32 when they scan all instances.
     const int lanes = first_pass ? 16 : (P.late_list ? 16 : 32);
     if constexpr (MODEL == MODEL_QUADROTOR) {   // Lie-group error state: dx = state_diff(xbar, x), gains m x (n - 1)
         if (P.lie) {
-            if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, FAST, (G <= 16 ? 16 : 32), true, INST>(P, trial0, first_pass, final_pass, s);
-            return launch_pass_l<MODEL, G, FAST, 32, true, INST>(P, trial0, first_pass, final_pass, s);
+            if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, PATH, (G <= 16 ? 16 : 32), true, INST>(P, trial0, first_pass, final_pass, s);
+            return launch_pass_l<MODEL, G, PATH, 32, true, INST>(P, trial0, first_pass, final_pass, s);
         }
     }
-    if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, FAST, (G <= 16 ? 16 : 32), false, INST>(P, trial0, first_pass, final_pass, s);
-    return launch_pass_l<MODEL, G, FAST, 32, false, INST>(P, trial0, first_pass, final_pass, s);
+    if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, PATH, (G <= 16 ? 16 : 32), false, INST>(P, trial0, first_pass, final_pass, s);
+    return launch_pass_l<MODEL, G, PATH, 32, false, INST>(P, trial0, first_pass, final_pass, s);
 }
 
 // per-instance linear cost terms / Goal values: a kernel variant of its own, so that the shared one is the code it has always been
-template <int MODEL, int G, bool FAST>
+template <int MODEL, int G, int PATH>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
-    if (P.qr) return launch_pass_i<MODEL, G, FAST, true>(P, trial0, first_pass, final_pass, s);
-    return launch_pass_i<MODEL, G, FAST, false>(P, trial0, first_pass, final_pass, s);
+    if (P.qr) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);
+    return launch_pass_i<MODEL, G, PATH, false>(P, trial0, first_pass, final_pass, s);
 }
 
 bool fast_path(const DevProblem& P) {
     return P.all_diag_cost && P.all_diag_con && P.N <= FWD_MAX_N && P.max_p_knot <= 2 * (P.n + P.m) && P.max_cons_knot <= 2;
+}
+
+// the compact class (DevProblem::fwd_compact) inside the fast path, with its costs cached in shared memory as rollout_fast caches them
+bool compact_path(const DevProblem& P) { return TO_FWD_COMPACT && fast_path(P) && P.fwd_compact && P.ncost <= FWD_MAX_COST; }
+
+template <int MODEL, int G>
+cudaError_t launch_any(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
+    if constexpr (TO_FWD_COMPACT) { if (compact_path(P)) return launch_pass<MODEL, G, FWD_COMPACT>(P, trial0, first_pass, final_pass, s); }
+    if (fast_path(P)) return launch_pass<MODEL, G, FWD_FAST>(P, trial0, first_pass, final_pass, s);
+    return launch_pass<MODEL, G, FWD_GENERIC>(P, trial0, first_pass, final_pass, s);
 }
 
 }  // namespace
@@ -512,8 +797,7 @@ cudaError_t launch_forward(const DevProblem& P, cudaStream_t s) {
     cudaError_t e = cudaErrorNotSupported;
     const int final_pass = P.opt.ls_iters < 4;
     if (P.late_list) { e = cudaMemsetAsync(P.late_count, 0, sizeof(int), s); if (e != cudaSuccess) return e; e = cudaErrorNotSupported; }
-    if (fast_path(P)) { TO_DISPATCH_MODEL(P.model, P.m, (e = launch_pass<MODEL, 4, true>(P, 0, 1, final_pass, s))); }
-    else { TO_DISPATCH_MODEL(P.model, P.m, (e = launch_pass<MODEL, 4, false>(P, 0, 1, final_pass, s))); }
+    TO_DISPATCH_MODEL(P.model, P.m, (e = launch_any<MODEL, 4>(P, 0, 1, final_pass, s)));
     return e;
 }
 
@@ -522,8 +806,7 @@ cudaError_t launch_ladder(const DevProblem& P, cudaStream_t s) {
     cudaError_t e = cudaSuccess;
     for (int trial0 = 4; trial0 <= P.opt.ls_iters && e == cudaSuccess; trial0 += 8) {
         const int final_pass = trial0 + 8 > P.opt.ls_iters;
-        if (fast_path(P)) { TO_DISPATCH_MODEL(P.model, P.m, (e = launch_pass<MODEL, 8, true>(P, trial0, 0, final_pass, s))); }
-        else { TO_DISPATCH_MODEL(P.model, P.m, (e = launch_pass<MODEL, 8, false>(P, trial0, 0, final_pass, s))); }
+        TO_DISPATCH_MODEL(P.model, P.m, (e = launch_any<MODEL, 8>(P, trial0, 0, final_pass, s)));
     }
     return e;
 }
