@@ -28,8 +28,8 @@
 //     positive-definiteness = positive leading minors a, det P, s00, det S (the pivots of LDL' are their ratios).
 //   * the record of knot k (1920 B: fragments of [A_e B_e] + compact expansion) arrives by ONE 1-D bulk TMA copy (cp.async.bulk +
 //     mbarrier, SASS UBLKCP) into a per-warp ring, issued one knot ahead.
-//   * 4-warp CTAs; 80 registers x 6 CTAs per SM = 24 resident warps, 1.29 waves of B = 4096 instances on 132 SMs (TO_FRAG_MINB below: the
-//     faster sweeps beat the 1.11 waves of a 72-register x 7-CTA build on one H100).
+//   * 4-warp CTAs; 128 registers x 4 CTAs per SM = 16 resident warps, two nearly full waves of B = 4096 instances on 132 SMs (1.94;
+//     TO_FRAG_MINB below).
 #include "costcon.cuh"
 #include "frag_layout.cuh"
 #include "kernels.h"
@@ -46,11 +46,13 @@
 #ifndef TO_FRAG_ROUNDS
 #define TO_FRAG_ROUNDS 2
 #endif
-// CTAs per SM the register allocation aims at: 7 (72 registers, 28 warps per SM, more spills) or 6 (80 registers, 24 warps, fewer spills: a sweep
-// is faster).  On one H100 (400 W) 6 is the faster build both on the BASELINE inputs (k_riccati_frag 0.55 vs 0.60 ms) and without regularisation
-// restarts (quadrotor_calm 0.46 vs 0.50 ms).  A build-time knob (-DTO_FRAG_MINB=7) for variant builds.
+// CTAs per SM the register allocation aims at.  A full SM does not make the sweeps faster in total: R grows almost in proportion to the
+// resident warps beyond 4 per scheduler, so 6 CTAs (80 registers, 24 warps, 180 / 368 B of spills) ran B = 4096 as a full wave of 3168
+// sweeps and then 928 more at lone-warp latency.  4 CTAs (128 registers, 16 warps, 12 B of spills) run two nearly full waves of 2112 and
+// 1984 sweeps, each faster per sweep.  On one H100 (700 W), k_riccati_frag: BASELINE 0.484 ms (6 CTAs 0.529, 5 CTAs 0.493, 7 CTAs 0.553),
+// quadrotor_calm 0.361 ms (6 CTAs 0.450, 5 CTAs 0.399, 7 CTAs 0.473).  A build-time knob (-DTO_FRAG_MINB=6) for variant builds.
 #ifndef TO_FRAG_MINB
-#define TO_FRAG_MINB 6
+#define TO_FRAG_MINB 4
 #endif
 // L2 prefetch distance of the record stream, in knots beyond the shared-memory ring (0 = off).  The ring hides the copy latency while the SM is
 // full (28 warps); a LONE warp -- the retry sweeps at the tail of the regularisation ladder, small batches -- waits for every record.
