@@ -5,7 +5,8 @@
  * calls for a BATCH of B independent problem instances that share model / objective / constraints and
  * differ in x0, X, U, multipliers -- and, after a per-instance goal call (to_set_goal_states,
  * to_update_trajectories, to_set_cost_terms), in the linear cost terms q, r and the Goal constraint values
- * (goal state / tracking reference per instance).  Every function cites the reference interface it stands in for.  The
+ * (goal state / tracking reference per instance) -- and, after to_set_model_params, in the model parameters (mass,
+ * inertia, lengths, motor constants, gravity).  Every function cites the reference interface it stands in for.  The
  * Julia-side binding (ccall) that a maintainer adds is shown in INTEGRATION.md.
  *
  * Conventions
@@ -226,6 +227,17 @@ int to_get_cost_terms(to_handle* h, double* q /*[B][ncost][n]*/, double* r /*[B]
 int to_set_cost_terms(to_handle* h, const double* q, const double* r);                              /* set_LQR_goal!(obj[k], ...) per instance, raw terms */
 int to_get_goal_values(to_handle* h, int32_t con, double* vals /*[B][p]*/);                        /* a Goal constraint's xf[inds] of every instance */
 int to_set_goal_values(to_handle* h, int32_t con, const double* vals);                             /* ... set per instance (TO_EINVAL: not a Goal) */
+
+/* ---- per-instance model parameters ---------------------------------------------------------------------------
+ * Instance b integrates its dynamics with its own parameter vector (a Problem owns its model, src/problem.jl:36-73): the entries and order of
+ * to_spec.params, nparams = 1 (DoubleIntegrator), 4 (Cartpole), 10 (Quadrotor), 8 (Acrobot).  Until the first call every instance uses the
+ * shared to_spec.params and every kernel runs as before.  A batch whose instance b holds p_b computes, bit for bit, what instance b of a batch
+ * created with p_b as to_spec.params computes.  X is not rolled out again: the next rollout / expansion / line search / solve uses the new
+ * values.  TO_EDIM: nparams is not the model's count.  TO_EINVAL: a hybrid problem, a non-finite entry, or a non-positive mass, inertia or
+ * length the dynamics divide by (DoubleIntegrator mass; Cartpole mc, mp, l; Quadrotor mass, J1..J3; Acrobot l1, l2, m1, m2); the message names
+ * the instance and the entry, and the rows stay as they were.  Multi-GPU: each rank passes its shard's rows, as for x0. */
+int to_set_model_params(to_handle* h, const double* params /*[B][nparams]*/, int32_t nparams);
+int to_get_model_params(to_handle* h, double* params /*[B][nparams]*/);                             /* the shared values broadcast when none are set */
 
 /* ---- kernel 1: batched RK4 rollout (+ dual-number Jacobians) ---------------------------------------- */
 int to_rollout(to_handle* h);                                                 /* rollout!           src/problem.jl:330-340 */

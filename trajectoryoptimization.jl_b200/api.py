@@ -1204,6 +1204,10 @@ class Problem:
                     vals = np.empty((self.B, con.p))
                     self._raw_call("to_get_goal_values", j, K._dp(vals))
                     goal_carry[cid] = vals
+        mparams = None
+        if getattr(self, "_mparams", False):   # per-instance model parameters: carried over as they are
+            mparams = np.empty((self.B, len(self.model.params)))
+            self._raw_call("to_get_model_params", K._dp(mparams))
         self.close()
         self.spec = self._make_spec(self._dt, float(t[0]))
         self._open()
@@ -1220,6 +1224,8 @@ class Problem:
             if id(c) in goal_carry:
                 self._raw_call("to_set_goal_values", j, K._dp(goal_carry[id(c)]))
         self._goal_snap = {cid: v for cid, v in getattr(self, "_goal_snap", {}).items() if cid in goal_carry}
+        if mparams is not None:
+            self._raw_call("to_set_model_params", K._dp(mparams), int(mparams.shape[1]))
         self._raw_call("to_set_initial_state", K._dp(self.x0))
         self._raw_call("to_set_controls", K._dp(U))
         if np.all(np.isfinite(X)):
@@ -1447,6 +1453,44 @@ def set_cost_terms(prob, q, r):
         raise DimensionMismatch("set_cost_terms: the objective changed its distinct costs; read cost_terms again")
     prob._call("to_set_cost_terms", K._dp(q), K._dp(r))
     prob._inst = True
+
+
+def _model_param_rows(prob, params):
+    """``params`` as the ``[B, nparams]`` rows ``to_set_model_params`` takes; every check that needs no device happens here"""
+    if getattr(prob, "hybrid", False):
+        raise ArgumentError("per-instance model parameters are not supported on hybrid problems (their constants live in the recorded programs)")
+    nparams = len(prob.model.params)
+    if isinstance(params, (list, tuple)) and any(isinstance(x, _Model) for x in params):
+        if len(params) != prob.B:
+            raise DimensionMismatch(f"set_model_params: {len(params)} models for a batch of {prob.B} instances")
+        for b, x in enumerate(params):
+            if type(x) is not type(prob.model) or x.dims() != prob.model.dims():
+                raise ArgumentError(f"set_model_params: instance {b} holds a {type(x).__name__} {getattr(x, 'dims', lambda: '')()}, the problem's model is "
+                                    f"a {type(prob.model).__name__} {prob.model.dims()}")
+        params = [x.params for x in params]
+    rows = np.ascontiguousarray(np.asarray(params, dtype=np.float64))
+    if rows.shape != (prob.B, nparams):
+        raise DimensionMismatch(f"set_model_params: expected [{prob.B}, {nparams}] parameters, got {rows.shape}")
+    return rows
+
+
+def set_model_params(prob, params):
+    """Instance ``b`` integrates its dynamics with its own model parameters: ``params[B, nparams]`` in the order of ``model.params``, or a
+    sequence of ``B`` models of ``type(prob.model)`` whose ``.params`` are taken.  A batch with per-instance parameters computes, bit for bit,
+    what each instance computes in a batch built with its model.  The trajectory is not rolled out again; the next rollout, expansion, line
+    search or solve uses the new values.  ``prob.model`` is left as it is."""
+    rows = _model_param_rows(prob, params)
+    prob._call("to_set_model_params", K._dp(rows), int(rows.shape[1]))
+    prob._mparams = True
+
+
+def model_params(prob):
+    """The model parameters of every instance, ``[B, nparams]`` (the shared ``model.params`` broadcast when none were set)."""
+    if getattr(prob, "hybrid", False):
+        raise ArgumentError("hybrid problems have no model parameter vector")
+    out = np.empty((prob.B, len(prob.model.params)))
+    prob._call("to_get_model_params", K._dp(out))
+    return out
 
 
 def shift_trajectory(prob, steps=1):

@@ -55,6 +55,7 @@ struct to_handle {
     // per-instance linear cost terms / Goal values (DevProblem::qr / goal), empty until the first per-instance call; the host copy is the
     // authoritative one and goes to the device whole after every change
     std::vector<double> h_qr, h_goal;
+    std::vector<double> h_mparams;   // per-instance model parameters (DevProblem::mparams), [B][TO_NPARAM]; empty until to_set_model_params
     int* d_fragerr = nullptr;     // sticky error word of that kernel (queue overflow / spin limit), read by to_synchronize
     double* d_fragpool = nullptr; // gains of its speculative regularisation candidates
     int* d_fragq = nullptr;       // work queue of the register-resident Riccati kernel (riccati_frag.cu)
@@ -202,6 +203,38 @@ void model_defaults(int model, int m, int& n_out, int& m_out, double* p) {
         case TO_MODEL_EXPR: n_out = 4; m_out = 2; break;       // recorded programs on the padded dimensions the kernels are instantiated for
         default: n_out = -1; m_out = -1;
     }
+}
+
+// The entries of a parameter vector the caller gives (to_spec.params, to_set_model_params), and the names of those the device dynamics
+// divide by or build a determinant from (models.cuh): they must be positive.
+int model_nparams(int model) {
+    switch (model) {
+        case TO_MODEL_DOUBLE_INTEGRATOR: return 1;
+        case TO_MODEL_CARTPOLE: return 4;
+        case TO_MODEL_QUADROTOR: return 10;
+        case TO_MODEL_ACROBOT: return 8;
+        default: return 0;
+    }
+}
+const char* positive_param_name(int model, int i) {
+    static const char* di[] = {"mass"};
+    static const char* cp[] = {"mc", "mp", "l"};
+    static const char* qr[] = {"mass", "J1", "J2", "J3"};
+    static const char* ac[] = {"l1", "l2", "m1", "m2"};
+    switch (model) {
+        case TO_MODEL_DOUBLE_INTEGRATOR: return i < 1 ? di[i] : nullptr;
+        case TO_MODEL_CARTPOLE: return i < 3 ? cp[i] : nullptr;
+        case TO_MODEL_QUADROTOR: return i < 4 ? qr[i] : nullptr;
+        case TO_MODEL_ACROBOT: return i < 4 ? ac[i] : nullptr;
+        default: return nullptr;
+    }
+}
+
+// The one place where a parameter vector is completed for the device: the reciprocals the dynamics multiply by (models.cuh).  to_create and
+// to_set_model_params both go through it, so a per-instance row and a shared vector with the same entries hold the same bits.
+void complete_model_params(int model, double* p) {
+    if (model == TO_MODEL_DOUBLE_INTEGRATOR) p[1] = 1.0 / p[0];
+    if (model == TO_MODEL_QUADROTOR) { p[10] = 1.0 / p[0]; p[11] = 1.0 / p[1]; p[12] = 1.0 / p[2]; p[13] = 1.0 / p[3]; }
 }
 
 int build_cost(to_handle* h, const to_cost_spec& tc, int n, int m, DevCost& c) {
@@ -457,10 +490,7 @@ int to_create(const to_spec* s, to_handle** out) {
     if (s->error_state && s->model != TO_MODEL_QUADROTOR)
         return fail(nullptr, TO_EINVAL, "error_state: the model has no Lie-group state (only the Quadrotor does)");
     if (s->params) for (int i = 0; i < s->nparams && i < 10; i++) params[i] = s->params[i];
-    if (s->model == TO_MODEL_DOUBLE_INTEGRATOR) params[1] = 1.0 / params[0];
-    if (s->model == TO_MODEL_QUADROTOR) {   // reciprocals used by the device dynamics (models.cuh)
-        params[10] = 1.0 / params[0]; params[11] = 1.0 / params[1]; params[12] = 1.0 / params[2]; params[13] = 1.0 / params[3];
-    }
+    complete_model_params(s->model, params);
 
     auto* h = new to_handle();
     h->device = s->device;
@@ -922,6 +952,54 @@ int to_set_cost_terms(to_handle* h, const double* q, const double* r) {
         }
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return upload_inst(h);
+}
+
+// ---- per-instance model parameters (DevProblem::mparams) ----------------------------------------------------------
+// params [B][nparams] in the order of to_spec.params.  The whole batch is checked before anything changes: a refused call leaves the rows
+// (or their absence) as they were.  X is not rolled out again (set_initial_state! does not either); the next rollout, expansion, line
+// search or solve integrates with the new values.
+int to_set_model_params(to_handle* h, const double* params, int32_t nparams) {
+    JOIN(h);
+    if (!h || !params) return TO_EINVAL;
+    const int model = h->P.model, B = h->P.B;
+    if (model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance model parameters are not supported on hybrid problems (their constants live in the recorded programs)");
+    const int np = model_nparams(model);
+    if (nparams != np)
+        return fail(h, TO_EDIM, "to_set_model_params: the model takes " + std::to_string(np) + " parameters per instance, got " + std::to_string(nparams));
+    std::vector<double> rows((size_t)B * TO_NPARAM, 0.0);
+    for (int b = 0; b < B; b++) {
+        double* row = rows.data() + (size_t)b * TO_NPARAM;
+        for (int i = 0; i < np; i++) {
+            const double v = params[(size_t)b * np + i];
+            const char* pos = positive_param_name(model, i);
+            if (!std::isfinite(v))
+                return fail(h, TO_EINVAL, "to_set_model_params: instance " + std::to_string(b) + ", parameter " + std::to_string(i) + " is not finite");
+            if (pos && !(v > 0))
+                return fail(h, TO_EINVAL, "to_set_model_params: instance " + std::to_string(b) + ", parameter " + std::to_string(i) + " (" + pos + ") must be positive");
+            row[i] = v;
+        }
+        complete_model_params(model, row);
+    }
+    if (!h->P.mparams) {
+        double* d = nullptr;
+        int rc = dalloc(h, &d, rows.size()); if (rc) return rc;
+        h->P.mparams = d;
+    }
+    h->h_mparams.swap(rows);
+    CU(h, cudaMemcpyAsync(const_cast<double*>(h->P.mparams), h->h_mparams.data(), sizeof(double) * h->h_mparams.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));   // a later call replaces the host rows
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return TO_OK;
+}
+// params [B][nparams]: every instance's parameters (the shared ones broadcast when none are set)
+int to_get_model_params(to_handle* h, double* params) {
+    JOIN(h);
+    if (!h || !params) return TO_EINVAL;
+    const int np = model_nparams(h->P.model);
+    if (np == 0) return fail(h, TO_EINVAL, "hybrid problems have no model parameter vector");
+    for (int b = 0; b < h->P.B; b++)
+        std::memcpy(params + (size_t)b * np, h->P.mparams ? h->h_mparams.data() + (size_t)b * TO_NPARAM : h->P.params, sizeof(double) * np);
+    return TO_OK;
 }
 
 // ---- kernel 1 ---------------------------------------------------------------------------------------------

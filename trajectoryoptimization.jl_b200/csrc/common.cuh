@@ -169,7 +169,11 @@ struct DevProblem {
     // knot, at most one Bound with finite limits on every control and none on the state, on every stage knot, and at most one Goal, on the
     // terminal knot only.  Set at to_create (the structure of the costs and constraints never changes afterwards).
     int fwd_compact;
+    // Per-instance model parameters (to_set_model_params): [B][TO_NPARAM] in the layout of `params`, the host-computed reciprocals included.
+    // nullptr until the first per-instance call; every kernel then reads the shared `params`.
+    const double* mparams;
 };
+#define TO_NPARAM 16         // slots of DevProblem::params and of a row of DevProblem::mparams (one 128-byte line)
 
 enum { SOLVE_ACTIVE = 0, SOLVE_WAITING = 1, SOLVE_DONE = 2 };
 __host__ __device__ inline bool retired(const DevProblem& P, int b) { return P.active != nullptr && P.active[b] != SOLVE_ACTIVE; }
@@ -191,6 +195,14 @@ template <bool INST>
 __host__ __device__ __forceinline__ const double* goal_values(const DevProblem& P, int b, int ci) {
     if constexpr (INST) { if (P.goal) return P.goal + (size_t)b * P.ngoal + P.cons[ci].goff; }
     return P.cons[ci].a;
+}
+// Model parameter i of instance b: the only place that decides between the rows of DevProblem::mparams and the shared vector.  A value, not a
+// pointer: the shared vector lives in the kernel's parameter bank, and a pointer that may point there makes the kernel copy it to local memory.
+// The kernels stage an instance's parameters with it (models.cuh stage_model_params) and run the dynamics on the copy.
+template <bool INST>
+__device__ __forceinline__ double model_param(const DevProblem& P, int b, int i) {
+    if constexpr (INST) { if (P.mparams) return P.mparams[(size_t)b * TO_NPARAM + i]; }
+    return P.params[i];
 }
 
 __host__ __device__ inline const double* traj_X(const DevProblem& P, int buf, int b) { return P.X + buf * P.strideX + (size_t)b * P.N * P.n; }

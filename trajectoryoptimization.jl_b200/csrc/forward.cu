@@ -224,8 +224,8 @@ __device__ __forceinline__ void prefetch_knot(double* base, int g, int l, int k,
 // The candidate trajectory goes to buffer `cbuf`.  Returns the merit; `ok` = no blow-up.
 // INST: the instance's own linear cost terms and Goal values (DevProblem::qr / goal, read from global memory instead of the CTA's table).
 template <int MODEL, int IPB, int G, bool LIE, bool INST>
-__device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab& tab, double* stage, int b, int g, int l, unsigned gmask,
-                                               double alpha, int cbuf, bool& ok, double& viol) {
+__device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab& tab, double* stage, const double* prm, int b, int g, int l,
+                                               unsigned gmask, double alpha, int cbuf, bool& ok, double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     using S = Stage<n, m, IPB, NE>;
     const int N = P.N, buf = P.cur[b];
@@ -378,7 +378,7 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
             }
         }
         if (!last) {
-            rk4_step<MODEL, double>(model_params<MODEL>(P, k), x, u, tab.dt[k], xn);
+            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, tab.dt[k], xn);
 #pragma unroll
             for (int i = 0; i < n; i++) { x[i] = xn[i]; if (!(fabs(xn[i]) <= P.opt.max_state_value)) ok = false; }
             // a blown-up trial keeps integrating (the group stays in lock step); its result is rejected through `ok`
@@ -400,8 +400,8 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
 //   * RK4 writes the next state over the current one (rk4_step reads x_i for the last time where it writes xn_i), so the loop carries
 //     no x <- xn copies.  (Unrolled by two with x / xn swapping roles instead, the loop took 40 more registers and spilled.)
 template <int MODEL, int IPB, int G, bool LIE, bool INST>
-__device__ __forceinline__ double rollout_compact(const DevProblem& P, const FwdCompactTab& tab, double* stage, double* ost, int b, int g,
-                                                  int l, unsigned gmask, double alpha, int cbuf, bool& ok, double& viol) {
+__device__ __forceinline__ double rollout_compact(const DevProblem& P, const FwdCompactTab& tab, double* stage, double* ost, const double* prm,
+                                                  int b, int g, int l, unsigned gmask, double alpha, int cbuf, bool& ok, double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     using S = Stage<n, m, IPB, NE>;
     const int N = P.N, buf = P.cur[b];
@@ -532,11 +532,11 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
         }
         if constexpr (MODEL == MODEL_EXPR_42) {   // a discrete jump map writes its outputs while it reads its inputs
             double xn[n];
-            rk4_step<MODEL, double>(model_params<MODEL>(P, k), x, u, tab.dt[k], xn);
+            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, tab.dt[k], xn);
 #pragma unroll
             for (int i = 0; i < n; i++) x[i] = xn[i];
         } else {
-            rk4_step<MODEL, double>(model_params<MODEL>(P, k), x, u, tab.dt[k], x);
+            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, tab.dt[k], x);
         }
 #pragma unroll
         for (int i = 0; i < n; i++) if (!(fabs(x[i]) <= P.opt.max_state_value)) ok = false;
@@ -579,7 +579,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
 
 // generic path (dense costs or general constraints): pointer-based evaluation, operands read directly from global
 template <int MODEL, bool LIE, bool INST>
-__device__ __forceinline__ double rollout_generic(const DevProblem& P, int b, double alpha, int cbuf, bool& ok, double& viol) {
+__device__ __forceinline__ double rollout_generic(const DevProblem& P, const double* prm, int b, double alpha, int cbuf, bool& ok, double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     const int N = P.N, buf = P.cur[b];
     const double* X = traj_X(P, buf, b);
@@ -625,7 +625,7 @@ __device__ __forceinline__ double rollout_generic(const DevProblem& P, int b, do
         J += cost_value(P.costs[cid], inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, !last);
         J += al_knot_penalty<INST>(P, k + 1, x, u, lam_b, viol, b);
         if (!last) {
-            rk4_step<MODEL, double>(model_params<MODEL>(P, k), x, u, P.dt[k], xn);
+            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, P.dt[k], xn);
 #pragma unroll
             for (int i = 0; i < n; i++) { x[i] = xn[i]; if (!(fabs(xn[i]) <= P.opt.max_state_value)) ok = false; }
             if (!ok) break;
@@ -649,6 +649,17 @@ enum { FWD_GENERIC = 0, FWD_FAST = 1, FWD_COMPACT = 2 };
 #ifndef TO_FWD_COMPACT
 #define TO_FWD_COMPACT 1
 #endif
+
+// dynamic shared memory of a line-search CTA: the cached tables, the operand ring and rollout_compact's output staging (the generic path
+// uses none of them); the INST variant keeps each group's model parameters behind them (launch_pass_l adds IPB rows of TO_NPARAM)
+template <int MODEL, int G, int PATH, int LANES, bool LIE>
+__host__ __device__ constexpr size_t ls_smem_bytes() {
+    constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
+    constexpr int IPB = LANES / G;
+    const size_t tab = PATH == FWD_COMPACT ? sizeof(FwdCompactTab) : sizeof(FwdTab);
+    const size_t ost = PATH == FWD_COMPACT ? (size_t)LANES * FWD_OKNOTS * (n + m) * sizeof(double) : 0;   // rollout_compact's output staging
+    return PATH != FWD_GENERIC ? tab + (size_t)FWD_STAGES * Stage<n, m, IPB, NE>::DOUBLES * sizeof(double) + ost : 0;
+}
 
 // One line-search pass: lane l of group g evaluates trial (trial0 + l) of instance b.
 //   first_pass : ignore / reset accepted[b];   final_pass : commit failures (no acceptable step size).
@@ -686,12 +697,18 @@ __device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0,
         const int cbuf = (P.cur[b] + 1 + l) % TO_NBUF;
         bool ok = false;
         double J, viol = 0.0;
+        double* prm = nullptr;
+        if constexpr (INST) {   // the instance's model parameters, one copy per group behind the rest of the CTA's shared memory
+            prm = reinterpret_cast<double*>(fwd_smem + ls_smem_bytes<MODEL, G, PATH, LANES, LIE>()) + g * TO_NPARAM;
+            if (l == 0) stage_model_params<INST>(P, b, prm);
+            __syncwarp(gmask);
+        }
         if constexpr (PATH == FWD_COMPACT) {
             double* ost = stage + FWD_STAGES * S::DOUBLES + (size_t)g * G * FWD_OKNOTS * (n + m);
-            J = rollout_compact<MODEL, IPB, G, LIE, INST>(P, *tab, stage, ost, b, g, l, gmask, alpha, cbuf, ok, viol);
+            J = rollout_compact<MODEL, IPB, G, LIE, INST>(P, *tab, stage, ost, prm, b, g, l, gmask, alpha, cbuf, ok, viol);
         }
-        else if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST>(P, *tab, stage, b, g, l, gmask, alpha, cbuf, ok, viol);
-        else J = rollout_generic<MODEL, LIE, INST>(P, b, alpha, cbuf, ok, viol);
+        else if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST>(P, *tab, stage, prm, b, g, l, gmask, alpha, cbuf, ok, viol);
+        else J = rollout_generic<MODEL, LIE, INST>(P, prm, b, alpha, cbuf, ok, viol);
         const bool good = (trial <= P.opt.ls_iters) && ls_accept(P, J, P.J[b], alpha, P.dV[2 * b], P.dV[2 * b + 1], ok);
         const unsigned votes = __ballot_sync(gmask, good) & gmask;
         if (votes) {
@@ -732,12 +749,9 @@ __global__ void __launch_bounds__(FWD_THREADS) k_linesearch_compact(const DevPro
 
 template <int MODEL, int G, int PATH, int LANES, bool LIE = false, bool INST = false>
 cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
-    constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     constexpr int IPB = LANES / G;
     const int blocks = (P.B + IPB - 1) / IPB;
-    const size_t tab = PATH == FWD_COMPACT ? sizeof(FwdCompactTab) : sizeof(FwdTab);
-    const size_t ost = PATH == FWD_COMPACT ? (size_t)LANES * FWD_OKNOTS * (n + m) * sizeof(double) : 0;   // rollout_compact's output staging
-    const size_t smem = PATH != FWD_GENERIC ? tab + (size_t)FWD_STAGES * Stage<n, m, IPB, NE>::DOUBLES * sizeof(double) + ost : 0;
+    const size_t smem = ls_smem_bytes<MODEL, G, PATH, LANES, LIE>() + (INST ? (size_t)IPB * TO_NPARAM * sizeof(double) : 0);
     auto kern = [] {
         if constexpr (PATH == FWD_COMPACT) return k_linesearch_compact<MODEL, G, LANES, LIE, INST>;
         else return k_linesearch<MODEL, G, PATH == FWD_FAST, LANES, LIE, INST>;
@@ -768,10 +782,11 @@ cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int f
     return launch_pass_l<MODEL, G, PATH, 32, false, INST>(P, trial0, first_pass, final_pass, s);
 }
 
-// per-instance linear cost terms / Goal values: a kernel variant of its own, so that the shared one is the code it has always been
+// per-instance linear cost terms / Goal values / model parameters: a kernel variant of its own, so that the shared one is the code it has
+// always been.  It serves every per-instance table; each accessor checks its own (inst_q, goal_values, model_param).
 template <int MODEL, int G, int PATH>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
-    if (P.qr) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);
+    if (P.qr || P.mparams) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);
     return launch_pass_i<MODEL, G, PATH, false>(P, trial0, first_pass, final_pass, s);
 }
 

@@ -97,6 +97,20 @@ template <> struct ModelDims<MODEL_DOUBLE_INTEGRATOR_2D> { static constexpr int 
 constexpr int MODEL_EXPR_42 = 20;
 template <> struct ModelDims<MODEL_EXPR_42> { static constexpr int n = 4, m = 2; };
 
+// a b - c c (the Cartpole's mass-matrix determinant).  With dual numbers the value is written as the one rounding fma(a, b, -(c c)): the
+// compiler is free to contract either product, and it chose differently when the parameters came from shared memory (per-instance
+// parameters) than from the parameter bank; this is the form the shared kernels have always computed.
+__device__ __forceinline__ double det_sub_square(double a, double b, double c) { return a * b - c * c; }
+template <int P>
+__device__ __forceinline__ Dual<P> det_sub_square(const Dual<P>& a, const Dual<P>& b, const Dual<P>& c) {
+    const Dual<P> ab = a * b, cc = c * c;
+    Dual<P> r;
+    r.v = fma(a.v, b.v, -cc.v);
+#pragma unroll
+    for (int i = 0; i < P; i++) r.d[i] = ab.d[i] - cc.d[i];
+    return r;
+}
+
 template <int MODEL, class S>
 __device__ __forceinline__ void dynamics(const double* __restrict__ p, const S* x, const S* u, S* xd) {
     if constexpr (MODEL == MODEL_EXPR_42) {
@@ -146,7 +160,7 @@ __device__ __forceinline__ void dynamics(const double* __restrict__ p, const S* 
         S h11 = lift<S>(mc + mp), h12 = (mp * l) * c, h22 = lift<S>(mp * l * l);
         S r1 = (-mp * l) * (qd2 * s) * qd2 - u[0];
         S r2 = (mp * g * l) * s;
-        S idet = lift<S>(1.0) / (h11 * h22 - h12 * h12);
+        S idet = lift<S>(1.0) / det_sub_square(h11, h22, h12);
         xd[0] = qd1; xd[1] = qd2;
         xd[2] = -(h22 * r1 - h12 * r2) * idet;
         xd[3] = -(h11 * r2 - h12 * r1) * idet;
@@ -236,9 +250,18 @@ __device__ __forceinline__ void rk4_step(const double* __restrict__ p, const S* 
         case MODEL_EXPR: { constexpr int MODEL = MODEL_EXPR_42; CALL; } break;                     \
     }
 
-// what rk4_step / dynamics take as `p`: the model's parameter vector, or -- recorded programs -- the DevDyn of knot k
-template <int MODEL>
-__device__ __forceinline__ const double* model_params(const DevProblem& P, int k) {
+// what rk4_step / dynamics take as `p` at knot k: the shared parameter vector (INST = false); INST: `row`, the copy of instance b's parameters
+// the kernel made with stage_model_params; recorded programs: the DevDyn of knot k (their constants are never per instance)
+template <int MODEL, bool INST = false>
+__device__ __forceinline__ const double* model_params(const DevProblem& P, const double* row, int k) {
     if constexpr (MODEL == MODEL_EXPR_42) return reinterpret_cast<const double*>(&P.dyn[P.dyn_index[k]]);
+    else if constexpr (INST) return row;
     else return P.params;
+}
+// row[0 .. TO_NPARAM) = the parameters of instance b (common.cuh model_param), `row` in shared memory: read from there, the dynamics compile
+// to the same FP64 operations as with the shared vector in the parameter bank (a copy in registers loses FMA contractions)
+template <bool INST>
+__device__ __forceinline__ void stage_model_params(const DevProblem& P, int b, double* row) {
+#pragma unroll
+    for (int i = 0; i < TO_NPARAM; i++) row[i] = model_param<INST>(P, b, i);
 }

@@ -17,7 +17,9 @@
 
 // One thread integrates one instance; the warp writes its 32 states of a knot through a shared-memory transpose, so that the stores are runs of
 // n contiguous doubles per instance (full 32-byte sectors) instead of 32 scattered 8-byte words per instruction.
-template <int MODEL>
+// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per lane.  (Copied to registers instead, the
+// parameter-only subexpressions of the dynamics were hoisted out of the knot loop and lost FMA contractions the shared kernel has.)
+template <int MODEL, bool INST>
 __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m;
     __shared__ double stage[32 * n];
@@ -28,6 +30,12 @@ __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
     const int bc = valid ? b : P.B - 1;                     // (idle lanes of the last warp shadow a real instance and store nothing)
     base[lane] = valid ? traj_Xw(P, P.cur[bc], bc) : nullptr;
     const double* U = traj_U(P, P.cur[bc], bc);
+    const double* prm = nullptr;
+    if constexpr (INST) {
+        __shared__ double prm_s[32][TO_NPARAM];
+        stage_model_params<INST>(P, bc, prm_s[lane]);
+        prm = prm_s[lane];
+    }
     double x[n], u[m], xn[n];
 #pragma unroll
     for (int i = 0; i < n; i++) x[i] = P.x0[(size_t)bc * n + i];
@@ -45,7 +53,7 @@ __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
         if (k == P.N - 1) break;
 #pragma unroll
         for (int i = 0; i < m; i++) u[i] = U[k * m + i];
-        rk4_step<MODEL, double>(model_params<MODEL>(P, k), x, u, P.dt[k], xn);
+        rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, P.dt[k], xn);
 #pragma unroll
         for (int i = 0; i < n; i++) x[i] = xn[i];
     }
@@ -68,7 +76,8 @@ template <> struct SeedList<MODEL_QUADROTOR> {
     __host__ __device__ static constexpr int trivial(int s) { return s < 3 ? s : 4 + s; }        // 0..2 (r), 7..9 (v)
 };
 
-template <int MODEL, int NP>
+// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per thread (see k_rollout)
+template <int MODEL, int NP, bool INST>
 __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, nm = n + m;
     constexpr int NSEED = SeedList<MODEL>::count;
@@ -103,7 +112,13 @@ __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
 #pragma unroll
         for (int q = 0; q < NP; q++) u[i].d[q] = (n + i == js[q]) ? 1.0 : 0.0;
     }
-    rk4_step<MODEL, D>(model_params<MODEL>(P, k), x, u, P.dt[k], xn);
+    const double* prm = nullptr;
+    if constexpr (INST) {
+        __shared__ double prm_s[128][TO_NPARAM];
+        stage_model_params<INST>(P, b, prm_s[threadIdx.x]);
+        prm = prm_s[threadIdx.x];
+    }
+    rk4_step<MODEL, D>(model_params<MODEL, INST>(P, prm, k), x, u, P.dt[k], xn);
 #pragma unroll
     for (int i = 0; i < n; i++) {
         if (NP == 2 && js[1] == js[0] + 1 && !(js[0] & 1)) *reinterpret_cast<double2*>(&AB[i * ld + js[0]]) = make_double2(xn[i].d[0], xn[i].d[1]);
@@ -175,9 +190,10 @@ __device__ __forceinline__ int lie_seed(int s) { return (int)((0xFEDCBA9543ULL >
 __device__ __forceinline__ int lie_trivial(int s) { return (int)((0x876210ULL >> (4 * s)) & 15); }        // 0,1,2,6,7,8
 
 // column j of [A_e B_e]_k: the RK4 step of knot k pushed through Dual<1> with the seed of error-state coordinate j (attitude: a column of G(q_k)),
-// projected on the error state of knot k + 1 with G(q_{k+1})'
-template <int MODEL>
-__device__ __forceinline__ void expand_lie_column(const DevProblem& P, int k, int j, const double* __restrict__ X, const double* __restrict__ U, double (&col)[ModelDims<MODEL>::n - 1]) {
+// projected on the error state of knot k + 1 with G(q_{k+1})'  (INST: with the instance's parameters, staged in `prm`)
+template <int MODEL, bool INST>
+__device__ __forceinline__ void expand_lie_column(const DevProblem& P, const double* prm, int k, int j, const double* __restrict__ X, const double* __restrict__ U,
+                                                  double (&col)[ModelDims<MODEL>::n - 1]) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, qs = 3;
     using D = Dual<1>;
     const double h = P.dt[k];
@@ -197,7 +213,7 @@ __device__ __forceinline__ void expand_lie_column(const DevProblem& P, int k, in
 #pragma unroll
         for (int i = qs + 4; i < n; i++) x[i].d[0] = (i == j + 1) ? 1.0 : 0.0;
     }
-    rk4_step<MODEL, D>(model_params<MODEL>(P, k), x, u, h, xn);
+    rk4_step<MODEL, D>(model_params<MODEL, INST>(P, prm, k), x, u, h, xn);
     const double* q1 = X + n + qs;                                     // attitude of knot k + 1
     const double w1 = q1[0], x1 = q1[1], y1 = q1[2], z1 = q1[3];
 #pragma unroll
@@ -218,7 +234,8 @@ __device__ __forceinline__ void expand_lie_column(const DevProblem& P, int k, in
 #ifndef TO_EXPAND_LIE_THREADS
 #define TO_EXPAND_LIE_THREADS 64
 #endif
-template <int MODEL>
+// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per thread (see k_rollout)
+template <int MODEL, bool INST>
 __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 128 / TO_EXPAND_LIE_THREADS) k_expand_lie(const DevProblem P, int mode) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, nme = ne + m, NS = 10;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -233,8 +250,14 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
     if (retired(P, b)) return;                                     // to_solve: not ACTIVE
     const double* X = traj_X(P, P.cur[b], b) + (size_t)k * n;
     const double* U = traj_U(P, P.cur[b], b) + (size_t)k * m;
+    const double* prm = nullptr;
+    if constexpr (INST) {
+        __shared__ double prm_s[TO_EXPAND_LIE_THREADS][TO_NPARAM];
+        stage_model_params<INST>(P, b, prm_s[threadIdx.x]);
+        prm = prm_s[threadIdx.x];
+    }
     double col[ne];
-    expand_lie_column<MODEL>(P, k, j, X, U, col);
+    expand_lie_column<MODEL, INST>(P, prm, k, j, X, U, col);
     double* out = P.ABe + ((size_t)bk * nme + j) * ne;                 // column j of [A_e B_e]: 12 contiguous doubles
 #pragma unroll
     for (int e = 0; e < ne; e++) out[e] = col[e];
@@ -254,9 +277,10 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
 //   image     record order (frag_layout.cuh) with the 16-byte chunks of each 128-byte line permuted by fraglayout::stage_swz: the column
 //             stores of a warp spread over the banks, the line stores read every bank once.
 // tests/test_expand_staging.py restates the staging map and the write-out in NumPy.
+// INST: the instance's own model parameters (DevProblem::mparams), staged in shared memory once per CTA (the CTA's one instance)
 #define EXPB_KPB 6
 #define EXPB_T 64
-template <int MODEL>
+template <int MODEL, bool INST>
 __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_expand_lie_rec(const DevProblem P, int mode, int nkb) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, NS = 10;
     static_assert(ne == 12 && m == 4 && EXPB_KPB * NS <= EXPB_T, "record layout of the error-state Quadrotor");
@@ -271,6 +295,13 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
     const int k0 = kb * EXPB_KPB;
     const int nk = (P.N - 1 - k0 < EXPB_KPB) ? P.N - 1 - k0 : EXPB_KPB;
     const int tid = threadIdx.x, kk = tid / NS, sd = tid - kk * NS;
+    const double* prm = nullptr;
+    if constexpr (INST) {
+        __shared__ double prm_s[TO_NPARAM];
+        if (tid == 0) stage_model_params<INST>(P, b, prm_s);
+        __syncthreads();
+        prm = prm_s;
+    }
     if (kk < nk) {
         const int k = k0 + kk;
         const int buf = P.cur[b];
@@ -285,7 +316,7 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
             for (int e = 0; e < ne; e++) img[fraglayout::stage_swz(fraglayout::ab_index(e, 12) | cb, kk)] = col[e];
         };
         double col[ne];
-        expand_lie_column<MODEL>(P, k, lie_seed(sd), X, U, col);
+        expand_lie_column<MODEL, INST>(P, prm, k, lie_seed(sd), X, U, col);
         put(lie_seed(sd), col);
         if (sd < 6) {                                                                  // closed-form column jt: d x+/d r = I, d r+/d v = h I, d v+/d v = I
             const int jt = lie_trivial(sd);
@@ -534,14 +565,19 @@ cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
     if (P.frag) {
         // one CTA per (instance, block of EXPB_KPB knots); mode 2 with the late list: the first *late_count instance slots carry work
         const int nkb = (P.N - 1 + EXPB_KPB - 1) / EXPB_KPB;
-        k_expand_lie_rec<MODEL_QUADROTOR><<<(unsigned)((long long)P.B * nkb), EXPB_T, 0, s>>>(P, mode, nkb);
-    } else k_expand_lie<MODEL_QUADROTOR><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
+        const unsigned blocks = (unsigned)((long long)P.B * nkb);
+        if (P.mparams) k_expand_lie_rec<MODEL_QUADROTOR, true><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
+        else k_expand_lie_rec<MODEL_QUADROTOR, false><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
+    } else if (P.mparams) k_expand_lie<MODEL_QUADROTOR, true><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
+    else k_expand_lie<MODEL_QUADROTOR, false><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
 
+// the dynamics kernels read nothing per instance but the model parameters: their INST variant runs exactly when the rows exist
 cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s) {
     const int threads = 32, blocks = (P.B + threads - 1) / threads;
-    TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL><<<blocks, threads, 0, s>>>(P)));
+    if (P.mparams) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true><<<blocks, threads, 0, s>>>(P))); }
+    else { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, false><<<blocks, threads, 0, s>>>(P))); }
     return cudaGetLastError();
 }
 
@@ -550,7 +586,9 @@ static cudaError_t launch_expand_t(const DevProblem& P, cudaStream_t s, int mode
     constexpr int TPK = (SeedList<MODEL>::count + NP - 1) / NP;
     const long long total = (long long)P.B * (P.N - 1) * TPK;
     const int threads = 128;
-    k_expand<MODEL, NP><<<(unsigned)((total + threads - 1) / threads), threads, 0, s>>>(P, mode);
+    const unsigned blocks = (unsigned)((total + threads - 1) / threads);
+    if (P.mparams) k_expand<MODEL, NP, true><<<blocks, threads, 0, s>>>(P, mode);
+    else k_expand<MODEL, NP, false><<<blocks, threads, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
 

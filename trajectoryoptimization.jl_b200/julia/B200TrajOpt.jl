@@ -324,6 +324,16 @@ function TO.set_goal_state!(p::BatchedProblem, xf::AbstractMatrix{Float64}; obje
     size(xf, 2) == p.B || throw(DimensionMismatch("xf must be (n, B)"))
     check(p.h, ccall((:to_set_goal_states, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Cint, Cint), p.h, Matrix{Float64}(xf), objective, constraint))
 end
+# per-instance model parameters: column b of P (nparams, B) is instance b's parameter vector, in the order of to_spec.params
+function set_model_params!(p::BatchedProblem, P::AbstractMatrix)
+    size(P, 2) == p.B || throw(DimensionMismatch("P must be (nparams, B)"))
+    check(p.h, ccall((:to_set_model_params, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Int32), p.h, Matrix{Float64}(P), size(P, 1)))
+end
+function model_params(p::BatchedProblem, nparams::Integer)
+    P = Matrix{Float64}(undef, nparams, p.B)
+    check(p.h, ccall((:to_get_model_params, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}), p.h, P))
+    P
+end
 
 # ---- what Altro.jl's iLQR / AL loop does with the API above, fused on the device ------------------------------
 expand!(p::BatchedProblem) = check(p.h, ccall((:to_expand, libb200), Cint, (Ptr{Cvoid},), p.h))
