@@ -315,6 +315,21 @@ int to_backward_algebra(const to_handle* h, int32_t* variant);             /* wh
                                                                              (riccati.cu, riccati_small.cu, lie.cu), 1 = 2 x 2 block inverse + W'K update
                                                                              (riccati_frag.cu).  Same mathematics (Altro backwardpass!); the oracle mirrors
                                                                              either so that parity tests compare like with like (DESIGN.md 4a) */
+/* DIAGNOSTIC (test / tuning hook, not part of the Julia shim): which kernels the next solver calls launch, as picked from the problem's
+ * shape, the options and the device (DESIGN.md 4a lists the thresholds).  choice[TO_CHOICE_COUNT]:
+ *   LINESEARCH  the line search's knot loop (TO_LS_*);  COST_CACHED  1: that loop reads the costs from shared memory (0 on the generic loop);
+ *   BACKWARD  the backward-pass kernel (TO_BK_*);  FASTAL  1: k_riccati holds the AL terms lane-resident (0 for the other kernels);
+ *   REC_FUSED  1: the records' cost expansion reads the host-built term table (0 off the record path);  LATE_LIST  1: the later line-search
+ *   passes walk the list of late instances;  INST_FORWARD / INST_BACKWARD  1: the line search / the backward pass's cost and AL reads
+ *   launch their per-instance (INST) variant;  RESIDENT  k_riccati_frag warps (= instances) resident at once on this device (0 off the
+ *   record path): a larger batch is pulled from the work queue after the first wave.  Reads the handle only. */
+enum to_choice { TO_CHOICE_LINESEARCH = 0, TO_CHOICE_COST_CACHED = 1, TO_CHOICE_BACKWARD = 2, TO_CHOICE_FASTAL = 3, TO_CHOICE_REC_FUSED = 4,
+                 TO_CHOICE_LATE_LIST = 5, TO_CHOICE_INST_FORWARD = 6, TO_CHOICE_INST_BACKWARD = 7, TO_CHOICE_RESIDENT = 8, TO_CHOICE_COUNT = 9 };
+enum to_linesearch_loop { TO_LS_GENERIC = 0, TO_LS_FAST = 1, TO_LS_COMPACT = 2 };
+enum to_backward_kernel { TO_BK_THREAD = 0 /* k_riccati_small */, TO_BK_WARP_MMA = 1 /* k_riccati, tensor MMA */, TO_BK_WARP_DFMA = 2 /* k_riccati, DFMA */,
+                          TO_BK_FRAGMENT = 3 /* k_riccati_frag, the record path */, TO_BK_DENSE_MMA = 4 /* k_riccati_dense_mma */,
+                          TO_BK_DENSE_DFMA = 5 /* k_riccati_dense */ };
+int to_kernel_choice(const to_handle* h, int32_t* choice);
 int to_error_state_dim(const to_handle* h, int32_t* ne);                      /* RD.errstate_dim(model): n, or n - 1 with spec.error_state */
 /* RD.state_diff(model, xbar, x) of every knot against the current trajectory: Xbar [B][N][n] (host) -> dx [B][N][n_e] */
 int to_state_diff(to_handle* h, const double* Xbar, double* dx);

@@ -30,6 +30,10 @@ CON_GOAL, CON_BOUND, CON_LINEAR, CON_CIRCLE, CON_SPHERE, CON_NORM, CON_COLLISION
 # to_solve_status
 SOLVE_UNSOLVED, SOLVE_SUCCEEDED, SOLVE_MAX_ITERATIONS, SOLVE_MAX_ITERATIONS_OUTER, SOLVE_MAX_REGULARIZATION = 0, 1, 2, 3, 4
 PHASE_EXPAND, PHASE_BACKWARD, PHASE_FORWARD, PHASE_LADDER, PHASE_ACCEPT, PHASE_COSTEXP, PHASE_LATE, PHASE_COUNT = 0, 1, 2, 3, 4, 5, 6, 8
+# to_kernel_choice: the entries of choice[] in order, and the names of the TO_LS_* / TO_BK_* values
+CHOICE_FIELDS = ("linesearch", "cost_cached", "backward", "fastal", "rec_fused", "late_list", "inst_forward", "inst_backward", "resident")
+LINESEARCH_LOOPS = ("generic", "fast", "compact")
+BACKWARD_KERNELS = ("thread", "warp_mma", "warp_dfma", "fragment", "dense_mma", "dense_dfma")
 
 c_double_p = C.POINTER(C.c_double)
 c_int32_p = C.POINTER(C.c_int32)
@@ -192,7 +196,7 @@ def load_library():
         "to_reduce_merit": [H], "to_reduce_merit_async": [H, C.c_void_p], "to_merit_device_ptr": [H, C.POINTER(C.c_void_p)],
         "to_set_phase_timing": [H, C.c_int], "to_get_phase_times": [H, c_double_p, C.POINTER(C.c_int64), C.c_int],
         "to_algorithmic_bytes": [H, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64)],
-        "to_backward_algebra": [H, c_int32_p], "to_error_state_dim": [H, c_int32_p], "to_state_diff": [H, c_double_p, c_double_p], "to_get_error_dynamics": [H, c_double_p],
+        "to_backward_algebra": [H, c_int32_p], "to_kernel_choice": [H, c_int32_p], "to_error_state_dim": [H, c_int32_p], "to_state_diff": [H, c_double_p, c_double_p], "to_get_error_dynamics": [H, c_double_p],
         "to_error_expansion": [H, c_double_p, c_double_p], "to_get_expansion_records": [H, c_double_p],
         "to_default_solve_options": [C.POINTER(to_solve_options)],
         "to_solve": [H, C.POINTER(to_solve_options), c_int32_p, c_int32_p, c_int32_p, c_double_p, c_double_p, c_double_p, c_double_p],
@@ -220,7 +224,7 @@ EXPORTED_SYMBOLS = [
     "to_set_goal_states", "to_update_trajectories", "to_get_cost_terms", "to_set_cost_terms", "to_get_goal_values", "to_set_goal_values",
     "to_set_model_params", "to_get_model_params",
     "to_set_phase_timing", "to_get_phase_times", "to_launch_count", "to_algorithmic_bytes",
-    "to_backward_algebra", "to_error_state_dim", "to_state_diff", "to_get_error_dynamics", "to_error_expansion",
+    "to_backward_algebra", "to_kernel_choice", "to_error_state_dim", "to_state_diff", "to_get_error_dynamics", "to_error_expansion",
     "to_get_expansion_records", "to_default_solve_options", "to_solve",
 ]
 

@@ -1756,6 +1756,21 @@ def backward_algebra(prob):
     return int(v.value)
 
 
+def kernel_choice(prob):
+    """which kernels the next solver calls launch, as the library picks them from the problem's shape (``to_kernel_choice``) -> dict:
+    ``linesearch`` ("generic" / "fast" / "compact"), ``backward`` ("thread", "warp_mma", "warp_dfma", "fragment", "dense_mma",
+    "dense_dfma"), the flags ``cost_cached``, ``fastal``, ``rec_fused``, ``late_list``, ``inst_forward``, ``inst_backward`` and ``resident``
+    (k_riccati_frag instances resident at once on the device, 0 off the record path)"""
+    v = (C.c_int32 * len(K.CHOICE_FIELDS))()
+    prob._call("to_kernel_choice", v)
+    d = dict(zip(K.CHOICE_FIELDS, (int(x) for x in v)))
+    d["linesearch"] = K.LINESEARCH_LOOPS[d["linesearch"]]
+    d["backward"] = K.BACKWARD_KERNELS[d["backward"]]
+    for f in ("cost_cached", "fastal", "rec_fused", "late_list", "inst_forward", "inst_backward"):
+        d[f] = bool(d[f])
+    return d
+
+
 def solver_state(prob):
     B = prob.B
     rho, dV, alpha = np.empty(B), np.empty((B, 2)), np.empty(B)

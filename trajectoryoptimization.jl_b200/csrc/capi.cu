@@ -1044,6 +1044,9 @@ int to_rollout(to_handle* h) {
 // the records' cost + AL expansion comes from the host-built term table (common.cuh ExpTab) when the Goal / Bound rows fit it:
 // <= 3 rows per z entry, knot indices < 4095, < 128 rows per knot; otherwise k_expansion_rec walks the descriptors
 static bool rec_fused(const DevProblem& P) { return P.frag && P.max_terms_per_z <= 3 && P.N < 4095 && P.max_p_knot < 128; }
+// the record path (k_riccati_frag) unless to_options.backward_kernel forces a shared-memory kernel: 3 generic DFMA kernel on the full
+// expansion, 5 tensor kernel on the compact expansion
+static bool record_path(const DevProblem& P) { return P.frag && P.opt.pad != 3 && P.opt.pad != 5; }
 int to_expand(to_handle* h) {
     JOIN(h);
     if (!h) return TO_EINVAL;
@@ -1216,8 +1219,7 @@ static int materialise_expansion(to_handle* h, double* EG, double* EH) {
     return TO_OK;
 }
 static int do_backward(to_handle* h, bool costexp_done = false) {
-    // to_options.backward_kernel: 0 automatic, 3 generic DFMA kernel on the full expansion, 5 shared-memory tensor kernel on the compact expansion
-    if (h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5) {
+    if (record_path(h->P)) {
         if (!costexp_done) {   // cost + AL expansion of every record: always from the current trajectory, multipliers and penalties
             PhaseScope pe(h, TO_PHASE_COSTEXP);
             if (rec_fused(h->P)) CU(h, launch_expansion_rec16(h->P, h->stream, 0));      // 16 lanes per knot, host-built term table
@@ -1295,7 +1297,7 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
     // (error state: only [A_e B_e] is needed by the solver kernels -- k_expand_lie; the full [A B] is produced by to_expand on request)
     auto expand = [&](cudaStream_t st, int mode) { return h->P.lie ? launch_expand_lie(h->P, st, mode) : launch_expand(h->P, st, mode); };
     bool costexp_done = false;
-    const bool rec = h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5 && rec_fused(h->P);
+    const bool rec = record_path(h->P) && rec_fused(h->P);
     if (h->side_pending) {
         {
             PhaseScope pl(h, TO_PHASE_LATE, h->stream2);
@@ -1459,7 +1461,27 @@ int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* 
 // ---- Lie-group error state (lie.cu) ---------------------------------------------------------------------------
 int to_backward_algebra(const to_handle* h, int32_t* variant) {
     if (!h || !variant) return TO_EINVAL;
-    *variant = (h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5) ? 1 : 0;
+    *variant = record_path(h->P) ? 1 : 0;
+    return TO_OK;
+}
+static_assert(TO_LS_GENERIC == KC_LS_GENERIC && TO_LS_FAST == KC_LS_FAST && TO_LS_COMPACT == KC_LS_COMPACT, "to_linesearch_loop");
+static_assert(TO_BK_THREAD == KC_BK_THREAD && TO_BK_WARP_MMA == KC_BK_WARP_MMA && TO_BK_WARP_DFMA == KC_BK_WARP_DFMA && TO_BK_FRAGMENT == KC_BK_FRAGMENT &&
+              TO_BK_DENSE_MMA == KC_BK_DENSE_MMA && TO_BK_DENSE_DFMA == KC_BK_DENSE_DFMA, "to_backward_kernel");
+int to_kernel_choice(const to_handle* h, int32_t* choice) {
+    if (!h || !choice) return TO_EINVAL;
+    DeviceGuard device_guard(h);     // the SM count (riccati_small_supported) and the resident warps are those of the handle's device
+    const DevProblem& P = h->P;
+    const int ls = linesearch_path(P);
+    const int bk = record_path(P) ? KC_BK_FRAGMENT : backward_kernel_of(P);   // do_backward
+    choice[TO_CHOICE_LINESEARCH] = ls;
+    choice[TO_CHOICE_COST_CACHED] = (ls != KC_LS_GENERIC && linesearch_costs_cached(P)) ? 1 : 0;
+    choice[TO_CHOICE_BACKWARD] = bk;
+    choice[TO_CHOICE_FASTAL] = ((bk == KC_BK_WARP_MMA || bk == KC_BK_WARP_DFMA) && riccati_fastal(P)) ? 1 : 0;
+    choice[TO_CHOICE_REC_FUSED] = (record_path(P) && rec_fused(P)) ? 1 : 0;
+    choice[TO_CHOICE_LATE_LIST] = P.late_list ? 1 : 0;
+    choice[TO_CHOICE_INST_FORWARD] = (P.qr || P.mparams) ? 1 : 0;   // launch_pass
+    choice[TO_CHOICE_INST_BACKWARD] = P.qr ? 1 : 0;                 // k_riccati, k_riccati_small, k_expansion_rec(16b), k_expansion_compact, k_al_expansion
+    choice[TO_CHOICE_RESIDENT] = bk == KC_BK_FRAGMENT ? frag_resident_warps() : 0;
     return TO_OK;
 }
 int to_error_state_dim(const to_handle* h, int32_t* ne) {

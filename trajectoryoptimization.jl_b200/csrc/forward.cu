@@ -625,7 +625,8 @@ __device__ __forceinline__ double rollout_generic(const DevProblem& P, const dou
         J += cost_value(P.costs[cid], inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, !last);
         J += al_knot_penalty<INST>(P, k + 1, x, u, lam_b, viol, b);
         if (!last) {
-            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, P.dt[k], xn);
+            // INST: the determinant form the shared kernel compiles to, written out (models.cuh det_sub_square)
+            rk4_step<MODEL, double, INST>(model_params<MODEL, INST>(P, prm, k), x, u, P.dt[k], xn);
 #pragma unroll
             for (int i = 0; i < n; i++) { x[i] = xn[i]; if (!(fabs(xn[i]) <= P.opt.max_state_value)) ok = false; }
             if (!ok) break;
@@ -790,21 +791,28 @@ cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int fin
     return launch_pass_i<MODEL, G, PATH, false>(P, trial0, first_pass, final_pass, s);
 }
 
-bool fast_path(const DevProblem& P) {
-    return P.all_diag_cost && P.all_diag_con && P.N <= FWD_MAX_N && P.max_p_knot <= 2 * (P.n + P.m) && P.max_cons_knot <= 2;
-}
-
-// the compact class (DevProblem::fwd_compact) inside the fast path, with its costs cached in shared memory as rollout_fast caches them
-bool compact_path(const DevProblem& P) { return TO_FWD_COMPACT && fast_path(P) && P.fwd_compact && P.ncost <= FWD_MAX_COST; }
+static_assert(FWD_GENERIC == KC_LS_GENERIC && FWD_FAST == KC_LS_FAST && FWD_COMPACT == KC_LS_COMPACT, "kernels.h KC_LS_*");
 
 template <int MODEL, int G>
 cudaError_t launch_any(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
-    if constexpr (TO_FWD_COMPACT) { if (compact_path(P)) return launch_pass<MODEL, G, FWD_COMPACT>(P, trial0, first_pass, final_pass, s); }
-    if (fast_path(P)) return launch_pass<MODEL, G, FWD_FAST>(P, trial0, first_pass, final_pass, s);
+    const int path = linesearch_path(P);
+    if constexpr (TO_FWD_COMPACT) { if (path == FWD_COMPACT) return launch_pass<MODEL, G, FWD_COMPACT>(P, trial0, first_pass, final_pass, s); }
+    if (path == FWD_FAST) return launch_pass<MODEL, G, FWD_FAST>(P, trial0, first_pass, final_pass, s);
     return launch_pass<MODEL, G, FWD_GENERIC>(P, trial0, first_pass, final_pass, s);
 }
 
 }  // namespace
+
+// load_tables makes the same test on the device
+bool linesearch_costs_cached(const DevProblem& P) { return P.ncost <= FWD_MAX_COST; }
+
+// the fast loop (rollout_fast) needs its tables to fit FwdTab: the horizon, 2 (n + m) multipliers and two constraints per knot.  The
+// compact loop is the compact class (DevProblem::fwd_compact) inside the fast path, with its costs cached as rollout_fast caches them.
+int linesearch_path(const DevProblem& P) {
+    const bool fast = P.all_diag_cost && P.all_diag_con && P.N <= FWD_MAX_N && P.max_p_knot <= 2 * (P.n + P.m) && P.max_cons_knot <= 2;
+    if (TO_FWD_COMPACT && fast && P.fwd_compact && linesearch_costs_cached(P)) return FWD_COMPACT;
+    return fast ? FWD_FAST : FWD_GENERIC;
+}
 
 // pass 1: trials 0..3 (alpha = 1, 1/2, 1/4, 1/8), 4 lanes per instance.
 // (The alternative, the whole ladder in one 16-lane pass, computes 11x the FLOPs, and its uncoalesced candidate stores load the LSU.)

@@ -43,6 +43,16 @@ cudaError_t launch_export_abe(const DevProblem& P, cudaStream_t s);             
 size_t frag_queue_ints(int B);
 size_t frag_pool_doubles(int B, int N);                                                 // doubles of the speculative candidates' gain pool                                                         // ints of the kernel's work queue (allocated by the handle)
 cudaError_t launch_backward_frag(const DevProblem& P, int* queue, double* pool, int* sticky_err, cudaStream_t s);
+// Kernel choices made from the problem's shape.  The launchers and to_kernel_choice (capi.cu) both call these, so the diagnostic reports
+// what the launch does.  The values are those of include/trajopt_b200.h (TO_LS_*, TO_BK_*).
+enum { KC_LS_GENERIC = 0, KC_LS_FAST = 1, KC_LS_COMPACT = 2 };
+enum { KC_BK_THREAD = 0, KC_BK_WARP_MMA = 1, KC_BK_WARP_DFMA = 2, KC_BK_FRAGMENT = 3, KC_BK_DENSE_MMA = 4, KC_BK_DENSE_DFMA = 5 };
+int linesearch_path(const DevProblem& P);          // forward.cu: the knot loop of the line search (KC_LS_*)
+bool linesearch_costs_cached(const DevProblem& P);  // forward.cu: the fast / compact loop reads the costs from shared memory
+int backward_kernel_of(const DevProblem& P);       // riccati.cu: the kernel launch_backward launches (KC_BK_*, never KC_BK_FRAGMENT)
+bool riccati_fastal(const DevProblem& P);           // riccati.cu: k_riccati holds the AL terms lane-resident (FASTAL)
+bool dense_backward_mma(const DevProblem& P);       // lie.cu: launch_backward_dense takes the tensor-MMA kernel
+int frag_resident_warps();                          // riccati_frag.cu: k_riccati_frag warps (= instances) resident at once on this device
 // forward pass: closed-loop rollout + merit + line search                     (forward.cu)
 cudaError_t launch_forward(const DevProblem& P, cudaStream_t s);
 cudaError_t launch_ladder(const DevProblem& P, cudaStream_t s);

@@ -688,9 +688,11 @@ cudaError_t launch_expansion_compact(const DevProblem& P, cudaStream_t s) {
     else k_expansion_compact<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }
+// to_options.backward_kernel = 3 forces the DFMA kernel (A/B, tests)
+bool dense_backward_mma(const DevProblem& P) { return P.ne == 12 && P.m == 4 && P.opt.pad != 3; }
 cudaError_t launch_backward_dense(const DevProblem& P, cudaStream_t s) {
-    // to_options.backward_kernel = 3 forces the DFMA kernel (A/B, tests)
-    if (P.ne == 12 && P.m == 4) return P.opt.pad == 3 ? launch_dense_t<12, 4>(P, s) : launch_dense_mma(P, s);
+    if (dense_backward_mma(P)) return launch_dense_mma(P, s);
+    if (P.ne == 12 && P.m == 4) return launch_dense_t<12, 4>(P, s);
     if (P.ne == 13 && P.m == 4) return launch_dense_t<13, 4>(P, s);
     if (P.ne == 4 && P.m == 1) return launch_dense_t<4, 1>(P, s);
     if (P.ne == 4 && P.m == 2) return launch_dense_t<4, 2>(P, s);

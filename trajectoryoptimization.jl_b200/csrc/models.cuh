@@ -100,8 +100,16 @@ template <> struct ModelDims<MODEL_EXPR_42> { static constexpr int n = 4, m = 2;
 // a b - c c (the Cartpole's mass-matrix determinant).  With dual numbers the value is written as the one rounding fma(a, b, -(c c)): the
 // compiler is free to contract either product, and it chose differently when the parameters came from shared memory (per-instance
 // parameters) than from the parameter bank; this is the form the shared kernels have always computed.
-__device__ __forceinline__ double det_sub_square(double a, double b, double c) { return a * b - c * c; }
-template <int P>
+// With doubles the shared kernels differ among themselves: the generic line search (rollout_generic) computes fma(a, b, -(c c)), and its
+// per-instance variant contracted c c instead (one ulp off in the merit).  DET_FMA writes that kernel's form out; every other instantiation
+// keeps the plain expression, and so the code it has always compiled to (writing fma everywhere changes the shared rollout and the fast
+// line-search kernels).
+template <bool DET_FMA>
+__device__ __forceinline__ double det_sub_square(double a, double b, double c) {
+    if constexpr (DET_FMA) return fma(a, b, -(c * c));
+    else return a * b - c * c;
+}
+template <bool DET_FMA, int P>
 __device__ __forceinline__ Dual<P> det_sub_square(const Dual<P>& a, const Dual<P>& b, const Dual<P>& c) {
     const Dual<P> ab = a * b, cc = c * c;
     Dual<P> r;
@@ -111,7 +119,7 @@ __device__ __forceinline__ Dual<P> det_sub_square(const Dual<P>& a, const Dual<P
     return r;
 }
 
-template <int MODEL, class S>
+template <int MODEL, class S, bool DET_FMA = false>
 __device__ __forceinline__ void dynamics(const double* __restrict__ p, const S* x, const S* u, S* xd) {
     if constexpr (MODEL == MODEL_EXPR_42) {
         // `p` is the knot's DevDyn (model_params): interpret the recorded program with the scalar type S (double or dual numbers); the
@@ -160,7 +168,7 @@ __device__ __forceinline__ void dynamics(const double* __restrict__ p, const S* 
         S h11 = lift<S>(mc + mp), h12 = (mp * l) * c, h22 = lift<S>(mp * l * l);
         S r1 = (-mp * l) * (qd2 * s) * qd2 - u[0];
         S r2 = (mp * g * l) * s;
-        S idet = lift<S>(1.0) / det_sub_square(h11, h22, h12);
+        S idet = lift<S>(1.0) / det_sub_square<DET_FMA>(h11, h22, h12);
         xd[0] = qd1; xd[1] = qd2;
         xd[2] = -(h22 * r1 - h12 * r2) * idet;
         xd[3] = -(h11 * r2 - h12 * r1) * idet;
@@ -216,23 +224,24 @@ __device__ __forceinline__ void dynamics(const double* __restrict__ p, const S* 
 }
 
 // RK4, zero-order hold:  k_i scaled by h as RobotDynamics does; x+ = x + (k1 + 2k2 + 2k3 + k4)/6
-template <int MODEL, class S>
+// DET_FMA: the Cartpole's determinant as one explicit fma (det_sub_square)
+template <int MODEL, class S, bool DET_FMA = false>
 __device__ __forceinline__ void rk4_step(const double* __restrict__ p, const S* x, const S* u, double h, S* xn) {
     constexpr int n = ModelDims<MODEL>::n;
     if constexpr (MODEL == MODEL_EXPR_42) {     // a discrete jump map is applied as is
         if (reinterpret_cast<const DevDyn*>(p)->discrete) { dynamics<MODEL, S>(p, x, u, xn); return; }
     }
     S k[n], acc[n], xt[n];
-    dynamics<MODEL, S>(p, x, u, k);
+    dynamics<MODEL, S, DET_FMA>(p, x, u, k);
 #pragma unroll
     for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = k[i]; xt[i] = x[i] + k[i] * 0.5; }
-    dynamics<MODEL, S>(p, xt, u, k);
+    dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
 #pragma unroll
     for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = acc[i] + 2.0 * k[i]; xt[i] = x[i] + k[i] * 0.5; }
-    dynamics<MODEL, S>(p, xt, u, k);
+    dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
 #pragma unroll
     for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = acc[i] + 2.0 * k[i]; xt[i] = x[i] + k[i]; }
-    dynamics<MODEL, S>(p, xt, u, k);
+    dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
 #pragma unroll
     for (int i = 0; i < n; i++) { k[i] = k[i] * h; xn[i] = x[i] + (acc[i] + k[i]) * (1.0 / 6.0); }
 }

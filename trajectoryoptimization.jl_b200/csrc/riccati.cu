@@ -986,7 +986,7 @@ cudaError_t launch_riccati_v(const DevProblem& P, int* work_counter, cudaStream_
 template <int N_, int M_, bool FASTAL, bool INST>
 cudaError_t launch_riccati_t(const DevProblem& P, int* work_counter, cudaStream_t s) {
     if constexpr (N_ >= 8 && M_ <= 4) {
-        if (P.all_diag_cost && P.all_diag_con) {   // tensor-MMA kernel: diagonal lzz (DiagonalCost + Goal/Bound)
+        if (backward_kernel_of(P) == KC_BK_WARP_MMA) {   // tensor-MMA kernel: diagonal lzz (DiagonalCost + Goal/Bound)
             // 2-stage ring, 16 one-warp CTAs per SM.  NSLOT stays MAXT (the loop bound of the slot loop).
             return launch_riccati_v<N_, M_, FASTAL, TO_RICCATI_STAGES, TO_RICCATI_MINB, true, MAXT, INST>(P, work_counter, s);
         }
@@ -998,20 +998,29 @@ cudaError_t launch_riccati_t(const DevProblem& P, int* work_counter, cudaStream_
 
 template <int N_, int M_>
 cudaError_t launch_riccati_nm(const DevProblem& P, int* work_counter, cudaStream_t s) {
-    // the lane-resident AL terms hold at most MAXT rows per z entry (upper + lower bound + goal)
-    const bool fastal = P.max_terms_per_z <= MAXT && P.N < 4095 && P.max_p_knot < 128;
+    const bool fastal = riccati_fastal(P);
     if (P.qr) return fastal ? launch_riccati_t<N_, M_, true, true>(P, work_counter, s) : launch_riccati_t<N_, M_, false, true>(P, work_counter, s);
     return fastal ? launch_riccati_t<N_, M_, true, false>(P, work_counter, s) : launch_riccati_t<N_, M_, false, false>(P, work_counter, s);
 }
 
 }  // namespace
 
-cudaError_t launch_backward(const DevProblem& P, int* work_counter, cudaStream_t s) {
-    if (P.dense_riccati) return launch_backward_dense(P, s);   // lie.cu: error state / quaternion costs (expansion materialised by the caller)
+// the lane-resident AL terms hold at most MAXT rows per z entry (upper + lower bound + goal); knot and row indices are packed in bit fields
+bool riccati_fastal(const DevProblem& P) { return P.max_terms_per_z <= MAXT && P.N < 4095 && P.max_p_knot < 128; }
+
+int backward_kernel_of(const DevProblem& P) {
+    // lie.cu: error state / quaternion costs (expansion materialised by the caller)
+    if (P.dense_riccati) return dense_backward_mma(P) ? KC_BK_DENSE_MMA : KC_BK_DENSE_DFMA;
     // small models: one thread per instance, everything in registers (riccati_small.cu); backward_kernel = 1 forces the warp kernel
     const int choice = P.opt.pad;   // to_options.backward_kernel: 0 automatic, 1 warp kernel, 2 thread kernel where it applies
-    if (choice == 2 && riccati_small_supported(P, true)) return launch_backward_small(P, s);
-    if (choice == 0 && riccati_small_supported(P, false)) return launch_backward_small(P, s);
+    if ((choice == 2 && riccati_small_supported(P, true)) || (choice == 0 && riccati_small_supported(P, false))) return KC_BK_THREAD;
+    // tensor-MMA k_riccati (n >= 8): diagonal lzz (DiagonalCost + Goal/Bound); otherwise the DFMA micro-block kernel
+    return (P.n >= 8 && P.m <= 4 && P.all_diag_cost && P.all_diag_con) ? KC_BK_WARP_MMA : KC_BK_WARP_DFMA;
+}
+
+cudaError_t launch_backward(const DevProblem& P, int* work_counter, cudaStream_t s) {
+    if (P.dense_riccati) return launch_backward_dense(P, s);
+    if (backward_kernel_of(P) == KC_BK_THREAD) return launch_backward_small(P, s);
     if (P.n == 13 && P.m == 4) return launch_riccati_nm<13, 4>(P, work_counter, s);
     if (P.n == 4 && P.m == 1) return launch_riccati_nm<4, 1>(P, work_counter, s);
     if (P.n == 4 && P.m == 2) return launch_riccati_nm<4, 2>(P, work_counter, s);

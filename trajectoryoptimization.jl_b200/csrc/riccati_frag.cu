@@ -618,24 +618,38 @@ int frag_pool_slots(int B, int N) {
 }
 size_t frag_pool_doubles(int B, int N) { return (size_t)frag_pool_slots(B, N) * ((size_t)(N - 1) * 52 + 2); }
 
+namespace {
+constexpr int FRAG_WARPS = TO_FRAG_WARPS;
+// per-device launch configuration (one process may hold handles on several GPUs): the SM count and the CTAs the occupancy API fits per SM
+int ctas_per_sm[TO_MAXDEV] = {0}, num_sms[TO_MAXDEV] = {0};
+cudaError_t frag_configure(int dev) {
+    if (ctas_per_sm[dev]) return cudaSuccess;
+    auto kern = k_riccati_frag<TO_FRAG_STAGES, FRAG_WARPS, TO_FRAG_MINB>;
+    const int smem = (int)sizeof(FragSmem<TO_FRAG_STAGES, FRAG_WARPS>);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return e;
+    cudaDeviceGetAttribute(&num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
+    int c = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kern, 32 * FRAG_WARPS, smem);
+    if (e != cudaSuccess) return e;
+    ctas_per_sm[dev] = c < 1 ? 1 : c;
+    return cudaSuccess;
+}
+}  // namespace
+
+int frag_resident_warps() {
+    const int dev = current_device_slot();
+    return frag_configure(dev) == cudaSuccess ? num_sms[dev] * ctas_per_sm[dev] * FRAG_WARPS : 0;
+}
+
 cudaError_t launch_backward_frag(const DevProblem& P, int* queue, double* pool, int* sticky_err, cudaStream_t s) {
-    constexpr int STAGES = TO_FRAG_STAGES, WARPS = TO_FRAG_WARPS;
+    constexpr int STAGES = TO_FRAG_STAGES, WARPS = FRAG_WARPS;
     using SM = FragSmem<STAGES, WARPS>;
     auto kern = k_riccati_frag<STAGES, WARPS, TO_FRAG_MINB>;
     const int smem = (int)sizeof(SM);
-    // per-device launch configuration (one process may hold handles on several GPUs)
-    static int ctas_per_sm[TO_MAXDEV] = {0}, num_sms[TO_MAXDEV] = {0};
     const int dev = current_device_slot();
-    cudaError_t e = cudaSuccess;
-    if (!ctas_per_sm[dev]) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-        if (e != cudaSuccess) return e;
-        cudaDeviceGetAttribute(&num_sms[dev], cudaDevAttrMultiProcessorCount, dev);
-        int c = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&c, kern, 32 * WARPS, smem);
-        if (e != cudaSuccess) return e;
-        ctas_per_sm[dev] = c < 1 ? 1 : c;
-    }
+    cudaError_t e = frag_configure(dev);
+    if (e != cudaSuccess) return e;
     // queue layout (k_riccati_frag): head, tail, nfinal, error, pool slots, 3 x pad | cnt[B] = 0 | items[16 B + 8192] = -1 | best[B] = 0x7f7f7f7f
     const size_t qcap = 16 * (size_t)P.B + 8192;
     e = cudaMemsetAsync(queue, 0, sizeof(int) * (8 + (size_t)P.B), s);
