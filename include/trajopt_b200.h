@@ -6,7 +6,8 @@
  * differ in x0, X, U, multipliers -- and, after a per-instance goal call (to_set_goal_states,
  * to_update_trajectories, to_set_cost_terms), in the linear cost terms q, r and the Goal constraint values
  * (goal state / tracking reference per instance) -- and, after to_set_model_params, in the model parameters (mass,
- * inertia, lengths, motor constants, gravity).  Every function cites the reference interface it stands in for.  The
+ * inertia, lengths, motor constants, gravity) -- and, after to_set_constraint_data, in the constraint data (bounds, obstacles, collision
+ * radii, norm values, linear right-hand sides).  Every function cites the reference interface it stands in for.  The
  * Julia-side binding (ccall) that a maintainer adds is shown in INTEGRATION.md.
  *
  * Conventions
@@ -238,6 +239,26 @@ int to_set_goal_values(to_handle* h, int32_t con, const double* vals);          
  * the instance and the entry, and the rows stay as they were.  Multi-GPU: each rank passes its shard's rows, as for x0. */
 int to_set_model_params(to_handle* h, const double* params /*[B][nparams]*/, int32_t nparams);
 int to_get_model_params(to_handle* h, double* params /*[B][nparams]*/);                             /* the shared values broadcast when none are set */
+
+/* ---- per-instance constraint data ----------------------------------------------------------------------------
+ * Instance b evaluates constraint con with its own data (a Problem owns its ConstraintList, src/problem.jl:36-73).  One instance's row, len doubles:
+ *   BOUND     2(n+m)  z_max[n+m] | z_min[n+m], +-Inf where the shared bound is +-Inf
+ *   LINEAR    p       b[p]  (A stays shared)
+ *   CIRCLE    3p      xc[p] | yc[p] | r[p]
+ *   SPHERE    4p      xc[p] | yc[p] | zc[p] | r[p]
+ *   NORM      1       val
+ *   COLLISION 1       radius
+ * to_constraint_data_len gives len (0 for GOAL, which has to_set_goal_values, and for QUATVEC / EXPR, whose constants stay shared).  Until the
+ * first to_set_constraint_data there is no table and every kernel runs as before; the first call fills every instance with the shared data of
+ * every constraint, then applies its rows.  The shape stays fixed: rows, knot ranges and the multiplier layout never change, so a BOUND row must
+ * be finite exactly where the shared bound is, with the same infinities.  TO_EINVAL, with the instance and the entry named, and nothing changed:
+ * a changed +-Inf pattern, z_max < z_min (src/constraints.jl:712), a non-finite entry of another kind, a NORM val < 0 (:451), a GOAL, QUATVEC or
+ * EXPR constraint, a hybrid problem.  to_shift_trajectory leaves the data alone (obstacles live in the world frame); to_bounds keeps returning
+ * the shared values.  A batch whose instance b holds d_b computes, bit for bit, what instance b of a batch created with d_b as the shared data
+ * computes, on every solver path.  Multi-GPU: each rank passes its shard's rows, as for x0. */
+int to_constraint_data_len(const to_handle* h, int32_t con, int32_t* len);                         /* doubles per instance of constraint con */
+int to_set_constraint_data(to_handle* h, int32_t con, const double* data /*[B][len]*/);
+int to_get_constraint_data(to_handle* h, int32_t con, double* data /*[B][len]*/);                  /* the shared values broadcast when none are set */
 
 /* ---- kernel 1: batched RK4 rollout (+ dual-number Jacobians) ---------------------------------------- */
 int to_rollout(to_handle* h);                                                 /* rollout!           src/problem.jl:330-340 */

@@ -1204,6 +1204,16 @@ class Problem:
                     vals = np.empty((self.B, con.p))
                     self._raw_call("to_get_goal_values", j, K._dp(vals))
                     goal_carry[cid] = vals
+        cdata_carry = {}   # per-instance constraint data: the rows of every constraint unchanged since the call
+        csnap = getattr(self, "_cdata_snap", {})
+        if csnap:
+            live = {id(c): c for c in self.constraints.constraints}
+            for j, cid in enumerate(self._sig[2]):
+                con = live.get(cid)
+                if cid in csnap and con is not None and np.array_equal(_con_row(con)[1], csnap[cid]):
+                    rows = np.empty((self.B, csnap[cid].size))
+                    self._raw_call("to_get_constraint_data", j, K._dp(rows))
+                    cdata_carry[cid] = rows
         mparams = None
         if getattr(self, "_mparams", False):   # per-instance model parameters: carried over as they are
             mparams = np.empty((self.B, len(self.model.params)))
@@ -1224,6 +1234,10 @@ class Problem:
             if id(c) in goal_carry:
                 self._raw_call("to_set_goal_values", j, K._dp(goal_carry[id(c)]))
         self._goal_snap = {cid: v for cid, v in getattr(self, "_goal_snap", {}).items() if cid in goal_carry}
+        for j, c in enumerate(self.constraints.constraints):
+            if id(c) in cdata_carry:
+                self._raw_call("to_set_constraint_data", j, K._dp(cdata_carry[id(c)]))
+        self._cdata_snap = {cid: v for cid, v in csnap.items() if cid in cdata_carry}
         if mparams is not None:
             self._raw_call("to_set_model_params", K._dp(mparams), int(mparams.shape[1]))
         self._raw_call("to_set_initial_state", K._dp(self.x0))
@@ -1490,6 +1504,117 @@ def model_params(prob):
         raise ArgumentError("hybrid problems have no model parameter vector")
     out = np.empty((prob.B, len(prob.model.params)))
     prob._call("to_get_model_params", K._dp(out))
+    return out
+
+
+# which fields of a constraint's _spec are its per-instance data, in the order of an instance's row (include/trajopt_b200.h
+# to_set_constraint_data); every other field stays shared
+_CON_DATA_FIELDS = {K.CON_BOUND: ("a", "b"), K.CON_LINEAR: ("b",), K.CON_CIRCLE: ("a", "b", "rad"), K.CON_SPHERE: ("a", "b", "c", "rad"),
+                    K.CON_NORM: ("val",), K.CON_COLLISION: ("val",)}
+
+
+def _con_row(con):
+    """(spec, row): the device description of ``con`` and its data in the layout of one instance's row (ArgumentError: no such data)"""
+    if isinstance(con, (QuatVecEq, AutodiffConstraint, IndexedConstraint)):
+        raise ArgumentError(f"the data of a {type(con).__name__} stays shared across the batch")
+    spec = con._spec(1, 1)
+    fields = _CON_DATA_FIELDS.get(spec["kind"])
+    if fields is None:
+        raise ArgumentError(f"{type(con).__name__} carries no per-instance constraint data")
+    return spec, np.concatenate([np.atleast_1d(np.asarray(spec[f], dtype=np.float64)).ravel() for f in fields])
+
+
+def _con_and_index(prob, con):
+    """(index, constraint) of ``con``: an index into the problem's constraint list or one of its constraint objects"""
+    j = _con_index(prob, con)
+    if not 0 <= j < len(prob.constraints):
+        raise ArgumentError(f"constraint index {j} outside 0:{len(prob.constraints) - 1}")
+    return j, prob.constraints[j]
+
+
+def _constraint_data_rows(prob, con, rows):
+    """(index, constraint, rows [B, len]) as to_set_constraint_data / to_set_goal_values take them; every check that needs no device happens here"""
+    if getattr(prob, "hybrid", False):
+        raise ArgumentError("per-instance constraint data is not supported on hybrid problems")
+    j, con = _con_and_index(prob, con)
+    objs = isinstance(rows, (list, tuple)) and any(isinstance(x, AbstractConstraint) for x in rows)
+    if isinstance(con, GoalConstraint):
+        if objs:
+            if len(rows) != prob.B:
+                raise DimensionMismatch(f"set_constraint_data: {len(rows)} constraints for a batch of {prob.B} instances")
+            if any(type(x) is not GoalConstraint or not np.array_equal(x.inds, con.inds) for x in rows):
+                raise ArgumentError("set_constraint_data: every instance's constraint must be a GoalConstraint on the same indices")
+            rows = [x.xf for x in rows]
+        out = np.ascontiguousarray(np.asarray(rows, dtype=np.float64))
+        if out.shape != (prob.B, con.p):
+            raise DimensionMismatch(f"set_constraint_data: expected [{prob.B}, {con.p}] Goal values, got {out.shape}")
+        return j, con, out
+    spec, shared = _con_row(con)
+    if objs:
+        if len(rows) != prob.B:
+            raise DimensionMismatch(f"set_constraint_data: {len(rows)} constraints for a batch of {prob.B} instances")
+        fields = _CON_DATA_FIELDS[spec["kind"]]
+        packed = []
+        for b, x in enumerate(rows):
+            if type(x) is not type(con):
+                raise ArgumentError(f"set_constraint_data: instance {b} holds a {type(x).__name__}, the constraint is a {type(con).__name__}")
+            xs, xr = _con_row(x)
+            same = all(np.array_equal(np.asarray(xs[k]), np.asarray(spec[k])) for k in spec if k not in fields and k in xs) and set(xs) == set(spec)
+            if xr.shape != shared.shape or not same:
+                raise DimensionMismatch(f"set_constraint_data: instance {b}'s {type(x).__name__} differs from the problem's in more than its data")
+            packed.append(xr)
+        rows = packed
+    out = np.ascontiguousarray(np.asarray(rows, dtype=np.float64))
+    if out.shape != (prob.B, shared.size):
+        raise DimensionMismatch(f"set_constraint_data: expected [{prob.B}, {shared.size}] rows, got {out.shape}")
+    for b in range(prob.B):
+        r = out[b]
+        if spec["kind"] == K.CON_BOUND:
+            nm = shared.size // 2
+            fin = np.isfinite(shared)
+            bad = np.nonzero(np.where(fin, ~np.isfinite(r), r != shared))[0]
+            if bad.size:
+                raise ArgumentError(f"set_constraint_data: instance {b}, entry {bad[0]}: BoundConstraint entries must be finite exactly where the "
+                                    "shared bound is, with the same infinities")
+            bad = np.nonzero(~(r[:nm] >= r[nm:]))[0]
+            if bad.size:
+                raise ArgumentError(f"set_constraint_data: instance {b}, entry {bad[0]}: Upper bounds must be greater than or equal to lower bounds")
+        else:
+            bad = np.nonzero(~np.isfinite(r))[0]
+            if bad.size:
+                raise ArgumentError(f"set_constraint_data: instance {b}, entry {bad[0]} is not finite")
+            if spec["kind"] == K.CON_NORM and not r[0] >= 0:
+                raise ArgumentError(f"set_constraint_data: instance {b}: NormConstraint value must be non-negative")
+    return j, con, out
+
+
+def set_constraint_data(prob, con, rows):
+    """Instance ``b`` evaluates constraint ``con`` (an index into the problem's constraint list, or the constraint object) with its own data.
+    ``rows`` is ``[B, len]`` in the layout of include/trajopt_b200.h (BoundConstraint ``z_max | z_min``, LinearConstraint ``b``,
+    CircleConstraint ``xc | yc | r``, SphereConstraint ``xc | yc | zc | r``, NormConstraint ``val``, CollisionConstraint ``radius``;
+    GoalConstraint ``xf[inds]``), or a sequence of ``B`` constraints of the same type and shape whose data are taken.  A batch whose
+    instance ``b`` holds ``d_b`` computes, bit for bit, what instance ``b`` of a batch built with ``d_b`` computes.  The constraint objects
+    are left as they are; a later in-place change to one of them, picked up when the handle is rebuilt, wins in every instance.
+    An ``IndexedConstraint`` (a constraint applied to a slice of a larger model) keeps its data shared: ``ArgumentError``."""
+    j, con, out = _constraint_data_rows(prob, con, rows)
+    if isinstance(con, GoalConstraint):
+        prob._call("to_set_goal_values", j, K._dp(out))
+        prob._inst = True
+        prob._goal_snap = {**getattr(prob, "_goal_snap", {}), id(con): np.array(con.xf, dtype=float)}
+        return
+    prob._call("to_set_constraint_data", j, K._dp(out))
+    prob._cdata_snap = {**getattr(prob, "_cdata_snap", {}), id(con): _con_row(con)[1]}
+
+
+def constraint_data(prob, con):
+    """The data of constraint ``con`` of every instance, ``[B, len]`` (the shared data broadcast when none was set)."""
+    j, con = _con_and_index(prob, con)
+    if isinstance(con, GoalConstraint):
+        out = np.empty((prob.B, con.p))
+        prob._call("to_get_goal_values", j, K._dp(out))
+        return out
+    out = np.empty((prob.B, _con_row(con)[1].size))
+    prob._call("to_get_constraint_data", j, K._dp(out))
     return out
 
 

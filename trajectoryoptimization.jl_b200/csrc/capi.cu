@@ -56,6 +56,7 @@ struct to_handle {
     // authoritative one and goes to the device whole after every change
     std::vector<double> h_qr, h_goal;
     std::vector<double> h_mparams;   // per-instance model parameters (DevProblem::mparams), [B][TO_NPARAM]; empty until to_set_model_params
+    std::vector<double> h_cdata;     // per-instance constraint data (DevProblem::cdata), [B][ncdata]; empty until to_set_constraint_data
     int* d_fragerr = nullptr;     // sticky error word of that kernel (queue overflow / spin limit), read by to_synchronize
     double* d_fragpool = nullptr; // gains of its speculative regularisation candidates
     int* d_fragq = nullptr;       // work queue of the register-resident Riccati kernel (riccati_frag.cu)
@@ -131,7 +132,7 @@ int upload_exptab(to_handle* h) {
                     t.nms[nterm][i] = -mu * sign; t.bound[nterm][i] = bound;
                     t.pkx[nterm][i] = (unsigned)con.first | ((unsigned)(con.last - con.first) << 12) | ((unsigned)con.p << 24) | (eq ? 0x80000000u : 0u);
                     t.pky[nterm][i] = (unsigned)(con.offset + row - con.first * con.p);
-                    if (eq) t.goal[nterm][i] = con.goff + row;
+                    t.goal[nterm][i] = eq ? con.goff + row : -2 - (con.cdoff + (side ? nm : 0) + i);
                 }
                 nterm++;
             }
@@ -283,6 +284,34 @@ int build_cost(to_handle* h, const to_cost_spec& tc, int n, int m, DevCost& c) {
         c.zeroH = (hn == 0.0);   // is_blockdiag(cost) = zeroH, src/cost_functions.jl:445,455
     }
     return TO_OK;
+}
+
+// doubles of constraint c in an instance's row of DevProblem::cdata (0: no per-instance data; a Goal has its own table)
+int con_data_len(const DevCon& c, int nm) {
+    switch (c.kind) {
+        case CON_BOUND: return 2 * nm;
+        case CON_LINEAR: return c.p;
+        case CON_CIRCLE: return 3 * c.p;
+        case CON_SPHERE: return 4 * c.p;
+        case CON_NORM: case CON_COLLISION: return 1;
+    }
+    return 0;
+}
+// the shared data of constraint c in the layout of its row (common.cuh con_data)
+void con_shared_row(const DevCon& c, int nm, double* row) {
+    const int p = c.p;
+    switch (c.kind) {
+        case CON_BOUND: std::memcpy(row, c.a, sizeof(double) * nm); std::memcpy(row + nm, c.b, sizeof(double) * nm); break;
+        case CON_LINEAR: std::memcpy(row, c.b, sizeof(double) * p); break;
+        case CON_CIRCLE: case CON_SPHERE: {
+            const bool sph = c.kind == CON_SPHERE;
+            std::memcpy(row, c.a, sizeof(double) * p); std::memcpy(row + p, c.b, sizeof(double) * p);
+            if (sph) std::memcpy(row + 2 * p, c.c3, sizeof(double) * p);
+            std::memcpy(row + (sph ? 3 : 2) * p, c.rad, sizeof(double) * p);
+            break;
+        }
+        case CON_NORM: case CON_COLLISION: row[0] = c.val; break;
+    }
 }
 
 int build_con(to_handle* h, const to_constraint_spec& tc, int n, int m, int N, DevCon& c) {
@@ -554,6 +583,8 @@ int to_create(const to_spec* s, to_handle** out) {
         h->h_cons[i].offset = P.lambda_len;
         P.lambda_len += (h->h_cons[i].last - h->h_cons[i].first + 1) * h->h_cons[i].p;
         if (h->h_cons[i].kind == CON_GOAL) { h->h_cons[i].goff = P.ngoal; P.ngoal += h->h_cons[i].p; }
+        const int clen = con_data_len(h->h_cons[i], n + m);
+        h->h_cons[i].cdoff = clen ? P.ncdata : -1; P.ncdata += clen;
         if (!h->h_cons[i].diagonal) P.all_diag_con = 0;
     }
     P.ncost = s->ncost; P.ncon = s->ncon;
@@ -999,6 +1030,80 @@ int to_get_model_params(to_handle* h, double* params) {
     if (np == 0) return fail(h, TO_EINVAL, "hybrid problems have no model parameter vector");
     for (int b = 0; b < h->P.B; b++)
         std::memcpy(params + (size_t)b * np, h->P.mparams ? h->h_mparams.data() + (size_t)b * TO_NPARAM : h->P.params, sizeof(double) * np);
+    return TO_OK;
+}
+
+// ---- per-instance constraint data (DevProblem::cdata) ----------------------------------------------------------
+int to_constraint_data_len(const to_handle* h, int32_t con, int32_t* len) {
+    if (!h || !len) return TO_EINVAL;
+    if (con < 0 || con >= (int)h->h_cons.size()) return TO_EINVAL;
+    *len = con_data_len(h->h_cons[con], h->P.n + h->P.m);
+    return TO_OK;
+}
+// data [B][len] of constraint con (the layout of con_shared_row).  The whole batch is checked before anything changes: a refused call leaves the
+// table (or its absence) as it was.  The first call creates the table with the shared data of every constraint in every row.
+int to_set_constraint_data(to_handle* h, int32_t con, const double* data) {
+    JOIN(h);
+    if (!h || !data) return TO_EINVAL;
+    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance constraint data is not supported on hybrid problems");
+    if (con < 0 || con >= (int)h->h_cons.size()) return fail(h, TO_EINVAL, "to_set_constraint_data: no constraint " + std::to_string(con));
+    const DevCon& c = h->h_cons[con];
+    if (c.kind == CON_GOAL) return fail(h, TO_EINVAL, "to_set_constraint_data: a Goal constraint's values are set with to_set_goal_values");
+    const int nm = h->P.n + h->P.m, len = con_data_len(c, nm), B = h->P.B;
+    if (len == 0) return fail(h, TO_EINVAL, "to_set_constraint_data: the data of QuatVecEq and recorded (expression) constraints stays shared");
+    auto where = [](int b, int j) { return "instance " + std::to_string(b) + ", entry " + std::to_string(j); };
+    for (int b = 0; b < B; b++) {
+        const double* row = data + (size_t)b * len;
+        if (c.kind == CON_BOUND) {   // the rows, and so p and the multiplier layout, stay those of the shared bound
+            for (int j = 0; j < 2 * nm; j++) {
+                const double v = row[j], s = j < nm ? c.a[j] : c.b[j - nm];
+                if (std::isfinite(s) ? !std::isfinite(v) : !(v == s))
+                    return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, j) + ": BoundConstraint entries must be finite exactly where the shared "
+                                              "bound is, with the same infinities");
+            }
+            for (int j = 0; j < nm; j++)
+                if (!(row[j] >= row[nm + j]))
+                    return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, j) + ": Upper bounds must be greater than or equal to lower bounds");   // src/constraints.jl:712
+        } else {
+            for (int j = 0; j < len; j++)
+                if (!std::isfinite(row[j])) return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, j) + " is not finite");
+            if (c.kind == CON_NORM && !(row[0] >= 0))
+                return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, 0) + ": NormConstraint value must be non-negative");   // src/constraints.jl:451
+        }
+    }
+    // the new rows are staged and become the host table only once the device holds them: if a copy fails, to_get_constraint_data still
+    // reports the rows of the last successful call (or the shared data, and no table exists)
+    const int nc = h->P.ncdata;
+    std::vector<double> rows;
+    if (h->P.cdata) rows = h->h_cdata;
+    else {
+        rows.resize((size_t)B * nc);
+        for (int b = 0; b < B; b++)
+            for (const auto& k : h->h_cons)
+                if (k.cdoff >= 0) con_shared_row(k, nm, rows.data() + (size_t)b * nc + k.cdoff);
+    }
+    for (int b = 0; b < B; b++) std::memcpy(rows.data() + (size_t)b * nc + c.cdoff, data + (size_t)b * len, sizeof(double) * len);
+    double* d = const_cast<double*>(h->P.cdata);
+    if (!d) { int rc = dalloc(h, &d, rows.size()); if (rc) return rc; }
+    CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));   // `rows` is the source of the copy
+    h->h_cdata.swap(rows);
+    h->P.cdata = d;
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return TO_OK;
+}
+// data [B][len]: constraint con's data of every instance (the shared data broadcast when none is set)
+int to_get_constraint_data(to_handle* h, int32_t con, double* data) {
+    JOIN(h);
+    if (!h || !data) return TO_EINVAL;
+    if (con < 0 || con >= (int)h->h_cons.size()) return fail(h, TO_EINVAL, "to_get_constraint_data: no constraint " + std::to_string(con));
+    const DevCon& c = h->h_cons[con];
+    const int nm = h->P.n + h->P.m, len = con_data_len(c, nm);
+    if (len == 0) return fail(h, TO_EINVAL, "to_get_constraint_data: the constraint has no per-instance data here (Goal: to_get_goal_values)");
+    std::vector<double> shared(len);
+    con_shared_row(c, nm, shared.data());
+    for (int b = 0; b < h->P.B; b++)
+        std::memcpy(data + (size_t)b * len, h->P.cdata ? h->h_cdata.data() + (size_t)b * h->P.ncdata + c.cdoff : shared.data(), sizeof(double) * len);
     return TO_OK;
 }
 
@@ -1479,8 +1584,10 @@ int to_kernel_choice(const to_handle* h, int32_t* choice) {
     choice[TO_CHOICE_FASTAL] = ((bk == KC_BK_WARP_MMA || bk == KC_BK_WARP_DFMA) && riccati_fastal(P)) ? 1 : 0;
     choice[TO_CHOICE_REC_FUSED] = (record_path(P) && rec_fused(P)) ? 1 : 0;
     choice[TO_CHOICE_LATE_LIST] = P.late_list ? 1 : 0;
-    choice[TO_CHOICE_INST_FORWARD] = (P.qr || P.mparams) ? 1 : 0;   // launch_pass
-    choice[TO_CHOICE_INST_BACKWARD] = P.qr ? 1 : 0;                 // k_riccati, k_riccati_small, k_expansion_rec(16b), k_expansion_compact, k_al_expansion
+    choice[TO_CHOICE_INST_FORWARD] = (P.qr || P.mparams || P.cdata) ? 1 : 0;   // launch_pass
+    choice[TO_CHOICE_INST_BACKWARD] = (P.qr || P.cdata) ? 1 : 0;                // k_riccati, k_riccati_small, k_expansion_rec(16b), k_expansion_compact,
+                                                                                // k_al_expansion, k_al_update, k_cost, k_eval_constraints,
+                                                                                // k_constraint_jacobians (cdata)
     choice[TO_CHOICE_RESIDENT] = bk == KC_BK_FRAGMENT ? frag_resident_warps() : 0;
     return TO_OK;
 }

@@ -66,7 +66,9 @@ struct DevCon {
     double c3[TO_MAXP];      // SPHERE zc[p]
     double rad[TO_MAXP];
     // CON_EXPR: user constraint recorded as a program (outputs = the last p instructions); to_constraint_spec TO_CON_EXPR
-    int prog_len, pad4[3];
+    int prog_len;
+    int cdoff;               // BOUND / LINEAR / CIRCLE / SPHERE / NORM / COLLISION: offset of its data in an instance's row of DevProblem::cdata
+    int pad4[2];
     int prog[3 * TO_EXPR_LEN];
     double pconst[TO_EXPR_CONST];
 };
@@ -80,7 +82,8 @@ struct ExpTab {
     double bound[TO_EXP_MAXT][TO_MAXNM];
     unsigned pkx[TO_EXP_MAXT][TO_MAXNM];    // first knot (12 bits) | last - first (12) | rows p of the constraint (7) | equality (1)
     unsigned pky[TO_EXP_MAXT][TO_MAXNM];    // lambda index of the row at knot 0
-    int goal[TO_EXP_MAXT][TO_MAXNM];        // Goal term: index of its bound in an instance's row of DevProblem::goal (-1: other terms)
+    int goal[TO_EXP_MAXT][TO_MAXNM];        // Goal term: index i >= 0 of its bound in an instance's row of DevProblem::goal; Bound term: -2 - j,
+                                            // j = index of its bound in an instance's row of DevProblem::cdata; -1: no term
 };
 
 // one dynamics model of a hybrid problem (to_dynamics_spec): a recorded program, RK4-discretised or a discrete jump map
@@ -172,8 +175,12 @@ struct DevProblem {
     // Per-instance model parameters (to_set_model_params): [B][TO_NPARAM] in the layout of `params`, the host-computed reciprocals included.
     // nullptr until the first per-instance call; every kernel then reads the shared `params`.
     const double* mparams;
+    // Per-instance constraint data (to_set_constraint_data): row b holds, at DevCon::cdoff, the data of every constraint that carries data
+    // other than a Goal (see con_data).  nullptr until the first call; every kernel then reads the shared DevCon fields.
+    const double* cdata;      // [B][ncdata]
+    int ncdata;
 };
-#define TO_NPARAM 16         // slots of DevProblem::params and of a row of DevProblem::mparams (one 128-byte line)
+#define TO_NPARAM 16        // slots of DevProblem::params and of a row of DevProblem::mparams (one 128-byte line)
 
 enum { SOLVE_ACTIVE = 0, SOLVE_WAITING = 1, SOLVE_DONE = 2 };
 __host__ __device__ inline bool retired(const DevProblem& P, int b) { return P.active != nullptr && P.active[b] != SOLVE_ACTIVE; }
@@ -203,6 +210,31 @@ template <bool INST>
 __device__ __forceinline__ double model_param(const DevProblem& P, int b, int i) {
     if constexpr (INST) { if (P.mparams) return P.mparams[(size_t)b * TO_NPARAM + i]; }
     return P.params[i];
+}
+// The data of constraint ci for instance b, in the fields of DevCon it replaces: a (GOAL xf | BOUND z_max | CIRCLE / SPHERE xc), b (BOUND z_min |
+// LINEAR b | yc), c3 (zc), rad (CIRCLE / SPHERE r), val (NORM val | COLLISION radius).  LINEAR's A and every other field stay shared.  The only
+// place that decides between an instance's row of DevProblem::goal / cdata and the descriptor; INST = false returns the descriptor's fields.
+// An instance's row of cdata, at DevCon::cdoff: BOUND z_max[n+m] | z_min[n+m], LINEAR b[p], CIRCLE xc[p] | yc[p] | r[p],
+// SPHERE xc[p] | yc[p] | zc[p] | r[p], NORM val, COLLISION radius.
+struct ConData { const double *a, *b, *c3, *rad; double val; };
+template <bool INST>
+__device__ __forceinline__ ConData con_data(const DevProblem& P, int b, int ci) {
+    const DevCon& con = P.cons[ci];
+    ConData d{con.a, con.b, con.c3, con.rad, con.val};
+    if constexpr (INST) {
+        if (con.kind == CON_GOAL) d.a = goal_values<true>(P, b, ci);
+        else if (P.cdata && con.cdoff >= 0) {
+            const double* row = P.cdata + (size_t)b * P.ncdata + con.cdoff;
+            switch (con.kind) {
+                case CON_BOUND: d.a = row; d.b = row + P.n + P.m; break;
+                case CON_LINEAR: d.b = row; break;
+                case CON_CIRCLE: d.a = row; d.b = row + con.p; d.rad = row + 2 * con.p; break;
+                case CON_SPHERE: d.a = row; d.b = row + con.p; d.c3 = row + 2 * con.p; d.rad = row + 3 * con.p; break;
+                case CON_NORM: case CON_COLLISION: d.val = row[0]; break;
+            }
+        }
+    }
+    return d;
 }
 
 __host__ __device__ inline const double* traj_X(const DevProblem& P, int buf, int b) { return P.X + buf * P.strideX + (size_t)b * P.N * P.n; }

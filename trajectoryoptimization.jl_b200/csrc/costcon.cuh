@@ -326,6 +326,91 @@ __device__ inline void con_jacobian(const DevCon& con, int n, int m, const doubl
     }
 }
 
+// The INST overloads: d = the data of an instance (con_data).  The kinds whose data may differ per instance are evaluated here with the shared
+// overloads' arithmetic, operation for operation; the others go to the shared overloads (a Goal with d.a, its instance's values).
+__device__ inline void con_evaluate(const DevCon& con, const ConData& d, int n, int m, const double* x, const double* u, double* c) {
+    switch (con.kind) {
+        case CON_BOUND: {
+            int i = 0;
+            for (int r = 0; r < con.n_max; r++, i++) { int j = con.a_max[r]; c[i] = zget(n, x, u, j) - d.a[j]; }
+            for (int r = 0; r < con.n_min; r++, i++) { int j = con.a_min[r]; c[i] = d.b[j] - zget(n, x, u, j); }
+            break;
+        }
+        case CON_LINEAR: {
+            const double* y = con.flag ? u : x;
+            const int w = con.flag ? m : n;
+            for (int i = 0; i < con.p; i++) {
+                double s = -d.b[i];
+                for (int j = 0; j < w; j++) s = fma(con.a[j * con.p + i], y[j], s);
+                c[i] = s;
+            }
+            break;
+        }
+        case CON_CIRCLE:
+            for (int i = 0; i < con.p; i++) {
+                double dx = x[con.inds[0]] - d.a[i], dy = x[con.inds[1]] - d.b[i];
+                c[i] = -(dx * dx) - (dy * dy) + d.rad[i] * d.rad[i];
+            }
+            break;
+        case CON_SPHERE:
+            for (int i = 0; i < con.p; i++) {
+                double dx = x[con.inds[0]] - d.a[i], dy = x[con.inds[1]] - d.b[i], dz = x[con.inds[2]] - d.c3[i];
+                c[i] = -(dx * dx) - (dy * dy) - (dz * dz) + d.rad[i] * d.rad[i];
+            }
+            break;
+        case CON_NORM:
+            if (con.sense == CONE_SECOND_ORDER) {
+                for (int i = 0; i < con.ninds; i++) c[i] = zget(n, x, u, con.inds[i]);
+                c[con.ninds] = d.val;
+            } else {
+                double s = 0;
+                for (int i = 0; i < con.ninds; i++) { double z = zget(n, x, u, con.inds[i]); s = fma(z, z, s); }
+                c[0] = s - d.val * d.val;
+            }
+            break;
+        case CON_COLLISION: {
+            const int D = con.ninds / 2;
+            double s = d.val * d.val;
+            for (int i = 0; i < D; i++) { const double dd = x[con.inds[i]] - x[con.inds[D + i]]; s -= dd * dd; }
+            c[0] = s;
+            break;
+        }
+        default: con_evaluate(con, d.a, n, m, x, u, c);
+    }
+}
+__device__ inline void con_jacobian(const DevCon& con, const ConData& d, int n, int m, const double* x, const double* u, double* jac) {
+    const int p = con.p, w = n + m;
+    switch (con.kind) {
+        case CON_CIRCLE:
+            for (int i = 0; i < p * w; i++) jac[i] = 0;
+            for (int i = 0; i < p; i++) {
+                jac[con.inds[0] * p + i] = -2 * (x[con.inds[0]] - d.a[i]);
+                jac[con.inds[1] * p + i] = -2 * (x[con.inds[1]] - d.b[i]);
+            }
+            break;
+        case CON_SPHERE:
+            for (int i = 0; i < p * w; i++) jac[i] = 0;
+            for (int i = 0; i < p; i++) {
+                jac[con.inds[0] * p + i] = -2 * (x[con.inds[0]] - d.a[i]);
+                jac[con.inds[1] * p + i] = -2 * (x[con.inds[1]] - d.b[i]);
+                jac[con.inds[2] * p + i] = -2 * (x[con.inds[2]] - d.c3[i]);
+            }
+            break;
+        default: con_jacobian(con, n, m, x, u, jac);   // independent of the data that may differ per instance
+    }
+}
+// the values / Jacobian of constraint con = P.cons[ci] for instance b: the INST overloads with its data (con_data), or the shared overloads
+template <bool INST>
+__device__ __forceinline__ void con_evaluate_b(const DevProblem& P, const DevCon& con, int b, int ci, int n, int m, const double* x, const double* u, double* c) {
+    if constexpr (INST) con_evaluate(con, con_data<true>(P, b, ci), n, m, x, u, c);
+    else con_evaluate(con, goal_values<false>(P, b, ci), n, m, x, u, c);
+}
+template <bool INST>
+__device__ __forceinline__ void con_jacobian_b(const DevProblem& P, const DevCon& con, int b, int ci, int n, int m, const double* x, const double* u, double* jac) {
+    if constexpr (INST) con_jacobian(con, con_data<true>(P, b, ci), n, m, x, u, jac);
+    else con_jacobian(con, n, m, x, u, jac);
+}
+
 // H[(n+m)^2] col-major = d/dz (cz' lambda) = sum_i lambda_i Hess c_i(z), overwritten: the second-order constraint term the reference hands to
 // solvers through grad-constraint_jacobians! (src/abstract_constraint.jl:267-280; `∇jacobian!` is zero for Goal / Bound, src/constraints.jl:70-73,
 // :767-770, ForwardDiff for the rest).
@@ -486,7 +571,7 @@ __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const doub
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k1 - con.first) * con.p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
-        con_evaluate(con, goal_values<INST>(P, b, ci), P.n, P.m, x, u, c);
+        con_evaluate_b<INST>(P, con, b, ci, P.n, P.m, x, u, c);
         for (int i = 0; i < con.p; i++) lbar[i] = lam[i] - mu * c[i];
         cone_projection(dualcone(con.sense), lbar, con.p, lp);
         double a = 0, l2 = 0;
@@ -519,7 +604,7 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k0 + 1 - con.first) * p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
-        con_evaluate(con, goal_values<INST>(P, b, ci), n, m, x, u, c);
+        con_evaluate_b<INST>(P, con, b, ci, n, m, x, u, c);
         if (con.diagonal) {   // Goal / Bound: +-1 selector rows (src/constraints.jl:62-68, :757-765) -- row by row, no dense products
             const bool eq = (con.kind == CON_GOAL);
             const int nrow = eq ? p : con.n_max + con.n_min;
@@ -532,7 +617,7 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
             continue;
         }
         double jac[TO_MAXP * TO_MAXNM], Dm[TO_MAXP * TO_MAXP], tmp[TO_MAXP * TO_MAXNM];
-        con_jacobian(con, n, m, x, u, jac);
+        con_jacobian_b<INST>(P, con, b, ci, n, m, x, u, jac);
         for (int i = 0; i < p; i++) lbar[i] = lam[i] - mu * c[i];
         const int dc = dualcone(con.sense);
         cone_projection(dc, lbar, p, lp);

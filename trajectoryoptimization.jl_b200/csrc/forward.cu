@@ -350,27 +350,31 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
                     }
                 } else if (c.ubox) {
                     // u_min <= u <= u_max on every control: rows 0..m-1 = upper, m..2m-1 = lower (src/constraints.jl:738-755)
+                    const double* ca = c.a; const double* cb = c.b;
+                    if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ca = cd.a; cb = cd.b; }
 #pragma unroll
                     for (int i = 0; i < m; i++) {
                         const double lu = st[S::sidx(lo + i, g)], ll = st[S::sidx(lo + m + i, g)];
-                        const double cu = u[i] - c.a[n + i], cl = c.b[n + i] - u[i];
+                        const double cu = u[i] - ca[n + i], cl = cb[n + i] - u[i];
                         const double pu = fmin(0.0, fma(-mu, cu, lu)), pl = fmin(0.0, fma(-mu, cl, ll));
                         a = fma(pu, pu, a); a = fma(pl, pl, a); l2 = fma(lu, lu, l2); l2 = fma(ll, ll, l2);
                         viol = fmax(viol, fmax(cu, cl));
                     }
                 } else {
                     const unsigned mx = c.mask_max, mn = c.mask_min;
+                    const double* ca = c.a; const double* cb = c.b;
+                    if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ca = cd.a; cb = cd.b; }
                     if ((mx | mn) & ((1u << n) - 1u)) {
 #pragma unroll
                         for (int i = 0; i < n; i++) {
-                            if (mx & (1u << i)) { const double lm = st[S::sidx(lo + c.row_max[i], g)]; const double cv = x[i] - c.a[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
-                            if (mn & (1u << i)) { const double lm = st[S::sidx(lo + c.row_min[i], g)]; const double cv = c.b[i] - x[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
+                            if (mx & (1u << i)) { const double lm = st[S::sidx(lo + c.row_max[i], g)]; const double cv = x[i] - ca[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
+                            if (mn & (1u << i)) { const double lm = st[S::sidx(lo + c.row_min[i], g)]; const double cv = cb[i] - x[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
                         }
                     }
 #pragma unroll
                     for (int i = 0; i < m; i++) {
-                        if (mx & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_max[n + i], g)]; const double cv = u[i] - c.a[n + i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
-                        if (mn & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_min[n + i], g)]; const double cv = c.b[n + i] - u[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
+                        if (mx & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_max[n + i], g)]; const double cv = u[i] - ca[n + i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
+                        if (mn & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_min[n + i], g)]; const double cv = cb[n + i] - u[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
                     }
                 }
                 J = fma(a - l2, c.inv2mu, J);
@@ -399,9 +403,11 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
 //     candidate stores ran pass 1 in about half the time);
 //   * RK4 writes the next state over the current one (rk4_step reads x_i for the last time where it writes xn_i), so the loop carries
 //     no x <- xn copies.  (Unrolled by two with x / xn swapping roles instead, the loop took 40 more registers and spilled.)
+// INST: gbox = the instance's control box {u_max_i, u_min_i}, staged for the group by linesearch_pass
 template <int MODEL, int IPB, int G, bool LIE, bool INST>
 __device__ __forceinline__ double rollout_compact(const DevProblem& P, const FwdCompactTab& tab, double* stage, double* ost, const double* prm,
-                                                  int b, int g, int l, unsigned gmask, double alpha, int cbuf, bool& ok, double& viol) {
+                                                  const double2* gbox, int b, int g, int l, unsigned gmask, double alpha, int cbuf, bool& ok,
+                                                  double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     using S = Stage<n, m, IPB, NE>;
     const int N = P.N, buf = P.cur[b];
@@ -520,7 +526,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
 #pragma unroll
             for (int i = 0; i < m; i++) {
                 const double lu = st[S::sidx(S::OFF_L + i, g)], ll = st[S::sidx(S::OFF_L + m + i, g)];
-                const double2 bx = tab.box[i];
+                const double2 bx = INST ? gbox[i] : tab.box[i];
                 const double cu = u[i] - bx.x, cl = bx.y - u[i];
                 const double vu = fma(-mu, cu, lu), vl = fma(-mu, cl, ll);
                 const double pu = vu < 0.0 ? vu : 0.0, pl = vl < 0.0 ? vl : 0.0;
@@ -699,14 +705,24 @@ __device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0,
         bool ok = false;
         double J, viol = 0.0;
         double* prm = nullptr;
+        double2* gbox = nullptr;
         if constexpr (INST) {   // the instance's model parameters, one copy per group behind the rest of the CTA's shared memory
             prm = reinterpret_cast<double*>(fwd_smem + ls_smem_bytes<MODEL, G, PATH, LANES, LIE>()) + g * TO_NPARAM;
             if (l == 0) stage_model_params<INST>(P, b, prm);
+            if constexpr (PATH == FWD_COMPACT) {   // ... and its control box, behind the parameter rows of the CTA's groups
+                gbox = reinterpret_cast<double2*>(reinterpret_cast<double*>(fwd_smem + ls_smem_bytes<MODEL, G, PATH, LANES, LIE>()) + IPB * TO_NPARAM) + g * TO_MAXM;
+                if (tab->box_p != 0)
+                    for (int ci = 0; ci < P.ncon; ci++)
+                        if (P.cons[ci].kind == CON_BOUND) {
+                            const ConData cd = con_data<true>(P, b, ci);
+                            for (int i = l; i < m; i += G) gbox[i] = make_double2(cd.a[n + i], cd.b[n + i]);
+                        }
+            }
             __syncwarp(gmask);
         }
         if constexpr (PATH == FWD_COMPACT) {
             double* ost = stage + FWD_STAGES * S::DOUBLES + (size_t)g * G * FWD_OKNOTS * (n + m);
-            J = rollout_compact<MODEL, IPB, G, LIE, INST>(P, *tab, stage, ost, prm, b, g, l, gmask, alpha, cbuf, ok, viol);
+            J = rollout_compact<MODEL, IPB, G, LIE, INST>(P, *tab, stage, ost, prm, gbox, b, g, l, gmask, alpha, cbuf, ok, viol);
         }
         else if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST>(P, *tab, stage, prm, b, g, l, gmask, alpha, cbuf, ok, viol);
         else J = rollout_generic<MODEL, LIE, INST>(P, prm, b, alpha, cbuf, ok, viol);
@@ -752,7 +768,9 @@ template <int MODEL, int G, int PATH, int LANES, bool LIE = false, bool INST = f
 cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     constexpr int IPB = LANES / G;
     const int blocks = (P.B + IPB - 1) / IPB;
-    const size_t smem = ls_smem_bytes<MODEL, G, PATH, LANES, LIE>() + (INST ? (size_t)IPB * TO_NPARAM * sizeof(double) : 0);
+    static_assert(ls_smem_bytes<MODEL, G, PATH, LANES, LIE>() % 16 == 0, "the parameter rows and the staged boxes (double2) follow the tables");
+    const size_t smem = ls_smem_bytes<MODEL, G, PATH, LANES, LIE>() + (INST ? (size_t)IPB * TO_NPARAM * sizeof(double) : 0)
+                      + (INST && PATH == FWD_COMPACT ? (size_t)IPB * TO_MAXM * sizeof(double2) : 0);
     auto kern = [] {
         if constexpr (PATH == FWD_COMPACT) return k_linesearch_compact<MODEL, G, LANES, LIE, INST>;
         else return k_linesearch<MODEL, G, PATH == FWD_FAST, LANES, LIE, INST>;
@@ -787,7 +805,7 @@ cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int f
 // always been.  It serves every per-instance table; each accessor checks its own (inst_q, goal_values, model_param).
 template <int MODEL, int G, int PATH>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
-    if (P.qr || P.mparams) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);
+    if (P.qr || P.mparams || P.cdata) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);
     return launch_pass_i<MODEL, G, PATH, false>(P, trial0, first_pass, final_pass, s);
 }
 

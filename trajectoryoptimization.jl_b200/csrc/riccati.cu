@@ -220,7 +220,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
     }
 
     // ---- lane-resident AL terms of z_lane (Goal / Bound constraints) ----------------------------------------
-    int tgoal[MAXT];   // (INST) index of a Goal term's value in an instance's row of P.goal, -1 for the other terms
+    int tgoal[MAXT];   // (INST) where a term's bound sits in an instance's rows: i >= 0 in P.goal (Goal), -2 - j in P.cdata (Bound), -1: none
 #pragma unroll
     for (int t = 0; t < MAXT; t++) tgoal[t] = -1;
     if (FASTAL) {
@@ -240,9 +240,10 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     else { row = con.row_min[lane]; bound = con.b[lane]; sign = -1.0; }
                     if (row < 0) continue;
                     if (nterm < MAXT) { sm.tnms[nterm][lane] = -mu * sign; sm.tbound[nterm][lane] = bound; sm.tpk[nterm][lane] = pack_term(con.first, con.last, con.offset + row, con.p, eq); }
-                    if (INST && eq && nterm < MAXT) {
+                    if (INST && nterm < MAXT) {
+                        const int src = eq ? con.goff + row : -2 - (con.cdoff + (side ? n + m : 0) + lane);
 #pragma unroll
-                        for (int t = 0; t < MAXT; t++) if (t == nterm) tgoal[t] = con.goff + row;
+                        for (int t = 0; t < MAXT; t++) if (t == nterm) tgoal[t] = src;
                     }
                     nterm++;
                 }
@@ -266,10 +267,13 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         b = __shfl_sync(0xffffffffu, b, 0);
         if (b >= P.B) break;
         if (retired(P, b)) continue;            // to_solve: not ACTIVE
-        if constexpr (INST && FASTAL) {         // this instance's Goal values into the lane-resident terms (read back by this lane only)
-            if (P.goal && lane < NM) {
+        if constexpr (INST && FASTAL) {         // this instance's Goal / Bound values into the lane-resident terms (read back by this lane only)
+            if (lane < NM) {
 #pragma unroll
-                for (int t = 0; t < MAXT; t++) if (tgoal[t] >= 0) sm.tbound[t][lane] = P.goal[(size_t)b * P.ngoal + tgoal[t]];
+                for (int t = 0; t < MAXT; t++) {
+                    if (P.goal && tgoal[t] >= 0) sm.tbound[t][lane] = P.goal[(size_t)b * P.ngoal + tgoal[t]];
+                    else if (P.cdata && tgoal[t] <= -2) sm.tbound[t][lane] = P.cdata[(size_t)b * P.ncdata + (-2 - tgoal[t])];
+                }
             }
         }
 
@@ -343,8 +347,14 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     if (lane == 0) {
                         double uz[M_];
                         for (int a = 0; a < m; a++) uz[a] = terminal ? 0.0 : U[(size_t)(k1 - 1) * m + a];
-                        con_evaluate(con, n, m, xk, uz, sm.gc);
-                        con_jacobian(con, n, m, xk, uz, sm.gjac);
+                        if constexpr (INST) {
+                            const ConData cd = con_data<true>(P, b, ci);
+                            con_evaluate(con, cd, n, m, xk, uz, sm.gc);
+                            con_jacobian(con, cd, n, m, xk, uz, sm.gjac);
+                        } else {
+                            con_evaluate(con, n, m, xk, uz, sm.gc);
+                            con_jacobian(con, n, m, xk, uz, sm.gjac);
+                        }
                     }
                     __syncwarp();
                     if (lane < p) sm.glbar[lane] = lam[lane] - mu * sm.gc[lane];
@@ -423,10 +433,12 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                                 const int row = con.row_max[i];
                                 if (row >= 0) { const double lp = lam[row] - mu * (xi - goal_values<INST>(P, b, ci)[row]); gi -= lp; hi += mu; }
                             } else if (con.kind == CON_BOUND) {
+                                const double* ba = con.a; const double* bb = con.b;
+                                if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ba = cd.a; bb = cd.b; }
                                 int row = con.row_max[i];
-                                if (row >= 0) { const double lb = lam[row] - mu * (xi - con.a[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
+                                if (row >= 0) { const double lb = lam[row] - mu * (xi - ba[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
                                 row = con.row_min[i];
-                                if (row >= 0) { const double lb = lam[row] - mu * (con.b[i] - xi); if (lb <= 0) { gi += lb; hi += mu; } }
+                                if (row >= 0) { const double lb = lam[row] - mu * (bb[i] - xi); if (lb <= 0) { gi += lb; hi += mu; } }
                             }
                         }
                         if (cost.diag) sm.S[i * LDS_ + i] = hi; else sm.S[i * LDS_ + i] += hi;
@@ -505,10 +517,12 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                                     const int row = (i < n) ? con.row_max[i] : -1;
                                     if (row >= 0) { const double lp = lam[row] - mu * (zi - goal_values<INST>(P, b, ci)[row]); gi -= lp; hi += mu; }
                                 } else if (con.kind == CON_BOUND) {
+                                    const double* ba = con.a; const double* bb = con.b;
+                                    if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ba = cd.a; bb = cd.b; }
                                     int row = con.row_max[i];
-                                    if (row >= 0) { const double lb = lam[row] - mu * (zi - con.a[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
+                                    if (row >= 0) { const double lb = lam[row] - mu * (zi - ba[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
                                     row = con.row_min[i];
-                                    if (row >= 0) { const double lb = lam[row] - mu * (con.b[i] - zi); if (lb <= 0) { gi += lb; hi += mu; } }
+                                    if (row >= 0) { const double lb = lam[row] - mu * (bb[i] - zi); if (lb <= 0) { gi += lb; hi += mu; } }
                                 }
                             }
                         }
@@ -999,7 +1013,7 @@ cudaError_t launch_riccati_t(const DevProblem& P, int* work_counter, cudaStream_
 template <int N_, int M_>
 cudaError_t launch_riccati_nm(const DevProblem& P, int* work_counter, cudaStream_t s) {
     const bool fastal = riccati_fastal(P);
-    if (P.qr) return fastal ? launch_riccati_t<N_, M_, true, true>(P, work_counter, s) : launch_riccati_t<N_, M_, false, true>(P, work_counter, s);
+    if (P.qr || P.cdata) return fastal ? launch_riccati_t<N_, M_, true, true>(P, work_counter, s) : launch_riccati_t<N_, M_, false, true>(P, work_counter, s);
     return fastal ? launch_riccati_t<N_, M_, true, false>(P, work_counter, s) : launch_riccati_t<N_, M_, false, false>(P, work_counter, s);
 }
 

@@ -145,12 +145,12 @@ __global__ void __launch_bounds__(128) k_expansion_rec(const DevProblem P) {
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
         const bool eq = (con.kind == CON_GOAL);
-        const double* ga = goal_values<INST>(P, b, ci);
+        const ConData cd = con_data<INST>(P, b, ci);
         const int nrow = eq ? con.p : con.n_max + con.n_min;
         for (int r = 0; r < nrow; r++) {
             const int j = eq ? con.inds[r] : (r < con.n_max ? con.a_max[r] : con.a_min[r - con.n_max]);
             const bool lower = !eq && r >= con.n_max;
-            const double cv = eq ? z[j] - ga[r] : (lower ? con.b[j] - z[j] : z[j] - con.a[j]);
+            const double cv = eq ? z[j] - cd.a[r] : (lower ? cd.b[j] - z[j] : z[j] - cd.a[j]);
             const double lb = lam[r] - mu * cv;
             if ((eq || lb <= 0.0) && j < lim) { g[j] -= lower ? -lb : lb; h[j] += mu; }
         }
@@ -599,7 +599,7 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_riccati_frag(const DevProb
 }  // namespace
 
 cudaError_t launch_expansion_rec(const DevProblem& P, cudaStream_t s) {
-    if (P.qr) k_expansion_rec<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
+    if (P.qr || P.cdata) k_expansion_rec<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     else k_expansion_rec<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }

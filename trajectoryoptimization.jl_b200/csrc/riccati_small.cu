@@ -47,8 +47,9 @@ __device__ __forceinline__ void expand_knot(const DevProblem& P, int b, int k0, 
         if (k0 + 1 < con.first || k0 + 1 > con.last) continue;
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k0 + 1 - con.first) * con.p;
+        const ConData cd = con_data<INST>(P, b, ci);
         if (con.kind == CON_GOAL) {
-            const double* ga = goal_values<INST>(P, b, ci);
+            const double* ga = cd.a;
             for (int r = 0; r < con.p; r++) {
                 const int j = con.inds[r];
 #pragma unroll
@@ -59,13 +60,13 @@ __device__ __forceinline__ void expand_knot(const DevProblem& P, int b, int k0, 
                 const int j = con.a_max[r];
                 if (j >= lim) continue;
 #pragma unroll
-                for (int i = 0; i < nm; i++) if (i == j) { const double lb = lam[r] - mu * (z[i] - con.a[j]); if (lb <= 0.0) { g[i] -= lb; H[i * nm + i] += mu; } }
+                for (int i = 0; i < nm; i++) if (i == j) { const double lb = lam[r] - mu * (z[i] - cd.a[j]); if (lb <= 0.0) { g[i] -= lb; H[i * nm + i] += mu; } }
             }
             for (int r = 0; r < con.n_min; r++) {
                 const int j = con.a_min[r];
                 if (j >= lim) continue;
 #pragma unroll
-                for (int i = 0; i < nm; i++) if (i == j) { const double lb = lam[con.n_max + r] - mu * (con.b[j] - z[i]); if (lb <= 0.0) { g[i] += lb; H[i * nm + i] += mu; } }
+                for (int i = 0; i < nm; i++) if (i == j) { const double lb = lam[con.n_max + r] - mu * (cd.b[j] - z[i]); if (lb <= 0.0) { g[i] += lb; H[i * nm + i] += mu; } }
             }
         }
     }
@@ -245,7 +246,7 @@ __global__ void __maxnreg__(255) k_riccati_small(const DevProblem P) {
 
 template <int N_, int M_>
 cudaError_t launch_small(const DevProblem& P, cudaStream_t s) {
-    if (P.qr) k_riccati_small<N_, M_, true><<<(P.B + 31) / 32, 32, 0, s>>>(P);
+    if (P.qr || P.cdata) k_riccati_small<N_, M_, true><<<(P.B + 31) / 32, 32, 0, s>>>(P);
     else k_riccati_small<N_, M_, false><<<(P.B + 31) / 32, 32, 0, s>>>(P);
     return cudaGetLastError();
 }

@@ -157,7 +157,14 @@ cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s) {
 // + the AL terms of the Goal / Bound rows acting on z_i (src/constraints.jl:55-68, :738-765; projection on the dual cone src/cones.jl:96-145).
 // The compact problem class only (P.compact): every cost diagonal, every constraint Goal or Bound, at most TO_EXP_MAXT rows per entry
 // (the host-built table P.exptab; walking the constraint descriptors per thread instead adds work comparable to the RK4 itself).
-// (INST: the linear cost terms and Goal bounds of instance b)
+// The bound of term t of z entry i for instance b: its row of DevProblem::goal (Goal) or cdata (Bound) when those exist, else `shared`
+__device__ __forceinline__ double exp_term_bound(const DevProblem& P, const ExpTab& tab, int b, int t, int i, double shared) {
+    const int gi = tab.goal[t][i];
+    if (P.goal && gi >= 0) return P.goal[(size_t)b * P.ngoal + gi];
+    if (P.cdata && gi <= -2) return P.cdata[(size_t)b * P.ncdata + (-2 - gi)];
+    return shared;
+}
+// (INST: the linear cost terms and Goal / Bound bounds of instance b)
 template <bool INST>
 __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, const ExpTab& tab, int b, int k, int i, double zi, const double* __restrict__ lam_b, double& g, double& h) {
     const int n = P.n;
@@ -174,7 +181,7 @@ __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, con
             const double nms = __ldg(&tab.nms[t][i]);
             const double lam = lam_b[(int)(__ldg(&tab.pky[t][i]) + (unsigned)(k + 1) * ((px >> 24) & 0x7fu))];
             double bound = __ldg(&tab.bound[t][i]);
-            if constexpr (INST) { const int gi = tab.goal[t][i]; if (P.goal && gi >= 0) bound = P.goal[(size_t)b * P.ngoal + gi]; }
+            if constexpr (INST) bound = exp_term_bound(P, tab, b, t, i, bound);
             const double lb = fma(nms, zi - bound, lam);          // lambda - mu c
             if ((px >> 31) || lb <= 0.0) { g += (nms < 0.0) ? -lb : lb; h += fabs(nms); }   // g -= sign lb ; h += mu
         }
@@ -415,11 +422,9 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
         const double* __restrict__ Ub = traj_U(P, buf, b);
         const double* __restrict__ lam_b = P.lambda + (size_t)b * P.lambda_len;
         double* __restrict__ recb = P.REC + ((size_t)b * N + kb) * TO_REC_LEN + TO_REC_G;
-        if constexpr (INST) {                                                         // this instance's Goal bounds into the lane's terms
-            if (P.goal) {
+        if constexpr (INST) {                                                         // this instance's Goal / Bound bounds into the lane's terms
 #pragma unroll
-                for (int t = 0; t < TO_EXP_MAXT; t++) { const int gi = tab.goal[t][i]; if (gi >= 0) bnd[t] = P.goal[(size_t)b * P.ngoal + gi]; }
-            }
+            for (int t = 0; t < TO_EXP_MAXT; t++) bnd[t] = exp_term_bound(P, tab, b, t, i, tab.bound[t][i]);
         }
         const int nk = (N - kb < 16) ? N - kb : 16;
         const int mycid = (i < nk) ? P.cost_index[kb + i] : 0;                        // lane j <-> knot kb + j (phases B, C; broadcast in phase A)
@@ -526,7 +531,9 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
                         const unsigned rx = __ldg(&tab.pkx[t][n + a]);
                         if ((unsigned)(k + 1) - (rx & 0xfffu) <= ((rx >> 12) & 0xfffu)) {
                             const double rn = __ldg(&tab.nms[t][n + a]);
-                            const double lb = fma(rn, zu[a] - __ldg(&tab.bound[t][n + a]), lu[a][t]);
+                            double bd = __ldg(&tab.bound[t][n + a]);
+                            if constexpr (INST) bd = exp_term_bound(P, tab, b, t, n + a, bd);
+                            const double lb = fma(rn, zu[a] - bd, lu[a][t]);
                             if ((rx >> 31) || lb <= 0.0) { g += (rn < 0.0) ? -lb : lb; h += fabs(rn); }
                         }
                     }
@@ -552,7 +559,7 @@ cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode
     constexpr int GPB = TO_CEXP2_THREADS / 16;                                       // 16-lane groups per CTA
     long long blocks = (units + GPB - 1) / GPB;
     if (blocks < sms) blocks = sms;
-    if (P.qr) k_expansion_rec16b<true><<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
+    if (P.qr || P.cdata) k_expansion_rec16b<true><<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
     else k_expansion_rec16b<false><<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
     return cudaGetLastError();
 }

@@ -114,7 +114,7 @@ __global__ void k_eval_constraints(const DevProblem P, int ci, double* __restric
     const double* x = traj_X(P, P.cur[b], b) + (size_t)(k1 - 1) * P.n;
     const double* u = (k1 == P.N) ? zero_u : traj_U(P, P.cur[b], b) + (size_t)(k1 - 1) * P.m;
     double c[TO_MAXPV];
-    con_evaluate(con, goal_values<INST>(P, b, ci), P.n, P.m, x, u, c);
+    con_evaluate_b<INST>(P, con, b, ci, P.n, P.m, x, u, c);
     for (int i = 0; i < con.p; i++) vals[t * con.p + i] = c[i];
 }
 
@@ -133,6 +133,7 @@ __global__ void k_constraint_hessians(const DevProblem P, int ci, const double* 
     con_hess_vec(con, P.n, P.m, x, u, lam, H + t * w * w);
 }
 
+template <bool INST>
 __global__ void k_constraint_jacobians(const DevProblem P, int ci, double* __restrict__ jac) {
     const DevCon& con = P.cons[ci];
     const int len = con.last - con.first + 1;
@@ -143,7 +144,7 @@ __global__ void k_constraint_jacobians(const DevProblem P, int ci, double* __res
     double zero_u[TO_MAXM] = {0};
     const double* x = traj_X(P, P.cur[b], b) + (size_t)(k1 - 1) * P.n;
     const double* u = (k1 == P.N) ? zero_u : traj_U(P, P.cur[b], b) + (size_t)(k1 - 1) * P.m;
-    con_jacobian(con, P.n, P.m, x, u, jac + t * con.p * (P.n + P.m));
+    con_jacobian_b<INST>(P, con, b, ci, P.n, P.m, x, u, jac + t * con.p * (P.n + P.m));
 }
 
 __global__ void k_projection(int cone, int p, int count, const double* __restrict__ x, double* __restrict__ px, int* err) {
@@ -180,7 +181,7 @@ __global__ void k_al_update(const DevProblem P) {
             const double* u = (k1 == P.N) ? zero_u : U + (size_t)(k1 - 1) * P.m;
             double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
             double* lam = lam_b + con.offset + (size_t)(k1 - con.first) * con.p;
-            con_evaluate(con, goal_values<INST>(P, b, ci), P.n, P.m, x, u, c);
+            con_evaluate_b<INST>(P, con, b, ci, P.n, P.m, x, u, c);
             for (int i = 0; i < con.p; i++) lbar[i] = lam[i] - mu * c[i];
             cone_projection(dualcone(con.sense), lbar, con.p, lp);
             for (int i = 0; i < con.p; i++) lam[i] = fmax(-P.opt.dual_max, fmin(P.opt.dual_max, lp[i]));
@@ -237,17 +238,17 @@ __global__ void k_export_ab(const DevProblem P, double* __restrict__ out) {
 static inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
 cudaError_t launch_cost(const DevProblem& P, double* J, double* Jk, cudaStream_t s) {
-    if (P.qr) k_cost<false, true><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
+    if (P.qr || P.cdata) k_cost<false, true><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
     else k_cost<false, false><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
     return cudaGetLastError();
 }
 cudaError_t launch_merit(const DevProblem& P, double* J, double* viol, cudaStream_t s) {
-    if (P.qr) k_cost<true, true><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
+    if (P.qr || P.cdata) k_cost<true, true><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
     else k_cost<true, false><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
     return cudaGetLastError();
 }
 cudaError_t launch_cost_gradient(const DevProblem& P, double* grad, cudaStream_t s) {
-    if (P.qr) k_cost_gradient<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
+    if (P.qr || P.cdata) k_cost_gradient<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
     else k_cost_gradient<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
     return cudaGetLastError();
 }
@@ -256,13 +257,13 @@ cudaError_t launch_cost_hessian(const DevProblem& P, double* hess, cudaStream_t 
     return cudaGetLastError();
 }
 cudaError_t launch_al_expansion(const DevProblem& P, double* grad, double* hess, cudaStream_t s) {
-    if (P.qr) k_al_expansion<true><<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
+    if (P.qr || P.cdata) k_al_expansion<true><<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
     else k_al_expansion<false><<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
     return cudaGetLastError();
 }
 cudaError_t launch_eval_constraints(const DevProblem& P, int con, double* vals, cudaStream_t s) {
     // the knot-range length is read on the device; size the grid for the worst case N
-    if (P.qr) k_eval_constraints<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
+    if (P.qr || P.cdata) k_eval_constraints<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
     else k_eval_constraints<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
     return cudaGetLastError();
 }
@@ -272,7 +273,8 @@ cudaError_t launch_constraint_hessians(const DevProblem& P, int con, int len, co
     return cudaGetLastError();
 }
 cudaError_t launch_constraint_jacobians(const DevProblem& P, int con, double* jac, cudaStream_t s) {
-    k_constraint_jacobians<<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, jac);
+    if (P.cdata) k_constraint_jacobians<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, jac);
+    else k_constraint_jacobians<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, jac);
     return cudaGetLastError();
 }
 cudaError_t launch_projection(int cone, int p, int count, const double* x, double* px, int* err, cudaStream_t s) {
@@ -288,7 +290,7 @@ cudaError_t launch_hess_projection(int cone, int p, int count, const double* x, 
     return cudaGetLastError();
 }
 cudaError_t launch_al_update(const DevProblem& P, cudaStream_t s) {
-    if (P.qr) k_al_update<true><<<P.B, 128, 0, s>>>(P);
+    if (P.qr || P.cdata) k_al_update<true><<<P.B, 128, 0, s>>>(P);
     else k_al_update<false><<<P.B, 128, 0, s>>>(P);
     return cudaGetLastError();
 }

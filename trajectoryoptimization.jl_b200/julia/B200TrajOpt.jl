@@ -334,6 +334,22 @@ function model_params(p::BatchedProblem, nparams::Integer)
     check(p.h, ccall((:to_get_model_params, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}), p.h, P))
     P
 end
+# per-instance constraint data: column b of D (len, B) is instance b's data of constraint `con` (1-based), in the layout of
+# to_set_constraint_data (Bound z_max | z_min, Linear b, Circle xc | yc | r, Sphere xc | yc | zc | r, Norm val, Collision radius)
+function constraint_data_len(p::BatchedProblem, con::Integer)
+    len = Ref{Int32}(0)
+    check(p.h, ccall((:to_constraint_data_len, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Int32}), p.h, con - 1, len))
+    Int(len[])
+end
+function set_constraint_data!(p::BatchedProblem, con::Integer, D::AbstractMatrix)
+    size(D) == (constraint_data_len(p, con), p.B) || throw(DimensionMismatch("D must be (len, B)"))
+    check(p.h, ccall((:to_set_constraint_data, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}), p.h, con - 1, Matrix{Float64}(D)))
+end
+function constraint_data(p::BatchedProblem, con::Integer)
+    D = Matrix{Float64}(undef, constraint_data_len(p, con), p.B)
+    check(p.h, ccall((:to_get_constraint_data, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}), p.h, con - 1, D))
+    D
+end
 
 # ---- what Altro.jl's iLQR / AL loop does with the API above, fused on the device ------------------------------
 expand!(p::BatchedProblem) = check(p.h, ccall((:to_expand, libb200), Cint, (Ptr{Cvoid},), p.h))
