@@ -17,9 +17,9 @@ pytestmark = [pytest.mark.gpu,
 G = 3
 
 
-def _generic_spheres(B=48, cls=None):
+def _generic_spheres(B=48, cls=None, goal=False):
     """DoubleIntegrator(2) with a Sphere field on (x, y, vx), a Collision and a Linear constraint: the generic line search and general
-    constraint rows"""
+    constraint rows (goal: and a Goal on the last knot)"""
     cls = cls or TO.Problem
     model = TO.DoubleIntegrator(2)
     n, m, N = 4, 2, 21
@@ -30,6 +30,8 @@ def _generic_spheres(B=48, cls=None):
     TO.add_constraint(cons, TO.CollisionConstraint(n, [1], [2], 0.1), (2, N - 1))
     TO.add_constraint(cons, TO.LinearConstraint(n, m, np.array([[1.0, 1.0]]), [6.0], TO.Inequality(), "control"), (1, N - 1))
     TO.add_constraint(cons, TO.BoundConstraint(n, m, u_min=-8, u_max=8), (1, N - 1))
+    if goal:
+        TO.add_constraint(cons, TO.GoalConstraint(xf), N)
     r = np.random.default_rng(3)
     p = cls(model, obj, np.zeros((B, n)), 3.0, xf=xf, constraints=cons)
     TO.initial_controls(p, 0.3 * r.standard_normal((B, N - 1, m)))
@@ -411,6 +413,70 @@ def test_refusals_leave_the_table_as_it_was():
     if iq is not None:
         assert lie._lib.to_set_constraint_data(lie._h, iq, C._dp(np.zeros((4, 4)))) == C.TO_EINVAL
     lie.close()
+
+
+# a Goal next to data-carrying constraints, on the record path (ExpTab) and on the generic path
+GOAL_PATHS = {"quadrotor_rec": PATHS["quadrotor_rec"],
+              "double_integrator_spheres_generic": (lambda cls: _generic_spheres(48, cls, goal=True), {})}
+
+
+def _goals(p, seed):
+    rng = np.random.default_rng(seed)
+    out = []
+    for _ in range(G):
+        g = np.array(p.xf, dtype=float); g[:2] += rng.uniform(-0.3, 0.3, 2); out.append(g)
+    return out
+
+
+@pytest.mark.parametrize("path", sorted(GOAL_PATHS))
+def test_shared_goal_after_instance_data(path):
+    """per-instance data on every data-carrying constraint, then a shared set_goal_state: every instance goes to the new goal, and keeps its data.
+    objective=False: a new goal for the cost objects would rebuild the handle from them (set_LQR_goal!), this one reaches the handle as it is"""
+    factory, opts = GOAL_PATHS[path]
+    per = factory(None)
+    if opts:
+        TO.set_options(per, **opts)
+    sets = _data_sets(per, seed=17)
+    cons = per.constraints.constraints
+    igoal = next(j for j, c in enumerate(cons) if isinstance(c, TO.GoalConstraint))
+    g = _goals(per, 19)[0]
+    shared = []
+    for s in sets:   # each with a Goal object of its own: set_goal_state assigns its xf
+        q = _rebuilt(per, {igoal: copy.copy(cons[igoal]), **{j: _con_with(cons[j], row) for j, row in s.items()}}, opts)
+        TO.set_goal_state(q, g, objective=False)
+        shared.append(q)
+    for j in sets[0]:
+        TO.set_constraint_data(per, j, np.stack([sets[b % G][j] for b in range(per.B)]))
+    TO.set_goal_state(per, g, objective=False)
+    assert np.array_equal(TO.constraint_data(per, igoal), np.tile(cons[igoal].xf, (per.B, 1)))
+    _compare_pipeline(per, shared, f"{path}: instance data, then a shared goal")
+    for p in [per] + shared:
+        p.close()
+
+
+@pytest.mark.parametrize("path", sorted(GOAL_PATHS))
+def test_instance_goal_values_then_bound_data(path):
+    """per-instance Goal values, then per-instance Bound data: the Bound call keeps the Goal rows"""
+    factory, opts = GOAL_PATHS[path]
+    per = factory(None)
+    if opts:
+        TO.set_options(per, **opts)
+    cons = per.constraints.constraints
+    igoal = next(j for j, c in enumerate(cons) if isinstance(c, TO.GoalConstraint))
+    ibox = next(j for j, c in enumerate(cons) if isinstance(c, TO.BoundConstraint))
+    goal = cons[igoal]
+    vals = [g[goal.inds - 1] for g in _goals(per, 23)]
+    boxes = [s[ibox] for s in _data_sets(per, seed=29)]
+    shared = []
+    for j in range(G):
+        gc = copy.copy(goal); gc.xf = vals[j].copy()
+        shared.append(_rebuilt(per, {igoal: gc, ibox: _con_with(cons[ibox], boxes[j])}, opts))
+    TO.set_constraint_data(per, igoal, np.stack([vals[b % G] for b in range(per.B)]))
+    TO.set_constraint_data(per, ibox, np.stack([boxes[b % G] for b in range(per.B)]))
+    assert np.array_equal(TO.constraint_data(per, igoal), np.stack([vals[b % G] for b in range(per.B)]))
+    _compare_pipeline(per, shared, f"{path}: instance Goal values, then instance Bound data")
+    for p in [per] + shared:
+        p.close()
 
 
 def test_goal_routes_to_the_goal_values():

@@ -1190,30 +1190,21 @@ class Problem:
         # Per-instance state is carried over row by row.  The later change wins: a cost mutated since the handle was built, or a Goal
         # constraint whose xf changed since the per-instance call, takes its new (shared) value in every instance; a constraint added
         # since keeps the value it was built with.
-        carry, goal_carry = {}, {}
+        carry = {}
         if getattr(self, "_inst", False):
             q, r = np.empty((self.B, len(self._cost_objs), self.n)), np.empty((self.B, len(self._cost_objs), self.m))
             self._raw_call("to_get_cost_terms", K._dp(q), K._dp(r))
             built = self._sig[1]
             carry = {id(c): (q[:, j].copy(), r[:, j].copy()) for j, c in enumerate(self._cost_objs) if getattr(c, "_version", 0) == built[j]}
-            snap = getattr(self, "_goal_snap", {})
-            live = {id(c): c for c in self.constraints.constraints}
-            for j, cid in enumerate(self._sig[2]):
-                con = live.get(cid)
-                if cid in snap and con is not None and np.array_equal(np.asarray(con.xf), snap[cid]):
-                    vals = np.empty((self.B, con.p))
-                    self._raw_call("to_get_goal_values", j, K._dp(vals))
-                    goal_carry[cid] = vals
-        cdata_carry = {}   # per-instance constraint data: the rows of every constraint unchanged since the call
-        csnap = getattr(self, "_cdata_snap", {})
-        if csnap:
-            live = {id(c): c for c in self.constraints.constraints}
-            for j, cid in enumerate(self._sig[2]):
-                con = live.get(cid)
-                if cid in csnap and con is not None and np.array_equal(_con_row(con)[1], csnap[cid]):
-                    rows = np.empty((self.B, csnap[cid].size))
-                    self._raw_call("to_get_constraint_data", j, K._dp(rows))
-                    cdata_carry[cid] = rows
+        con_carry = {}   # per-instance constraint rows (Goal values, constraint data): those of every constraint unchanged since the call
+        snap = getattr(self, "_con_snap", {})
+        live = {id(c): c for c in self.constraints.constraints}
+        for j, cid in enumerate(self._sig[2]):
+            con = live.get(cid)
+            if cid in snap and con is not None and np.array_equal(_con_snap_row(con), snap[cid]):
+                rows = np.empty((self.B, snap[cid].size))
+                self._raw_call(_con_rows_call(con, "get"), j, K._dp(rows))
+                con_carry[cid] = rows
         mparams = None
         if getattr(self, "_mparams", False):   # per-instance model parameters: carried over as they are
             mparams = np.empty((self.B, len(self.model.params)))
@@ -1222,7 +1213,7 @@ class Problem:
         self.spec = self._make_spec(self._dt, float(t[0]))
         self._open()
         self._sig = self._signature()
-        self._inst = bool(carry or goal_carry)
+        self._inst = bool(carry)
         if carry:
             q, r = np.empty((self.B, len(self._cost_objs), self.n)), np.empty((self.B, len(self._cost_objs), self.m))
             self._raw_call("to_get_cost_terms", K._dp(q), K._dp(r))
@@ -1231,13 +1222,9 @@ class Problem:
                     q[:, j], r[:, j] = carry[id(c)]
             self._raw_call("to_set_cost_terms", K._dp(q), K._dp(r))
         for j, c in enumerate(self.constraints.constraints):
-            if id(c) in goal_carry:
-                self._raw_call("to_set_goal_values", j, K._dp(goal_carry[id(c)]))
-        self._goal_snap = {cid: v for cid, v in getattr(self, "_goal_snap", {}).items() if cid in goal_carry}
-        for j, c in enumerate(self.constraints.constraints):
-            if id(c) in cdata_carry:
-                self._raw_call("to_set_constraint_data", j, K._dp(cdata_carry[id(c)]))
-        self._cdata_snap = {cid: v for cid, v in csnap.items() if cid in cdata_carry}
+            if id(c) in con_carry:
+                self._raw_call(_con_rows_call(c, "set"), j, K._dp(con_carry[id(c)]))
+        self._con_snap = {cid: v for cid, v in snap.items() if cid in con_carry}
         if mparams is not None:
             self._raw_call("to_set_model_params", K._dp(mparams), int(mparams.shape[1]))
         self._raw_call("to_set_initial_state", K._dp(self.x0))
@@ -1400,9 +1387,11 @@ def set_goal_state(prob, xf, objective=True, constraint=True):   # set_goal_stat
         if xf.shape != (prob.B, prob.n):
             raise DimensionMismatch(f"set_goal_state!: xf has shape {xf.shape}, expected ({prob.n},) or ({prob.B}, {prob.n})")
         prob._call("to_set_goal_states", K._dp(xf), int(objective), int(constraint))
-        prob._inst = True
+        if objective:
+            prob._inst = True
         if constraint:   # the Goal constraints that now hold per-instance values, with the xf they had (a later change to it wins)
-            prob._goal_snap = {id(c): np.array(c.xf, dtype=float) for c in prob.constraints if isinstance(c, GoalConstraint)}
+            prob._con_snap = {**getattr(prob, "_con_snap", {}),
+                              **{id(c): _con_snap_row(c) for c in prob.constraints if isinstance(c, GoalConstraint)}}
         prob.xf = xf.copy()
         return
     if objective:
@@ -1414,8 +1403,9 @@ def set_goal_state(prob, xf, objective=True, constraint=True):   # set_goal_stat
             if isinstance(con, GoalConstraint):
                 con.xf = xf[con.inds - 1].copy() if xf.size != con.xf.size else xf.copy()
     prob.xf = xf.copy()
-    if constraint:
-        prob._goal_snap = {}       # every instance takes the shared Goal values
+    if constraint:   # every instance takes the shared Goal values
+        goals = {id(c) for c in prob.constraints if isinstance(c, GoalConstraint)}
+        prob._con_snap = {cid: v for cid, v in getattr(prob, "_con_snap", {}).items() if cid not in goals}
     prob._call("to_set_goal_state", K._dp(xf), int(objective), int(constraint))
 
 
@@ -1524,6 +1514,16 @@ def _con_row(con):
     return spec, np.concatenate([np.atleast_1d(np.asarray(spec[f], dtype=np.float64)).ravel() for f in fields])
 
 
+def _con_snap_row(con):
+    """the row ``con`` holds in every instance until a per-instance call: a Goal's ``xf``, another kind's data (``_con_row``)"""
+    return np.array(con.xf, dtype=float) if isinstance(con, GoalConstraint) else _con_row(con)[1]
+
+
+def _con_rows_call(con, verb):
+    """the C call that sets (``verb = "set"``) or reads (``"get"``) the per-instance rows of ``con``: a Goal's values or another kind's data"""
+    return f"to_{verb}_goal_values" if isinstance(con, GoalConstraint) else f"to_{verb}_constraint_data"
+
+
 def _con_and_index(prob, con):
     """(index, constraint) of ``con``: an index into the problem's constraint list or one of its constraint objects"""
     j = _con_index(prob, con)
@@ -1597,24 +1597,15 @@ def set_constraint_data(prob, con, rows):
     are left as they are; a later in-place change to one of them, picked up when the handle is rebuilt, wins in every instance.
     An ``IndexedConstraint`` (a constraint applied to a slice of a larger model) keeps its data shared: ``ArgumentError``."""
     j, con, out = _constraint_data_rows(prob, con, rows)
-    if isinstance(con, GoalConstraint):
-        prob._call("to_set_goal_values", j, K._dp(out))
-        prob._inst = True
-        prob._goal_snap = {**getattr(prob, "_goal_snap", {}), id(con): np.array(con.xf, dtype=float)}
-        return
-    prob._call("to_set_constraint_data", j, K._dp(out))
-    prob._cdata_snap = {**getattr(prob, "_cdata_snap", {}), id(con): _con_row(con)[1]}
+    prob._call(_con_rows_call(con, "set"), j, K._dp(out))
+    prob._con_snap = {**getattr(prob, "_con_snap", {}), id(con): _con_snap_row(con)}
 
 
 def constraint_data(prob, con):
     """The data of constraint ``con`` of every instance, ``[B, len]`` (the shared data broadcast when none was set)."""
     j, con = _con_and_index(prob, con)
-    if isinstance(con, GoalConstraint):
-        out = np.empty((prob.B, con.p))
-        prob._call("to_get_goal_values", j, K._dp(out))
-        return out
-    out = np.empty((prob.B, _con_row(con)[1].size))
-    prob._call("to_get_constraint_data", j, K._dp(out))
+    out = np.empty((prob.B, _con_snap_row(con).size))
+    prob._call(_con_rows_call(con, "get"), j, K._dp(out))
     return out
 
 

@@ -52,11 +52,11 @@ struct to_handle {
     double* d_merit2 = nullptr;   // {sum J, max viol}
     int* d_work = nullptr;
     ExpTab* d_exptab = nullptr;   // (frag) AL rows per z entry, rebuilt with the constraint tables / penalties
-    // per-instance linear cost terms / Goal values (DevProblem::qr / goal), empty until the first per-instance call; the host copy is the
-    // authoritative one and goes to the device whole after every change
-    std::vector<double> h_qr, h_goal;
-    std::vector<double> h_mparams;   // per-instance model parameters (DevProblem::mparams), [B][TO_NPARAM]; empty until to_set_model_params
-    std::vector<double> h_cdata;     // per-instance constraint data (DevProblem::cdata), [B][ncdata]; empty until to_set_constraint_data
+    // host copies of the per-instance tables, empty until the first per-instance call (commit_rows); each goes to the device whole after every change
+    std::vector<double> h_qr;        // linear cost terms (DevProblem::qr), [B][ncost][n+m]
+    std::vector<double> h_mparams;   // model parameters (DevProblem::mparams), [B][TO_NPARAM]
+    std::vector<double> h_cdata;     // constraint data and Goal values (DevProblem::cdata), [B][ncdata]
+    std::vector<double> stage;       // the rows a setter is building, committed by commit_rows (kept to reuse its allocation)
     int* d_fragerr = nullptr;     // sticky error word of that kernel (queue overflow / spin limit), read by to_synchronize
     double* d_fragpool = nullptr; // gains of its speculative regularisation candidates
     int* d_fragq = nullptr;       // work queue of the register-resident Riccati kernel (riccati_frag.cu)
@@ -117,7 +117,7 @@ int upload_exptab(to_handle* h) {
     const int nm = h->P.n + h->P.m, n = h->P.n;
     for (int i = 0; i < nm; i++) {
         int nterm = 0;
-        for (int k = 0; k < TO_EXP_MAXT; k++) { t.nms[k][i] = -1.0; t.pkx[k][i] = 4095u; t.goal[k][i] = -1; }      // empty knot range
+        for (int k = 0; k < TO_EXP_MAXT; k++) { t.nms[k][i] = -1.0; t.pkx[k][i] = 4095u; t.inst[k][i] = -1; }      // empty knot range
         for (size_t ci = 0; ci < h->h_cons.size(); ci++) {
             const DevCon& con = h->h_cons[ci];
             if (!con.diagonal) continue;
@@ -132,7 +132,7 @@ int upload_exptab(to_handle* h) {
                     t.nms[nterm][i] = -mu * sign; t.bound[nterm][i] = bound;
                     t.pkx[nterm][i] = (unsigned)con.first | ((unsigned)(con.last - con.first) << 12) | ((unsigned)con.p << 24) | (eq ? 0x80000000u : 0u);
                     t.pky[nterm][i] = (unsigned)(con.offset + row - con.first * con.p);
-                    t.goal[nterm][i] = eq ? con.goff + row : -2 - (con.cdoff + (side ? nm : 0) + i);
+                    t.inst[nterm][i] = con.cdoff + (eq ? row : (side ? nm : 0) + i);
                 }
                 nterm++;
             }
@@ -149,10 +149,18 @@ void lqr_linear_term(const double* M, int dim, const double* xf, double* out) {
     for (int i = 0; i < dim; i++) { double t = 0; for (int j = 0; j < dim; j++) t += M[j * dim + i] * xf[j]; out[i] = -t; }
 }
 
-int upload_inst(to_handle* h) {
-    CU(h, cudaMemcpyAsync(const_cast<double*>(h->P.qr), h->h_qr.data(), sizeof(double) * h->h_qr.size(), cudaMemcpyHostToDevice, h->stream));
-    CU(h, cudaMemcpyAsync(const_cast<double*>(h->P.goal), h->h_goal.data(), sizeof(double) * h->h_goal.size(), cudaMemcpyHostToDevice, h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));   // the host tables may change right after
+// Commits the complete rows staged in h->stage as the per-instance table whose host copy is `host` and whose device pointer is `dev`
+// (DevProblem::qr / mparams / cdata): the device buffer is allocated on first use, the rows are copied, and only once the device holds them
+// do they become the host copy and is the pointer published.  A failed call leaves the table, or its absence, as it was: no kernel reads
+// rows the device lacks and no getter reports them.
+int commit_rows(to_handle* h, std::vector<double>& host, const double*& dev) {
+    std::vector<double>& rows = h->stage;
+    double* d = const_cast<double*>(dev);
+    if (!d) { int rc = dalloc(h, &d, rows.size()); if (rc) return rc; }
+    CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));   // the staged rows are the source of the copy
+    host.swap(rows);
+    dev = d;
     return TO_OK;
 }
 
@@ -286,9 +294,10 @@ int build_cost(to_handle* h, const to_cost_spec& tc, int n, int m, DevCost& c) {
     return TO_OK;
 }
 
-// doubles of constraint c in an instance's row of DevProblem::cdata (0: no per-instance data; a Goal has its own table)
-int con_data_len(const DevCon& c, int nm) {
+// doubles of constraint c in an instance's row of DevProblem::cdata (0: no per-instance data)
+int con_row_len(const DevCon& c, int nm) {
     switch (c.kind) {
+        case CON_GOAL: return c.p;
         case CON_BOUND: return 2 * nm;
         case CON_LINEAR: return c.p;
         case CON_CIRCLE: return 3 * c.p;
@@ -297,10 +306,13 @@ int con_data_len(const DevCon& c, int nm) {
     }
     return 0;
 }
+// ... as to_constraint_data_len reports it: a Goal's values are set with to_set_goal_values, not to_set_constraint_data
+int con_data_len(const DevCon& c, int nm) { return c.kind == CON_GOAL ? 0 : con_row_len(c, nm); }
 // the shared data of constraint c in the layout of its row (common.cuh con_data)
 void con_shared_row(const DevCon& c, int nm, double* row) {
     const int p = c.p;
     switch (c.kind) {
+        case CON_GOAL: std::memcpy(row, c.a, sizeof(double) * p); break;
         case CON_BOUND: std::memcpy(row, c.a, sizeof(double) * nm); std::memcpy(row + nm, c.b, sizeof(double) * nm); break;
         case CON_LINEAR: std::memcpy(row, c.b, sizeof(double) * p); break;
         case CON_CIRCLE: case CON_SPHERE: {
@@ -582,8 +594,7 @@ int to_create(const to_spec* s, to_handle** out) {
         if (rc) return bail(rc);
         h->h_cons[i].offset = P.lambda_len;
         P.lambda_len += (h->h_cons[i].last - h->h_cons[i].first + 1) * h->h_cons[i].p;
-        if (h->h_cons[i].kind == CON_GOAL) { h->h_cons[i].goff = P.ngoal; P.ngoal += h->h_cons[i].p; }
-        const int clen = con_data_len(h->h_cons[i], n + m);
+        const int clen = con_row_len(h->h_cons[i], n + m);
         h->h_cons[i].cdoff = clen ? P.ncdata : -1; P.ncdata += clen;
         if (!h->h_cons[i].diagonal) P.all_diag_con = 0;
     }
@@ -853,31 +864,32 @@ int to_set_initial_time(to_handle* h, double t0, double* tf_out) {
     if (tf_out) { double t = t0; for (double d : h->h_dt) t += d; *tf_out = t; }
     return TO_OK;
 }
-// ---- per-instance goals (DevProblem::qr / goal) -------------------------------------------------------------
-// The tables are created by the first per-instance call, filled from the shared values; later shared calls write through to every row.
-static int inst_tables(to_handle* h) {
-    if (h->P.qr) return TO_OK;
-    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance goals are not supported on hybrid problems");
-    const int B = h->P.B, ncost = h->P.ncost, n = h->P.n, m = h->P.m, nm = n + m, ngoal = h->P.ngoal;
-    h->h_qr.assign((size_t)B * ncost * nm, 0.0);
-    h->h_goal.assign((size_t)B * std::max(1, ngoal), 0.0);
-    for (int b = 0; b < B; b++) {
+// ---- per-instance goals (DevProblem::qr, and the Goal rows of DevProblem::cdata) ------------------------------------------------------
+// A setter stages the complete new rows of a table in h->stage and commits them (commit_rows).  The first per-instance call creates a table
+// from the shared values; later shared calls write through to every row.
+static int hybrid_goals(to_handle* h) { return fail(h, TO_EINVAL, "per-instance goals are not supported on hybrid problems"); }
+static size_t q_off(const to_handle* h, int b, int cid) { return ((size_t)b * h->P.ncost + cid) * (h->P.n + h->P.m); }
+static size_t cd_off(const to_handle* h, int b, const DevCon& c) { return (size_t)b * h->P.ncdata + c.cdoff; }
+// h->stage := the rows of the cost-term table, or every instance's shared terms when it does not exist yet
+static void stage_qr(to_handle* h) {
+    if (h->P.qr) { h->stage = h->h_qr; return; }
+    const int B = h->P.B, ncost = h->P.ncost, n = h->P.n, m = h->P.m;
+    h->stage.resize((size_t)B * ncost * (n + m));
+    for (int b = 0; b < B; b++)
         for (int ci = 0; ci < ncost; ci++) {
-            double* row = h->h_qr.data() + ((size_t)b * ncost + ci) * nm;
-            std::memcpy(row, h->h_costs[ci].q, sizeof(double) * n);
-            std::memcpy(row + n, h->h_costs[ci].r, sizeof(double) * m);
+            std::memcpy(h->stage.data() + q_off(h, b, ci), h->h_costs[ci].q, sizeof(double) * n);
+            std::memcpy(h->stage.data() + q_off(h, b, ci) + n, h->h_costs[ci].r, sizeof(double) * m);
         }
-        for (const auto& c : h->h_cons)
-            if (c.kind == CON_GOAL) std::memcpy(h->h_goal.data() + (size_t)b * std::max(1, ngoal) + c.goff, c.a, sizeof(double) * c.p);
-    }
-    double *dq = nullptr, *dg = nullptr;
-    int rc = dalloc(h, &dq, h->h_qr.size()); if (rc) return rc;
-    rc = dalloc(h, &dg, h->h_goal.size()); if (rc) return rc;
-    h->P.ngoal = std::max(1, ngoal);      // row stride of the Goal table (a problem without Goal constraints keeps one unused slot)
-    h->P.qr = dq; h->P.goal = dg;
-    return TO_OK;
 }
-static double* inst_q_row(to_handle* h, int b, int cid) { return h->h_qr.data() + ((size_t)b * h->P.ncost + cid) * (h->P.n + h->P.m); }
+// h->stage := the rows of the constraint-data table, or every instance's shared data of every constraint when it does not exist yet
+static void stage_cdata(to_handle* h) {
+    if (h->P.cdata) { h->stage = h->h_cdata; return; }
+    const int nm = h->P.n + h->P.m;
+    h->stage.resize((size_t)h->P.B * h->P.ncdata);
+    for (int b = 0; b < h->P.B; b++)
+        for (const auto& c : h->h_cons)
+            if (c.cdoff >= 0) con_shared_row(c, nm, h->stage.data() + cd_off(h, b, c));
+}
 
 // set_goal_state! src/problem.jl:294-310 with set_LQR_goal! (q = -Q xf; c untouched) src/cost_functions.jl:245-248
 int to_set_goal_state(to_handle* h, const double* xf, int objective, int constraint) {
@@ -891,32 +903,44 @@ int to_set_goal_state(to_handle* h, const double* xf, int objective, int constra
             if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) c.a[i] = xf[c.inds[i]];
     h->J_valid = false;
     int rc = upload_tables(h); if (rc) return rc;
-    if (!h->P.qr) return TO_OK;
-    for (int b = 0; b < h->P.B; b++) {     // the later call wins: every instance takes the shared goal
-        if (objective)
-            for (int ci = 0; ci < h->P.ncost; ci++) std::memcpy(inst_q_row(h, b, ci), h->h_costs[ci].q, sizeof(double) * n);
-        if (constraint)
-            for (const auto& c : h->h_cons)
-                if (c.kind == CON_GOAL) std::memcpy(h->h_goal.data() + (size_t)b * h->P.ngoal + c.goff, c.a, sizeof(double) * c.p);
+    // the later call wins: every instance takes the shared goal
+    if (objective && h->P.qr) {
+        stage_qr(h);
+        for (int b = 0; b < h->P.B; b++)
+            for (int ci = 0; ci < h->P.ncost; ci++) std::memcpy(h->stage.data() + q_off(h, b, ci), h->h_costs[ci].q, sizeof(double) * n);
+        rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
     }
-    return upload_inst(h);
+    if (constraint && h->P.cdata) {
+        stage_cdata(h);
+        for (int b = 0; b < h->P.B; b++)
+            for (const auto& c : h->h_cons)
+                if (c.kind == CON_GOAL) std::memcpy(h->stage.data() + cd_off(h, b, c), c.a, sizeof(double) * c.p);
+        rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
+    }
+    return TO_OK;
 }
 // set_goal_state! per instance: xf [B][n]
 int to_set_goal_states(to_handle* h, const double* xf, int objective, int constraint) {
     JOIN(h);
     if (!h || !xf) return TO_EINVAL;
-    int rc = inst_tables(h); if (rc) return rc;
+    if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
     const int n = h->P.n;
-    for (int b = 0; b < h->P.B; b++) {
-        const double* xb = xf + (size_t)b * n;
-        if (objective)
-            for (int ci = 0; ci < h->P.ncost; ci++) lqr_linear_term(h->h_costs[ci].Q, n, xb, inst_q_row(h, b, ci));
-        if (constraint)
-            for (const auto& c : h->h_cons)
-                if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) h->h_goal[(size_t)b * h->P.ngoal + c.goff + i] = xb[c.inds[i]];
+    if (objective) {
+        stage_qr(h);
+        for (int b = 0; b < h->P.B; b++)
+            for (int ci = 0; ci < h->P.ncost; ci++) lqr_linear_term(h->h_costs[ci].Q, n, xf + (size_t)b * n, h->stage.data() + q_off(h, b, ci));
+        int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
+        h->J_valid = false;
     }
-    h->J_valid = false;
-    return upload_inst(h);
+    if (constraint) {
+        stage_cdata(h);
+        for (int b = 0; b < h->P.B; b++)
+            for (const auto& c : h->h_cons)
+                if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) h->stage[cd_off(h, b, c) + i] = xf[(size_t)b * n + c.inds[i]];
+        int rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
+        h->J_valid = false;
+    }
+    return TO_OK;
 }
 // update_trajectory! per instance: Xref [B][nref][n], Uref [B][nref][m], one start for the batch
 int to_update_trajectories(to_handle* h, const double* Xref, const double* Uref, int32_t nref, int32_t start) {
@@ -924,17 +948,19 @@ int to_update_trajectories(to_handle* h, const double* Xref, const double* Uref,
     if (!h || !Xref || !Uref) return TO_EINVAL;
     const int n = h->P.n, m = h->P.m, N = h->P.N;
     if (start < 1 || start - 1 + N > nref) return fail(h, TO_EDIM, "update_trajectory!: the reference is shorter than start + N - 1");
-    int rc = inst_tables(h); if (rc) return rc;
+    if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
+    stage_qr(h);
     for (int b = 0; b < h->P.B; b++)
         for (int i = 0; i < N; i++) {                   // set_LQR_goal!(obj[i], state(Z[k]), control(Z[k])) of instance b
             const int cid = h->h_cost_index[i];
             const DevCost& c = h->h_costs[cid];
-            double* row = inst_q_row(h, b, cid);
+            double* row = h->stage.data() + q_off(h, b, cid);
             lqr_linear_term(c.Q, n, Xref + ((size_t)b * nref + start - 1 + i) * n, row);
             lqr_linear_term(c.R, m, Uref + ((size_t)b * nref + start - 1 + i) * m, row + n);
         }
+    int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
-    return upload_inst(h);
+    return TO_OK;
 }
 // the linear terms of every cost of every instance: q [B][ncost][n], r [B][ncost][m] (the shared ones broadcast when none are set)
 int to_get_cost_terms(to_handle* h, double* q, double* r) {
@@ -943,8 +969,8 @@ int to_get_cost_terms(to_handle* h, double* q, double* r) {
     const int n = h->P.n, m = h->P.m, ncost = h->P.ncost;
     for (int b = 0; b < h->P.B; b++)
         for (int ci = 0; ci < ncost; ci++) {
-            const double* sq = h->P.qr ? inst_q_row(h, b, ci) : h->h_costs[ci].q;
-            const double* sr = h->P.qr ? inst_q_row(h, b, ci) + n : h->h_costs[ci].r;
+            const double* sq = h->P.qr ? h->h_qr.data() + q_off(h, b, ci) : h->h_costs[ci].q;
+            const double* sr = h->P.qr ? h->h_qr.data() + q_off(h, b, ci) + n : h->h_costs[ci].r;
             std::memcpy(q + ((size_t)b * ncost + ci) * n, sq, sizeof(double) * n);
             std::memcpy(r + ((size_t)b * ncost + ci) * m, sr, sizeof(double) * m);
         }
@@ -957,32 +983,36 @@ int to_get_goal_values(to_handle* h, int32_t con, double* vals) {
     if (con < 0 || con >= (int)h->h_cons.size() || h->h_cons[con].kind != CON_GOAL) return fail(h, TO_EINVAL, "to_get_goal_values: not a Goal constraint");
     const DevCon& c = h->h_cons[con];
     for (int b = 0; b < h->P.B; b++)
-        std::memcpy(vals + (size_t)b * c.p, h->P.goal ? h->h_goal.data() + (size_t)b * h->P.ngoal + c.goff : c.a, sizeof(double) * c.p);
+        std::memcpy(vals + (size_t)b * c.p, h->P.cdata ? h->h_cdata.data() + cd_off(h, b, c) : c.a, sizeof(double) * c.p);
     return TO_OK;
 }
 int to_set_goal_values(to_handle* h, int32_t con, const double* vals) {
     JOIN(h);
     if (!h || !vals) return TO_EINVAL;
     if (con < 0 || con >= (int)h->h_cons.size() || h->h_cons[con].kind != CON_GOAL) return fail(h, TO_EINVAL, "to_set_goal_values: not a Goal constraint");
-    int rc = inst_tables(h); if (rc) return rc;
+    if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
     const DevCon& c = h->h_cons[con];
-    for (int b = 0; b < h->P.B; b++) std::memcpy(h->h_goal.data() + (size_t)b * h->P.ngoal + c.goff, vals + (size_t)b * c.p, sizeof(double) * c.p);
+    stage_cdata(h);
+    for (int b = 0; b < h->P.B; b++) std::memcpy(h->stage.data() + cd_off(h, b, c), vals + (size_t)b * c.p, sizeof(double) * c.p);
+    int rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
     h->J_valid = false;
-    return upload_inst(h);
+    return TO_OK;
 }
 // set_LQR_goal!(obj[k], ...) per instance with the raw terms: q [B][ncost][n], r [B][ncost][m]
 int to_set_cost_terms(to_handle* h, const double* q, const double* r) {
     JOIN(h);
     if (!h || !q || !r) return TO_EINVAL;
-    int rc = inst_tables(h); if (rc) return rc;
+    if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
     const int n = h->P.n, m = h->P.m, ncost = h->P.ncost;
+    h->stage.resize((size_t)h->P.B * ncost * (n + m));    // every row is written
     for (int b = 0; b < h->P.B; b++)
         for (int ci = 0; ci < ncost; ci++) {
-            std::memcpy(inst_q_row(h, b, ci), q + ((size_t)b * ncost + ci) * n, sizeof(double) * n);
-            std::memcpy(inst_q_row(h, b, ci) + n, r + ((size_t)b * ncost + ci) * m, sizeof(double) * m);
+            std::memcpy(h->stage.data() + q_off(h, b, ci), q + ((size_t)b * ncost + ci) * n, sizeof(double) * n);
+            std::memcpy(h->stage.data() + q_off(h, b, ci) + n, r + ((size_t)b * ncost + ci) * m, sizeof(double) * m);
         }
+    int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
-    return upload_inst(h);
+    return TO_OK;
 }
 
 // ---- per-instance model parameters (DevProblem::mparams) ----------------------------------------------------------
@@ -997,7 +1027,8 @@ int to_set_model_params(to_handle* h, const double* params, int32_t nparams) {
     const int np = model_nparams(model);
     if (nparams != np)
         return fail(h, TO_EDIM, "to_set_model_params: the model takes " + std::to_string(np) + " parameters per instance, got " + std::to_string(nparams));
-    std::vector<double> rows((size_t)B * TO_NPARAM, 0.0);
+    std::vector<double>& rows = h->stage;
+    rows.assign((size_t)B * TO_NPARAM, 0.0);
     for (int b = 0; b < B; b++) {
         double* row = rows.data() + (size_t)b * TO_NPARAM;
         for (int i = 0; i < np; i++) {
@@ -1011,14 +1042,7 @@ int to_set_model_params(to_handle* h, const double* params, int32_t nparams) {
         }
         complete_model_params(model, row);
     }
-    if (!h->P.mparams) {
-        double* d = nullptr;
-        int rc = dalloc(h, &d, rows.size()); if (rc) return rc;
-        h->P.mparams = d;
-    }
-    h->h_mparams.swap(rows);
-    CU(h, cudaMemcpyAsync(const_cast<double*>(h->P.mparams), h->h_mparams.data(), sizeof(double) * h->h_mparams.size(), cudaMemcpyHostToDevice, h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));   // a later call replaces the host rows
+    int rc = commit_rows(h, h->h_mparams, h->P.mparams); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1071,24 +1095,9 @@ int to_set_constraint_data(to_handle* h, int32_t con, const double* data) {
                 return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, 0) + ": NormConstraint value must be non-negative");   // src/constraints.jl:451
         }
     }
-    // the new rows are staged and become the host table only once the device holds them: if a copy fails, to_get_constraint_data still
-    // reports the rows of the last successful call (or the shared data, and no table exists)
-    const int nc = h->P.ncdata;
-    std::vector<double> rows;
-    if (h->P.cdata) rows = h->h_cdata;
-    else {
-        rows.resize((size_t)B * nc);
-        for (int b = 0; b < B; b++)
-            for (const auto& k : h->h_cons)
-                if (k.cdoff >= 0) con_shared_row(k, nm, rows.data() + (size_t)b * nc + k.cdoff);
-    }
-    for (int b = 0; b < B; b++) std::memcpy(rows.data() + (size_t)b * nc + c.cdoff, data + (size_t)b * len, sizeof(double) * len);
-    double* d = const_cast<double*>(h->P.cdata);
-    if (!d) { int rc = dalloc(h, &d, rows.size()); if (rc) return rc; }
-    CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));   // `rows` is the source of the copy
-    h->h_cdata.swap(rows);
-    h->P.cdata = d;
+    stage_cdata(h);
+    for (int b = 0; b < B; b++) std::memcpy(h->stage.data() + cd_off(h, b, c), data + (size_t)b * len, sizeof(double) * len);
+    int rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1103,7 +1112,7 @@ int to_get_constraint_data(to_handle* h, int32_t con, double* data) {
     std::vector<double> shared(len);
     con_shared_row(c, nm, shared.data());
     for (int b = 0; b < h->P.B; b++)
-        std::memcpy(data + (size_t)b * len, h->P.cdata ? h->h_cdata.data() + (size_t)b * h->P.ncdata + c.cdoff : shared.data(), sizeof(double) * len);
+        std::memcpy(data + (size_t)b * len, h->P.cdata ? h->h_cdata.data() + cd_off(h, b, c) : shared.data(), sizeof(double) * len);
     return TO_OK;
 }
 
@@ -1121,13 +1130,14 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     int rc = upload_tables(h); if (rc) return rc;
     if (!h->P.qr) return TO_OK;
+    stage_qr(h);
     for (int b = 0; b < h->P.B; b++)                    // the later call wins: every instance takes the shared reference
         for (int i = 0; i < N; i++) {
             const int cid = h->h_cost_index[i];
-            std::memcpy(inst_q_row(h, b, cid), h->h_costs[cid].q, sizeof(double) * n);
-            std::memcpy(inst_q_row(h, b, cid) + n, h->h_costs[cid].r, sizeof(double) * m);
+            std::memcpy(h->stage.data() + q_off(h, b, cid), h->h_costs[cid].q, sizeof(double) * n);
+            std::memcpy(h->stage.data() + q_off(h, b, cid) + n, h->h_costs[cid].r, sizeof(double) * m);
         }
-    return upload_inst(h);
+    return commit_rows(h, h->h_qr, h->P.qr);
 }
 int to_shift_trajectory(to_handle* h, int32_t steps) {
     JOIN(h);
@@ -1584,10 +1594,9 @@ int to_kernel_choice(const to_handle* h, int32_t* choice) {
     choice[TO_CHOICE_FASTAL] = ((bk == KC_BK_WARP_MMA || bk == KC_BK_WARP_DFMA) && riccati_fastal(P)) ? 1 : 0;
     choice[TO_CHOICE_REC_FUSED] = (record_path(P) && rec_fused(P)) ? 1 : 0;
     choice[TO_CHOICE_LATE_LIST] = P.late_list ? 1 : 0;
-    choice[TO_CHOICE_INST_FORWARD] = (P.qr || P.mparams || P.cdata) ? 1 : 0;   // launch_pass
-    choice[TO_CHOICE_INST_BACKWARD] = (P.qr || P.cdata) ? 1 : 0;                // k_riccati, k_riccati_small, k_expansion_rec(16b), k_expansion_compact,
-                                                                                // k_al_expansion, k_al_update, k_cost, k_eval_constraints,
-                                                                                // k_constraint_jacobians (cdata)
+    choice[TO_CHOICE_INST_FORWARD] = inst_forward(P) ? 1 : 0;     // launch_pass
+    choice[TO_CHOICE_INST_BACKWARD] = inst_backward(P) ? 1 : 0;   // k_riccati, k_riccati_small, k_expansion_rec(16b), k_expansion_compact,
+                                                                  // k_al_expansion, k_al_update, k_cost, k_eval_constraints, k_constraint_jacobians
     choice[TO_CHOICE_RESIDENT] = bk == KC_BK_FRAGMENT ? frag_resident_warps() : 0;
     return TO_OK;
 }

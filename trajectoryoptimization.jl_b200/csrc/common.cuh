@@ -54,7 +54,7 @@ struct DevCon {
     int kind, first, last, p, sense, offset, ninds, flag;   // first/last: 1-based inclusive knots; offset into lambda
     int diagonal;
     int n_max, n_min;
-    int goff;                // GOAL: offset of its rows in an instance's row of DevProblem::goal
+    int pad;
     int inds[TO_MAXNM];      // GOAL: state index per row (0-based); NORM: indices into z; CIRCLE/SPHERE: xi,yi,zi
     int a_max[TO_MAXNM];     // BOUND: z index of each finite upper bound (row i)        src/constraints.jl:675
     int a_min[TO_MAXNM];     // BOUND: z index of each finite lower bound (row n_max+i)  src/constraints.jl:676
@@ -67,7 +67,7 @@ struct DevCon {
     double rad[TO_MAXP];
     // CON_EXPR: user constraint recorded as a program (outputs = the last p instructions); to_constraint_spec TO_CON_EXPR
     int prog_len;
-    int cdoff;               // BOUND / LINEAR / CIRCLE / SPHERE / NORM / COLLISION: offset of its data in an instance's row of DevProblem::cdata
+    int cdoff;               // GOAL / BOUND / LINEAR / CIRCLE / SPHERE / NORM / COLLISION: offset of its data in an instance's row of DevProblem::cdata
     int pad4[2];
     int prog[3 * TO_EXPR_LEN];
     double pconst[TO_EXPR_CONST];
@@ -82,8 +82,7 @@ struct ExpTab {
     double bound[TO_EXP_MAXT][TO_MAXNM];
     unsigned pkx[TO_EXP_MAXT][TO_MAXNM];    // first knot (12 bits) | last - first (12) | rows p of the constraint (7) | equality (1)
     unsigned pky[TO_EXP_MAXT][TO_MAXNM];    // lambda index of the row at knot 0
-    int goal[TO_EXP_MAXT][TO_MAXNM];        // Goal term: index i >= 0 of its bound in an instance's row of DevProblem::goal; Bound term: -2 - j,
-                                            // j = index of its bound in an instance's row of DevProblem::cdata; -1: no term
+    int inst[TO_EXP_MAXT][TO_MAXNM];        // index of the term's bound in an instance's row of DevProblem::cdata; -1: no term
 };
 
 // one dynamics model of a hybrid problem (to_dynamics_spec): a recorded program, RK4-discretised or a discrete jump map
@@ -163,11 +162,8 @@ struct DevProblem {
     // nullptr outside to_solve: every instance is worked on.
     const int* active;        // [B]
     // Per-instance goals / tracking references (to_set_goal_states, to_update_trajectories, to_set_cost_terms): the linear terms of every
-    // cost and the values of every Goal constraint, per instance.  nullptr until the first per-instance call; every kernel then reads the
-    // shared DevCost::q / r and DevCon::a.
+    // cost, per instance.  nullptr until the first per-instance call; every kernel then reads the shared DevCost::q / r.
     const double* qr;         // [B][ncost][n+m]: q | r of cost cid for instance b
-    const double* goal;       // [B][ngoal]: a[row] of Goal constraint ci at DevCon::goff
-    int ngoal;
     // The line search's compact problem class (forward.cu rollout_compact): one cost on every stage knot and another on the terminal
     // knot, at most one Bound with finite limits on every control and none on the state, on every stage knot, and at most one Goal, on the
     // terminal knot only.  Set at to_create (the structure of the costs and constraints never changes afterwards).
@@ -175,8 +171,9 @@ struct DevProblem {
     // Per-instance model parameters (to_set_model_params): [B][TO_NPARAM] in the layout of `params`, the host-computed reciprocals included.
     // nullptr until the first per-instance call; every kernel then reads the shared `params`.
     const double* mparams;
-    // Per-instance constraint data (to_set_constraint_data): row b holds, at DevCon::cdoff, the data of every constraint that carries data
-    // other than a Goal (see con_data).  nullptr until the first call; every kernel then reads the shared DevCon fields.
+    // Per-instance constraint data (to_set_constraint_data, and the Goal values of to_set_goal_values / to_set_goal_states): row b holds, at
+    // DevCon::cdoff, the data of every constraint that carries data (see con_data).  nullptr until the first call; every kernel then reads
+    // the shared DevCon fields.
     const double* cdata;      // [B][ncdata]
     int ncdata;
 };
@@ -185,7 +182,14 @@ struct DevProblem {
 enum { SOLVE_ACTIVE = 0, SOLVE_WAITING = 1, SOLVE_DONE = 2 };
 __host__ __device__ inline bool retired(const DevProblem& P, int b) { return P.active != nullptr && P.active[b] != SOLVE_ACTIVE; }
 
-// Linear cost terms and Goal values of instance b: the only place that decides between the per-instance tables and the shared descriptors.
+// Which variant of a kernel family runs: INST = true when a per-instance table the family reads exists.  The only place that decides; every
+// launcher and to_kernel_choice ask here.  The line search reads the linear cost terms, the model parameters and the constraint data; the
+// expansion, backward and sweep kernels the cost terms and the constraint data; the dynamics kernels the model parameters alone.
+__host__ __device__ inline bool inst_forward(const DevProblem& P) { return P.qr || P.mparams || P.cdata; }
+__host__ __device__ inline bool inst_backward(const DevProblem& P) { return P.qr || P.cdata; }
+__host__ __device__ inline bool inst_dynamics(const DevProblem& P) { return P.mparams; }
+
+// Linear cost terms of instance b: the only place that decides between the per-instance table and the shared descriptors.
 // INST = false is the shared path, compiled without a look at the tables; the hot kernels take INST as a template parameter and are
 // launched with INST = true only when the tables exist.
 template <bool INST>
@@ -198,11 +202,6 @@ __host__ __device__ __forceinline__ const double* inst_r(const DevProblem& P, in
     if constexpr (INST) { if (P.qr) return P.qr + ((size_t)b * P.ncost + cid) * (P.n + P.m) + P.n; }
     return P.costs[cid].r;
 }
-template <bool INST>
-__host__ __device__ __forceinline__ const double* goal_values(const DevProblem& P, int b, int ci) {
-    if constexpr (INST) { if (P.goal) return P.goal + (size_t)b * P.ngoal + P.cons[ci].goff; }
-    return P.cons[ci].a;
-}
 // Model parameter i of instance b: the only place that decides between the rows of DevProblem::mparams and the shared vector.  A value, not a
 // pointer: the shared vector lives in the kernel's parameter bank, and a pointer that may point there makes the kernel copy it to local memory.
 // The kernels stage an instance's parameters with it (models.cuh stage_model_params) and run the dynamics on the copy.
@@ -212,20 +211,27 @@ __device__ __forceinline__ double model_param(const DevProblem& P, int b, int i)
     return P.params[i];
 }
 // The data of constraint ci for instance b, in the fields of DevCon it replaces: a (GOAL xf | BOUND z_max | CIRCLE / SPHERE xc), b (BOUND z_min |
-// LINEAR b | yc), c3 (zc), rad (CIRCLE / SPHERE r), val (NORM val | COLLISION radius).  LINEAR's A and every other field stay shared.  The only
-// place that decides between an instance's row of DevProblem::goal / cdata and the descriptor; INST = false returns the descriptor's fields.
-// An instance's row of cdata, at DevCon::cdoff: BOUND z_max[n+m] | z_min[n+m], LINEAR b[p], CIRCLE xc[p] | yc[p] | r[p],
+// LINEAR b | yc), c3 (zc), rad (CIRCLE / SPHERE r), val (NORM val | COLLISION radius).  LINEAR's A and every other field stay shared.  With
+// con_row, the only place that decides between an instance's row of DevProblem::cdata and the descriptor; INST = false returns the descriptor's
+// fields.  An instance's row of cdata, at DevCon::cdoff: GOAL xf[inds], BOUND z_max[n+m] | z_min[n+m], LINEAR b[p], CIRCLE xc[p] | yc[p] | r[p],
 // SPHERE xc[p] | yc[p] | zc[p] | r[p], NORM val, COLLISION radius.
+// con_row: constraint ci's part of instance b's row when the table exists, else `shared`.  For a constraint that carries data (DevCon::cdoff
+// >= 0); the Goal read sites take their values with it (con_row<INST>(P, b, ci, con.a)).
+template <bool INST>
+__host__ __device__ __forceinline__ const double* con_row(const DevProblem& P, int b, int ci, const double* shared) {
+    if constexpr (INST) { if (P.cdata) return P.cdata + (size_t)b * P.ncdata + P.cons[ci].cdoff; }
+    return shared;
+}
 struct ConData { const double *a, *b, *c3, *rad; double val; };
 template <bool INST>
 __device__ __forceinline__ ConData con_data(const DevProblem& P, int b, int ci) {
     const DevCon& con = P.cons[ci];
     ConData d{con.a, con.b, con.c3, con.rad, con.val};
     if constexpr (INST) {
-        if (con.kind == CON_GOAL) d.a = goal_values<true>(P, b, ci);
-        else if (P.cdata && con.cdoff >= 0) {
-            const double* row = P.cdata + (size_t)b * P.ncdata + con.cdoff;
+        if (P.cdata && con.cdoff >= 0) {
+            const double* row = con_row<true>(P, b, ci, nullptr);
             switch (con.kind) {
+                case CON_GOAL: d.a = row; break;
                 case CON_BOUND: d.a = row; d.b = row + P.n + P.m; break;
                 case CON_LINEAR: d.b = row; break;
                 case CON_CIRCLE: d.a = row; d.b = row + con.p; d.rad = row + 2 * con.p; break;

@@ -191,7 +191,7 @@ __device__ inline void cost_hessian_quadratic(const DevCost& c, int n, int m, bo
 
 __device__ __forceinline__ double zget(int n, const double* x, const double* u, int j) { return j < n ? x[j] : u[j - n]; }
 
-// goal: the Goal values to use (con.a, or an instance's row of DevProblem::goal, goal_values); read for CON_GOAL only
+// goal: the Goal values to use (con.a, or an instance's row of DevProblem::cdata, con_data); read for CON_GOAL only
 __device__ inline void con_evaluate(const DevCon& con, const double* goal, int n, int m, const double* x, const double* u, double* c) {
     switch (con.kind) {
         case CON_GOAL:
@@ -403,7 +403,7 @@ __device__ inline void con_jacobian(const DevCon& con, const ConData& d, int n, 
 template <bool INST>
 __device__ __forceinline__ void con_evaluate_b(const DevProblem& P, const DevCon& con, int b, int ci, int n, int m, const double* x, const double* u, double* c) {
     if constexpr (INST) con_evaluate(con, con_data<true>(P, b, ci), n, m, x, u, c);
-    else con_evaluate(con, goal_values<false>(P, b, ci), n, m, x, u, c);
+    else con_evaluate(con, P.cons[ci].a, n, m, x, u, c);
 }
 template <bool INST>
 __device__ __forceinline__ void con_jacobian_b(const DevProblem& P, const DevCon& con, int b, int ci, int n, int m, const double* x, const double* u, double* jac) {

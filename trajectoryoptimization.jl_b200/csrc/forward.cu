@@ -337,7 +337,7 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
                 if (c.kind == CON_GOAL) {
                     const unsigned mk = c.mask_max;
                     const double* ga = c.a;
-                    if constexpr (INST) ga = goal_values<true>(P, b, ci);
+                    if constexpr (INST) ga = con_row<true>(P, b, ci, P.cons[ci].a);
 #pragma unroll
                     for (int i = 0; i < n; i++) {
                         if (mk & (1u << i)) {
@@ -565,7 +565,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
             double a = 0.0, l2 = 0.0;
             const unsigned mk = c.mask_max;
             const double* ga = c.a;
-            if constexpr (INST) ga = goal_values<true>(P, b, tab.goal_ci);
+            if constexpr (INST) ga = con_row<true>(P, b, tab.goal_ci, P.cons[tab.goal_ci].a);
 #pragma unroll
             for (int i = 0; i < n; i++) {
                 if (mk & (1u << i)) {
@@ -801,11 +801,11 @@ cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int f
     return launch_pass_l<MODEL, G, PATH, 32, false, INST>(P, trial0, first_pass, final_pass, s);
 }
 
-// per-instance linear cost terms / Goal values / model parameters: a kernel variant of its own, so that the shared one is the code it has
-// always been.  It serves every per-instance table; each accessor checks its own (inst_q, goal_values, model_param).
+// per-instance linear cost terms / model parameters / constraint data: a kernel variant of its own, so that the shared one is the code it has
+// always been.  It serves every per-instance table; each accessor checks its own (inst_q, model_param, con_data / con_row).
 template <int MODEL, int G, int PATH>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
-    if (P.qr || P.mparams || P.cdata) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);
+    if (inst_forward(P)) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);
     return launch_pass_i<MODEL, G, PATH, false>(P, trial0, first_pass, final_pass, s);
 }
 

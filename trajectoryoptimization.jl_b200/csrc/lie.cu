@@ -684,7 +684,7 @@ cudaError_t launch_error_expansion(const DevProblem& P, const double* gfull, con
     return cudaGetLastError();
 }
 cudaError_t launch_expansion_compact(const DevProblem& P, cudaStream_t s) {
-    if (P.qr || P.cdata) k_expansion_compact<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
+    if (inst_backward(P)) k_expansion_compact<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     else k_expansion_compact<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }

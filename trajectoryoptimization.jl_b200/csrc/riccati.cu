@@ -220,9 +220,9 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
     }
 
     // ---- lane-resident AL terms of z_lane (Goal / Bound constraints) ----------------------------------------
-    int tgoal[MAXT];   // (INST) where a term's bound sits in an instance's rows: i >= 0 in P.goal (Goal), -2 - j in P.cdata (Bound), -1: none
+    int tinst[MAXT];   // (INST) index of a term's bound in an instance's row of P.cdata, -1: none
 #pragma unroll
-    for (int t = 0; t < MAXT; t++) tgoal[t] = -1;
+    for (int t = 0; t < MAXT; t++) tinst[t] = -1;
     if (FASTAL) {
         if (lane < SM::NMT) {
 #pragma unroll
@@ -241,9 +241,9 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     if (row < 0) continue;
                     if (nterm < MAXT) { sm.tnms[nterm][lane] = -mu * sign; sm.tbound[nterm][lane] = bound; sm.tpk[nterm][lane] = pack_term(con.first, con.last, con.offset + row, con.p, eq); }
                     if (INST && nterm < MAXT) {
-                        const int src = eq ? con.goff + row : -2 - (con.cdoff + (side ? n + m : 0) + lane);
+                        const int src = con.cdoff + (eq ? row : (side ? n + m : 0) + lane);
 #pragma unroll
-                        for (int t = 0; t < MAXT; t++) if (t == nterm) tgoal[t] = src;
+                        for (int t = 0; t < MAXT; t++) if (t == nterm) tinst[t] = src;
                     }
                     nterm++;
                 }
@@ -270,10 +270,8 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         if constexpr (INST && FASTAL) {         // this instance's Goal / Bound values into the lane-resident terms (read back by this lane only)
             if (lane < NM) {
 #pragma unroll
-                for (int t = 0; t < MAXT; t++) {
-                    if (P.goal && tgoal[t] >= 0) sm.tbound[t][lane] = P.goal[(size_t)b * P.ngoal + tgoal[t]];
-                    else if (P.cdata && tgoal[t] <= -2) sm.tbound[t][lane] = P.cdata[(size_t)b * P.ncdata + (-2 - tgoal[t])];
-                }
+                for (int t = 0; t < MAXT; t++)
+                    if (P.cdata && tinst[t] >= 0) sm.tbound[t][lane] = P.cdata[(size_t)b * P.ncdata + tinst[t]];
             }
         }
 
@@ -431,7 +429,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                             const double* lam = lam_b + con.offset + (size_t)(N - con.first) * con.p;
                             if (con.kind == CON_GOAL) {
                                 const int row = con.row_max[i];
-                                if (row >= 0) { const double lp = lam[row] - mu * (xi - goal_values<INST>(P, b, ci)[row]); gi -= lp; hi += mu; }
+                                if (row >= 0) { const double lp = lam[row] - mu * (xi - con_row<INST>(P, b, ci, con.a)[row]); gi -= lp; hi += mu; }
                             } else if (con.kind == CON_BOUND) {
                                 const double* ba = con.a; const double* bb = con.b;
                                 if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ba = cd.a; bb = cd.b; }
@@ -515,7 +513,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                                 const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
                                 if (con.kind == CON_GOAL) {
                                     const int row = (i < n) ? con.row_max[i] : -1;
-                                    if (row >= 0) { const double lp = lam[row] - mu * (zi - goal_values<INST>(P, b, ci)[row]); gi -= lp; hi += mu; }
+                                    if (row >= 0) { const double lp = lam[row] - mu * (zi - con_row<INST>(P, b, ci, con.a)[row]); gi -= lp; hi += mu; }
                                 } else if (con.kind == CON_BOUND) {
                                     const double* ba = con.a; const double* bb = con.b;
                                     if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ba = cd.a; bb = cd.b; }
@@ -996,7 +994,7 @@ cudaError_t launch_riccati_v(const DevProblem& P, int* work_counter, cudaStream_
     return cudaGetLastError();
 }
 
-// INST: per-instance linear cost terms / Goal values (P.qr), a kernel variant of its own so that the shared one stays as it is
+// INST: per-instance linear cost terms (P.qr) and constraint data (P.cdata), a kernel variant of its own so that the shared one stays as it is
 template <int N_, int M_, bool FASTAL, bool INST>
 cudaError_t launch_riccati_t(const DevProblem& P, int* work_counter, cudaStream_t s) {
     if constexpr (N_ >= 8 && M_ <= 4) {
@@ -1013,7 +1011,7 @@ cudaError_t launch_riccati_t(const DevProblem& P, int* work_counter, cudaStream_
 template <int N_, int M_>
 cudaError_t launch_riccati_nm(const DevProblem& P, int* work_counter, cudaStream_t s) {
     const bool fastal = riccati_fastal(P);
-    if (P.qr || P.cdata) return fastal ? launch_riccati_t<N_, M_, true, true>(P, work_counter, s) : launch_riccati_t<N_, M_, false, true>(P, work_counter, s);
+    if (inst_backward(P)) return fastal ? launch_riccati_t<N_, M_, true, true>(P, work_counter, s) : launch_riccati_t<N_, M_, false, true>(P, work_counter, s);
     return fastal ? launch_riccati_t<N_, M_, true, false>(P, work_counter, s) : launch_riccati_t<N_, M_, false, false>(P, work_counter, s);
 }
 

@@ -599,7 +599,7 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_riccati_frag(const DevProb
 }  // namespace
 
 cudaError_t launch_expansion_rec(const DevProblem& P, cudaStream_t s) {
-    if (P.qr || P.cdata) k_expansion_rec<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
+    if (inst_backward(P)) k_expansion_rec<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     else k_expansion_rec<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }

@@ -246,7 +246,7 @@ __global__ void __maxnreg__(255) k_riccati_small(const DevProblem P) {
 
 template <int N_, int M_>
 cudaError_t launch_small(const DevProblem& P, cudaStream_t s) {
-    if (P.qr || P.cdata) k_riccati_small<N_, M_, true><<<(P.B + 31) / 32, 32, 0, s>>>(P);
+    if (inst_backward(P)) k_riccati_small<N_, M_, true><<<(P.B + 31) / 32, 32, 0, s>>>(P);
     else k_riccati_small<N_, M_, false><<<(P.B + 31) / 32, 32, 0, s>>>(P);
     return cudaGetLastError();
 }

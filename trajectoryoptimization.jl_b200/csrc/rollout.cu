@@ -157,11 +157,10 @@ cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s) {
 // + the AL terms of the Goal / Bound rows acting on z_i (src/constraints.jl:55-68, :738-765; projection on the dual cone src/cones.jl:96-145).
 // The compact problem class only (P.compact): every cost diagonal, every constraint Goal or Bound, at most TO_EXP_MAXT rows per entry
 // (the host-built table P.exptab; walking the constraint descriptors per thread instead adds work comparable to the RK4 itself).
-// The bound of term t of z entry i for instance b: its row of DevProblem::goal (Goal) or cdata (Bound) when those exist, else `shared`
+// The bound of term t of z entry i for instance b: its entry of the instance's row of DevProblem::cdata when the table exists, else `shared`
 __device__ __forceinline__ double exp_term_bound(const DevProblem& P, const ExpTab& tab, int b, int t, int i, double shared) {
-    const int gi = tab.goal[t][i];
-    if (P.goal && gi >= 0) return P.goal[(size_t)b * P.ngoal + gi];
-    if (P.cdata && gi <= -2) return P.cdata[(size_t)b * P.ncdata + (-2 - gi)];
+    const int j = __ldg(&tab.inst[t][i]);
+    if (P.cdata && j >= 0) return P.cdata[(size_t)b * P.ncdata + j];
     return shared;
 }
 // (INST: the linear cost terms and Goal / Bound bounds of instance b)
@@ -391,7 +390,7 @@ cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s) {
 #ifndef TO_CEXP2_THREADS
 #define TO_CEXP2_THREADS 64
 #endif
-// INST: the linear cost terms and Goal bounds of each instance (DevProblem::qr / goal), a variant of its own so that the shared one stays as it is
+// INST: the linear cost terms and Goal / Bound bounds of each instance (DevProblem::qr / cdata), a variant of its own so that the shared one stays as it is
 template <bool INST>
 __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_rec16b(const DevProblem P, int mode) {
     constexpr int qs = 3, n = 13, m = 4;
@@ -559,7 +558,7 @@ cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode
     constexpr int GPB = TO_CEXP2_THREADS / 16;                                       // 16-lane groups per CTA
     long long blocks = (units + GPB - 1) / GPB;
     if (blocks < sms) blocks = sms;
-    if (P.qr || P.cdata) k_expansion_rec16b<true><<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
+    if (inst_backward(P)) k_expansion_rec16b<true><<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
     else k_expansion_rec16b<false><<<(unsigned)blocks, TO_CEXP2_THREADS, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
@@ -573,9 +572,9 @@ cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
         // one CTA per (instance, block of EXPB_KPB knots); mode 2 with the late list: the first *late_count instance slots carry work
         const int nkb = (P.N - 1 + EXPB_KPB - 1) / EXPB_KPB;
         const unsigned blocks = (unsigned)((long long)P.B * nkb);
-        if (P.mparams) k_expand_lie_rec<MODEL_QUADROTOR, true><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
+        if (inst_dynamics(P)) k_expand_lie_rec<MODEL_QUADROTOR, true><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
         else k_expand_lie_rec<MODEL_QUADROTOR, false><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
-    } else if (P.mparams) k_expand_lie<MODEL_QUADROTOR, true><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
+    } else if (inst_dynamics(P)) k_expand_lie<MODEL_QUADROTOR, true><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
     else k_expand_lie<MODEL_QUADROTOR, false><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
@@ -583,7 +582,7 @@ cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
 // the dynamics kernels read nothing per instance but the model parameters: their INST variant runs exactly when the rows exist
 cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s) {
     const int threads = 32, blocks = (P.B + threads - 1) / threads;
-    if (P.mparams) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true><<<blocks, threads, 0, s>>>(P))); }
+    if (inst_dynamics(P)) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true><<<blocks, threads, 0, s>>>(P))); }
     else { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, false><<<blocks, threads, 0, s>>>(P))); }
     return cudaGetLastError();
 }
@@ -594,7 +593,7 @@ static cudaError_t launch_expand_t(const DevProblem& P, cudaStream_t s, int mode
     const long long total = (long long)P.B * (P.N - 1) * TPK;
     const int threads = 128;
     const unsigned blocks = (unsigned)((total + threads - 1) / threads);
-    if (P.mparams) k_expand<MODEL, NP, true><<<blocks, threads, 0, s>>>(P, mode);
+    if (inst_dynamics(P)) k_expand<MODEL, NP, true><<<blocks, threads, 0, s>>>(P, mode);
     else k_expand<MODEL, NP, false><<<blocks, threads, 0, s>>>(P, mode);
     return cudaGetLastError();
 }

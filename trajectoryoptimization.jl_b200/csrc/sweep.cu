@@ -238,17 +238,17 @@ __global__ void k_export_ab(const DevProblem P, double* __restrict__ out) {
 static inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
 cudaError_t launch_cost(const DevProblem& P, double* J, double* Jk, cudaStream_t s) {
-    if (P.qr || P.cdata) k_cost<false, true><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
+    if (inst_backward(P)) k_cost<false, true><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
     else k_cost<false, false><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
     return cudaGetLastError();
 }
 cudaError_t launch_merit(const DevProblem& P, double* J, double* viol, cudaStream_t s) {
-    if (P.qr || P.cdata) k_cost<true, true><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
+    if (inst_backward(P)) k_cost<true, true><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
     else k_cost<true, false><<<P.B, 128, 0, s>>>(P, J, nullptr, viol);
     return cudaGetLastError();
 }
 cudaError_t launch_cost_gradient(const DevProblem& P, double* grad, cudaStream_t s) {
-    if (P.qr || P.cdata) k_cost_gradient<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
+    if (inst_backward(P)) k_cost_gradient<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
     else k_cost_gradient<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, grad);
     return cudaGetLastError();
 }
@@ -257,13 +257,13 @@ cudaError_t launch_cost_hessian(const DevProblem& P, double* hess, cudaStream_t 
     return cudaGetLastError();
 }
 cudaError_t launch_al_expansion(const DevProblem& P, double* grad, double* hess, cudaStream_t s) {
-    if (P.qr || P.cdata) k_al_expansion<true><<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
+    if (inst_backward(P)) k_al_expansion<true><<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
     else k_al_expansion<false><<<nblk((long long)P.B * P.N, 64), 64, 0, s>>>(P, grad, hess);
     return cudaGetLastError();
 }
 cudaError_t launch_eval_constraints(const DevProblem& P, int con, double* vals, cudaStream_t s) {
     // the knot-range length is read on the device; size the grid for the worst case N
-    if (P.qr || P.cdata) k_eval_constraints<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
+    if (inst_backward(P)) k_eval_constraints<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
     else k_eval_constraints<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, vals);
     return cudaGetLastError();
 }
@@ -273,7 +273,7 @@ cudaError_t launch_constraint_hessians(const DevProblem& P, int con, int len, co
     return cudaGetLastError();
 }
 cudaError_t launch_constraint_jacobians(const DevProblem& P, int con, double* jac, cudaStream_t s) {
-    if (P.cdata) k_constraint_jacobians<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, jac);
+    if (inst_backward(P)) k_constraint_jacobians<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, jac);
     else k_constraint_jacobians<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, con, jac);
     return cudaGetLastError();
 }
@@ -290,7 +290,7 @@ cudaError_t launch_hess_projection(int cone, int p, int count, const double* x, 
     return cudaGetLastError();
 }
 cudaError_t launch_al_update(const DevProblem& P, cudaStream_t s) {
-    if (P.qr || P.cdata) k_al_update<true><<<P.B, 128, 0, s>>>(P);
+    if (inst_backward(P)) k_al_update<true><<<P.B, 128, 0, s>>>(P);
     else k_al_update<false><<<P.B, 128, 0, s>>>(P);
     return cudaGetLastError();
 }
