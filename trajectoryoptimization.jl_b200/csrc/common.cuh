@@ -211,36 +211,36 @@ __device__ __forceinline__ double model_param(const DevProblem& P, int b, int i)
     return P.params[i];
 }
 // The data of constraint ci for instance b, in the fields of DevCon it replaces: a (GOAL xf | BOUND z_max | CIRCLE / SPHERE xc), b (BOUND z_min |
-// LINEAR b | yc), c3 (zc), rad (CIRCLE / SPHERE r), val (NORM val | COLLISION radius).  LINEAR's A and every other field stay shared.  With
-// con_row, the only place that decides between an instance's row of DevProblem::cdata and the descriptor; INST = false returns the descriptor's
-// fields.  An instance's row of cdata, at DevCon::cdoff: GOAL xf[inds], BOUND z_max[n+m] | z_min[n+m], LINEAR b[p], CIRCLE xc[p] | yc[p] | r[p],
+// LINEAR b | yc), c3 (zc), rad (CIRCLE / SPHERE r), val (NORM val | COLLISION radius).  LINEAR's A and every other field stay shared.  The only
+// place that decides between an instance's row of DevProblem::cdata and the descriptor, and the only way a kernel reads a constraint's data.
+// An instance's row of cdata, at DevCon::cdoff: GOAL xf[inds], BOUND z_max[n+m] | z_min[n+m], LINEAR b[p], CIRCLE xc[p] | yc[p] | r[p],
 // SPHERE xc[p] | yc[p] | zc[p] | r[p], NORM val, COLLISION radius.
-// con_row: constraint ci's part of instance b's row when the table exists, else `shared`.  For a constraint that carries data (DevCon::cdoff
-// >= 0); the Goal read sites take their values with it (con_row<INST>(P, b, ci, con.a)).
+// Every field is a pointer, val included: building the view loads nothing, so with INST = false it is the address arithmetic of reading the
+// descriptor in place, and each value is loaded where it is used (a value field would load con.val before the stores that precede its use,
+// which may alias it).  `shared`: the descriptor's fields, or a kernel's staged copy of them (the line search's tables in shared memory).
+struct ConData { const double *a, *b, *c3, *rad, *val; };
 template <bool INST>
-__host__ __device__ __forceinline__ const double* con_row(const DevProblem& P, int b, int ci, const double* shared) {
-    if constexpr (INST) { if (P.cdata) return P.cdata + (size_t)b * P.ncdata + P.cons[ci].cdoff; }
-    return shared;
-}
-struct ConData { const double *a, *b, *c3, *rad; double val; };
-template <bool INST>
-__device__ __forceinline__ ConData con_data(const DevProblem& P, int b, int ci) {
-    const DevCon& con = P.cons[ci];
-    ConData d{con.a, con.b, con.c3, con.rad, con.val};
+__device__ __forceinline__ ConData con_data(const DevProblem& P, int b, int ci, ConData shared) {
     if constexpr (INST) {
+        const DevCon& con = P.cons[ci];
         if (P.cdata && con.cdoff >= 0) {
-            const double* row = con_row<true>(P, b, ci, nullptr);
+            const double* row = P.cdata + (size_t)b * P.ncdata + con.cdoff;
             switch (con.kind) {
-                case CON_GOAL: d.a = row; break;
-                case CON_BOUND: d.a = row; d.b = row + P.n + P.m; break;
-                case CON_LINEAR: d.b = row; break;
-                case CON_CIRCLE: d.a = row; d.b = row + con.p; d.rad = row + 2 * con.p; break;
-                case CON_SPHERE: d.a = row; d.b = row + con.p; d.c3 = row + 2 * con.p; d.rad = row + 3 * con.p; break;
-                case CON_NORM: case CON_COLLISION: d.val = row[0]; break;
+                case CON_GOAL: shared.a = row; break;
+                case CON_BOUND: shared.a = row; shared.b = row + P.n + P.m; break;
+                case CON_LINEAR: shared.b = row; break;
+                case CON_CIRCLE: shared.a = row; shared.b = row + con.p; shared.rad = row + 2 * con.p; break;
+                case CON_SPHERE: shared.a = row; shared.b = row + con.p; shared.c3 = row + 2 * con.p; shared.rad = row + 3 * con.p; break;
+                case CON_NORM: case CON_COLLISION: shared.val = row; break;
             }
         }
     }
-    return d;
+    return shared;
+}
+template <bool INST>
+__device__ __forceinline__ ConData con_data(const DevProblem& P, int b, int ci) {
+    const DevCon& con = P.cons[ci];
+    return con_data<INST>(P, b, ci, ConData{con.a, con.b, con.c3, con.rad, &con.val});
 }
 
 __host__ __device__ inline const double* traj_X(const DevProblem& P, int buf, int b) { return P.X + buf * P.strideX + (size_t)b * P.N * P.n; }

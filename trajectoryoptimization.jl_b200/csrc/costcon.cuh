@@ -191,146 +191,13 @@ __device__ inline void cost_hessian_quadratic(const DevCost& c, int n, int m, bo
 
 __device__ __forceinline__ double zget(int n, const double* x, const double* u, int j) { return j < n ? x[j] : u[j - n]; }
 
-// goal: the Goal values to use (con.a, or an instance's row of DevProblem::cdata, con_data); read for CON_GOAL only
-__device__ inline void con_evaluate(const DevCon& con, const double* goal, int n, int m, const double* x, const double* u, double* c) {
-    switch (con.kind) {
-        case CON_GOAL:
-            for (int i = 0; i < con.p; i++) c[i] = x[con.inds[i]] - goal[i];
-            break;
-        case CON_BOUND: {   // upper block first, then the lower block
-            int i = 0;
-            for (int r = 0; r < con.n_max; r++, i++) { int j = con.a_max[r]; c[i] = zget(n, x, u, j) - con.a[j]; }
-            for (int r = 0; r < con.n_min; r++, i++) { int j = con.a_min[r]; c[i] = con.b[j] - zget(n, x, u, j); }
-            break;
-        }
-        case CON_LINEAR: {
-            const double* y = con.flag ? u : x;
-            const int w = con.flag ? m : n;
-            for (int i = 0; i < con.p; i++) {
-                double s = -con.b[i];
-                for (int j = 0; j < w; j++) s = fma(con.a[j * con.p + i], y[j], s);
-                c[i] = s;
-            }
-            break;
-        }
-        case CON_CIRCLE:
-            for (int i = 0; i < con.p; i++) {
-                double dx = x[con.inds[0]] - con.a[i], dy = x[con.inds[1]] - con.b[i];
-                c[i] = -(dx * dx) - (dy * dy) + con.rad[i] * con.rad[i];
-            }
-            break;
-        case CON_SPHERE:
-            for (int i = 0; i < con.p; i++) {
-                double dx = x[con.inds[0]] - con.a[i], dy = x[con.inds[1]] - con.b[i], dz = x[con.inds[2]] - con.c3[i];
-                c[i] = -(dx * dx) - (dy * dy) - (dz * dz) + con.rad[i] * con.rad[i];
-            }
-            break;
-        case CON_NORM:
-            if (con.sense == CONE_SECOND_ORDER) {
-                for (int i = 0; i < con.ninds; i++) c[i] = zget(n, x, u, con.inds[i]);
-                c[con.ninds] = con.val;
-            } else {
-                double s = 0;
-                for (int i = 0; i < con.ninds; i++) { double z = zget(n, x, u, con.inds[i]); s = fma(z, z, s); }
-                c[0] = s - con.val * con.val;
-            }
-            break;
-        case CON_COLLISION: {   // src/constraints.jl:367-376: r^2 - sum_i (x[x1_i] - x[x2_i])^2, accumulated in that order
-            const int D = con.ninds / 2;
-            double s = con.val * con.val;
-            for (int i = 0; i < D; i++) { const double d = x[con.inds[i]] - x[con.inds[D + i]]; s -= d * d; }
-            c[0] = s;
-            break;
-        }
-        case CON_EXPR: {   // user constraint recorded as a program (docs/src/constraint_interface.md:52-72)
-            Hyper reg[TO_EXPR_LEN];
-            expr_run(con.prog, con.prog_len, con.pconst, n, x, u, true, -1, -1, reg);
-            for (int i = 0; i < con.p; i++) c[i] = reg[con.prog_len - con.p + i].v;
-            break;
-        }
-        case CON_QUATVEC: {   // QuatVecEq src/constraints.jl:947-956
-            double q[4], nrm = 0, dq = 0;
-            for (int i = 0; i < 4; i++) { q[i] = x[con.inds[i]]; nrm = fma(q[i], q[i], nrm); }
-            nrm = sqrt(nrm);
-            for (int i = 0; i < 4; i++) { q[i] /= nrm; dq = fma(con.a[i], q[i], dq); }
-            const double sg = dq < 0 ? -1.0 : 1.0;
-            for (int i = 0; i < 3; i++) c[i] = -(sg * con.a[i + 1] - q[i + 1]);
-            break;
-        }
-    }
-}
-__device__ inline void con_evaluate(const DevCon& con, int n, int m, const double* x, const double* u, double* c) {
-    con_evaluate(con, con.a, n, m, x, u, c);
-}
-
-// jac: p x (n+m) col-major, fully written
-__device__ inline void con_jacobian(const DevCon& con, int n, int m, const double* x, const double* u, double* jac) {
-    const int p = con.p, w = n + m;
-    for (int i = 0; i < p * w; i++) jac[i] = 0;
-    switch (con.kind) {
-        case CON_GOAL: for (int i = 0; i < p; i++) jac[con.inds[i] * p + i] = 1; break;
-        case CON_BOUND: {
-            int i = 0;
-            for (int r = 0; r < con.n_max; r++, i++) jac[con.a_max[r] * p + i] = 1;
-            for (int r = 0; r < con.n_min; r++, i++) jac[con.a_min[r] * p + i] = -1;
-            break;
-        }
-        case CON_LINEAR: {
-            const int off = con.flag ? n : 0, wd = con.flag ? m : n;
-            for (int j = 0; j < wd; j++) for (int i = 0; i < p; i++) jac[(off + j) * p + i] = con.a[j * p + i];
-            break;
-        }
-        case CON_CIRCLE:
-            for (int i = 0; i < p; i++) {
-                jac[con.inds[0] * p + i] = -2 * (x[con.inds[0]] - con.a[i]);
-                jac[con.inds[1] * p + i] = -2 * (x[con.inds[1]] - con.b[i]);
-            }
-            break;
-        case CON_SPHERE:
-            for (int i = 0; i < p; i++) {
-                jac[con.inds[0] * p + i] = -2 * (x[con.inds[0]] - con.a[i]);
-                jac[con.inds[1] * p + i] = -2 * (x[con.inds[1]] - con.b[i]);
-                jac[con.inds[2] * p + i] = -2 * (x[con.inds[2]] - con.c3[i]);
-            }
-            break;
-        case CON_NORM:
-            if (con.sense == CONE_SECOND_ORDER) for (int i = 0; i < con.ninds; i++) jac[con.inds[i] * p + i] = 1;
-            else for (int i = 0; i < con.ninds; i++) jac[con.inds[i] * p + 0] = 2 * zget(n, x, u, con.inds[i]);
-            break;
-        case CON_COLLISION: {   // :378-389 (assignments, as in the reference)
-            const int D = con.ninds / 2;
-            for (int i = 0; i < D; i++) {
-                const double d = x[con.inds[i]] - x[con.inds[D + i]];
-                jac[con.inds[i] * p] = -2 * d;
-                jac[con.inds[D + i] * p] = 2 * d;
-            }
-            break;
-        }
-        case CON_EXPR: {   // RD.jacobian!(ForwardAD): one first-order pass per input
-            Hyper reg[TO_EXPR_LEN];
-            for (int j = 0; j < w; j++) {
-                expr_run(con.prog, con.prog_len, con.pconst, n, x, u, true, j, -1, reg);
-                for (int i = 0; i < p; i++) jac[j * p + i] = reg[con.prog_len - p + i].d1;
-            }
-            break;
-        }
-        case CON_QUATVEC: {   // d normalize(q)/dq = (I - qh qh')/|q|, rows 2:4 (what ForwardAD gives, src/constraints.jl:938,962)
-            double q[4], nrm = 0;
-            for (int i = 0; i < 4; i++) { q[i] = x[con.inds[i]]; nrm = fma(q[i], q[i], nrm); }
-            nrm = sqrt(nrm);
-            for (int i = 0; i < 4; i++) q[i] /= nrm;
-            for (int j = 0; j < 4; j++)
-                for (int i = 0; i < 3; i++) jac[con.inds[j] * p + i] = ((i + 1 == j ? 1.0 : 0.0) - q[i + 1] * q[j]) / nrm;
-            break;
-        }
-    }
-}
-
-// The INST overloads: d = the data of an instance (con_data).  The kinds whose data may differ per instance are evaluated here with the shared
-// overloads' arithmetic, operation for operation; the others go to the shared overloads (a Goal with d.a, its instance's values).
+// d: the constraint's data (con_data); every other field is read from the descriptor
 __device__ inline void con_evaluate(const DevCon& con, const ConData& d, int n, int m, const double* x, const double* u, double* c) {
     switch (con.kind) {
-        case CON_BOUND: {
+        case CON_GOAL:
+            for (int i = 0; i < con.p; i++) c[i] = x[con.inds[i]] - d.a[i];
+            break;
+        case CON_BOUND: {   // upper block first, then the lower block
             int i = 0;
             for (int r = 0; r < con.n_max; r++, i++) { int j = con.a_max[r]; c[i] = zget(n, x, u, j) - d.a[j]; }
             for (int r = 0; r < con.n_min; r++, i++) { int j = con.a_min[r]; c[i] = d.b[j] - zget(n, x, u, j); }
@@ -361,54 +228,99 @@ __device__ inline void con_evaluate(const DevCon& con, const ConData& d, int n, 
         case CON_NORM:
             if (con.sense == CONE_SECOND_ORDER) {
                 for (int i = 0; i < con.ninds; i++) c[i] = zget(n, x, u, con.inds[i]);
-                c[con.ninds] = d.val;
+                c[con.ninds] = *d.val;
             } else {
                 double s = 0;
                 for (int i = 0; i < con.ninds; i++) { double z = zget(n, x, u, con.inds[i]); s = fma(z, z, s); }
-                c[0] = s - d.val * d.val;
+                c[0] = s - *d.val * *d.val;
             }
             break;
-        case CON_COLLISION: {
+        case CON_COLLISION: {   // src/constraints.jl:367-376: r^2 - sum_i (x[x1_i] - x[x2_i])^2, accumulated in that order
             const int D = con.ninds / 2;
-            double s = d.val * d.val;
+            double s = *d.val * *d.val;
             for (int i = 0; i < D; i++) { const double dd = x[con.inds[i]] - x[con.inds[D + i]]; s -= dd * dd; }
             c[0] = s;
             break;
         }
-        default: con_evaluate(con, d.a, n, m, x, u, c);
+        case CON_EXPR: {   // user constraint recorded as a program (docs/src/constraint_interface.md:52-72)
+            Hyper reg[TO_EXPR_LEN];
+            expr_run(con.prog, con.prog_len, con.pconst, n, x, u, true, -1, -1, reg);
+            for (int i = 0; i < con.p; i++) c[i] = reg[con.prog_len - con.p + i].v;
+            break;
+        }
+        case CON_QUATVEC: {   // QuatVecEq src/constraints.jl:947-956
+            double q[4], nrm = 0, dq = 0;
+            for (int i = 0; i < 4; i++) { q[i] = x[con.inds[i]]; nrm = fma(q[i], q[i], nrm); }
+            nrm = sqrt(nrm);
+            for (int i = 0; i < 4; i++) { q[i] /= nrm; dq = fma(con.a[i], q[i], dq); }
+            const double sg = dq < 0 ? -1.0 : 1.0;
+            for (int i = 0; i < 3; i++) c[i] = -(sg * con.a[i + 1] - q[i + 1]);
+            break;
+        }
     }
 }
+
+// jac: p x (n+m) col-major, fully written; d as in con_evaluate
 __device__ inline void con_jacobian(const DevCon& con, const ConData& d, int n, int m, const double* x, const double* u, double* jac) {
     const int p = con.p, w = n + m;
+    for (int i = 0; i < p * w; i++) jac[i] = 0;
     switch (con.kind) {
+        case CON_GOAL: for (int i = 0; i < p; i++) jac[con.inds[i] * p + i] = 1; break;
+        case CON_BOUND: {
+            int i = 0;
+            for (int r = 0; r < con.n_max; r++, i++) jac[con.a_max[r] * p + i] = 1;
+            for (int r = 0; r < con.n_min; r++, i++) jac[con.a_min[r] * p + i] = -1;
+            break;
+        }
+        case CON_LINEAR: {
+            const int off = con.flag ? n : 0, wd = con.flag ? m : n;
+            for (int j = 0; j < wd; j++) for (int i = 0; i < p; i++) jac[(off + j) * p + i] = con.a[j * p + i];
+            break;
+        }
         case CON_CIRCLE:
-            for (int i = 0; i < p * w; i++) jac[i] = 0;
             for (int i = 0; i < p; i++) {
                 jac[con.inds[0] * p + i] = -2 * (x[con.inds[0]] - d.a[i]);
                 jac[con.inds[1] * p + i] = -2 * (x[con.inds[1]] - d.b[i]);
             }
             break;
         case CON_SPHERE:
-            for (int i = 0; i < p * w; i++) jac[i] = 0;
             for (int i = 0; i < p; i++) {
                 jac[con.inds[0] * p + i] = -2 * (x[con.inds[0]] - d.a[i]);
                 jac[con.inds[1] * p + i] = -2 * (x[con.inds[1]] - d.b[i]);
                 jac[con.inds[2] * p + i] = -2 * (x[con.inds[2]] - d.c3[i]);
             }
             break;
-        default: con_jacobian(con, n, m, x, u, jac);   // independent of the data that may differ per instance
+        case CON_NORM:
+            if (con.sense == CONE_SECOND_ORDER) for (int i = 0; i < con.ninds; i++) jac[con.inds[i] * p + i] = 1;
+            else for (int i = 0; i < con.ninds; i++) jac[con.inds[i] * p + 0] = 2 * zget(n, x, u, con.inds[i]);
+            break;
+        case CON_COLLISION: {   // :378-389 (assignments, as in the reference)
+            const int D = con.ninds / 2;
+            for (int i = 0; i < D; i++) {
+                const double dd = x[con.inds[i]] - x[con.inds[D + i]];
+                jac[con.inds[i] * p] = -2 * dd;
+                jac[con.inds[D + i] * p] = 2 * dd;
+            }
+            break;
+        }
+        case CON_EXPR: {   // RD.jacobian!(ForwardAD): one first-order pass per input
+            Hyper reg[TO_EXPR_LEN];
+            for (int j = 0; j < w; j++) {
+                expr_run(con.prog, con.prog_len, con.pconst, n, x, u, true, j, -1, reg);
+                for (int i = 0; i < p; i++) jac[j * p + i] = reg[con.prog_len - p + i].d1;
+            }
+            break;
+        }
+        case CON_QUATVEC: {   // d normalize(q)/dq = (I - qh qh')/|q|, rows 2:4 (what ForwardAD gives, src/constraints.jl:938,962)
+            double q[4], nrm = 0;
+            for (int i = 0; i < 4; i++) { q[i] = x[con.inds[i]]; nrm = fma(q[i], q[i], nrm); }
+            nrm = sqrt(nrm);
+            for (int i = 0; i < 4; i++) q[i] /= nrm;
+            for (int j = 0; j < 4; j++)
+                for (int i = 0; i < 3; i++) jac[con.inds[j] * p + i] = ((i + 1 == j ? 1.0 : 0.0) - q[i + 1] * q[j]) / nrm;
+            break;
+        }
     }
-}
-// the values / Jacobian of constraint con = P.cons[ci] for instance b: the INST overloads with its data (con_data), or the shared overloads
-template <bool INST>
-__device__ __forceinline__ void con_evaluate_b(const DevProblem& P, const DevCon& con, int b, int ci, int n, int m, const double* x, const double* u, double* c) {
-    if constexpr (INST) con_evaluate(con, con_data<true>(P, b, ci), n, m, x, u, c);
-    else con_evaluate(con, P.cons[ci].a, n, m, x, u, c);
-}
-template <bool INST>
-__device__ __forceinline__ void con_jacobian_b(const DevProblem& P, const DevCon& con, int b, int ci, int n, int m, const double* x, const double* u, double* jac) {
-    if constexpr (INST) con_jacobian(con, con_data<true>(P, b, ci), n, m, x, u, jac);
-    else con_jacobian(con, n, m, x, u, jac);
 }
 
 // H[(n+m)^2] col-major = d/dz (cz' lambda) = sum_i lambda_i Hess c_i(z), overwritten: the second-order constraint term the reference hands to
@@ -560,7 +472,7 @@ __device__ inline int cone_hess_projection(int cone, const double* x, const doub
 }
 
 // AL penalty of one knot (conic form): sum_c (|Pi_{K*}(lambda - mu c)|^2 - |lambda|^2) / (2 mu); also the
-// knot's constraint violation |c - Pi_K(c)|_inf.  k1 = 1-based knot, b = instance (its Goal values when INST).  x/u may be registers, local or global.
+// knot's constraint violation |c - Pi_K(c)|_inf.  k1 = 1-based knot, b = instance (its constraint data when INST).  x/u may be registers, local or global.
 template <bool INST = false>
 __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const double* x, const double* u,
                                          const double* lam_b, double& viol, int b = 0) {
@@ -571,7 +483,7 @@ __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const doub
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k1 - con.first) * con.p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
-        con_evaluate_b<INST>(P, con, b, ci, P.n, P.m, x, u, c);
+        con_evaluate(con, con_data<INST>(P, b, ci), P.n, P.m, x, u, c);
         for (int i = 0; i < con.p; i++) lbar[i] = lam[i] - mu * c[i];
         cone_projection(dualcone(con.sense), lbar, con.p, lp);
         double a = 0, l2 = 0;
@@ -585,7 +497,7 @@ __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const doub
 
 // Cost expansion of one knot with the AL terms (Gauss-Newton):
 //   grad += -cz' D' lp ; hess += mu cz' D'D cz,  D = grad Pi_{K*}(lambda - mu c), lp = Pi_{K*}(lambda - mu c)
-// k0 = 0-based knot, b = instance (its linear cost terms and Goal values when INST).  grad[n+m], hess[(n+m)^2] col-major symmetric.
+// k0 = 0-based knot, b = instance (its linear cost terms and constraint data when INST).  grad[n+m], hess[(n+m)^2] col-major symmetric.
 template <bool INST = false>
 __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const double* x, const double* u, const double* lam_b,
                                          double* grad, double* hess, int b = 0) {
@@ -604,7 +516,8 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k0 + 1 - con.first) * p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
-        con_evaluate_b<INST>(P, con, b, ci, n, m, x, u, c);
+        const ConData cd = con_data<INST>(P, b, ci);
+        con_evaluate(con, cd, n, m, x, u, c);
         if (con.diagonal) {   // Goal / Bound: +-1 selector rows (src/constraints.jl:62-68, :757-765) -- row by row, no dense products
             const bool eq = (con.kind == CON_GOAL);
             const int nrow = eq ? p : con.n_max + con.n_min;
@@ -617,7 +530,7 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
             continue;
         }
         double jac[TO_MAXP * TO_MAXNM], Dm[TO_MAXP * TO_MAXP], tmp[TO_MAXP * TO_MAXNM];
-        con_jacobian_b<INST>(P, con, b, ci, n, m, x, u, jac);
+        con_jacobian(con, cd, n, m, x, u, jac);
         for (int i = 0; i < p; i++) lbar[i] = lam[i] - mu * c[i];
         const int dc = dualcone(con.sense);
         cone_projection(dc, lbar, p, lp);
@@ -663,4 +576,57 @@ __device__ __forceinline__ void state_diff(bool lie, int n, int qs, const double
     for (int i = 0; i < qs; i++) dx[i] = xbar[i] - x[i];
     quat_diff(x + qs, xbar + qs, dx + qs);
     for (int i = qs + 4; i < n; i++) dx[i - 1] = xbar[i] - x[i];
+}
+
+// Compact error-state expansion of knot k of instance b (P.compact: DiagonalCost objective, Goal / Bound constraints, n_e + m = 16 -- the
+// BASELINE problem class).  The full-state expansion is a gradient g and a DIAGONAL h, so the error-state one is G'g, the same diagonal
+// outside the attitude and the 3 x 3 block G_q' diag(h_q) G_q - (q'g_q) I3 (Altro error_expansion!).  Cost: RD.gradient!/hessian! of
+// DiagonalCost (src/cost_functions.jl:137-233); AL rows of Goal / Bound constraints as in al_knot_expansion.  Logical order: ge = G'g and
+// hd = the diagonal, over the error state and the controls; b01, b02, b12 = the off-diagonal entries of the attitude block.  lie.cu
+// k_expansion_compact (EC) and riccati_frag.cu k_expansion_rec (the record) store it, each in its own layout.
+template <bool INST>   // INST: the linear cost terms and constraint data of each instance
+__device__ __forceinline__ void compact_expansion(const DevProblem& P, int b, int k, double (&ge)[16], double (&hd)[16],
+                                                  double& b01, double& b02, double& b12) {
+    const int n = P.n, m = P.m, nm = n + m, qs = P.qs;
+    const bool last = (k == P.N - 1);
+    const double* xg = traj_X(P, P.cur[b], b) + (size_t)k * n;
+    const double* ug = traj_U(P, P.cur[b], b) + (size_t)k * m;
+    const double* lam_b = P.lambda + (size_t)b * P.lambda_len;
+    double z[TO_MAXNM], g[TO_MAXNM], h[TO_MAXNM];
+    for (int i = 0; i < n; i++) z[i] = xg[i];
+    for (int a = 0; a < m; a++) z[n + a] = last ? 0.0 : ug[a];
+    const int cid = P.cost_index[k];
+    const DevCost& c = P.costs[cid];
+    const double* cq = inst_q<INST>(P, b, cid); const double* cr = inst_r<INST>(P, b, cid);
+    for (int i = 0; i < n; i++) { g[i] = fma(c.Qd[i], z[i], cq[i]); h[i] = c.Qd[i]; }
+    for (int a = 0; a < m; a++) { g[n + a] = last ? 0.0 : fma(c.Rd[a], z[n + a], cr[a]); h[n + a] = last ? 0.0 : c.Rd[a]; }
+    const int lim = last ? n : nm;
+    for (int ci = 0; ci < P.ncon; ci++) {
+        const DevCon& con = P.cons[ci];
+        if (k + 1 < con.first || k + 1 > con.last) continue;
+        const double mu = P.mu[ci];
+        const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
+        const bool eq = (con.kind == CON_GOAL);
+        const ConData cd = con_data<INST>(P, b, ci);
+        const int nrow = eq ? con.p : con.n_max + con.n_min;
+        for (int r = 0; r < nrow; r++) {
+            const int j = eq ? con.inds[r] : (r < con.n_max ? con.a_max[r] : con.a_min[r - con.n_max]);
+            const bool lower = !eq && r >= con.n_max;
+            const double cv = eq ? z[j] - cd.a[r] : (lower ? cd.b[j] - z[j] : z[j] - cd.a[j]);
+            const double lb = lam[r] - mu * cv;
+            if ((eq || lb <= 0.0) && j < lim) { g[j] -= lower ? -lb : lb; h[j] += mu; }
+        }
+    }
+    double G[12]; quat_G(z + qs, G);
+    for (int e = 0; e < qs; e++) { ge[e] = g[e]; hd[e] = h[e]; }
+    for (int e = qs + 3; e < n - 1 + m; e++) { ge[e] = g[e + 1]; hd[e] = h[e + 1]; }
+    double qb = 0;
+    for (int r = 0; r < 4; r++) qb += z[qs + r] * g[qs + r];
+    for (int cc = 0; cc < 3; cc++) {
+        double s = 0, d = 0;
+        for (int r = 0; r < 4; r++) { s += G[cc * 4 + r] * g[qs + r]; d += G[cc * 4 + r] * h[qs + r] * G[cc * 4 + r]; }
+        ge[qs + cc] = s; hd[qs + cc] = d - qb;
+    }
+    b01 = 0; b02 = 0; b12 = 0;
+    for (int r = 0; r < 4; r++) { b01 += G[r] * h[qs + r] * G[4 + r]; b02 += G[r] * h[qs + r] * G[8 + r]; b12 += G[4 + r] * h[qs + r] * G[8 + r]; }
 }

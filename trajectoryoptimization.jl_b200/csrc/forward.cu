@@ -41,6 +41,8 @@ struct FwdCon {
     int row_max[TO_MAXNM], row_min[TO_MAXNM];
     double a[TO_MAXNM], b[TO_MAXNM];
 };
+// the data view (common.cuh con_data) of a staged constraint: its Goal values / Bound limits in shared memory
+__device__ __forceinline__ ConData staged(const FwdCon& c) { return ConData{c.a, c.b}; }
 struct FwdCost {
     double Qd[TO_MAXN], Rd[TO_MAXM], q[TO_MAXN], r[TO_MAXM], c;
 };
@@ -336,8 +338,7 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
                 double a = 0.0, l2 = 0.0;
                 if (c.kind == CON_GOAL) {
                     const unsigned mk = c.mask_max;
-                    const double* ga = c.a;
-                    if constexpr (INST) ga = con_row<true>(P, b, ci, P.cons[ci].a);
+                    const double* ga = con_data<INST>(P, b, ci, staged(c)).a;
 #pragma unroll
                     for (int i = 0; i < n; i++) {
                         if (mk & (1u << i)) {
@@ -350,31 +351,29 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
                     }
                 } else if (c.ubox) {
                     // u_min <= u <= u_max on every control: rows 0..m-1 = upper, m..2m-1 = lower (src/constraints.jl:738-755)
-                    const double* ca = c.a; const double* cb = c.b;
-                    if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ca = cd.a; cb = cd.b; }
+                    const ConData cd = con_data<INST>(P, b, ci, staged(c));
 #pragma unroll
                     for (int i = 0; i < m; i++) {
                         const double lu = st[S::sidx(lo + i, g)], ll = st[S::sidx(lo + m + i, g)];
-                        const double cu = u[i] - ca[n + i], cl = cb[n + i] - u[i];
+                        const double cu = u[i] - cd.a[n + i], cl = cd.b[n + i] - u[i];
                         const double pu = fmin(0.0, fma(-mu, cu, lu)), pl = fmin(0.0, fma(-mu, cl, ll));
                         a = fma(pu, pu, a); a = fma(pl, pl, a); l2 = fma(lu, lu, l2); l2 = fma(ll, ll, l2);
                         viol = fmax(viol, fmax(cu, cl));
                     }
                 } else {
                     const unsigned mx = c.mask_max, mn = c.mask_min;
-                    const double* ca = c.a; const double* cb = c.b;
-                    if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ca = cd.a; cb = cd.b; }
+                    const ConData cd = con_data<INST>(P, b, ci, staged(c));
                     if ((mx | mn) & ((1u << n) - 1u)) {
 #pragma unroll
                         for (int i = 0; i < n; i++) {
-                            if (mx & (1u << i)) { const double lm = st[S::sidx(lo + c.row_max[i], g)]; const double cv = x[i] - ca[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
-                            if (mn & (1u << i)) { const double lm = st[S::sidx(lo + c.row_min[i], g)]; const double cv = cb[i] - x[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
+                            if (mx & (1u << i)) { const double lm = st[S::sidx(lo + c.row_max[i], g)]; const double cv = x[i] - cd.a[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
+                            if (mn & (1u << i)) { const double lm = st[S::sidx(lo + c.row_min[i], g)]; const double cv = cd.b[i] - x[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
                         }
                     }
 #pragma unroll
                     for (int i = 0; i < m; i++) {
-                        if (mx & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_max[n + i], g)]; const double cv = u[i] - ca[n + i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
-                        if (mn & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_min[n + i], g)]; const double cv = cb[n + i] - u[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
+                        if (mx & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_max[n + i], g)]; const double cv = u[i] - cd.a[n + i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
+                        if (mn & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_min[n + i], g)]; const double cv = cd.b[n + i] - u[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
                     }
                 }
                 J = fma(a - l2, c.inv2mu, J);
@@ -564,8 +563,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
             const double mu = c.mu;
             double a = 0.0, l2 = 0.0;
             const unsigned mk = c.mask_max;
-            const double* ga = c.a;
-            if constexpr (INST) ga = con_row<true>(P, b, tab.goal_ci, P.cons[tab.goal_ci].a);
+            const double* ga = con_data<INST>(P, b, tab.goal_ci, staged(c)).a;
 #pragma unroll
             for (int i = 0; i < n; i++) {
                 if (mk & (1u << i)) {
@@ -802,7 +800,7 @@ cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int f
 }
 
 // per-instance linear cost terms / model parameters / constraint data: a kernel variant of its own, so that the shared one is the code it has
-// always been.  It serves every per-instance table; each accessor checks its own (inst_q, model_param, con_data / con_row).
+// always been.  It serves every per-instance table; each accessor checks its own (inst_q, model_param, con_data).
 template <int MODEL, int G, int PATH>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     if (inst_forward(P)) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);

@@ -128,60 +128,20 @@ __global__ void __launch_bounds__(128) k_error_expansion(const DevProblem P, con
     }
 }
 
-// Compact error-state expansion (P.compact: DiagonalCost objective, Goal / Bound constraints -- the BASELINE problem
-// class).  The full-state expansion is a gradient g and a DIAGONAL h, so the error-state one is G'g, the same diagonal outside the
-// attitude and the 3 x 3 block G_q' diag(h_q) G_q - (q'g_q) I3: 40 doubles per knot (TO_EC_LEN) instead of 272.  One thread per
-// (instance, knot); cost: RD.gradient!/hessian! of DiagonalCost (src/cost_functions.jl:137-233),
-// AL rows of Goal / Bound constraints as in al_knot_expansion (costcon.cuh).
-template <bool INST>   // INST: the linear cost terms and Goal values of each instance
+// Compact error-state expansion (P.compact): one thread per (instance, knot), costcon.cuh compact_expansion stored in logical order
+// into EC, 40 doubles per knot (TO_EC_LEN) instead of the 272 of EG + EH.  riccati_frag.cu k_expansion_rec stores the same numbers
+// in the record's order for the register-resident kernel.
+template <bool INST>   // INST: the linear cost terms and constraint data of each instance
 __global__ void __launch_bounds__(128) k_expansion_compact(const DevProblem P) {
-    const int n = P.n, m = P.m, nm = n + m, qs = P.qs;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)P.B * P.N) return;
     const int k = (int)(t % P.N), b = (int)(t / P.N);
     if (retired(P, b)) return;                                     // to_solve: not ACTIVE
-    const bool last = (k == P.N - 1);
-    const double* xg = traj_X(P, P.cur[b], b) + (size_t)k * n;
-    const double* ug = traj_U(P, P.cur[b], b) + (size_t)k * m;
-    const double* lam_b = P.lambda + (size_t)b * P.lambda_len;
-    double z[TO_MAXNM], g[TO_MAXNM], h[TO_MAXNM];
-    for (int i = 0; i < n; i++) z[i] = xg[i];
-    for (int a = 0; a < m; a++) z[n + a] = last ? 0.0 : ug[a];
-    const int cid = P.cost_index[k];
-    const DevCost& c = P.costs[cid];
-    const double* cq = inst_q<INST>(P, b, cid); const double* cr = inst_r<INST>(P, b, cid);
-    for (int i = 0; i < n; i++) { g[i] = fma(c.Qd[i], z[i], cq[i]); h[i] = c.Qd[i]; }
-    for (int a = 0; a < m; a++) { g[n + a] = last ? 0.0 : fma(c.Rd[a], z[n + a], cr[a]); h[n + a] = last ? 0.0 : c.Rd[a]; }
-    const int lim = last ? n : nm;
-    for (int ci = 0; ci < P.ncon; ci++) {
-        const DevCon& con = P.cons[ci];
-        if (k + 1 < con.first || k + 1 > con.last) continue;
-        const double mu = P.mu[ci];
-        const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
-        const bool eq = (con.kind == CON_GOAL);
-        const ConData cd = con_data<INST>(P, b, ci);
-        const int nrow = eq ? con.p : con.n_max + con.n_min;
-        for (int r = 0; r < nrow; r++) {
-            const int j = eq ? con.inds[r] : (r < con.n_max ? con.a_max[r] : con.a_min[r - con.n_max]);
-            const bool lower = !eq && r >= con.n_max;
-            const double cv = eq ? z[j] - cd.a[r] : (lower ? cd.b[j] - z[j] : z[j] - cd.a[j]);
-            const double lb = lam[r] - mu * cv;
-            if ((eq || lb <= 0.0) && j < lim) { g[j] -= lower ? -lb : lb; h[j] += mu; }
-        }
-    }
+    double ge[16], hd[16], b01, b02, b12;
+    compact_expansion<INST>(P, b, k, ge, hd, b01, b02, b12);
     double* out = P.EC + t * TO_EC_LEN;
-    double G[12]; quat_G(z + qs, G);
-    for (int e = 0; e < qs; e++) { out[e] = g[e]; out[16 + e] = h[e]; }
-    for (int e = qs + 3; e < n - 1 + m; e++) { out[e] = g[e + 1]; out[16 + e] = h[e + 1]; }
-    double qb = 0;
-    for (int r = 0; r < 4; r++) qb += z[qs + r] * g[qs + r];
-    for (int cc = 0; cc < 3; cc++) {
-        double s = 0, d = 0;
-        for (int r = 0; r < 4; r++) { s += G[cc * 4 + r] * g[qs + r]; d += G[cc * 4 + r] * h[qs + r] * G[cc * 4 + r]; }
-        out[qs + cc] = s; out[16 + qs + cc] = d - qb;
-    }
-    double b01 = 0, b02 = 0, b12 = 0;
-    for (int r = 0; r < 4; r++) { b01 += G[r] * h[qs + r] * G[4 + r]; b02 += G[r] * h[qs + r] * G[8 + r]; b12 += G[4 + r] * h[qs + r] * G[8 + r]; }
+#pragma unroll
+    for (int e = 0; e < 16; e++) { out[e] = ge[e]; out[16 + e] = hd[e]; }
     out[32] = b01; out[33] = b02; out[34] = b12;
     for (int e = 35; e < TO_EC_LEN; e++) out[e] = 0.0;
 }

@@ -345,14 +345,9 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     if (lane == 0) {
                         double uz[M_];
                         for (int a = 0; a < m; a++) uz[a] = terminal ? 0.0 : U[(size_t)(k1 - 1) * m + a];
-                        if constexpr (INST) {
-                            const ConData cd = con_data<true>(P, b, ci);
-                            con_evaluate(con, cd, n, m, xk, uz, sm.gc);
-                            con_jacobian(con, cd, n, m, xk, uz, sm.gjac);
-                        } else {
-                            con_evaluate(con, n, m, xk, uz, sm.gc);
-                            con_jacobian(con, n, m, xk, uz, sm.gjac);
-                        }
+                        const ConData cd = con_data<INST>(P, b, ci);
+                        con_evaluate(con, cd, n, m, xk, uz, sm.gc);
+                        con_jacobian(con, cd, n, m, xk, uz, sm.gjac);
                     }
                     __syncwarp();
                     if (lane < p) sm.glbar[lane] = lam[lane] - mu * sm.gc[lane];
@@ -429,14 +424,13 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                             const double* lam = lam_b + con.offset + (size_t)(N - con.first) * con.p;
                             if (con.kind == CON_GOAL) {
                                 const int row = con.row_max[i];
-                                if (row >= 0) { const double lp = lam[row] - mu * (xi - con_row<INST>(P, b, ci, con.a)[row]); gi -= lp; hi += mu; }
+                                if (row >= 0) { const double lp = lam[row] - mu * (xi - con_data<INST>(P, b, ci).a[row]); gi -= lp; hi += mu; }
                             } else if (con.kind == CON_BOUND) {
-                                const double* ba = con.a; const double* bb = con.b;
-                                if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ba = cd.a; bb = cd.b; }
+                                const ConData cd = con_data<INST>(P, b, ci);
                                 int row = con.row_max[i];
-                                if (row >= 0) { const double lb = lam[row] - mu * (xi - ba[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
+                                if (row >= 0) { const double lb = lam[row] - mu * (xi - cd.a[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
                                 row = con.row_min[i];
-                                if (row >= 0) { const double lb = lam[row] - mu * (bb[i] - xi); if (lb <= 0) { gi += lb; hi += mu; } }
+                                if (row >= 0) { const double lb = lam[row] - mu * (cd.b[i] - xi); if (lb <= 0) { gi += lb; hi += mu; } }
                             }
                         }
                         if (cost.diag) sm.S[i * LDS_ + i] = hi; else sm.S[i * LDS_ + i] += hi;
@@ -513,14 +507,13 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                                 const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
                                 if (con.kind == CON_GOAL) {
                                     const int row = (i < n) ? con.row_max[i] : -1;
-                                    if (row >= 0) { const double lp = lam[row] - mu * (zi - con_row<INST>(P, b, ci, con.a)[row]); gi -= lp; hi += mu; }
+                                    if (row >= 0) { const double lp = lam[row] - mu * (zi - con_data<INST>(P, b, ci).a[row]); gi -= lp; hi += mu; }
                                 } else if (con.kind == CON_BOUND) {
-                                    const double* ba = con.a; const double* bb = con.b;
-                                    if constexpr (INST) { const ConData cd = con_data<true>(P, b, ci); ba = cd.a; bb = cd.b; }
+                                    const ConData cd = con_data<INST>(P, b, ci);
                                     int row = con.row_max[i];
-                                    if (row >= 0) { const double lb = lam[row] - mu * (zi - ba[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
+                                    if (row >= 0) { const double lb = lam[row] - mu * (zi - cd.a[i]); if (lb <= 0) { gi -= lb; hi += mu; } }
                                     row = con.row_min[i];
-                                    if (row >= 0) { const double lb = lam[row] - mu * (bb[i] - zi); if (lb <= 0) { gi += lb; hi += mu; } }
+                                    if (row >= 0) { const double lb = lam[row] - mu * (cd.b[i] - zi); if (lb <= 0) { gi += lb; hi += mu; } }
                                 }
                             }
                         }

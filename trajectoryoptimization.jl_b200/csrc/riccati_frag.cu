@@ -116,59 +116,19 @@ __device__ __forceinline__ double rcp_pos(double x) {
 }
 
 // ---- compact error-state expansion into the record --------------------------------------------------------------------------------
-// One thread per (instance, knot).  Full-state expansion of a DiagonalCost + Goal / Bound AL rows is a gradient g and a DIAGONAL h;
-// on the error state it is G'g, the same diagonal outside the attitude, and the 3 x 3 block G_q' diag(h_q) G_q - (q'g_q) I3
-// (Altro error_expansion!; lie.cu k_expansion_compact computes the same numbers in logical order for the shared-memory kernel).
-template <bool INST>   // INST: the linear cost terms and Goal values of each instance
+// One thread per (instance, knot): costcon.cuh compact_expansion, stored in the record's physical order (lie.cu k_expansion_compact stores
+// the same numbers in logical order for the shared-memory kernel).  rollout.cu k_expansion_rec16b computes them by another schedule from the
+// host-built term table; this kernel is its fallback where that table does not reach (capi.cu rec_fused: more than TO_EXP_MAXT Goal / Bound
+// rows on one z entry, N >= 4095, or 128 rows at one knot).
+template <bool INST>   // INST: the linear cost terms and constraint data of each instance
 __global__ void __launch_bounds__(128) k_expansion_rec(const DevProblem P) {
-    const int n = P.n, m = P.m, nm = n + m, qs = P.qs;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)P.B * P.N) return;
     const int k = (int)(t % P.N), b = (int)(t / P.N);
     if (retired(P, b)) return;                                     // to_solve: not ACTIVE
-    const bool last = (k == P.N - 1);
-    const double* xg = traj_X(P, P.cur[b], b) + (size_t)k * n;
-    const double* ug = traj_U(P, P.cur[b], b) + (size_t)k * m;
-    const double* lam_b = P.lambda + (size_t)b * P.lambda_len;
-    double z[TO_MAXNM], g[TO_MAXNM], h[TO_MAXNM];
-    for (int i = 0; i < n; i++) z[i] = xg[i];
-    for (int a = 0; a < m; a++) z[n + a] = last ? 0.0 : ug[a];
-    const int cid = P.cost_index[k];
-    const DevCost& c = P.costs[cid];
-    const double* cq = inst_q<INST>(P, b, cid); const double* cr = inst_r<INST>(P, b, cid);
-    for (int i = 0; i < n; i++) { g[i] = fma(c.Qd[i], z[i], cq[i]); h[i] = c.Qd[i]; }
-    for (int a = 0; a < m; a++) { g[n + a] = last ? 0.0 : fma(c.Rd[a], z[n + a], cr[a]); h[n + a] = last ? 0.0 : c.Rd[a]; }
-    const int lim = last ? n : nm;
-    for (int ci = 0; ci < P.ncon; ci++) {
-        const DevCon& con = P.cons[ci];
-        if (k + 1 < con.first || k + 1 > con.last) continue;
-        const double mu = P.mu[ci];
-        const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
-        const bool eq = (con.kind == CON_GOAL);
-        const ConData cd = con_data<INST>(P, b, ci);
-        const int nrow = eq ? con.p : con.n_max + con.n_min;
-        for (int r = 0; r < nrow; r++) {
-            const int j = eq ? con.inds[r] : (r < con.n_max ? con.a_max[r] : con.a_min[r - con.n_max]);
-            const bool lower = !eq && r >= con.n_max;
-            const double cv = eq ? z[j] - cd.a[r] : (lower ? cd.b[j] - z[j] : z[j] - cd.a[j]);
-            const double lb = lam[r] - mu * cv;
-            if ((eq || lb <= 0.0) && j < lim) { g[j] -= lower ? -lb : lb; h[j] += mu; }
-        }
-    }
+    double ge[16], hd[16], b01, b02, b12;
+    compact_expansion<INST>(P, b, k, ge, hd, b01, b02, b12);
     double* out = P.REC + t * TO_REC_LEN;
-    double G[12]; quat_G(z + qs, G);
-    double ge[16], hd[16];
-    for (int e = 0; e < qs; e++) { ge[e] = g[e]; hd[e] = h[e]; }
-    for (int e = qs + 3; e < n - 1 + m; e++) { ge[e] = g[e + 1]; hd[e] = h[e + 1]; }
-    double qb = 0;
-    for (int r = 0; r < 4; r++) qb += z[qs + r] * g[qs + r];
-    for (int cc = 0; cc < 3; cc++) {
-        double s = 0, d = 0;
-        for (int r = 0; r < 4; r++) { s += G[cc * 4 + r] * g[qs + r]; d += G[cc * 4 + r] * h[qs + r] * G[cc * 4 + r]; }
-        ge[qs + cc] = s; hd[qs + cc] = d - qb;
-    }
-    double b01 = 0, b02 = 0, b12 = 0;
-    for (int r = 0; r < 4; r++) { b01 += G[r] * h[qs + r] * G[4 + r]; b02 += G[r] * h[qs + r] * G[8 + r]; b12 += G[4 + r] * h[qs + r] * G[8 + r]; }
 #pragma unroll
     for (int j = 0; j < 16; j++) { out[TO_REC_G + fraglayout::phys_z(j)] = ge[j]; out[TO_REC_HD + fraglayout::phys_z(j)] = hd[j]; }
     // Hb[a][b] = H~[8+2a][8+2b]: a, b = 0..2 the attitude error (e = 3..5), a = 3 is p = 14 (e = 7)

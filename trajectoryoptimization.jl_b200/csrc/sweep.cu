@@ -25,7 +25,7 @@ __device__ __forceinline__ double warp_max(double v) {
     return v;
 }
 
-// INST (here and below): per-instance linear cost terms / Goal values, a variant of its own so that the shared one stays as it is
+// INST (here and below): per-instance linear cost terms / constraint data, a variant of its own so that the shared one stays as it is
 template <bool WITH_AL, bool INST>
 __global__ void __launch_bounds__(128) k_cost(const DevProblem P, double* __restrict__ J, double* __restrict__ Jk,
                                               double* __restrict__ viol_out) {
@@ -114,7 +114,7 @@ __global__ void k_eval_constraints(const DevProblem P, int ci, double* __restric
     const double* x = traj_X(P, P.cur[b], b) + (size_t)(k1 - 1) * P.n;
     const double* u = (k1 == P.N) ? zero_u : traj_U(P, P.cur[b], b) + (size_t)(k1 - 1) * P.m;
     double c[TO_MAXPV];
-    con_evaluate_b<INST>(P, con, b, ci, P.n, P.m, x, u, c);
+    con_evaluate(con, con_data<INST>(P, b, ci), P.n, P.m, x, u, c);
     for (int i = 0; i < con.p; i++) vals[t * con.p + i] = c[i];
 }
 
@@ -144,7 +144,7 @@ __global__ void k_constraint_jacobians(const DevProblem P, int ci, double* __res
     double zero_u[TO_MAXM] = {0};
     const double* x = traj_X(P, P.cur[b], b) + (size_t)(k1 - 1) * P.n;
     const double* u = (k1 == P.N) ? zero_u : traj_U(P, P.cur[b], b) + (size_t)(k1 - 1) * P.m;
-    con_jacobian_b<INST>(P, con, b, ci, P.n, P.m, x, u, jac + t * con.p * (P.n + P.m));
+    con_jacobian(con, con_data<INST>(P, b, ci), P.n, P.m, x, u, jac + t * con.p * (P.n + P.m));
 }
 
 __global__ void k_projection(int cone, int p, int count, const double* __restrict__ x, double* __restrict__ px, int* err) {
@@ -181,7 +181,7 @@ __global__ void k_al_update(const DevProblem P) {
             const double* u = (k1 == P.N) ? zero_u : U + (size_t)(k1 - 1) * P.m;
             double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
             double* lam = lam_b + con.offset + (size_t)(k1 - con.first) * con.p;
-            con_evaluate_b<INST>(P, con, b, ci, P.n, P.m, x, u, c);
+            con_evaluate(con, con_data<INST>(P, b, ci), P.n, P.m, x, u, c);
             for (int i = 0; i < con.p; i++) lbar[i] = lam[i] - mu * c[i];
             cone_projection(dualcone(con.sense), lbar, con.p, lp);
             for (int i = 0; i < con.p; i++) lam[i] = fmax(-P.opt.dual_max, fmin(P.opt.dual_max, lp[i]));
