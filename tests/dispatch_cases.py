@@ -4,9 +4,9 @@ straddles its threshold, the oracle runs both sides) and tests/test_gpu_dispatch
 built for, and matches the oracle there).
 
 Every builder takes the Problem class (CUDA or oracle) and returns the same problem for both.  The restatement mirrors, constant for
-constant, the launch-time predicates of csrc/forward.cu (linesearch_path), riccati.cu (backward_kernel_of, riccati_fastal),
-riccati_small.cu (riccati_small_supported), riccati_frag.cu and capi.cu (to_create's problem flags, rec_fused); `to_kernel_choice`
-reports what the library itself decided.  A change to one of those constants has to move the matching case here."""
+constant, the launch-time predicates of csrc/forward.cu (linesearch_path), riccati.cu (backward_plan: the backward kernel, FASTAL and
+the records' term table), riccati_small.cu (riccati_small_supported), riccati_frag.cu and capi.cu (to_create's problem flags);
+`to_kernel_choice` reports what the library itself decided.  A change to one of those constants has to move the matching case here."""
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -16,8 +16,8 @@ import trajopt_b200 as TO
 # the thresholds, as the library has them
 FWD_MAX_N = 512          # forward.cu: FwdTab::dt / cost_index / lam_off / lam_cnt
 FWD_MAX_COST = 4         # forward.cu: costs cached in shared memory
-MAXT = 3                 # riccati.cu: lane-resident AL terms per z entry (FASTAL); the records' term table (rec_fused)
-MAXP_KNOT_PACKED = 128   # riccati.cu / capi.cu: rows per knot of the packed term fields (FASTAL, rec_fused)
+MAXT = 3                 # common.cuh TO_EXP_MAXT: lane-resident AL terms per z entry (FASTAL); the records' term table (rec_fused)
+MAXP_KNOT_PACKED = 128   # riccati.cu backward_plan: rows per knot of the packed term fields (FASTAL, rec_fused)
 SOLVER_MAXP = 16         # capi.cu solver_supported: rows per general constraint in the solver kernels
 CREATE_MAXP = 32         # capi.cu build_con (TO_MAXP): rows per general constraint
 SMALL_WAVE = 16          # riccati_small.cu: the thread kernel past 16 one-warp CTAs per SM

@@ -194,7 +194,7 @@ struct PhaseScope {
 
 void set_default_options(DevOptions& o) {
     o.bp_reg_increase_factor = 1.6; o.bp_reg_max = 1e8; o.bp_reg_min = 1e-8; o.bp_reg_initial = 0.0; o.bp_reg_fp = 10.0;
-    o.ls_lower = 1e-8; o.ls_upper = 10.0; o.ls_iters = 10; o.pad = 0;
+    o.ls_lower = 1e-8; o.ls_upper = 10.0; o.ls_iters = 10; o.backward_kernel = 0;
     o.max_state_value = 1e8; o.max_control_value = 1e8;
     o.penalty_initial = 1.0; o.penalty_scaling = 10.0; o.penalty_max = 1e8; o.dual_max = 1e8;
 }
@@ -739,7 +739,7 @@ int to_set_options(to_handle* h, const to_options* o) {
     d.bp_reg_increase_factor = o->bp_reg_increase_factor; d.bp_reg_max = o->bp_reg_max; d.bp_reg_min = o->bp_reg_min;
     d.bp_reg_initial = o->bp_reg_initial; d.bp_reg_fp = o->bp_reg_fp;
     d.ls_lower = o->line_search_lower_bound; d.ls_upper = o->line_search_upper_bound; d.ls_iters = o->iterations_linesearch;
-    d.pad = o->backward_kernel;   // kernel choice of launch_backward (0 automatic)
+    d.backward_kernel = o->backward_kernel;
     d.max_state_value = o->max_state_value; d.max_control_value = o->max_control_value;
     d.penalty_initial = o->penalty_initial; d.penalty_scaling = o->penalty_scaling; d.penalty_max = o->penalty_max; d.dual_max = o->dual_max;
     if (reset_mu) for (auto& mu : h->h_mu) mu = d.penalty_initial;
@@ -1156,12 +1156,6 @@ int to_rollout(to_handle* h) {
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
-// the records' cost + AL expansion comes from the host-built term table (common.cuh ExpTab) when the Goal / Bound rows fit it:
-// <= 3 rows per z entry, knot indices < 4095, < 128 rows per knot; otherwise k_expansion_rec walks the descriptors
-static bool rec_fused(const DevProblem& P) { return P.frag && P.max_terms_per_z <= 3 && P.N < 4095 && P.max_p_knot < 128; }
-// the record path (k_riccati_frag) unless to_options.backward_kernel forces a shared-memory kernel: 3 generic DFMA kernel on the full
-// expansion, 5 tensor kernel on the compact expansion
-static bool record_path(const DevProblem& P) { return P.frag && P.opt.pad != 3 && P.opt.pad != 5; }
 int to_expand(to_handle* h) {
     JOIN(h);
     if (!h) return TO_EINVAL;
@@ -1333,28 +1327,26 @@ static int materialise_expansion(to_handle* h, double* EG, double* EH) {
     CU(h, launch_error_expansion(P, gf, hf, EG, EH, h->stream)); h->launches++;
     return TO_OK;
 }
-static int do_backward(to_handle* h, bool costexp_done = false) {
-    if (record_path(h->P)) {
+static int do_backward(to_handle* h, const BackwardPlan& plan, bool costexp_done = false) {
+    if (plan.kernel == KC_BK_FRAGMENT) {
         if (!costexp_done) {   // cost + AL expansion of every record: always from the current trajectory, multipliers and penalties
             PhaseScope pe(h, TO_PHASE_COSTEXP);
-            if (rec_fused(h->P)) CU(h, launch_expansion_rec16(h->P, h->stream, 0));      // 16 lanes per knot, host-built term table
-            else CU(h, launch_expansion_rec(h->P, h->stream));                          // more than 3 rows on one z entry: descriptor walk
+            if (plan.expansion == BackwardPlan::REC_TABLE) CU(h, launch_expansion_rec16(h->P, h->stream, 0));   // 16 lanes per knot
+            else CU(h, launch_expansion_rec(h->P, h->stream));
             h->launches++; h->phase_launches[TO_PHASE_COSTEXP]++;
         }
         h->rec_costexp = true;     // (costexp_done: to_ilqr_step launched it, split or not)
         PhaseScope ps(h, TO_PHASE_BACKWARD);
         CU(h, launch_backward_frag(h->P, h->d_fragq, h->d_fragpool, h->d_fragerr, h->stream));
-    } else if (h->P.dense_riccati) {
-        PhaseScope ps(h, TO_PHASE_BACKWARD);
-        if (h->P.frag) { CU(h, launch_export_abe(h->P, h->stream)); h->launches++; }     // the shared-memory kernels read P.ABe
-        DevProblem Q = h->P;
-        Q.compact = (h->P.compact && h->P.opt.pad != 3) ? 1 : 0;      // backward_kernel = 3: the generic (DFMA, full expansion) kernel
-        if (Q.compact) { CU(h, launch_expansion_compact(Q, h->stream)); h->launches++; }
-        else { int rc = materialise_expansion(h, h->P.EG, h->P.EH); if (rc) return rc; }
-        if (!Q.lie) { CU(h, launch_error_dynamics(Q, h->stream)); h->launches++; }   // error state: [A_e B_e] comes from k_expand_lie
-        CU(h, launch_backward_dense(Q, h->stream));
     } else {
-        PhaseScope ps(h, TO_PHASE_BACKWARD); CU(h, launch_backward(h->P, h->d_work, h->stream));
+        PhaseScope ps(h, TO_PHASE_BACKWARD);
+        if (plan.expansion != BackwardPlan::IN_KERNEL) {   // lie.cu: the expansion and [A_e B_e] in HBM before the kernel
+            if (h->P.frag) { CU(h, launch_export_abe(h->P, h->stream)); h->launches++; }     // the shared-memory kernels read P.ABe
+            if (plan.expansion == BackwardPlan::COMPACT) { CU(h, launch_expansion_compact(h->P, h->stream)); h->launches++; }
+            else { int rc = materialise_expansion(h, h->P.EG, h->P.EH); if (rc) return rc; }
+            if (!h->P.lie) { CU(h, launch_error_dynamics(h->P, h->stream)); h->launches++; }   // error state: [A_e B_e] comes from k_expand_lie
+        }
+        CU(h, launch_backward(h->P, plan, h->d_work, h->stream));
     }
     h->launches++; h->phase_launches[TO_PHASE_BACKWARD]++;
     h->backward_done = true;
@@ -1374,7 +1366,7 @@ int to_backward(to_handle* h, int32_t* status) {
     if (!h) return TO_EINVAL;
     int rc = solver_supported(h); if (rc) return rc;
     if (!h->expanded) return fail(h, TO_ESTATE, "to_backward before to_expand");
-    rc = do_backward(h); if (rc) return rc;
+    rc = do_backward(h, backward_plan(h->P)); if (rc) return rc;
     if (status) {
         CU(h, cudaMemcpyAsync(status, h->P.bp_status, sizeof(int) * h->P.B, cudaMemcpyDeviceToHost, h->stream));
         CU(h, cudaStreamSynchronize(h->stream));
@@ -1412,7 +1404,8 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
     // (error state: only [A_e B_e] is needed by the solver kernels -- k_expand_lie; the full [A B] is produced by to_expand on request)
     auto expand = [&](cudaStream_t st, int mode) { return h->P.lie ? launch_expand_lie(h->P, st, mode) : launch_expand(h->P, st, mode); };
     bool costexp_done = false;
-    const bool rec = record_path(h->P) && rec_fused(h->P);
+    const BackwardPlan plan = backward_plan(h->P);
+    const bool rec = plan.expansion == BackwardPlan::REC_TABLE;
     if (h->side_pending) {
         {
             PhaseScope pl(h, TO_PHASE_LATE, h->stream2);
@@ -1431,7 +1424,7 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
     h->launches++; h->phase_launches[TO_PHASE_EXPAND]++;
     JOIN(h);
     h->expanded = true;
-    int rc = do_backward(h, costexp_done); if (rc) return rc;
+    int rc = do_backward(h, plan, costexp_done); if (rc) return rc;
     { PhaseScope ps(h, TO_PHASE_FORWARD); CU(h, launch_forward(h->P, h->stream)); }
     h->launches++; h->phase_launches[TO_PHASE_FORWARD]++;
     if (h->overlap) {
@@ -1576,7 +1569,7 @@ int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* 
 // ---- Lie-group error state (lie.cu) ---------------------------------------------------------------------------
 int to_backward_algebra(const to_handle* h, int32_t* variant) {
     if (!h || !variant) return TO_EINVAL;
-    *variant = record_path(h->P) ? 1 : 0;
+    *variant = backward_plan(h->P).kernel == KC_BK_FRAGMENT ? 1 : 0;
     return TO_OK;
 }
 static_assert(TO_LS_GENERIC == KC_LS_GENERIC && TO_LS_FAST == KC_LS_FAST && TO_LS_COMPACT == KC_LS_COMPACT, "to_linesearch_loop");
@@ -1584,20 +1577,20 @@ static_assert(TO_BK_THREAD == KC_BK_THREAD && TO_BK_WARP_MMA == KC_BK_WARP_MMA &
               TO_BK_DENSE_MMA == KC_BK_DENSE_MMA && TO_BK_DENSE_DFMA == KC_BK_DENSE_DFMA, "to_backward_kernel");
 int to_kernel_choice(const to_handle* h, int32_t* choice) {
     if (!h || !choice) return TO_EINVAL;
-    DeviceGuard device_guard(h);     // the SM count (riccati_small_supported) and the resident warps are those of the handle's device
+    DeviceGuard device_guard(h);     // the SM count (backward_plan) and the resident warps are those of the handle's device
     const DevProblem& P = h->P;
     const int ls = linesearch_path(P);
-    const int bk = record_path(P) ? KC_BK_FRAGMENT : backward_kernel_of(P);   // do_backward
+    const BackwardPlan plan = backward_plan(P);
     choice[TO_CHOICE_LINESEARCH] = ls;
     choice[TO_CHOICE_COST_CACHED] = (ls != KC_LS_GENERIC && linesearch_costs_cached(P)) ? 1 : 0;
-    choice[TO_CHOICE_BACKWARD] = bk;
-    choice[TO_CHOICE_FASTAL] = ((bk == KC_BK_WARP_MMA || bk == KC_BK_WARP_DFMA) && riccati_fastal(P)) ? 1 : 0;
-    choice[TO_CHOICE_REC_FUSED] = (record_path(P) && rec_fused(P)) ? 1 : 0;
+    choice[TO_CHOICE_BACKWARD] = plan.kernel;
+    choice[TO_CHOICE_FASTAL] = plan.fastal ? 1 : 0;
+    choice[TO_CHOICE_REC_FUSED] = plan.expansion == BackwardPlan::REC_TABLE ? 1 : 0;
     choice[TO_CHOICE_LATE_LIST] = P.late_list ? 1 : 0;
     choice[TO_CHOICE_INST_FORWARD] = inst_forward(P) ? 1 : 0;     // launch_pass
     choice[TO_CHOICE_INST_BACKWARD] = inst_backward(P) ? 1 : 0;   // k_riccati, k_riccati_small, k_expansion_rec(16b), k_expansion_compact,
                                                                   // k_al_expansion, k_al_update, k_cost, k_eval_constraints, k_constraint_jacobians
-    choice[TO_CHOICE_RESIDENT] = bk == KC_BK_FRAGMENT ? frag_resident_warps() : 0;
+    choice[TO_CHOICE_RESIDENT] = plan.kernel == KC_BK_FRAGMENT ? frag_resident_warps() : 0;
     return TO_OK;
 }
 int to_error_state_dim(const to_handle* h, int32_t* ne) {
@@ -1644,7 +1637,7 @@ int to_error_expansion(to_handle* h, double* grad, double* hess) {
 int to_get_expansion_records(to_handle* h, double* out) {
     JOIN(h);
     if (!h || !out) return TO_EINVAL;
-    if (!(h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5)) return fail(h, TO_ESTATE, "to_get_expansion_records: the handle is not on the record path");
+    if (backward_plan(h->P).kernel != KC_BK_FRAGMENT) return fail(h, TO_ESTATE, "to_get_expansion_records: the handle is not on the record path");
     if (!h->rec_costexp) return fail(h, TO_ESTATE, "to_get_expansion_records before any backward pass wrote the records' expansion");
     constexpr int W = TO_REC_LEN - TO_REC_G;
     CU(h, cudaMemcpy2DAsync(out, W * sizeof(double), h->P.REC + TO_REC_G, TO_REC_LEN * sizeof(double), W * sizeof(double), (size_t)h->P.B * h->P.N,
@@ -1767,13 +1760,13 @@ int to_algorithmic_bytes(const to_handle* h, int64_t* E, int64_t* R, int64_t* F)
     //   compact (error state, diagonal costs, Goal/Bound): XU + L -> EC (40 per knot) ; EC + [A_e B_e] -> K, d
     //   generic: full-state expansion (scratch) -> error-state expansion (HES) ; [A B] -> [A_e B_e] unless k_expand_lie wrote it
     const int64_t EC = (int64_t)TO_EC_LEN * N, HESF = ((n + m) * (n + m) + (n + m)) * N;
-    if (R) {
+    if (R) switch (backward_plan(h->P).expansion) {
         // record path (riccati_frag.cu): the Riccati kernel is timed alone; its compulsory inputs are [A_e B_e], the trajectory and the
         // multipliers (what the expansion it consumes is made of), its outputs the gains -- SURVEY 8(d)'s R column on the error state
-        if (h->P.frag && h->P.opt.pad != 3 && h->P.opt.pad != 5) *R = (ABe + XU + KD + L) * w;
-        else if (h->P.compact && h->P.opt.pad != 3) *R = (XU + L + 2 * EC + ABe + KD) * w;
-        else if (h->P.dense_riccati) *R = (XU + L + 2 * HESF + 2 * HES + (h->P.lie ? 0 : AB + ABe) + ABe + KD) * w;
-        else *R = (AB + XU + KD + L) * w;
+        case BackwardPlan::REC_TABLE: case BackwardPlan::REC_WALK: *R = (ABe + XU + KD + L) * w; break;
+        case BackwardPlan::COMPACT: *R = (XU + L + 2 * EC + ABe + KD) * w; break;
+        case BackwardPlan::MATERIALISED: *R = (XU + L + 2 * HESF + 2 * HES + (h->P.lie ? 0 : AB + ABe) + ABe + KD) * w; break;
+        case BackwardPlan::IN_KERNEL: *R = (AB + XU + KD + L) * w; break;
     }
     if (E && h->P.lie) *E = (XU + ABe) * w;     // k_expand_lie writes [A_e B_e] only
     if (F) *F = (2 * XU + KD + L) * w + 8;

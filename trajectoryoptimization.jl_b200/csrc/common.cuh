@@ -96,7 +96,7 @@ struct DevDyn {
 struct DevOptions {
     double bp_reg_increase_factor, bp_reg_max, bp_reg_min, bp_reg_initial, bp_reg_fp;
     double ls_lower, ls_upper;
-    int ls_iters, pad;
+    int ls_iters, backward_kernel;   // to_options.backward_kernel (riccati.cu backward_plan)
     double max_state_value, max_control_value;
     double penalty_initial, penalty_scaling, penalty_max, dual_max;
 };

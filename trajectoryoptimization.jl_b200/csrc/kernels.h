@@ -23,15 +23,30 @@ cudaError_t launch_shift_traj(const DevProblem& P, int steps, cudaStream_t s);
 cudaError_t launch_gather_traj(const DevProblem& P, double* Xout, double* Uout, cudaStream_t s);
 cudaError_t launch_scatter_traj(const DevProblem& P, const double* Xin, const double* Uin, cudaStream_t s);
 cudaError_t launch_export_ab(const DevProblem& P, double* ABout, cudaStream_t s);
+// Kernel choices made from the problem's shape.  The launchers and the diagnostics (capi.cu) ask the functions below, so each reports what
+// the launch does.  The values are those of include/trajopt_b200.h (TO_LS_*, TO_BK_*).
+enum { KC_LS_GENERIC = 0, KC_LS_FAST = 1, KC_LS_COMPACT = 2 };
+enum { KC_BK_THREAD = 0, KC_BK_WARP_MMA = 1, KC_BK_WARP_DFMA = 2, KC_BK_FRAGMENT = 3, KC_BK_DENSE_MMA = 4, KC_BK_DENSE_DFMA = 5 };
+struct BackwardPlan {
+    int kernel;   // KC_BK_*: the kernel launch_backward / launch_backward_frag launches
+    // where it reads the cost + AL expansion: in k_riccati / k_riccati_small; the records, by k_expansion_rec16b from the term table
+    // (common.cuh ExpTab) or by k_expansion_rec walking the descriptors; EC (k_expansion_compact); EG / EH (k_al_expansion + k_error_expansion)
+    enum Expansion { IN_KERNEL, REC_TABLE, REC_WALK, COMPACT, MATERIALISED } expansion;
+    bool fastal;  // k_riccati holds the AL terms lane-resident
+};
+BackwardPlan backward_plan(const DevProblem& P);   // riccati.cu: the only place that chooses the backward pass
+int linesearch_path(const DevProblem& P);          // forward.cu: the knot loop of the line search (KC_LS_*)
+bool linesearch_costs_cached(const DevProblem& P);  // forward.cu: the fast / compact loop reads the costs from shared memory
+int frag_resident_warps();                          // riccati_frag.cu: k_riccati_frag warps (= instances) resident at once on this device
 // kernel 3: Riccati backward pass                                             (riccati.cu)
-cudaError_t launch_backward(const DevProblem& P, int* work_counter, cudaStream_t s);
+cudaError_t launch_backward(const DevProblem& P, const BackwardPlan& plan, int* work_counter, cudaStream_t s);   // every kernel but KC_BK_FRAGMENT
 bool riccati_small_supported(const DevProblem& P, bool any_batch);                     // riccati_small.cu: thread-per-instance pass for n <= 4, m <= 2
 cudaError_t launch_backward_small(const DevProblem& P, cudaStream_t s);
 // Lie-group error state + Riccati pass on a materialised expansion               (lie.cu)
 cudaError_t launch_state_diff(const DevProblem& P, const double* Xbar, double* dx, cudaStream_t s);
 cudaError_t launch_error_dynamics(const DevProblem& P, cudaStream_t s);
 cudaError_t launch_error_expansion(const DevProblem& P, const double* gfull, const double* hfull, double* EG, double* EH, cudaStream_t s);
-cudaError_t launch_backward_dense(const DevProblem& P, cudaStream_t s);
+cudaError_t launch_backward_dense(const DevProblem& P, const BackwardPlan& plan, cudaStream_t s);
 cudaError_t launch_expansion_compact(const DevProblem& P, cudaStream_t s);             // EC of every knot (P.compact)
 cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode = 0);     // [A_e B_e] straight from the dual-number RK4 step (rollout.cu)
 // register-resident Riccati pass of the error-state Quadrotor + its record producers   (riccati_frag.cu)
@@ -43,16 +58,6 @@ cudaError_t launch_export_abe(const DevProblem& P, cudaStream_t s);             
 size_t frag_queue_ints(int B);
 size_t frag_pool_doubles(int B, int N);                                                 // doubles of the speculative candidates' gain pool                                                         // ints of the kernel's work queue (allocated by the handle)
 cudaError_t launch_backward_frag(const DevProblem& P, int* queue, double* pool, int* sticky_err, cudaStream_t s);
-// Kernel choices made from the problem's shape.  The launchers and to_kernel_choice (capi.cu) both call these, so the diagnostic reports
-// what the launch does.  The values are those of include/trajopt_b200.h (TO_LS_*, TO_BK_*).
-enum { KC_LS_GENERIC = 0, KC_LS_FAST = 1, KC_LS_COMPACT = 2 };
-enum { KC_BK_THREAD = 0, KC_BK_WARP_MMA = 1, KC_BK_WARP_DFMA = 2, KC_BK_FRAGMENT = 3, KC_BK_DENSE_MMA = 4, KC_BK_DENSE_DFMA = 5 };
-int linesearch_path(const DevProblem& P);          // forward.cu: the knot loop of the line search (KC_LS_*)
-bool linesearch_costs_cached(const DevProblem& P);  // forward.cu: the fast / compact loop reads the costs from shared memory
-int backward_kernel_of(const DevProblem& P);       // riccati.cu: the kernel launch_backward launches (KC_BK_*, never KC_BK_FRAGMENT)
-bool riccati_fastal(const DevProblem& P);           // riccati.cu: k_riccati holds the AL terms lane-resident (FASTAL)
-bool dense_backward_mma(const DevProblem& P);       // lie.cu: launch_backward_dense takes the tensor-MMA kernel
-int frag_resident_warps();                          // riccati_frag.cu: k_riccati_frag warps (= instances) resident at once on this device
 // forward pass: closed-loop rollout + merit + line search                     (forward.cu)
 cudaError_t launch_forward(const DevProblem& P, cudaStream_t s);
 cudaError_t launch_ladder(const DevProblem& P, cudaStream_t s);

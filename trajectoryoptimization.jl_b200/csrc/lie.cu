@@ -605,7 +605,7 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
 #ifndef TO_DENSE_WARPS
 #define TO_DENSE_WARPS 2     // warps (= instances) per CTA of k_riccati_dense_mma; A/B: profiles/build_lie_variants.sh
 #endif
-cudaError_t launch_dense_mma(const DevProblem& P, cudaStream_t s) {
+cudaError_t launch_dense_mma(const DevProblem& P, bool compact, cudaStream_t s) {
     constexpr int WARPS = TO_DENSE_WARPS;
     const int smem = (int)sizeof(MmaSmem) * WARPS;
     static bool configured[TO_MAXDEV] = {false};
@@ -616,7 +616,7 @@ cudaError_t launch_dense_mma(const DevProblem& P, cudaStream_t s) {
         if (e != cudaSuccess) return e;
         configured[dev] = true;
     }
-    if (P.compact) k_riccati_dense_mma<WARPS, true><<<(P.B + WARPS - 1) / WARPS, 32 * WARPS, smem, s>>>(P);
+    if (compact) k_riccati_dense_mma<WARPS, true><<<(P.B + WARPS - 1) / WARPS, 32 * WARPS, smem, s>>>(P);
     else k_riccati_dense_mma<WARPS, false><<<(P.B + WARPS - 1) / WARPS, 32 * WARPS, smem, s>>>(P);
     return cudaGetLastError();
 }
@@ -648,10 +648,8 @@ cudaError_t launch_expansion_compact(const DevProblem& P, cudaStream_t s) {
     else k_expansion_compact<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }
-// to_options.backward_kernel = 3 forces the DFMA kernel (A/B, tests)
-bool dense_backward_mma(const DevProblem& P) { return P.ne == 12 && P.m == 4 && P.opt.pad != 3; }
-cudaError_t launch_backward_dense(const DevProblem& P, cudaStream_t s) {
-    if (dense_backward_mma(P)) return launch_dense_mma(P, s);
+cudaError_t launch_backward_dense(const DevProblem& P, const BackwardPlan& plan, cudaStream_t s) {
+    if (plan.kernel == KC_BK_DENSE_MMA) return launch_dense_mma(P, plan.expansion == BackwardPlan::COMPACT, s);
     if (P.ne == 12 && P.m == 4) return launch_dense_t<12, 4>(P, s);
     if (P.ne == 13 && P.m == 4) return launch_dense_t<13, 4>(P, s);
     if (P.ne == 4 && P.m == 1) return launch_dense_t<4, 1>(P, s);

@@ -52,7 +52,7 @@
 namespace {
 
 __host__ __device__ constexpr int even_up(int v) { return (v + 1) & ~1; }
-constexpr int MAXT = 3;   // AL terms per z entry kept in registers (e.g. upper bound + lower bound + goal)
+constexpr int MAXT = TO_EXP_MAXT;   // AL terms per z entry kept in registers (e.g. upper bound + lower bound + goal)
 
 __device__ __forceinline__ double2 lds128(const double* p) { return *reinterpret_cast<const double2*>(p); }
 __device__ __forceinline__ void sts128(double* p, double a, double b) { *reinterpret_cast<double2*>(p) = make_double2(a, b); }
@@ -989,9 +989,9 @@ cudaError_t launch_riccati_v(const DevProblem& P, int* work_counter, cudaStream_
 
 // INST: per-instance linear cost terms (P.qr) and constraint data (P.cdata), a kernel variant of its own so that the shared one stays as it is
 template <int N_, int M_, bool FASTAL, bool INST>
-cudaError_t launch_riccati_t(const DevProblem& P, int* work_counter, cudaStream_t s) {
+cudaError_t launch_riccati_t(const DevProblem& P, const BackwardPlan& plan, int* work_counter, cudaStream_t s) {
     if constexpr (N_ >= 8 && M_ <= 4) {
-        if (backward_kernel_of(P) == KC_BK_WARP_MMA) {   // tensor-MMA kernel: diagonal lzz (DiagonalCost + Goal/Bound)
+        if (plan.kernel == KC_BK_WARP_MMA) {   // tensor-MMA kernel: diagonal lzz (DiagonalCost + Goal/Bound)
             // 2-stage ring, 16 one-warp CTAs per SM.  NSLOT stays MAXT (the loop bound of the slot loop).
             return launch_riccati_v<N_, M_, FASTAL, TO_RICCATI_STAGES, TO_RICCATI_MINB, true, MAXT, INST>(P, work_counter, s);
         }
@@ -1002,33 +1002,39 @@ cudaError_t launch_riccati_t(const DevProblem& P, int* work_counter, cudaStream_
 }
 
 template <int N_, int M_>
-cudaError_t launch_riccati_nm(const DevProblem& P, int* work_counter, cudaStream_t s) {
-    const bool fastal = riccati_fastal(P);
-    if (inst_backward(P)) return fastal ? launch_riccati_t<N_, M_, true, true>(P, work_counter, s) : launch_riccati_t<N_, M_, false, true>(P, work_counter, s);
-    return fastal ? launch_riccati_t<N_, M_, true, false>(P, work_counter, s) : launch_riccati_t<N_, M_, false, false>(P, work_counter, s);
+cudaError_t launch_riccati_nm(const DevProblem& P, const BackwardPlan& plan, int* work_counter, cudaStream_t s) {
+    if (inst_backward(P)) return plan.fastal ? launch_riccati_t<N_, M_, true, true>(P, plan, work_counter, s) : launch_riccati_t<N_, M_, false, true>(P, plan, work_counter, s);
+    return plan.fastal ? launch_riccati_t<N_, M_, true, false>(P, plan, work_counter, s) : launch_riccati_t<N_, M_, false, false>(P, plan, work_counter, s);
 }
 
 }  // namespace
 
-// the lane-resident AL terms hold at most MAXT rows per z entry (upper + lower bound + goal); knot and row indices are packed in bit fields
-bool riccati_fastal(const DevProblem& P) { return P.max_terms_per_z <= MAXT && P.N < 4095 && P.max_p_knot < 128; }
-
-int backward_kernel_of(const DevProblem& P) {
-    // lie.cu: error state / quaternion costs (expansion materialised by the caller)
-    if (P.dense_riccati) return dense_backward_mma(P) ? KC_BK_DENSE_MMA : KC_BK_DENSE_DFMA;
-    // small models: one thread per instance, everything in registers (riccati_small.cu); backward_kernel = 1 forces the warp kernel
-    const int choice = P.opt.pad;   // to_options.backward_kernel: 0 automatic, 1 warp kernel, 2 thread kernel where it applies
-    if ((choice == 2 && riccati_small_supported(P, true)) || (choice == 0 && riccati_small_supported(P, false))) return KC_BK_THREAD;
+// Reads the options and, for the thread kernel, the SM count of the current device: called where the choice is needed, never cached.
+BackwardPlan backward_plan(const DevProblem& P) {
+    // to_options.backward_kernel.  BK_WARP, like any value not named here, only keeps the small models off the thread kernel.
+    enum { BK_AUTOMATIC = 0, BK_WARP = 1, BK_THREAD = 2, BK_DENSE_GENERIC = 3, BK_DENSE_COMPACT = 5 };
+    const int o = P.opt.backward_kernel;
+    // FASTAL's lane-resident AL terms and the records' term table: <= TO_EXP_MAXT rows per z entry, indices packed in bit fields
+    const bool packed = P.max_terms_per_z <= TO_EXP_MAXT && P.N < 4095 && P.max_p_knot < 128;
+    // compact error-state problems: the register-resident k_riccati_frag on per-knot records, unless a shared-memory kernel is forced
+    if (P.frag && o != BK_DENSE_GENERIC && o != BK_DENSE_COMPACT)
+        return {KC_BK_FRAGMENT, packed ? BackwardPlan::REC_TABLE : BackwardPlan::REC_WALK, false};
+    // lie.cu: error state / quaternion costs, on an expansion written before the kernel (BK_DENSE_GENERIC: DFMA kernel, full expansion)
+    if (P.dense_riccati)
+        return {(P.ne == 12 && P.m == 4 && o != BK_DENSE_GENERIC) ? KC_BK_DENSE_MMA : KC_BK_DENSE_DFMA,
+                (P.compact && o != BK_DENSE_GENERIC) ? BackwardPlan::COMPACT : BackwardPlan::MATERIALISED, false};
+    // small models: one thread per instance, everything in registers (riccati_small.cu), automatically past one wave of the warp kernel
+    if ((o == BK_THREAD || o == BK_AUTOMATIC) && riccati_small_supported(P, o == BK_THREAD)) return {KC_BK_THREAD, BackwardPlan::IN_KERNEL, false};
     // tensor-MMA k_riccati (n >= 8): diagonal lzz (DiagonalCost + Goal/Bound); otherwise the DFMA micro-block kernel
-    return (P.n >= 8 && P.m <= 4 && P.all_diag_cost && P.all_diag_con) ? KC_BK_WARP_MMA : KC_BK_WARP_DFMA;
+    return {(P.n >= 8 && P.m <= 4 && P.all_diag_cost && P.all_diag_con) ? KC_BK_WARP_MMA : KC_BK_WARP_DFMA, BackwardPlan::IN_KERNEL, packed};
 }
 
-cudaError_t launch_backward(const DevProblem& P, int* work_counter, cudaStream_t s) {
-    if (P.dense_riccati) return launch_backward_dense(P, s);
-    if (backward_kernel_of(P) == KC_BK_THREAD) return launch_backward_small(P, s);
-    if (P.n == 13 && P.m == 4) return launch_riccati_nm<13, 4>(P, work_counter, s);
-    if (P.n == 4 && P.m == 1) return launch_riccati_nm<4, 1>(P, work_counter, s);
-    if (P.n == 4 && P.m == 2) return launch_riccati_nm<4, 2>(P, work_counter, s);
-    if (P.n == 2 && P.m == 1) return launch_riccati_nm<2, 1>(P, work_counter, s);
+cudaError_t launch_backward(const DevProblem& P, const BackwardPlan& plan, int* work_counter, cudaStream_t s) {
+    if (plan.kernel == KC_BK_DENSE_MMA || plan.kernel == KC_BK_DENSE_DFMA) return launch_backward_dense(P, plan, s);
+    if (plan.kernel == KC_BK_THREAD) return launch_backward_small(P, s);
+    if (P.n == 13 && P.m == 4) return launch_riccati_nm<13, 4>(P, plan, work_counter, s);
+    if (P.n == 4 && P.m == 1) return launch_riccati_nm<4, 1>(P, plan, work_counter, s);
+    if (P.n == 4 && P.m == 2) return launch_riccati_nm<4, 2>(P, plan, work_counter, s);
+    if (P.n == 2 && P.m == 1) return launch_riccati_nm<2, 1>(P, plan, work_counter, s);
     return cudaErrorNotSupported;
 }

@@ -118,7 +118,7 @@ __device__ __forceinline__ double rcp_pos(double x) {
 // ---- compact error-state expansion into the record --------------------------------------------------------------------------------
 // One thread per (instance, knot): costcon.cuh compact_expansion, stored in the record's physical order (lie.cu k_expansion_compact stores
 // the same numbers in logical order for the shared-memory kernel).  rollout.cu k_expansion_rec16b computes them by another schedule from the
-// host-built term table; this kernel is its fallback where that table does not reach (capi.cu rec_fused: more than TO_EXP_MAXT Goal / Bound
+// host-built term table; this kernel is its fallback where that table does not reach (backward_plan REC_WALK: more than TO_EXP_MAXT Goal / Bound
 // rows on one z entry, N >= 4095, or 128 rows at one knot).
 template <bool INST>   // INST: the linear cost terms and constraint data of each instance
 __global__ void __launch_bounds__(128) k_expansion_rec(const DevProblem P) {
