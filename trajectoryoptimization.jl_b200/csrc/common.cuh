@@ -262,3 +262,17 @@ __host__ __device__ inline void reg_decrease(const DevOptions& o, double& rho, d
     drho = fmin(drho / o.bp_reg_increase_factor, 1.0 / o.bp_reg_increase_factor);
     rho = rho * drho * ((rho * drho > o.bp_reg_min) ? 1.0 : 0.0);
 }
+// The regularisation ladder of a backward pass (Altro backwardpass!), for every backward kernel.
+// A failed sweep: raise rho and count the restart; true when rho went past bp_reg_max, where the ladder gives up.
+__host__ __device__ inline bool reg_restart(const DevOptions& o, double& rho, double& drho, int& restarts) {
+    reg_increase(o, rho, drho);
+    restarts++;
+    return rho > o.bp_reg_max;
+}
+// The end of instance b's pass, called by every lane of the instance's warp (the thread kernel passes lane 0): lower rho unless the
+// ladder gave up, then lane 0 stores rho, drho and bp_status = the restarts, or -1 when the ladder gave up.  solve.cu and forward.cu
+// read bp_status in that encoding.
+__device__ inline void reg_finish(const DevProblem& P, int b, double rho, double drho, int restarts, bool failed, int lane) {
+    if (!failed) reg_decrease(P.opt, rho, drho);
+    if (lane == 0) { P.rho[b] = rho; P.drho[b] = drho; P.bp_status[b] = failed ? -1 : restarts; }
+}

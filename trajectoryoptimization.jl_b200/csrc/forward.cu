@@ -26,6 +26,7 @@
 #include "costcon.cuh"
 #include "kernels.h"
 #include "models.cuh"
+#include "ptx.cuh"
 
 namespace {
 
@@ -144,13 +145,6 @@ __device__ inline void load_compact_tables(const DevProblem& P, FwdCompactTab& t
     __syncthreads();
 }
 
-__device__ __forceinline__ void cp_async8(double* smem_dst, const double* gsrc) {
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async16(double* smem_dst, const double* gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 // Depth of the operand ring of the closed-loop rollout: knot k + FWD_STAGES - 1 is in flight while knot k is consumed.  One knot ahead
 // (2 stages) is the default; deeper rings cost registers and shared memory (TO_FWD_STAGES at build time).
 #ifndef TO_FWD_STAGES
@@ -159,7 +153,6 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 constexpr int FWD_STAGES = TO_FWD_STAGES;
 // knots of candidate trajectory staged in shared memory per lane before the group writes them out (rollout_compact)
 constexpr int FWD_OKNOTS = 4;
-template <int NPEND> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(NPEND) : "memory"); }
 
 // shared-memory stage of one knot's operands for the IPB instances of a CTA.
 // K_k is stored as 16-byte pairs [pair][IPB][2] (when n*m is even), everything else as 8-byte slots [slot][IPB].

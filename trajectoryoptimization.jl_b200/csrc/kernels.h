@@ -2,6 +2,9 @@
 #pragma once
 #include "common.cuh"
 
+// blocks of `threads` threads that cover `total` threads (the grid of a launcher)
+inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
+
 // kernel 1: batched RK4 rollout / dual-number dynamics expansion           (rollout.cu)
 cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s);
 cudaError_t launch_expand(const DevProblem& P, cudaStream_t s, int mode = 0);   // mode 1 / 2: only instances with acc1 == 1 / == 0

@@ -18,16 +18,18 @@
 //   k_error_dynamics    [A_e B_e] from [A B] (rollout.cu k_expand) -- one thread per (instance, knot, column)
 //   k_error_expansion   error-state cost + AL expansion from the full-state one (sweep.cu k_al_expansion) -- one thread per
 //                       (instance, knot, column)
+//   k_expansion_compact the compact error-state expansion EC of every knot (P.compact) -- one thread per (instance, knot)
 //   k_riccati_dense     backward pass, one warp per instance, reading [A_e B_e]_k, E_k from HBM: 3.7 KB per knot instead of the
 //                       2 KB of the fused kernel (riccati.cu), in exchange for taking ANY cost / constraint type -- the expansion
-//                       is whatever the sweep kernels wrote.  First correct version: DFMA on shared-memory operands, lane-strided.
-//                       (n_e = 12, n_e + m = 16 tiles the FP64 MMA shapes exactly: the tensor-core variant is the next step.)
+//                       is whatever the sweep kernels wrote.  DFMA on shared-memory operands, lane-strided.
+//   k_riccati_dense_mma the same pass for n_e = 12, m = 4 on the FP64 tensor cores, on EG / EH or on EC
+// Both backward passes take their gain step (LDL' of Quu + rho I, the solves, dV) from gains.cuh, as riccati.cu does.
 #include "costcon.cuh"
+#include "gains.cuh"
 #include "kernels.h"
+#include "ptx.cuh"
 
 namespace {
-
-inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
 __global__ void k_state_diff(const DevProblem P, const double* __restrict__ Xbar, double* __restrict__ dx) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -229,61 +231,24 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense(const DevProblem P
             for (int a = 0; a < M; a++)
 #pragma unroll
                 for (int c = 0; c <= a; c++) Quu[a * (a + 1) / 2 + c] = 0.5 * (sm.Q[(NR + c) * NME + NR + a] + sm.Q[(NR + a) * NME + NR + c]);
-#pragma unroll
-            for (int j = 0; j < M; j++) {
-                double t = Quu[j * (j + 1) / 2 + j] + rho;
-#pragma unroll
-                for (int r = 0; r < j; r++) t = fma(-Lf[j * (j + 1) / 2 + r] * Lf[j * (j + 1) / 2 + r], dj[r], t);
-                if (!(t > 0.0) || !isfinite(t)) ok = false;
-                dj[j] = t;
-                const double inv = 1.0 / t;
-                Lf[j * (j + 1) / 2 + j] = inv;
-#pragma unroll
-                for (int i = j + 1; i < M; i++) {
-                    double v = Quu[i * (i + 1) / 2 + j];
-#pragma unroll
-                    for (int r = 0; r < j; r++) v = fma(-Lf[i * (i + 1) / 2 + r] * Lf[j * (j + 1) / 2 + r], dj[r], v);
-                    Lf[i * (i + 1) / 2 + j] = v * inv;
-                }
-            }
+            if (!ldl_factor<M>(Quu, rho, Lf, dj, [](double t) { return 1.0 / t; })) ok = false;   // a division, where the other kernels take rcp_pos
             if (!ok) break;   // uniform across the warp
             if (lane <= NR) {
                 const int c = lane;
                 double rhs[M], kc[M];
 #pragma unroll
                 for (int a = 0; a < M; a++) rhs[a] = (c < NR) ? sm.Q[c * NME + NR + a] : sm.q[NR + a];   // Qux[a][c] | Qu[a]
-#pragma unroll
-                for (int a = 0; a < M; a++) {
-                    double t = -rhs[a];
-#pragma unroll
-                    for (int r = 0; r < a; r++) t = fma(-Lf[a * (a + 1) / 2 + r], kc[r], t);
-                    kc[a] = t;
-                }
-#pragma unroll
-                for (int a = 0; a < M; a++) kc[a] *= Lf[a * (a + 1) / 2 + a];
-#pragma unroll
-                for (int a = M - 1; a >= 0; a--) {
-                    double t = kc[a];
-#pragma unroll
-                    for (int r = a + 1; r < M; r++) t = fma(-Lf[r * (r + 1) / 2 + a], kc[r], t);
-                    kc[a] = t;
-                }
+                ldl_solve<M>(Lf, rhs, kc);
 #pragma unroll
                 for (int a = 0; a < M; a++) { sm.K[a * (NR + 1) + c] = kc[a]; sm.W[a * (NR + 1) + c] = fma(-rho, kc[a], rhs[a]); }
                 if (c < NR) {
 #pragma unroll
                     for (int a = 0; a < M; a++) Kg[(size_t)k * NR * M + c * M + a] = kc[a];
                 } else {
-                    double t1 = 0.0, t2 = 0.0;
 #pragma unroll
-                    for (int a = 0; a < M; a++) {
-                        dg[(size_t)k * M + a] = kc[a];
-                        t1 = fma(kc[a], rhs[a], t1);
-                        double qd = 0.0;
-#pragma unroll
-                        for (int r = 0; r < M; r++) qd = fma((r <= a) ? Quu[a * (a + 1) / 2 + r] : Quu[r * (r + 1) / 2 + a], kc[r], qd);
-                        t2 = fma(0.5 * kc[a], qd, t2);
-                    }
+                    for (int a = 0; a < M; a++) dg[(size_t)k * M + a] = kc[a];
+                    double t1, t2;
+                    expected_decrease<M>(Quu, kc, rhs, t1, t2);
                     dV1 += t1; dV2 += t2;
                 }
             }
@@ -311,13 +276,10 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense(const DevProblem P
             if (lane == NR) { P.dV[2 * b] = dV1; P.dV[2 * b + 1] = dV2; }
             break;
         }
-        reg_increase(P.opt, rho, drho);
-        restarts++;
-        if (rho > P.opt.bp_reg_max) { failed = true; break; }
+        if (reg_restart(P.opt, rho, drho, restarts)) { failed = true; break; }
         __syncwarp();
     }
-    if (!failed) reg_decrease(P.opt, rho, drho);
-    if (lane == 0) { P.rho[b] = rho; P.drho[b] = drho; P.bp_status[b] = failed ? -1 : restarts; }
+    reg_finish(P, b, rho, drho, restarts, failed, lane);
 }
 
 // ---- the same pass for n_e = 12, m = 4 on the FP64 tensor cores -----------------------------------------------------------------
@@ -327,24 +289,6 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense(const DevProblem P
 // wavefronts (the minimum for 32 x 8 B): column-major with leading dimension 12 for S, [A B], T (12 = 4 mod 8), 20 for Q, 24 for K / W.
 // The next knot's [A_e B_e], E.hess, E.grad are fetched with cp.async (LDGSTS) into the other half of a double buffer while this
 // knot computes.
-// 1/x for a positive finite pivot: hardware seed + two Newton steps (<= 1 ulp), without the slow path of the IEEE division
-__device__ __forceinline__ double rcp_pos(double x) {
-    double y;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
-    double e = fma(-x, y, 1.0);
-    y = fma(y, e, y);
-    e = fma(-x, y, 1.0);
-    return fma(y, e, y);
-}
-__device__ __forceinline__ void dmma884(double& d0, double& d1, double a, double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
-}
-__device__ __forceinline__ void cp16(double* smem_dst, const double* gsrc) {
-    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
-}
-__device__ __forceinline__ void cp_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int NPEND> __device__ __forceinline__ void cp_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(NPEND) : "memory"); }
-
 struct MmaSmem {   // one warp; NR = 12, M = 4, NME = 16
     static constexpr int LDQ = 20, LDK = 24;
     double ab[2][12 * 16];      // [A_e B_e]_k col-major ld 12, double buffered
@@ -383,13 +327,13 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
     // async copies of knot k into buffer st: [A_e B_e] (96 sixteen-byte chunks) + the expansion (128 + 8 chunks, or the 20 of the compact record)
     auto fetch = [&](int st, int k) {
         const double* srcab = ABg + (size_t)k * NR * NME;
-        for (int c = lane; c < 96; c += 32) cp16(&sm.ab[st][2 * c], srcab + 2 * c);
+        for (int c = lane; c < 96; c += 32) cp_async16(&sm.ab[st][2 * c], srcab + 2 * c);
         if constexpr (COMPACT) {
-            if (lane < TO_EC_LEN / 2) cp16(&sm.rec[st][2 * lane], ECg + (size_t)k * TO_EC_LEN + 2 * lane);
+            if (lane < TO_EC_LEN / 2) cp_async16(&sm.rec[st][2 * lane], ECg + (size_t)k * TO_EC_LEN + 2 * lane);
         } else {
             const double* srch = EHg + (size_t)k * NME * NME;
-            for (int c = lane; c < 128; c += 32) { const int j = c >> 3, i = (c & 7) * 2; cp16(&sm.Q[st][j * LDQ + i], srch + j * NME + i); }
-            if (lane < 8) cp16(&sm.q[st][2 * lane], EGg + (size_t)k * NME + 2 * lane);
+            for (int c = lane; c < 128; c += 32) { const int j = c >> 3, i = (c & 7) * 2; cp_async16(&sm.Q[st][j * LDQ + i], srch + j * NME + i); }
+            if (lane < 8) cp_async16(&sm.q[st][2 * lane], EGg + (size_t)k * NME + 2 * lane);
         }
     };
     // entry (row, col) of the compact record's Hessian: diagonal + the symmetric 3 x 3 attitude block
@@ -409,15 +353,15 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
             for (int e = lane; e < NR * NR; e += 32) sm.S[e] = H[(e / NR) * NME + (e % NR)];
             if (lane < NR) sm.s[lane] = EGg[(size_t)(N - 1) * NME + lane];
         }
-        fetch(0, N - 2); cp_commit();
+        fetch(0, N - 2); cp_async_commit();
         __syncwarp();
         double dV1 = 0.0, dV2 = 0.0;
         bool ok = true;
         int st = 0;
         for (int k = N - 2; k >= 0; k--, st ^= 1) {
             if (k > 0) fetch(st ^ 1, k - 1);
-            cp_commit();
-            cp_wait<1>();                  // this lane's copies of knot k have landed ...
+            cp_async_commit();
+            cp_async_wait<1>();            // this lane's copies of knot k have landed ...
             __syncwarp();                  // ... and everybody else's
             const double* ab = sm.ab[st];
             double* Qs = sm.Q[st];
@@ -442,7 +386,7 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
 #pragma unroll
                     for (int mi = 0; mi < 2; mi++)
 #pragma unroll
-                        for (int ni = 0; ni < 2; ni++) dmma884(d[mi][ni][0], d[mi][ni][1], a[mi], bfr[kk][ni]);
+                        for (int ni = 0; ni < 2; ni++) dmma(d[mi][ni][0], d[mi][ni][1], a[mi], bfr[kk][ni]);
                 }
 #pragma unroll
                 for (int mi = 0; mi < 2; mi++)
@@ -471,7 +415,7 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
 #pragma unroll
                     for (int mi = 0; mi < 2; mi++)
 #pragma unroll
-                        for (int ni = 0; ni < 2; ni++) dmma884(c[mi][ni][0], c[mi][ni][1], bfr[kk][mi], bt[ni]);
+                        for (int ni = 0; ni < 2; ni++) dmma(c[mi][ni][0], c[mi][ni][1], bfr[kk][mi], bt[ni]);
                 }
                 double qz = 0.0;
                 if (lane < NME) {
@@ -492,72 +436,28 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
             __syncwarp();
             // ---- gains: LDL' of Quu + rho I (every lane factors the same 4 x 4 matrix), one lane per column of [Qux | Qu] ----
             double Quu[M * (M + 1) / 2], Lf[M * (M + 1) / 2], dj[M];
-#ifdef TO_DENSE_HALFLDL
-            if (lane < 16) {   // A/B: FP64 instructions of a half-empty warp take one pipe pass
-#endif
 #pragma unroll
             for (int a = 0; a < M; a++)
 #pragma unroll
                 for (int c = 0; c <= a; c++) Quu[a * (a + 1) / 2 + c] = 0.5 * (Qs[(NR + c) * LDQ + NR + a] + Qs[(NR + a) * LDQ + NR + c]);
-#pragma unroll
-            for (int j = 0; j < M; j++) {
-                double t = Quu[j * (j + 1) / 2 + j] + rho;
-#pragma unroll
-                for (int r = 0; r < j; r++) t = fma(-Lf[j * (j + 1) / 2 + r] * Lf[j * (j + 1) / 2 + r], dj[r], t);
-                if (!(t > 0.0) || !isfinite(t)) ok = false;
-                dj[j] = t;
-                const double inv = rcp_pos(t);
-                Lf[j * (j + 1) / 2 + j] = inv;
-#pragma unroll
-                for (int i = j + 1; i < M; i++) {
-                    double v = Quu[i * (i + 1) / 2 + j];
-#pragma unroll
-                    for (int r = 0; r < j; r++) v = fma(-Lf[i * (i + 1) / 2 + r] * Lf[j * (j + 1) / 2 + r], dj[r], v);
-                    Lf[i * (i + 1) / 2 + j] = v * inv;
-                }
-            }
-#ifdef TO_DENSE_HALFLDL
-            }
-            ok = __shfl_sync(0xffffffffu, ok ? 1 : 0, 0) != 0;
-#endif
+            if (!ldl_factor<M>(Quu, rho, Lf, dj, rcp_pos)) ok = false;
             if (!ok) break;   // uniform across the warp
             if (lane <= NR) {
                 const int c = lane;
                 double rhs[M], kc[M];
 #pragma unroll
                 for (int a = 0; a < M; a++) rhs[a] = (c < NR) ? Qs[c * LDQ + NR + a] : qs[NR + a];   // Qux[a][c] | Qu[a]
-#pragma unroll
-                for (int a = 0; a < M; a++) {
-                    double t = -rhs[a];
-#pragma unroll
-                    for (int r = 0; r < a; r++) t = fma(-Lf[a * (a + 1) / 2 + r], kc[r], t);
-                    kc[a] = t;
-                }
-#pragma unroll
-                for (int a = 0; a < M; a++) kc[a] *= Lf[a * (a + 1) / 2 + a];
-#pragma unroll
-                for (int a = M - 1; a >= 0; a--) {
-                    double t = kc[a];
-#pragma unroll
-                    for (int r = a + 1; r < M; r++) t = fma(-Lf[r * (r + 1) / 2 + a], kc[r], t);
-                    kc[a] = t;
-                }
+                ldl_solve<M>(Lf, rhs, kc);
 #pragma unroll
                 for (int a = 0; a < M; a++) { sm.K[a * LDK + c] = kc[a]; sm.W[a * LDK + c] = fma(-rho, kc[a], rhs[a]); }
                 if (c < NR) {
 #pragma unroll
                     for (int a = 0; a < M; a++) Kg[(size_t)k * NR * M + c * M + a] = kc[a];
                 } else {
-                    double t1 = 0.0, t2 = 0.0;
 #pragma unroll
-                    for (int a = 0; a < M; a++) {
-                        dg[(size_t)k * M + a] = kc[a];
-                        t1 = fma(kc[a], rhs[a], t1);
-                        double qd = 0.0;
-#pragma unroll
-                        for (int r = 0; r < M; r++) qd = fma((r <= a) ? Quu[a * (a + 1) / 2 + r] : Quu[r * (r + 1) / 2 + a], kc[r], qd);
-                        t2 = fma(0.5 * kc[a], qd, t2);
-                    }
+                    for (int a = 0; a < M; a++) dg[(size_t)k * M + a] = kc[a];
+                    double t1, t2;
+                    expected_decrease<M>(Quu, kc, rhs, t1, t2);
                     dV1 += t1; dV2 += t2;
                 }
             }
@@ -573,7 +473,7 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
                     for (int ni = mi; ni < 2; ni++) {
                         const int row = 8 * mi + fr, col = 8 * ni + 2 * fc;
                         double a0 = Qs[col * LDQ + row], a1 = Qs[(col + 1) * LDQ + row];
-                        dmma884(a0, a1, af[mi], bk[ni]);
+                        dmma(a0, a1, af[mi], bk[ni]);
                         if (row < NR && col < NR) {        // NR is even: col + 1 < NR too
                             sm.S[col * 12 + row] = a0; sm.S[(col + 1) * 12 + row] = a1;
                             if (ni != mi) { sm.S[row * 12 + col] = a0; sm.S[row * 12 + col + 1] = a1; }
@@ -588,18 +488,15 @@ __global__ void __launch_bounds__(32 * WARPS) k_riccati_dense_mma(const DevProbl
             }
             __syncwarp();
         }
-        cp_wait<0>();
+        cp_async_wait<0>();
         __syncwarp();
         if (ok) {
             if (lane == NR) { P.dV[2 * b] = dV1; P.dV[2 * b + 1] = dV2; }
             break;
         }
-        reg_increase(P.opt, rho, drho);
-        restarts++;
-        if (rho > P.opt.bp_reg_max) { failed = true; break; }
+        if (reg_restart(P.opt, rho, drho, restarts)) { failed = true; break; }
     }
-    if (!failed) reg_decrease(P.opt, rho, drho);
-    if (lane == 0) { P.rho[b] = rho; P.drho[b] = drho; P.bp_status[b] = failed ? -1 : restarts; }
+    reg_finish(P, b, rho, drho, restarts, failed, lane);
 }
 
 #ifndef TO_DENSE_WARPS

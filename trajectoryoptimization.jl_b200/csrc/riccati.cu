@@ -28,11 +28,14 @@
 //   * lane i < n+m owns z_i: its cost / AL descriptors live in registers for the whole kernel, and z_i, lambda of the
 //     NEXT knot are prefetched while the current knot's products run (global latency off the critical path).
 //   * Quu + rho I is m x m (m <= 8): LDL' with reciprocal pivots (no fp64 sqrt / division chain) and the triangular
-//     solves are done per right-hand-side column, one lane per column of [Qux Qu], in registers.
+//     solves are done per right-hand-side column, one lane per column of [Qux Qu], in registers (gains.cuh, shared with
+//     lie.cu's kernels).
 #include <cstddef>
 
 #include "costcon.cuh"
+#include "gains.cuh"
 #include "kernels.h"
+#include "ptx.cuh"
 
 #ifndef TO_RICCATI_STAGES
 #define TO_RICCATI_STAGES 2     // depth of the [A B] ring
@@ -54,31 +57,7 @@ namespace {
 __host__ __device__ constexpr int even_up(int v) { return (v + 1) & ~1; }
 constexpr int MAXT = TO_EXP_MAXT;   // AL terms per z entry kept in registers (e.g. upper bound + lower bound + goal)
 
-__device__ __forceinline__ double2 lds128(const double* p) { return *reinterpret_cast<const double2*>(p); }
 __device__ __forceinline__ void sts128(double* p, double a, double b) { *reinterpret_cast<double2*>(p) = make_double2(a, b); }
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-// 1-D bulk TMA copy global -> shared, completion signalled on an mbarrier (SASS: UBLKCP)
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
 
 // global load the compiler may not sink towards its use (prefetch of the next knot's operands)
 __device__ __forceinline__ double ldg_pinned(const double* p) {
@@ -93,27 +72,12 @@ __device__ __forceinline__ int ldg_pinned(const int* p) {
     return v;
 }
 
-// 1/x for a positive finite pivot: hardware seed (MUFU.RCP64H, >= 20 bits) + two Newton steps -> <= 1 ulp, without
-// the rounding / special-case fix-up of __drcp_rn (12 dependent instructions + a branch on the knot's critical chain)
-__device__ __forceinline__ double rcp_pivot(double x) {
-    double y;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
-    double e = fma(-x, y, 1.0);
-    y = fma(y, e, y);
-    e = fma(-x, y, 1.0);
-    return fma(y, e, y);
-}
-
 // 2x2 micro-block outer-product accumulate
 __device__ __forceinline__ void fma2x2(double (&acc)[4], const double2& a, const double2& b) {
     acc[0] = fma(a.x, b.x, acc[0]);
     acc[1] = fma(a.x, b.y, acc[1]);
     acc[2] = fma(a.y, b.x, acc[2]);
     acc[3] = fma(a.y, b.y, acc[3]);
-}
-
-__device__ __forceinline__ void dmma(double& d0, double& d1, double a, double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
 }
 
 template <int N_, int M_, int STAGES, bool MMA>
@@ -256,7 +220,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
     if (lane == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; s++) mbar_init(&sm.bar[s], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     __syncwarp();
     uint32_t phase_bits = 0;   // per-stage parity of the next completion to wait for
@@ -645,43 +609,12 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                         for (int a = 0; a < m; a++)
 #pragma unroll
                             for (int c = 0; c <= a; c++) Quu[a * (a + 1) / 2 + c] = Qs_[(n + c) * LDQS + a];
-#pragma unroll
-                        for (int j = 0; j < m; j++) {
-                            double t = Quu[j * (j + 1) / 2 + j] + rho;
-#pragma unroll
-                            for (int r = 0; r < j; r++) t = fma(-Lf[j * (j + 1) / 2 + r] * Lf[j * (j + 1) / 2 + r], dj[r], t);
-                            if (!(t > 0.0) || !isfinite(t)) okl = false;
-                            dj[j] = t;
-                            const double inv = rcp_pivot(t);
-                            Lf[j * (j + 1) / 2 + j] = inv;
-#pragma unroll
-                            for (int i = j + 1; i < m; i++) {
-                                double v = Quu[i * (i + 1) / 2 + j];
-#pragma unroll
-                                for (int r = 0; r < j; r++) v = fma(-Lf[i * (i + 1) / 2 + r] * Lf[j * (j + 1) / 2 + r], dj[r], v);
-                                Lf[i * (i + 1) / 2 + j] = v * inv;
-                            }
-                        }
+                        if (!ldl_factor<M_>(Quu, rho, Lf, dj, rcp_pos)) okl = false;
                         const int c = (lane <= n) ? lane : n;
                         double rhs[M_];
 #pragma unroll
                         for (int a = 0; a < m; a++) rhs[a] = (c < n) ? Qs_[c * LDQS + a] : Qs_[(n + a) * LDQS + m];   // Qux[a][c] | Qu[a]
-#pragma unroll
-                        for (int a = 0; a < m; a++) {
-                            double t = -rhs[a];
-#pragma unroll
-                            for (int r = 0; r < a; r++) t = fma(-Lf[a * (a + 1) / 2 + r], kc[r], t);
-                            kc[a] = t;
-                        }
-#pragma unroll
-                        for (int a = 0; a < m; a++) kc[a] *= Lf[a * (a + 1) / 2 + a];
-#pragma unroll
-                        for (int a = m - 1; a >= 0; a--) {
-                            double t = kc[a];
-#pragma unroll
-                            for (int r = a + 1; r < m; r++) t = fma(-Lf[r * (r + 1) / 2 + a], kc[r], t);
-                            kc[a] = t;
-                        }
+                        ldl_solve<M_>(Lf, rhs, kc);
 #pragma unroll
                         for (int a = 0; a < m; a++) wc[a] = fma(-rho, kc[a], rhs[a]);   // W = Qux - rho K
                         if (okl) {
@@ -693,16 +626,10 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
 #pragma unroll
                                 for (int a = 0; a < m; a++) Kg[(size_t)k * n * m + lane * m + a] = kc[a];
                             } else if (lane == n) {
-                                double t1 = 0.0, t2 = 0.0;
 #pragma unroll
-                                for (int a = 0; a < m; a++) {
-                                    dg[(size_t)k * m + a] = kc[a];
-                                    t1 = fma(kc[a], rhs[a], t1);
-                                    double qd = 0.0;
-#pragma unroll
-                                    for (int r = 0; r < m; r++) qd = fma((r <= a) ? Quu[a * (a + 1) / 2 + r] : Quu[r * (r + 1) / 2 + a], kc[r], qd);
-                                    t2 = fma(0.5 * kc[a], qd, t2);
-                                }
+                                for (int a = 0; a < m; a++) dg[(size_t)k * m + a] = kc[a];
+                                double t1, t2;
+                                expected_decrease<M_>(Quu, kc, rhs, t1, t2);
                                 dV1 += t1; dV2 += t2;
                             }
                         }
@@ -812,54 +739,19 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     if (!P.all_diag_con) { double dummy = 0.0; general_constraints(k + 1, false, dummy); }
 
                     // ---- gains: LDL' of Quu + rho I, one lane per column of [Qux | Qu] -------------------------
-                    double Quu[M_ * (M_ + 1) / 2];           // packed lower by rows
-                    double Lf[M_ * (M_ + 1) / 2];            // unit-lower L (off-diagonal), diagonal slots hold 1/d_j
-                    {
+                    double Quu[M_ * (M_ + 1) / 2], Lf[M_ * (M_ + 1) / 2], dj[M_];
     #pragma unroll
-                        for (int a = 0; a < m; a++)
+                    for (int a = 0; a < m; a++)
     #pragma unroll
-                            for (int c = 0; c <= a; c++) Quu[a * (a + 1) / 2 + c] = sm.Q[(n + c) * LDT + (n + a)];   // upper entry (c <= a)
-                        double dj[M_];
-    #pragma unroll
-                        for (int j = 0; j < m; j++) {
-                            double t = Quu[j * (j + 1) / 2 + j] + rho;
-    #pragma unroll
-                            for (int r = 0; r < j; r++) t = fma(-Lf[j * (j + 1) / 2 + r] * Lf[j * (j + 1) / 2 + r], dj[r], t);
-                            if (!(t > 0.0) || !isfinite(t)) ok = false;
-                            dj[j] = t;
-                            const double inv = rcp_pivot(t);
-                            Lf[j * (j + 1) / 2 + j] = inv;
-    #pragma unroll
-                            for (int i = j + 1; i < m; i++) {
-                                double v = Quu[i * (i + 1) / 2 + j];
-    #pragma unroll
-                                for (int r = 0; r < j; r++) v = fma(-Lf[i * (i + 1) / 2 + r] * Lf[j * (j + 1) / 2 + r], dj[r], v);
-                                Lf[i * (i + 1) / 2 + j] = v * inv;
-                            }
-                        }
-                    }
+                        for (int c = 0; c <= a; c++) Quu[a * (a + 1) / 2 + c] = sm.Q[(n + c) * LDT + (n + a)];   // upper entry (c <= a)
+                    if (!ldl_factor<M_>(Quu, rho, Lf, dj, rcp_pos)) ok = false;
                     if (!ok) break;   // uniform across the warp (every lane factors the same matrix)
                     {
                         const int c = (lane <= n) ? lane : n;
                         double rhs[M_], kc[M_];
     #pragma unroll
                         for (int a = 0; a < m; a++) rhs[a] = (c < n) ? sm.Q[c * LDT + (n + a)] : sm.Q[(n + a) * LDT + NM];   // Qux[a][c] | Qu[a]
-    #pragma unroll
-                        for (int a = 0; a < m; a++) {      // forward: L y = -rhs
-                            double t = -rhs[a];
-    #pragma unroll
-                            for (int r = 0; r < a; r++) t = fma(-Lf[a * (a + 1) / 2 + r], kc[r], t);
-                            kc[a] = t;
-                        }
-    #pragma unroll
-                        for (int a = 0; a < m; a++) kc[a] *= Lf[a * (a + 1) / 2 + a];   // D^-1
-    #pragma unroll
-                        for (int a = m - 1; a >= 0; a--) {  // backward: L' x = y
-                            double t = kc[a];
-    #pragma unroll
-                            for (int r = a + 1; r < m; r++) t = fma(-Lf[r * (r + 1) / 2 + a], kc[r], t);
-                            kc[a] = t;
-                        }
+                        ldl_solve<M_>(Lf, rhs, kc);
                         if (lane <= n) {
     #pragma unroll
                             for (int a = 0; a < m; a++) {
@@ -871,16 +763,10 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
     #pragma unroll
                             for (int a = 0; a < m; a++) Kg[(size_t)k * n * m + lane * m + a] = kc[a];
                         } else if (lane == n) {
-                            double t1 = 0.0, t2 = 0.0;
     #pragma unroll
-                            for (int a = 0; a < m; a++) {
-                                dg[(size_t)k * m + a] = kc[a];
-                                t1 = fma(kc[a], rhs[a], t1);
-                                double qd = 0.0;   // (Quu d)_a
-    #pragma unroll
-                                for (int r = 0; r < m; r++) qd = fma((r <= a) ? Quu[a * (a + 1) / 2 + r] : Quu[r * (r + 1) / 2 + a], kc[r], qd);
-                                t2 = fma(0.5 * kc[a], qd, t2);
-                            }
+                            for (int a = 0; a < m; a++) dg[(size_t)k * m + a] = kc[a];
+                            double t1, t2;
+                            expected_decrease<M_>(Quu, kc, rhs, t1, t2);
                             dV1 += t1; dV2 += t2;
                         }
                     }
@@ -949,15 +835,9 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                 }
             }
             __syncwarp();
-            reg_increase(P.opt, rho, drho);
-            restarts++;
-            if (rho > P.opt.bp_reg_max) { failed = true; break; }
+            if (reg_restart(P.opt, rho, drho, restarts)) { failed = true; break; }
         }
-        if (!failed) reg_decrease(P.opt, rho, drho);
-        if (lane == 0) {
-            P.rho[b] = rho; P.drho[b] = drho;
-            P.bp_status[b] = failed ? -1 : restarts;
-        }
+        reg_finish(P, b, rho, drho, restarts, failed, lane);
         __syncwarp();
     }
 }

@@ -33,6 +33,7 @@
 #include "costcon.cuh"
 #include "frag_layout.cuh"
 #include "kernels.h"
+#include "ptx.cuh"
 
 #ifndef TO_FRAG_STAGES
 #define TO_FRAG_STAGES 2
@@ -62,35 +63,8 @@
 
 namespace {
 
-inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "WAIT_LOOP:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra DONE;\n\t"
-        "bra WAIT_LOOP;\n\t"
-        "DONE:\n\t}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
 __device__ __forceinline__ void bulk_prefetch_l2(const void* src, uint32_t bytes) {
     asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ double2 lds128(const double* p) { return *reinterpret_cast<const double2*>(p); }
-__device__ __forceinline__ void dmma(double& d0, double& d1, double a, double b) {
-    asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(d0), "+d"(d1) : "d"(a), "d"(b));
 }
 __device__ __forceinline__ int ld_volatile_s32(const int* p) {
     int v;
@@ -104,15 +78,6 @@ __device__ __forceinline__ void tile_transpose(double x0, double x1, int src, in
     const double b0 = __shfl_sync(0xffffffffu, x0, src + 4), b1 = __shfl_sync(0xffffffffu, x1, src + 4);
     y0 = odd_row ? a1 : a0;
     y1 = odd_row ? b1 : b0;
-}
-// 1/x for a positive finite x: hardware seed + two Newton steps (<= 1 ulp), no IEEE-division slow path on the pivot chain
-__device__ __forceinline__ double rcp_pos(double x) {
-    double y;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(x));
-    double e = fma(-x, y, 1.0);
-    y = fma(y, e, y);
-    e = fma(-x, y, 1.0);
-    return fma(y, e, y);
 }
 
 // ---- compact error-state expansion into the record --------------------------------------------------------------------------------
@@ -200,7 +165,7 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_riccati_frag(const DevProb
     if (lane == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; s++) mbar_init(&bar[s], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_fence_init();
     }
     __syncwarp();
     uint32_t phase_bits = 0;
@@ -433,10 +398,10 @@ __global__ void __launch_bounds__(32 * WARPS, MINB) k_riccati_frag(const DevProb
             // 1/2 d'Quu d = -1/2 (d'Qu + rho d'd)   since (Quu + rho I) d = -Qu
             if (lane == 0) { dst[0] = acc1; dst[1] = -0.5 * fma(rho, acc2, acc1); }
         };
+        // status: the winning candidate (restarts), or -1 when the ladder gave up -- never another negative value
         auto finalise = [&](double rho, double drho, int status) {
-            if (status >= 0) reg_decrease(P.opt, rho, drho);
+            reg_finish(P, b, rho, drho, status, status < 0, lane);
             if (lane == 0) {
-                P.rho[b] = rho; P.drho[b] = drho; P.bp_status[b] = status;
                 __threadfence();
                 atomicAdd(q_nfinal, 1);
             }

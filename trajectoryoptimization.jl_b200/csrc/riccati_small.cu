@@ -235,13 +235,9 @@ __global__ void __maxnreg__(255) k_riccati_small(const DevProblem P) {
             }
         }
         if (ok) { P.dV[2 * b] = dV1; P.dV[2 * b + 1] = dV2; break; }
-        reg_increase(P.opt, rho, drho);
-        restarts++;
-        if (rho > P.opt.bp_reg_max) { failed = true; break; }
+        if (reg_restart(P.opt, rho, drho, restarts)) { failed = true; break; }
     }
-    if (!failed) reg_decrease(P.opt, rho, drho);
-    P.rho[b] = rho; P.drho[b] = drho;
-    P.bp_status[b] = failed ? -1 : restarts;
+    reg_finish(P, b, rho, drho, restarts, failed, 0);
 }
 
 template <int N_, int M_>

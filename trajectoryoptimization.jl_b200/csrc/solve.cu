@@ -96,23 +96,21 @@ __global__ void k_solve_outer(const DevProblem P, SolveDev S) {
     atomicAdd(S.n_active, 1);
 }
 
-inline unsigned nblk(int count) { return (unsigned)((count + 127) / 128); }
-
 }  // namespace
 
 cudaError_t launch_solve_init(const DevProblem& P, const SolveDev& S, cudaStream_t s) {
-    k_solve_init<<<nblk(P.B), 128, 0, s>>>(P, S);
+    k_solve_init<<<nblk(P.B, 128), 128, 0, s>>>(P, S);
     return cudaGetLastError();
 }
 cudaError_t launch_solve_begin(const DevProblem& P, const SolveDev& S, cudaStream_t s) {
-    k_solve_begin<<<nblk(P.B), 128, 0, s>>>(P, S);
+    k_solve_begin<<<nblk(P.B, 128), 128, 0, s>>>(P, S);
     return cudaGetLastError();
 }
 cudaError_t launch_solve_check(const DevProblem& P, const SolveDev& S, int mode, cudaStream_t s) {
-    k_solve_check<<<nblk(P.B), 128, 0, s>>>(P, S, mode);
+    k_solve_check<<<nblk(P.B, 128), 128, 0, s>>>(P, S, mode);
     return cudaGetLastError();
 }
 cudaError_t launch_solve_outer(const DevProblem& P, const SolveDev& S, cudaStream_t s) {
-    k_solve_outer<<<nblk(P.B), 128, 0, s>>>(P, S);
+    k_solve_outer<<<nblk(P.B, 128), 128, 0, s>>>(P, S);
     return cudaGetLastError();
 }

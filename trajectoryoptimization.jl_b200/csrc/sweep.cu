@@ -235,8 +235,6 @@ __global__ void k_export_ab(const DevProblem P, double* __restrict__ out) {
 }
 
 // ------------------------------------------------------------------------------------------------------
-static inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
-
 cudaError_t launch_cost(const DevProblem& P, double* J, double* Jk, cudaStream_t s) {
     if (inst_backward(P)) k_cost<false, true><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
     else k_cost<false, false><<<P.B, 128, 0, s>>>(P, J, Jk, nullptr);
