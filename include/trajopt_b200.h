@@ -7,7 +7,7 @@
  * to_update_trajectories, to_set_cost_terms), in the linear cost terms q, r and the Goal constraint values
  * (goal state / tracking reference per instance) -- and, after to_set_model_params, in the model parameters (mass,
  * inertia, lengths, motor constants, gravity) -- and, after to_set_constraint_data, in the constraint data (bounds, obstacles, collision
- * radii, norm values, linear right-hand sides).  Every function cites the reference interface it stands in for.  The
+ * radii, norm values, linear right-hand sides) -- and, after to_set_cost_weights, in the cost weights Q, R, H, c, w.  Every function cites the reference interface it stands in for.  The
  * Julia-side binding (ccall) that a maintainer adds is shown in INTEGRATION.md.
  *
  * Conventions
@@ -214,8 +214,8 @@ int to_shift_trajectory(to_handle* h, int32_t steps);
 
 /* ---- per-instance goals / tracking references ---------------------------------------------------------------
  * The same operations per instance b.  Per instance the handle holds the linear terms q_b, r_b of every distinct cost (cost_index aliasing
- * kept: a cost shared by several knots tracks the last of them, per instance) and the values of every Goal constraint; Q, R, H, c, the
- * quaternion cost's w / q_ref, program costs and every other constraint stay shared.  Until the first per-instance call there is no
+ * kept: a cost shared by several knots tracks the last of them, per instance) and the values of every Goal constraint; the weights Q, R, H,
+ * c and w are per instance after to_set_cost_weights (below); q_ref, program costs and every other constraint stay shared.  Until the first per-instance call there is no
  * per-instance data and every kernel runs as before.  The first per-instance call copies the shared values into every instance, then applies
  * its change; a later shared to_set_goal_state / to_update_trajectory writes through to every instance (the later call wins).
  * to_shift_trajectory leaves the objective alone: an MPC loop calls to_update_trajectories with the next start.  Multi-GPU: each rank passes
@@ -259,6 +259,27 @@ int to_get_model_params(to_handle* h, double* params /*[B][nparams]*/);         
 int to_constraint_data_len(const to_handle* h, int32_t con, int32_t* len);                         /* doubles per instance of constraint con */
 int to_set_constraint_data(to_handle* h, int32_t con, const double* data /*[B][len]*/);
 int to_get_constraint_data(to_handle* h, int32_t con, double* data /*[B][len]*/);                  /* the shared values broadcast when none are set */
+
+/* ---- per-instance cost weights -------------------------------------------------------------------------------
+ * Instance b evaluates distinct cost `cost` (0-based index into to_spec.costs) with its own weights (a Problem owns its Objective,
+ * src/problem.jl:36-73).  One instance's row, len doubles, in to_cost_spec order, matrices column-major:
+ *   DIAGONAL       n+m+1          Qd[n] | Rd[m] | c
+ *   QUADRATIC      n^2+m^2+mn+1   Q[n*n] | R[m*m] | H[m*n] | c
+ *   DIAGONAL_QUAT  n+m+2          Qd[n] | Rd[m] | c | w
+ *   EXPR           0              (the program's constants stay shared)
+ * With the diagonal layouts entry i of z reads row[i], as in a row of the linear terms (q[n] | r[m]).  to_cost_weights_len gives len.  Until
+ * the first to_set_cost_weights there is no table and every kernel runs as before; the first call fills every instance with the shared weights
+ * of every cost, then applies its rows.  The shape stays fixed: the kind, terminal flag, q_ind and q_ref stay shared, and a QUADRATIC cost
+ * whose shared H is zero keeps H zero in every row (the zero pattern selects kernel code).  Weights to_create would accept in a spec of that
+ * kind are accepted (indefinite Q or R included, as the reference only warns).  TO_EINVAL, with the instance and the entry named, and nothing
+ * changed: a non-finite entry, a non-zero H where the shared H is zero, an EXPR cost, a hybrid problem, a cost index out of range.  The linear
+ * terms stay as they are (mutating cost.Q leaves cost.q alone); from then on to_set_goal_state(s) and to_update_trajectory(ies) set
+ * q_b = -Q_b xf and r_b = -R_b uf with each instance's own weights, the shared setters writing through to every instance.  A batch whose
+ * instance b holds w_b computes, bit for bit, what instance b of a batch created with w_b as the shared cost computes, on every solver path.
+ * Multi-GPU: each rank passes its shard's rows, as for x0. */
+int to_cost_weights_len(const to_handle* h, int32_t cost, int32_t* len);                            /* doubles per instance of distinct cost `cost` */
+int to_set_cost_weights(to_handle* h, int32_t cost, const double* w /*[B][len]*/);
+int to_get_cost_weights(to_handle* h, int32_t cost, double* w /*[B][len]*/);                       /* the shared values broadcast when none are set */
 
 /* ---- kernel 1: batched RK4 rollout (+ dual-number Jacobians) ---------------------------------------- */
 int to_rollout(to_handle* h);                                                 /* rollout!           src/problem.jl:330-340 */

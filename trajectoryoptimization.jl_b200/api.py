@@ -1205,6 +1205,13 @@ class Problem:
                 rows = np.empty((self.B, snap[cid].size))
                 self._raw_call(_con_rows_call(con, "get"), j, K._dp(rows))
                 con_carry[cid] = rows
+        cw_carry = {}   # per-instance cost weights: those of every cost whose own weights are unchanged since the call
+        cw_snap = getattr(self, "_cw_snap", {})
+        for j, c in enumerate(self._cost_objs):
+            if id(c) in cw_snap and np.array_equal(_cost_weight_row(c), cw_snap[id(c)]):
+                rows = np.empty((self.B, cw_snap[id(c)].size))
+                self._raw_call("to_get_cost_weights", j, K._dp(rows))
+                cw_carry[id(c)] = rows
         mparams = None
         if getattr(self, "_mparams", False):   # per-instance model parameters: carried over as they are
             mparams = np.empty((self.B, len(self.model.params)))
@@ -1213,6 +1220,10 @@ class Problem:
         self.spec = self._make_spec(self._dt, float(t[0]))
         self._open()
         self._sig = self._signature()
+        for j, c in enumerate(self._cost_objs):
+            if id(c) in cw_carry:
+                self._raw_call("to_set_cost_weights", j, K._dp(cw_carry[id(c)]))
+        self._cw_snap = {cid: v for cid, v in cw_snap.items() if cid in cw_carry}
         self._inst = bool(carry)
         if carry:
             q, r = np.empty((self.B, len(self._cost_objs), self.n)), np.empty((self.B, len(self._cost_objs), self.m))
@@ -1457,6 +1468,100 @@ def set_cost_terms(prob, q, r):
         raise DimensionMismatch("set_cost_terms: the objective changed its distinct costs; read cost_terms again")
     prob._call("to_set_cost_terms", K._dp(q), K._dp(r))
     prob._inst = True
+
+
+def _cost_weight_row(cost):
+    """the weights of ``cost`` in the layout of one instance's row of ``to_set_cost_weights`` (include/trajopt_b200.h): DiagonalCost
+    ``Qd | Rd | c``, QuadraticCost ``Q | R | H | c`` (column-major), DiagonalQuatCost ``Qd | Rd | c | w``"""
+    if not isinstance(cost, QuadraticCostFunction):
+        raise ArgumentError(f"the constants of a {type(cost).__name__} stay shared across the batch")
+    if isinstance(cost, DiagonalQuatCost):
+        return np.concatenate([np.diagonal(cost.Q), np.diagonal(cost.R), [cost.c, cost.w]]).astype(np.float64)
+    if cost.is_diag:
+        return np.concatenate([np.diagonal(cost.Q), np.diagonal(cost.R), [cost.c]]).astype(np.float64)
+    return np.concatenate([cost.Q.ravel(order="F"), cost.R.ravel(order="F"), cost.H.ravel(order="F"), [cost.c]]).astype(np.float64)
+
+
+def _cost_and_index(prob, cost):
+    """(index, cost) of ``cost``: an index into ``cost_terms``' distinct costs (``prob._cost_objs``) or one of those cost objects"""
+    if isinstance(cost, CostFunction):
+        j = next((i for i, c in enumerate(prob._cost_objs) if c is cost), None)
+        if j is None:
+            raise ArgumentError("the cost is not one of the problem's distinct costs")
+        return j, cost
+    j = int(cost)
+    if not 0 <= j < len(prob._cost_objs):
+        raise ArgumentError(f"cost index {j} outside 0:{len(prob._cost_objs) - 1}")
+    return j, prob._cost_objs[j]
+
+
+def _cost_weight_rows(prob, cost, rows):
+    """(index, cost, rows [B, len], linear terms or None) as ``to_set_cost_weights`` takes them; every check that needs no device happens
+    here.  Given cost objects, their q and r come back as ``(q [B, n], r [B, m])``, the cost's linear terms of every instance."""
+    if getattr(prob, "hybrid", False):
+        raise ArgumentError("per-instance cost weights are not supported on hybrid problems")
+    j, cost = _cost_and_index(prob, cost)
+    shared = _cost_weight_row(cost)
+    lin = None
+    if isinstance(rows, (list, tuple)) and any(isinstance(x, CostFunction) for x in rows):
+        if len(rows) != prob.B:
+            raise DimensionMismatch(f"set_cost_weights: {len(rows)} costs for a batch of {prob.B} instances")
+        for b, x in enumerate(rows):
+            if type(x) is not type(cost):
+                raise ArgumentError(f"set_cost_weights: instance {b} holds a {type(x).__name__}, the cost is a {type(cost).__name__}")
+            if (x.state_dim, x.control_dim) != (cost.state_dim, cost.control_dim):
+                raise DimensionMismatch(f"set_cost_weights: instance {b}'s cost has dimensions {(x.state_dim, x.control_dim)}, "
+                                        f"the problem's {(cost.state_dim, cost.control_dim)}")
+            if x.terminal != cost.terminal:
+                raise ArgumentError(f"set_cost_weights: instance {b}'s cost differs in its terminal flag")
+            if isinstance(cost, DiagonalQuatCost) and not (np.array_equal(x.q_ind, cost.q_ind) and np.array_equal(x.q_ref, cost.q_ref)):
+                raise ArgumentError(f"set_cost_weights: instance {b}'s DiagonalQuatCost differs in q_ind / q_ref")
+            if not cost.is_diag and x.is_blockdiag() != cost.is_blockdiag():
+                raise ArgumentError(f"set_cost_weights: instance {b}'s QuadraticCost has another H-zero pattern (H == 0 selects kernel code)")
+        lin = (np.array([x.q for x in rows], dtype=np.float64), np.array([x.r for x in rows], dtype=np.float64))
+        rows = [_cost_weight_row(x) for x in rows]
+    out = np.ascontiguousarray(np.asarray(rows, dtype=np.float64))
+    if out.shape != (prob.B, shared.size):
+        raise DimensionMismatch(f"set_cost_weights: expected [{prob.B}, {shared.size}] rows, got {out.shape}")
+    for b in range(prob.B):
+        bad = np.nonzero(~np.isfinite(out[b]))[0]
+        if bad.size:
+            raise ArgumentError(f"set_cost_weights: instance {b}, entry {bad[0]} is not finite")
+    if not cost.is_diag and cost.is_blockdiag():   # QuadraticCost with H == 0: every row keeps H zero
+        n, m = cost.state_dim, cost.control_dim
+        h0 = n * n + m * m
+        for b in range(prob.B):
+            bad = np.nonzero(out[b, h0:h0 + m * n] != 0.0)[0]
+            if bad.size:
+                raise ArgumentError(f"set_cost_weights: instance {b}, entry {h0 + bad[0]}: H must stay zero where the shared H is zero")
+    return j, cost, out, lin
+
+
+def set_cost_weights(prob, cost, rows):
+    """Instance ``b`` evaluates distinct cost ``cost`` (an index in the order of ``cost_terms``, or the cost object) with its own weights.
+    ``rows`` is ``[B, len]`` in the layout of include/trajopt_b200.h (DiagonalCost ``Qd | Rd | c``, QuadraticCost ``Q | R | H | c``
+    column-major, DiagonalQuatCost ``Qd | Rd | c | w``), or a sequence of ``B`` costs of the cost's type, dimensions, terminal flag,
+    ``q_ind`` / ``q_ref`` and H-zero pattern: their Q, R, H, c and w become the rows and their q, r that cost's linear terms, so
+    ``[cost_b] * B`` gives exactly the batch built with ``cost_b``.  Raw rows leave the linear terms as they are; from then on the goal
+    setters derive them from each instance's weights.  A batch whose instance ``b`` holds ``w_b`` computes, bit for bit, what instance ``b``
+    of a batch built with ``w_b`` computes.  The cost objects are left as they are; a later change to one's weights, picked up when the
+    handle is rebuilt, wins in every instance."""
+    j, cost, out, lin = _cost_weight_rows(prob, cost, rows)
+    prob._call("to_set_cost_weights", j, K._dp(out))
+    prob._cw_snap = {**getattr(prob, "_cw_snap", {}), id(cost): _cost_weight_row(cost)}
+    if lin is not None:
+        q, r = cost_terms(prob)
+        q[:, j], r[:, j] = lin
+        prob._call("to_set_cost_terms", K._dp(q), K._dp(r))
+        prob._inst = True
+
+
+def cost_weights(prob, cost):
+    """The weights of distinct cost ``cost`` of every instance, ``[B, len]`` (the shared weights broadcast when none were set)."""
+    j, cost = _cost_and_index(prob, cost)
+    out = np.empty((prob.B, _cost_weight_row(cost).size))
+    prob._call("to_get_cost_weights", j, K._dp(out))
+    return out
 
 
 def _model_param_rows(prob, params):

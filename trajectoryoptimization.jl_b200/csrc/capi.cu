@@ -1,6 +1,7 @@
 // capi.cu -- the C ABI (include/trajopt_b200.h): opaque handle, device memory, descriptor tables, and the
 // sequencing of the hot-path kernels.  No compute happens on the host: every compute entry point launches the
 // sm_90a kernels of rollout.cu / sweep.cu / riccati.cu / forward.cu on the handle's stream.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -56,6 +57,7 @@ struct to_handle {
     std::vector<double> h_qr;        // linear cost terms (DevProblem::qr), [B][ncost][n+m]
     std::vector<double> h_mparams;   // model parameters (DevProblem::mparams), [B][TO_NPARAM]
     std::vector<double> h_cdata;     // constraint data and Goal values (DevProblem::cdata), [B][ncdata]
+    std::vector<double> h_cw;        // cost weights (DevProblem::cw), [B][ncw]
     std::vector<double> stage;       // the rows a setter is building, committed by commit_rows (kept to reuse its allocation)
     int* d_fragerr = nullptr;     // sticky error word of that kernel (queue overflow / spin limit), read by to_synchronize
     double* d_fragpool = nullptr; // gains of its speculative regularisation candidates
@@ -251,7 +253,7 @@ int build_cost(to_handle* h, const to_cost_spec& tc, int n, int m, DevCost& c) {
     if (tc.kind == TO_COST_EXPR) {   // user cost recorded as a program (RD.@autodiff CostFunction)
         if (!tc.prog || tc.prog_len < 1 || tc.prog_len > TO_EXPR_LEN || tc.nconst < 0 || tc.nconst > TO_EXPR_CONST || (tc.nconst > 0 && !tc.consts))
             return fail(h, TO_EINVAL, "expression cost: bad program size");
-        c.expr = 1; c.prog_len = tc.prog_len; c.terminal = tc.terminal != 0;
+        c.expr = 1; c.prog_len = tc.prog_len; c.terminal = tc.terminal != 0; c.cwoff = -1;
         for (int j = 0; j < tc.prog_len; j++) {
             const int op = tc.prog[3 * j], a = tc.prog[3 * j + 1], b = tc.prog[3 * j + 2];
             const bool bin = op >= TO_OP_ADD && op <= TO_OP_DIV;
@@ -292,6 +294,31 @@ int build_cost(to_handle* h, const to_cost_spec& tc, int n, int m, DevCost& c) {
         c.zeroH = (hn == 0.0);   // is_blockdiag(cost) = zeroH, src/cost_functions.jl:445,455
     }
     return TO_OK;
+}
+
+// A cost's row of DevProblem::cw with its shared weights (the layout of common.cuh cost_data): DIAGONAL Qd | Rd | c, QUADRATIC Q | R | H | c,
+// DIAGONAL_QUAT Qd | Rd | c | w.  The one place that lays out a row; the setter checks rows of this layout.
+void cost_shared_row(const DevCost& c, int n, int m, double* row) {
+    if (c.diag) {
+        std::memcpy(row, c.Qd, sizeof(double) * n); std::memcpy(row + n, c.Rd, sizeof(double) * m);
+        row[n + m] = c.c;
+        if (c.quat) row[n + m + 1] = c.w;
+    } else {
+        std::memcpy(row, c.Q, sizeof(double) * n * n); std::memcpy(row + n * n, c.R, sizeof(double) * m * m);
+        std::memcpy(row + n * n + m * m, c.H, sizeof(double) * m * n);
+        row[n * n + m * m + m * n] = c.c;
+    }
+}
+// The dense Q (n x n) and R (m x m) of a row, as build_cost fills DevCost::Q / R from a spec of the cost's kind (a diagonal row: zeros off
+// the diagonal), so that lqr_linear_term gives an instance the bits a batch built with its weights would have.
+void cost_row_QR(const DevCost& c, const double* row, int n, int m, double* Q, double* R) {
+    if (c.diag) {
+        std::fill(Q, Q + n * n, 0.0); std::fill(R, R + m * m, 0.0);
+        for (int i = 0; i < n; i++) Q[i * n + i] = row[i];
+        for (int i = 0; i < m; i++) R[i * m + i] = row[n + i];
+    } else {
+        std::memcpy(Q, row, sizeof(double) * n * n); std::memcpy(R, row + n * n, sizeof(double) * m * m);
+    }
 }
 
 // doubles of constraint c in an instance's row of DevProblem::cdata (0: no per-instance data)
@@ -569,6 +596,8 @@ int to_create(const to_spec* s, to_handle** out) {
         if (rc) return bail(rc);
         if (!h->h_costs[i].diag) P.all_diag_cost = 0;
         if (h->h_costs[i].quat || h->h_costs[i].expr) { P.all_diag_cost = 0; P.dense_riccati = 1; }   // the fused fast paths assume purely quadratic costs
+        const int wlen = cost_weights_len(h->h_costs[i], n, m);
+        h->h_costs[i].cwoff = wlen ? P.ncw : -1; P.ncw += wlen;
     }
     P.lie = s->error_state ? 1 : 0; P.qs = 3; P.ne = P.lie ? n - 1 : n;
     if (P.lie) P.dense_riccati = 1;
@@ -881,6 +910,26 @@ static void stage_qr(to_handle* h) {
             std::memcpy(h->stage.data() + q_off(h, b, ci) + n, h->h_costs[ci].r, sizeof(double) * m);
         }
 }
+static size_t cw_off(const to_handle* h, int b, const DevCost& c) { return (size_t)b * h->P.ncw + c.cwoff; }
+// q | r of cost ci for instance b from the goal xf and, when uf is given, the control reference uf: with the instance's own Q and R once the
+// weight table exists, else with the shared ones (the bits every instance had before)
+static void instance_linear_term(const to_handle* h, int b, int ci, const double* xf, const double* uf, double* row) {
+    const DevCost& c = h->h_costs[ci];
+    const int n = h->P.n, m = h->P.m;
+    const double* Q = c.Q; const double* R = c.R;
+    double Qb[TO_MAXN * TO_MAXN], Rb[TO_MAXM * TO_MAXM];
+    if (h->P.cw && c.cwoff >= 0) { cost_row_QR(c, h->h_cw.data() + cw_off(h, b, c), n, m, Qb, Rb); Q = Qb; R = Rb; }
+    lqr_linear_term(Q, n, xf, row);
+    if (uf) lqr_linear_term(R, m, uf, row + n);
+}
+// h->stage := the rows of the cost-weight table, or every instance's shared weights of every cost when it does not exist yet
+static void stage_cw(to_handle* h) {
+    if (h->P.cw) { h->stage = h->h_cw; return; }
+    h->stage.resize((size_t)h->P.B * h->P.ncw);
+    for (int b = 0; b < h->P.B; b++)
+        for (const auto& c : h->h_costs)
+            if (c.cwoff >= 0) cost_shared_row(c, h->P.n, h->P.m, h->stage.data() + cw_off(h, b, c));
+}
 // h->stage := the rows of the constraint-data table, or every instance's shared data of every constraint when it does not exist yet
 static void stage_cdata(to_handle* h) {
     if (h->P.cdata) { h->stage = h->h_cdata; return; }
@@ -903,11 +952,15 @@ int to_set_goal_state(to_handle* h, const double* xf, int objective, int constra
             if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) c.a[i] = xf[c.inds[i]];
     h->J_valid = false;
     int rc = upload_tables(h); if (rc) return rc;
-    // the later call wins: every instance takes the shared goal
-    if (objective && h->P.qr) {
+    // the later call wins: every instance takes the shared goal, through its own weights once they are per instance
+    if (objective && (h->P.qr || h->P.cw)) {
         stage_qr(h);
         for (int b = 0; b < h->P.B; b++)
-            for (int ci = 0; ci < h->P.ncost; ci++) std::memcpy(h->stage.data() + q_off(h, b, ci), h->h_costs[ci].q, sizeof(double) * n);
+            for (int ci = 0; ci < h->P.ncost; ci++) {
+                double* row = h->stage.data() + q_off(h, b, ci);
+                if (h->P.cw) instance_linear_term(h, b, ci, xf, nullptr, row);
+                else std::memcpy(row, h->h_costs[ci].q, sizeof(double) * n);
+            }
         rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
     }
     if (constraint && h->P.cdata) {
@@ -928,7 +981,7 @@ int to_set_goal_states(to_handle* h, const double* xf, int objective, int constr
     if (objective) {
         stage_qr(h);
         for (int b = 0; b < h->P.B; b++)
-            for (int ci = 0; ci < h->P.ncost; ci++) lqr_linear_term(h->h_costs[ci].Q, n, xf + (size_t)b * n, h->stage.data() + q_off(h, b, ci));
+            for (int ci = 0; ci < h->P.ncost; ci++) instance_linear_term(h, b, ci, xf + (size_t)b * n, nullptr, h->stage.data() + q_off(h, b, ci));
         int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
         h->J_valid = false;
     }
@@ -953,10 +1006,8 @@ int to_update_trajectories(to_handle* h, const double* Xref, const double* Uref,
     for (int b = 0; b < h->P.B; b++)
         for (int i = 0; i < N; i++) {                   // set_LQR_goal!(obj[i], state(Z[k]), control(Z[k])) of instance b
             const int cid = h->h_cost_index[i];
-            const DevCost& c = h->h_costs[cid];
-            double* row = h->stage.data() + q_off(h, b, cid);
-            lqr_linear_term(c.Q, n, Xref + ((size_t)b * nref + start - 1 + i) * n, row);
-            lqr_linear_term(c.R, m, Uref + ((size_t)b * nref + start - 1 + i) * m, row + n);
+            instance_linear_term(h, b, cid, Xref + ((size_t)b * nref + start - 1 + i) * n, Uref + ((size_t)b * nref + start - 1 + i) * m,
+                                 h->stage.data() + q_off(h, b, cid));
         }
     int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
@@ -1116,6 +1167,55 @@ int to_get_constraint_data(to_handle* h, int32_t con, double* data) {
     return TO_OK;
 }
 
+// ---- per-instance cost weights (DevProblem::cw) ----------------------------------------------------------
+int to_cost_weights_len(const to_handle* h, int32_t cost, int32_t* len) {
+    if (!h || !len) return TO_EINVAL;
+    if (cost < 0 || cost >= (int)h->h_costs.size()) return TO_EINVAL;
+    *len = cost_weights_len(h->h_costs[cost], h->P.n, h->P.m);
+    return TO_OK;
+}
+// w [B][len] of cost `cost` (the layout of cost_shared_row).  The whole batch is checked before anything changes: a refused call leaves the
+// table (or its absence) as it was.  The first call creates the table with the shared weights of every cost in every row.  The linear terms
+// stay as they are (mutating cost.Q leaves cost.q alone); the goal setters derive them from each instance's weights from then on.
+int to_set_cost_weights(to_handle* h, int32_t cost, const double* w) {
+    JOIN(h);
+    if (!h || !w) return TO_EINVAL;
+    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance cost weights are not supported on hybrid problems");
+    if (cost < 0 || cost >= (int)h->h_costs.size()) return fail(h, TO_EINVAL, "to_set_cost_weights: no cost " + std::to_string(cost));
+    const DevCost& c = h->h_costs[cost];
+    if (c.expr) return fail(h, TO_EINVAL, "to_set_cost_weights: the constants of a recorded (expression) cost stay shared");
+    const int n = h->P.n, m = h->P.m, len = cost_weights_len(c, n, m), B = h->P.B;
+    const int h0 = n * n + m * m;   // QUADRATIC: H sits at [h0, h0 + m n)
+    auto where = [](int b, int j) { return "instance " + std::to_string(b) + ", entry " + std::to_string(j); };
+    for (int b = 0; b < B; b++) {
+        const double* row = w + (size_t)b * len;
+        for (int j = 0; j < len; j++) {
+            if (!std::isfinite(row[j])) return fail(h, TO_EINVAL, "to_set_cost_weights: " + where(b, j) + " is not finite");
+            if (!c.diag && c.zeroH && j >= h0 && j < h0 + m * n && row[j] != 0.0)
+                return fail(h, TO_EINVAL, "to_set_cost_weights: " + where(b, j) + ": H must stay zero where the shared H is zero (it selects kernel code)");
+        }
+    }
+    stage_cw(h);
+    for (int b = 0; b < B; b++) std::memcpy(h->stage.data() + cw_off(h, b, c), w + (size_t)b * len, sizeof(double) * len);
+    int rc = commit_rows(h, h->h_cw, h->P.cw); if (rc) return rc;
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return TO_OK;
+}
+// w [B][len]: cost `cost`'s weights of every instance (the shared weights broadcast when none are set)
+int to_get_cost_weights(to_handle* h, int32_t cost, double* w) {
+    JOIN(h);
+    if (!h || !w) return TO_EINVAL;
+    if (cost < 0 || cost >= (int)h->h_costs.size()) return fail(h, TO_EINVAL, "to_get_cost_weights: no cost " + std::to_string(cost));
+    const DevCost& c = h->h_costs[cost];
+    const int n = h->P.n, m = h->P.m, len = cost_weights_len(c, n, m);
+    if (len == 0) return fail(h, TO_EINVAL, "to_get_cost_weights: a recorded (expression) cost has no weights");
+    std::vector<double> shared(len);
+    cost_shared_row(c, n, m, shared.data());
+    for (int b = 0; b < h->P.B; b++)
+        std::memcpy(w + (size_t)b * len, h->P.cw ? h->h_cw.data() + cw_off(h, b, c) : shared.data(), sizeof(double) * len);
+    return TO_OK;
+}
+
 // ---- kernel 1 ---------------------------------------------------------------------------------------------
 int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, int32_t nref, int32_t start) {
     JOIN(h);
@@ -1129,13 +1229,17 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
     }
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     int rc = upload_tables(h); if (rc) return rc;
-    if (!h->P.qr) return TO_OK;
+    if (!h->P.qr && !h->P.cw) return TO_OK;
     stage_qr(h);
-    for (int b = 0; b < h->P.B; b++)                    // the later call wins: every instance takes the shared reference
+    for (int b = 0; b < h->P.B; b++)                    // the later call wins: every instance takes the shared reference, through its own weights
         for (int i = 0; i < N; i++) {
             const int cid = h->h_cost_index[i];
-            std::memcpy(h->stage.data() + q_off(h, b, cid), h->h_costs[cid].q, sizeof(double) * n);
-            std::memcpy(h->stage.data() + q_off(h, b, cid) + n, h->h_costs[cid].r, sizeof(double) * m);
+            double* row = h->stage.data() + q_off(h, b, cid);
+            if (h->P.cw) instance_linear_term(h, b, cid, Xref + (size_t)(start - 1 + i) * n, Uref + (size_t)(start - 1 + i) * m, row);
+            else {
+                std::memcpy(row, h->h_costs[cid].q, sizeof(double) * n);
+                std::memcpy(row + n, h->h_costs[cid].r, sizeof(double) * m);
+            }
         }
     return commit_rows(h, h->h_qr, h->P.qr);
 }

@@ -32,7 +32,8 @@ enum { CON_GOAL = 0, CON_BOUND = 1, CON_LINEAR = 2, CON_CIRCLE = 3, CON_SPHERE =
 
 // QuadraticCostFunction (reference src/cost_functions.jl:326-347, :417-454); dense storage + diagonal copy
 struct DevCost {
-    int diag, terminal, zeroH, pad;
+    int diag, terminal, zeroH;
+    int cwoff;                     // offset of the cost's weights in an instance's row of DevProblem::cw (-1: EXPR, no weights)
     double c;
     double Qd[TO_MAXN], Rd[TO_MAXM];
     double q[TO_MAXN], r[TO_MAXM];
@@ -176,6 +177,10 @@ struct DevProblem {
     // the shared DevCon fields.
     const double* cdata;      // [B][ncdata]
     int ncdata;
+    // Per-instance cost weights (to_set_cost_weights): row b holds, at DevCost::cwoff, the weights of every quadratic cost (see cost_data).
+    // nullptr until the first call; every kernel then reads the shared DevCost fields.
+    int ncw;
+    const double* cw;         // [B][ncw]
 };
 #define TO_NPARAM 16        // slots of DevProblem::params and of a row of DevProblem::mparams (one 128-byte line)
 
@@ -185,22 +190,44 @@ __host__ __device__ inline bool retired(const DevProblem& P, int b) { return P.a
 // Which variant of a kernel family runs: INST = true when a per-instance table the family reads exists.  The only place that decides; every
 // launcher and to_kernel_choice ask here.  The line search reads the linear cost terms, the model parameters and the constraint data; the
 // expansion, backward and sweep kernels the cost terms and the constraint data; the dynamics kernels the model parameters alone.
-__host__ __device__ inline bool inst_forward(const DevProblem& P) { return P.qr || P.mparams || P.cdata; }
-__host__ __device__ inline bool inst_backward(const DevProblem& P) { return P.qr || P.cdata; }
+__host__ __device__ inline bool inst_forward(const DevProblem& P) { return P.qr || P.mparams || P.cdata || P.cw; }
+__host__ __device__ inline bool inst_backward(const DevProblem& P) { return P.qr || P.cdata || P.cw; }
 __host__ __device__ inline bool inst_dynamics(const DevProblem& P) { return P.mparams; }
 
-// Linear cost terms of instance b: the only place that decides between the per-instance table and the shared descriptors.
-// INST = false is the shared path, compiled without a look at the tables; the hot kernels take INST as a template parameter and are
-// launched with INST = true only when the tables exist.
+// The weights and linear terms of cost cid for instance b: the only place that decides between an instance's rows (DevProblem::cw for the
+// weights, DevProblem::qr for the linear terms) and the descriptor, and the only way a kernel reads them.  The cost's structure (diag, zeroH,
+// quat, q_ind, q_ref, the program) stays in the descriptor.  An instance's row of cw, at DevCost::cwoff, by kind:
+//   DIAGONAL Qd[n] | Rd[m] | c ;  QUADRATIC Q[n*n] | R[m*m] | H[m*n] | c ;  DIAGONAL_QUAT Qd[n] | Rd[m] | c | w.
+// So with the diagonal layout entry i of z reads row[i], as it does in the row of qr (q[n] | r[m]).  A diagonal row has no dense Q / R / H
+// and a dense one no Qd / Rd: those fields keep the descriptor's, and every reader takes the form the cost's `diag` selects.
+// INST = false is the shared path, compiled without a look at the tables; the hot kernels take INST as a template parameter and are launched
+// with INST = true only when a table exists.  Every field is a pointer, c and w included, as in ConData: building the view loads nothing.
+// `shared`: the descriptor's fields, or a kernel's staged copy of them (the line search's cost cache in shared memory).
+struct CostData { const double *Qd, *Rd, *Q, *R, *H, *q, *r, *c, *w; };
 template <bool INST>
-__host__ __device__ __forceinline__ const double* inst_q(const DevProblem& P, int b, int cid) {
-    if constexpr (INST) { if (P.qr) return P.qr + ((size_t)b * P.ncost + cid) * (P.n + P.m); }
-    return P.costs[cid].q;
+__device__ __forceinline__ CostData cost_data(const DevProblem& P, int b, int cid, CostData shared) {
+    if constexpr (INST) {
+        const int n = P.n, m = P.m;
+        if (P.qr) { const double* row = P.qr + ((size_t)b * P.ncost + cid) * (n + m); shared.q = row; shared.r = row + n; }
+        const DevCost& c = P.costs[cid];
+        if (P.cw && c.cwoff >= 0) {
+            const double* row = P.cw + (size_t)b * P.ncw + c.cwoff;
+            if (c.diag) { shared.Qd = row; shared.Rd = row + n; shared.c = row + n + m; shared.w = row + n + m + 1; }
+            else { shared.Q = row; shared.R = row + n * n; shared.H = row + n * n + m * m; shared.c = row + n * n + m * m + m * n; }
+        }
+    }
+    return shared;
 }
+__device__ __forceinline__ CostData cost_fields(const DevCost& c) { return CostData{c.Qd, c.Rd, c.Q, c.R, c.H, c.q, c.r, &c.c, &c.w}; }
 template <bool INST>
-__host__ __device__ __forceinline__ const double* inst_r(const DevProblem& P, int b, int cid) {
-    if constexpr (INST) { if (P.qr) return P.qr + ((size_t)b * P.ncost + cid) * (P.n + P.m) + P.n; }
-    return P.costs[cid].r;
+__device__ __forceinline__ CostData cost_data(const DevProblem& P, int b, int cid) {
+    return cost_data<INST>(P, b, cid, cost_fields(P.costs[cid]));
+}
+// Doubles of a cost's row of DevProblem::cw (the table above; 0 for a program cost)
+__host__ __device__ inline int cost_weights_len(const DevCost& c, int n, int m) {
+    if (c.expr) return 0;
+    if (c.diag) return n + m + 1 + (c.quat ? 1 : 0);
+    return n * n + m * m + m * n + 1;
 }
 // Model parameter i of instance b: the only place that decides between the rows of DevProblem::mparams and the shared vector.  A value, not a
 // pointer: the shared vector lives in the kernel's parameter bank, and a pointer that may point there makes the kernel copy it to local memory.

@@ -64,41 +64,42 @@ __device__ inline Hyper expr_eval(const DevCost& c, int n, const double* x, cons
 }
 
 // geodesic term of DiagonalQuatCost (src/lie_costs.jl:74-76): w min(1 + dq, 1 - dq), dq = q_ref'x[q_ind]
-__device__ __forceinline__ double quat_cost_term(const DevCost& c, const double* x) {
+__device__ __forceinline__ double quat_cost_term(const DevCost& c, const CostData& d, const double* x) {
     double dq = 0;
     for (int i = 0; i < 4; i++) dq = fma(c.q_ref[i], x[c.q_ind[i]], dq);
-    return c.w * fmin(1 + dq, 1 - dq);
+    return *d.w * fmin(1 + dq, 1 - dq);
 }
 
-// q, r: the linear terms to use (c.q / c.r, or an instance's row of DevProblem::qr, inst_q / inst_r)
-__device__ inline double cost_value(const DevCost& c, const double* q, const double* r, int n, int m, const double* x, const double* u, bool has_u) {
+// d: the cost's weights and linear terms (cost_data); the structure is read from the descriptor
+__device__ inline double cost_value(const DevCost& c, const CostData& d, int n, int m, const double* x, const double* u, bool has_u) {
     if (c.expr) return expr_eval(c, n, x, u, has_u, -1, -1).v;
+    const double* q = d.q; const double* r = d.r;
     double J = 0;
     if (c.diag) {
         double a = 0, l = 0;
-        for (int i = 0; i < n; i++) { a = fma(c.Qd[i] * x[i], x[i], a); l = fma(q[i], x[i], l); }
-        J = 0.5 * a + l + c.c;
+        for (int i = 0; i < n; i++) { a = fma(d.Qd[i] * x[i], x[i], a); l = fma(q[i], x[i], l); }
+        J = 0.5 * a + l + *d.c;
         if (has_u) {
             double au = 0, lu = 0;
-            for (int i = 0; i < m; i++) { au = fma(c.Rd[i] * u[i], u[i], au); lu = fma(r[i], u[i], lu); }
+            for (int i = 0; i < m; i++) { au = fma(d.Rd[i] * u[i], u[i], au); lu = fma(r[i], u[i], lu); }
             J += 0.5 * au + lu;
         }
-        if (c.quat) J += quat_cost_term(c, x);
+        if (c.quat) J += quat_cost_term(c, d, x);
         return J;
     }
     for (int j = 0; j < n; j++) {
         double qx = 0;
-        for (int i = 0; i < n; i++) qx = fma(c.Q[j * n + i], x[i], qx);
+        for (int i = 0; i < n; i++) qx = fma(d.Q[j * n + i], x[i], qx);
         J = fma(0.5 * qx, x[j], J);
     }
     double lin = 0;
     for (int i = 0; i < n; i++) lin = fma(q[i], x[i], lin);
-    J += lin + c.c;
+    J += lin + *d.c;
     if (has_u) {
         double Ju = 0, linu = 0;
         for (int j = 0; j < m; j++) {
             double ru = 0;
-            for (int i = 0; i < m; i++) ru = fma(c.R[j * m + i], u[i], ru);
+            for (int i = 0; i < m; i++) ru = fma(d.R[j * m + i], u[i], ru);
             Ju = fma(0.5 * ru, u[j], Ju);
         }
         for (int i = 0; i < m; i++) linu = fma(r[i], u[i], linu);
@@ -106,65 +107,69 @@ __device__ inline double cost_value(const DevCost& c, const double* q, const dou
         if (!c.zeroH) {
             double h = 0;
             for (int j = 0; j < n; j++)
-                for (int i = 0; i < m; i++) h = fma(u[i] * c.H[j * m + i], x[j], h);
+                for (int i = 0; i < m; i++) h = fma(u[i] * d.H[j * m + i], x[j], h);
             J += h;
         }
     }
     return J;
 }
 __device__ inline double cost_value(const DevCost& c, int n, int m, const double* x, const double* u, bool has_u) {
-    return cost_value(c, c.q, c.r, n, m, x, u, has_u);
+    return cost_value(c, cost_fields(c), n, m, x, u, has_u);
 }
 
 // grad[n+m]; the u-part is left untouched at the terminal knot (the reference skips it when is_terminal(z))
 template <bool QUAT = true>
-__device__ inline void cost_gradient_quadratic(const DevCost& c, const double* q, const double* r, int n, int m, const double* x, const double* u, bool is_terminal, double* grad);
-__device__ inline void cost_gradient(const DevCost& c, const double* q, const double* r, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
+__device__ inline void cost_gradient_quadratic(const DevCost& c, const CostData& d, int n, int m, const double* x, const double* u, bool is_terminal, double* grad);
+__device__ inline void cost_gradient(const DevCost& c, const CostData& d, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
     if (c.expr) {   // RD.gradient!(ForwardAD) of a user cost
         const int lim = is_terminal ? n : n + m;
         for (int i = 0; i < lim; i++) grad[i] = expr_eval(c, n, x, u, !is_terminal, i, -1).d1;
         return;
     }
-    cost_gradient_quadratic(c, q, r, n, m, x, u, is_terminal, grad);
+    cost_gradient_quadratic(c, d, n, m, x, u, is_terminal, grad);
 }
 __device__ inline void cost_gradient(const DevCost& c, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
-    cost_gradient(c, c.q, c.r, n, m, x, u, is_terminal, grad);
+    cost_gradient(c, cost_fields(c), n, m, x, u, is_terminal, grad);
 }
 // QuadraticCostFunction only (the register-resident kernels call this directly with QUAT = false: no dynamically indexed stores)
 template <bool QUAT>
-__device__ inline void cost_gradient_quadratic(const DevCost& c, const double* q, const double* r, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
+__device__ inline void cost_gradient_quadratic(const DevCost& c, const CostData& d, int n, int m, const double* x, const double* u, bool is_terminal, double* grad) {
     for (int i = 0; i < n; i++) {
-        double g = q[i];
-        if (c.diag) g = fma(c.Qd[i], x[i], g);
-        else for (int j = 0; j < n; j++) g = fma(c.Q[j * n + i], x[j], g);
+        double g = d.q[i];
+        if (c.diag) g = fma(d.Qd[i], x[i], g);
+        else for (int j = 0; j < n; j++) g = fma(d.Q[j * n + i], x[j], g);
         grad[i] = g;
     }
     if (QUAT && c.quat) {   // gradient!(::DiagonalQuatCost) src/lie_costs.jl:79-95: -+ w q_ref by the sign of q_ref'p
         double dq = 0;
         for (int i = 0; i < 4; i++) dq = fma(c.q_ref[i], x[c.q_ind[i]], dq);
-        const double sw = dq < 0 ? c.w : -c.w;
+        const double sw = dq < 0 ? *d.w : -*d.w;
         for (int i = 0; i < 4; i++) grad[c.q_ind[i]] = fma(sw, c.q_ref[i], grad[c.q_ind[i]]);
     }
     if (!is_terminal) {
         for (int i = 0; i < m; i++) {
-            double g = r[i];
-            if (c.diag) g = fma(c.Rd[i], u[i], g);
-            else for (int j = 0; j < m; j++) g = fma(c.R[j * m + i], u[j], g);
+            double g = d.r[i];
+            if (c.diag) g = fma(d.Rd[i], u[i], g);
+            else for (int j = 0; j < m; j++) g = fma(d.R[j * m + i], u[j], g);
             grad[n + i] = g;
         }
         if (!c.zeroH)
             for (int j = 0; j < n; j++)
                 for (int i = 0; i < m; i++) {
-                    grad[j] = fma(c.H[j * m + i], u[i], grad[j]);
-                    grad[n + i] = fma(c.H[j * m + i], x[j], grad[n + i]);
+                    grad[j] = fma(d.H[j * m + i], u[i], grad[j]);
+                    grad[n + i] = fma(d.H[j * m + i], x[j], grad[n + i]);
                 }
     }
 }
 
 // hess (n+m)x(n+m) col-major, written in full and symmetric (the reference writes only the lower-left H block
 // and leaves the rest to the caller's zero initialisation, SURVEY.md 2.4)
-__device__ inline void cost_hessian_quadratic(const DevCost& c, int n, int m, bool is_terminal, double* hess);
-__device__ inline void cost_hessian(const DevCost& c, int n, int m, const double* x, const double* u, bool is_terminal, double* hess) {
+// INST: a diagonal cost's entries are read from Qd / Rd, as an instance's row of DevProblem::cw has no dense Q / R; the shared path reads the
+// descriptor's dense Q / R, whose diagonals build_cost fills with the same values
+template <bool INST>
+__device__ inline void cost_hessian_quadratic(const DevCost& c, const CostData& d, int n, int m, bool is_terminal, double* hess);
+template <bool INST>
+__device__ inline void cost_hessian(const DevCost& c, const CostData& d, int n, int m, const double* x, const double* u, bool is_terminal, double* hess) {
     const int nm = n + m;
     if (c.expr) {   // RD.hessian!(ForwardAD) of a user cost: one second-order pass per entry of the lower triangle
         for (int i = 0; i < nm * nm; i++) hess[i] = 0;
@@ -173,19 +178,20 @@ __device__ inline void cost_hessian(const DevCost& c, int n, int m, const double
             for (int i = j; i < lim; i++) { const double h = expr_eval(c, n, x, u, !is_terminal, i, j).d12; hess[j * nm + i] = h; hess[i * nm + j] = h; }
         return;
     }
-    cost_hessian_quadratic(c, n, m, is_terminal, hess);
+    cost_hessian_quadratic<INST>(c, d, n, m, is_terminal, hess);
 }
-__device__ inline void cost_hessian_quadratic(const DevCost& c, int n, int m, bool is_terminal, double* hess) {
+template <bool INST>
+__device__ inline void cost_hessian_quadratic(const DevCost& c, const CostData& d, int n, int m, bool is_terminal, double* hess) {
     const int nm = n + m;
     for (int i = 0; i < nm * nm; i++) hess[i] = 0;
     for (int j = 0; j < n; j++)
-        for (int i = 0; i < n; i++) if (!c.diag || i == j) hess[j * nm + i] = c.Q[j * n + i];
+        for (int i = 0; i < n; i++) if (!c.diag || i == j) hess[j * nm + i] = (INST && c.diag) ? d.Qd[i] : d.Q[j * n + i];
     if (!is_terminal) {
         for (int j = 0; j < m; j++)
-            for (int i = 0; i < m; i++) if (!c.diag || i == j) hess[(n + j) * nm + n + i] = c.R[j * m + i];
+            for (int i = 0; i < m; i++) if (!c.diag || i == j) hess[(n + j) * nm + n + i] = (INST && c.diag) ? d.Rd[i] : d.R[j * m + i];
         if (!c.zeroH)
             for (int j = 0; j < n; j++)
-                for (int i = 0; i < m; i++) { hess[j * nm + n + i] = c.H[j * m + i]; hess[(n + i) * nm + j] = c.H[j * m + i]; }
+                for (int i = 0; i < m; i++) { hess[j * nm + n + i] = d.H[j * m + i]; hess[(n + i) * nm + j] = d.H[j * m + i]; }
     }
 }
 
@@ -497,7 +503,7 @@ __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const doub
 
 // Cost expansion of one knot with the AL terms (Gauss-Newton):
 //   grad += -cz' D' lp ; hess += mu cz' D'D cz,  D = grad Pi_{K*}(lambda - mu c), lp = Pi_{K*}(lambda - mu c)
-// k0 = 0-based knot, b = instance (its linear cost terms and constraint data when INST).  grad[n+m], hess[(n+m)^2] col-major symmetric.
+// k0 = 0-based knot, b = instance (its cost weights, linear cost terms and constraint data when INST).  grad[n+m], hess[(n+m)^2] col-major symmetric.
 template <bool INST = false>
 __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const double* x, const double* u, const double* lam_b,
                                          double* grad, double* hess, int b = 0) {
@@ -505,9 +511,10 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
     const bool last = (k0 == P.N - 1);
     const int cid = P.cost_index[k0];
     const DevCost& cost = P.costs[cid];
+    const CostData cd = cost_data<INST>(P, b, cid);
     for (int i = 0; i < nm; i++) grad[i] = 0;
-    cost_gradient(cost, inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, last, grad);
-    cost_hessian(cost, n, m, x, u, last, hess);
+    cost_gradient(cost, cd, n, m, x, u, last, grad);
+    cost_hessian<INST>(cost, cd, n, m, x, u, last, hess);
     const int lim = last ? n : nm;
     for (int ci = 0; ci < P.ncon; ci++) {
         const DevCon& con = P.cons[ci];
@@ -516,8 +523,8 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
         const double mu = P.mu[ci];
         const double* lam = lam_b + con.offset + (size_t)(k0 + 1 - con.first) * p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
-        const ConData cd = con_data<INST>(P, b, ci);
-        con_evaluate(con, cd, n, m, x, u, c);
+        const ConData dd = con_data<INST>(P, b, ci);
+        con_evaluate(con, dd, n, m, x, u, c);
         if (con.diagonal) {   // Goal / Bound: +-1 selector rows (src/constraints.jl:62-68, :757-765) -- row by row, no dense products
             const bool eq = (con.kind == CON_GOAL);
             const int nrow = eq ? p : con.n_max + con.n_min;
@@ -530,7 +537,7 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
             continue;
         }
         double jac[TO_MAXP * TO_MAXNM], Dm[TO_MAXP * TO_MAXP], tmp[TO_MAXP * TO_MAXNM];
-        con_jacobian(con, cd, n, m, x, u, jac);
+        con_jacobian(con, dd, n, m, x, u, jac);
         for (int i = 0; i < p; i++) lbar[i] = lam[i] - mu * c[i];
         const int dc = dualcone(con.sense);
         cone_projection(dc, lbar, p, lp);
@@ -584,7 +591,7 @@ __device__ __forceinline__ void state_diff(bool lie, int n, int qs, const double
 // DiagonalCost (src/cost_functions.jl:137-233); AL rows of Goal / Bound constraints as in al_knot_expansion.  Logical order: ge = G'g and
 // hd = the diagonal, over the error state and the controls; b01, b02, b12 = the off-diagonal entries of the attitude block.  lie.cu
 // k_expansion_compact (EC) and riccati_frag.cu k_expansion_rec (the record) store it, each in its own layout.
-template <bool INST>   // INST: the linear cost terms and constraint data of each instance
+template <bool INST>   // INST: the cost weights, linear cost terms and constraint data of each instance
 __device__ __forceinline__ void compact_expansion(const DevProblem& P, int b, int k, double (&ge)[16], double (&hd)[16],
                                                   double& b01, double& b02, double& b12) {
     const int n = P.n, m = P.m, nm = n + m, qs = P.qs;
@@ -596,10 +603,9 @@ __device__ __forceinline__ void compact_expansion(const DevProblem& P, int b, in
     for (int i = 0; i < n; i++) z[i] = xg[i];
     for (int a = 0; a < m; a++) z[n + a] = last ? 0.0 : ug[a];
     const int cid = P.cost_index[k];
-    const DevCost& c = P.costs[cid];
-    const double* cq = inst_q<INST>(P, b, cid); const double* cr = inst_r<INST>(P, b, cid);
-    for (int i = 0; i < n; i++) { g[i] = fma(c.Qd[i], z[i], cq[i]); h[i] = c.Qd[i]; }
-    for (int a = 0; a < m; a++) { g[n + a] = last ? 0.0 : fma(c.Rd[a], z[n + a], cr[a]); h[n + a] = last ? 0.0 : c.Rd[a]; }
+    const CostData c = cost_data<INST>(P, b, cid);
+    for (int i = 0; i < n; i++) { g[i] = fma(c.Qd[i], z[i], c.q[i]); h[i] = c.Qd[i]; }
+    for (int a = 0; a < m; a++) { g[n + a] = last ? 0.0 : fma(c.Rd[a], z[n + a], c.r[a]); h[n + a] = last ? 0.0 : c.Rd[a]; }
     const int lim = last ? n : nm;
     for (int ci = 0; ci < P.ncon; ci++) {
         const DevCon& con = P.cons[ci];

@@ -47,6 +47,8 @@ __device__ __forceinline__ ConData staged(const FwdCon& c) { return ConData{c.a,
 struct FwdCost {
     double Qd[TO_MAXN], Rd[TO_MAXM], q[TO_MAXN], r[TO_MAXM], c;
 };
+// the cost view (common.cuh cost_data) of a cached cost: its diagonal weights, linear terms and c in shared memory
+__device__ __forceinline__ CostData staged(const FwdCost& c) { return CostData{c.Qd, c.Rd, nullptr, nullptr, nullptr, c.q, c.r, &c.c, nullptr}; }
 struct alignas(16) FwdTab {
     int ncon, ncost_cached, pad0, pad1;
     FwdCon con[TO_MAXCON];
@@ -111,6 +113,12 @@ struct alignas(16) FwdCompactTab {
     FwdCost term;                    // terminal cost (Qd, q, c)
     FwdCon goal;                     // the Goal's mu, inv2mu, mask_max, row_max, a
     double dt[FWD_MAX_N];
+};
+// The per-instance variant's copy of an instance's two costs in the fields of FwdCompactTab, staged for each group by linesearch_pass
+struct alignas(16) FwdCompactCost {
+    double2 sx[TO_MAXN], su[TO_MAXM];
+    double sc, pad;
+    FwdCost term;
 };
 
 __device__ inline void load_compact_tables(const DevProblem& P, FwdCompactTab& tab) {
@@ -297,26 +305,23 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
             const int cid = tab.cost_index[k];
             double a2 = 0.0, l1 = 0.0, cc;
             if (tab.ncost_cached) {
-                const FwdCost& c = tab.cost[cid];
-                const double* cq = c.q; const double* cr = c.r;
-                if constexpr (INST) { cq = inst_q<true>(P, b, cid); cr = inst_r<true>(P, b, cid); }
+                const CostData c = cost_data<INST>(P, b, cid, staged(tab.cost[cid]));
 #pragma unroll
-                for (int i = 0; i < n; i++) { a2 = fma(c.Qd[i] * x[i], x[i], a2); l1 = fma(cq[i], x[i], l1); }
+                for (int i = 0; i < n; i++) { a2 = fma(c.Qd[i] * x[i], x[i], a2); l1 = fma(c.q[i], x[i], l1); }
                 if (!last) {
 #pragma unroll
-                    for (int i = 0; i < m; i++) { a2 = fma(c.Rd[i] * u[i], u[i], a2); l1 = fma(cr[i], u[i], l1); }
+                    for (int i = 0; i < m; i++) { a2 = fma(c.Rd[i] * u[i], u[i], a2); l1 = fma(c.r[i], u[i], l1); }
                 }
-                cc = c.c;
+                cc = *c.c;
             } else {
-                const DevCost& c = P.costs[cid];
-                const double* cq = inst_q<INST>(P, b, cid); const double* cr = inst_r<INST>(P, b, cid);
+                const CostData c = cost_data<INST>(P, b, cid);
 #pragma unroll
-                for (int i = 0; i < n; i++) { a2 = fma(c.Qd[i] * x[i], x[i], a2); l1 = fma(cq[i], x[i], l1); }
+                for (int i = 0; i < n; i++) { a2 = fma(c.Qd[i] * x[i], x[i], a2); l1 = fma(c.q[i], x[i], l1); }
                 if (!last) {
 #pragma unroll
-                    for (int i = 0; i < m; i++) { a2 = fma(c.Rd[i] * u[i], u[i], a2); l1 = fma(cr[i], u[i], l1); }
+                    for (int i = 0; i < m; i++) { a2 = fma(c.Rd[i] * u[i], u[i], a2); l1 = fma(c.r[i], u[i], l1); }
                 }
-                cc = c.c;
+                cc = *c.c;
             }
             J += fma(0.5, a2, l1) + cc;
         }
@@ -395,11 +400,11 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
 //     candidate stores ran pass 1 in about half the time);
 //   * RK4 writes the next state over the current one (rk4_step reads x_i for the last time where it writes xn_i), so the loop carries
 //     no x <- xn copies.  (Unrolled by two with x / xn swapping roles instead, the loop took 40 more registers and spilled.)
-// INST: gbox = the instance's control box {u_max_i, u_min_i}, staged for the group by linesearch_pass
+// INST: gbox = the instance's control box {u_max_i, u_min_i} and gcost = its two costs, staged for the group by linesearch_pass
 template <int MODEL, int IPB, int G, bool LIE, bool INST>
 __device__ __forceinline__ double rollout_compact(const DevProblem& P, const FwdCompactTab& tab, double* stage, double* ost, const double* prm,
-                                                  const double2* gbox, int b, int g, int l, unsigned gmask, double alpha, int cbuf, bool& ok,
-                                                  double& viol) {
+                                                  const double2* gbox, const FwdCompactCost* gcost, int b, int g, int l, unsigned gmask,
+                                                  double alpha, int cbuf, bool& ok, double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     using S = Stage<n, m, IPB, NE>;
     const int N = P.N, buf = P.cur[b];
@@ -413,8 +418,10 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
     constexpr int OX = FWD_OKNOTS * n, OL = FWD_OKNOTS * (n + m);
     double* myx = ost + l * OL;
     double* myu = myx + OX;
-    const double* cq = INST ? inst_q<true>(P, b, tab.cid) : nullptr;   // INST: the instance's linear terms, read as rollout_fast does
-    const double* cr = INST ? inst_r<true>(P, b, tab.cid) : nullptr;
+    const double2* sx = INST ? gcost->sx : tab.sx;
+    const double2* su = INST ? gcost->su : tab.su;
+    const double* sc = INST ? &gcost->sc : &tab.sc;
+    const FwdCost& term = INST ? gcost->term : tab.term;
     const bool box = tab.box_p != 0;
     double x[n], u[m];
     double J = 0.0;
@@ -499,10 +506,10 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
         {   // stage cost
             double a2 = 0.0, l1 = 0.0;
 #pragma unroll
-            for (int i = 0; i < n; i++) { const double2 c = tab.sx[i]; a2 = fma(c.x * x[i], x[i], a2); l1 = fma(INST ? cq[i] : c.y, x[i], l1); }
+            for (int i = 0; i < n; i++) { const double2 c = sx[i]; a2 = fma(c.x * x[i], x[i], a2); l1 = fma(c.y, x[i], l1); }
 #pragma unroll
-            for (int i = 0; i < m; i++) { const double2 c = tab.su[i]; a2 = fma(c.x * u[i], u[i], a2); l1 = fma(INST ? cr[i] : c.y, u[i], l1); }
-            J += fma(0.5, a2, l1) + tab.sc;
+            for (int i = 0; i < m; i++) { const double2 c = su[i]; a2 = fma(c.x * u[i], u[i], a2); l1 = fma(c.y, u[i], l1); }
+            J += fma(0.5, a2, l1) + *sc;
         }
         if (box) {
             // AL penalty of the control box, rollout_fast's ubox branch with two replacements:
@@ -546,11 +553,10 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
         const double* st = next_stage(N - 1);
 #pragma unroll
         for (int i = 0; i < n; i++) Xc[(size_t)(N - 1) * n + i] = x[i];
-        const double* tq = INST ? inst_q<true>(P, b, tab.tcid) : tab.term.q;
         double a2 = 0.0, l1 = 0.0;
 #pragma unroll
-        for (int i = 0; i < n; i++) { a2 = fma(tab.term.Qd[i] * x[i], x[i], a2); l1 = fma(tq[i], x[i], l1); }
-        J += fma(0.5, a2, l1) + tab.term.c;
+        for (int i = 0; i < n; i++) { a2 = fma(term.Qd[i] * x[i], x[i], a2); l1 = fma(term.q[i], x[i], l1); }
+        J += fma(0.5, a2, l1) + term.c;
         if (tab.goal_ci >= 0) {
             const FwdCon& c = tab.goal;
             const double mu = c.mu;
@@ -619,7 +625,7 @@ __device__ __forceinline__ double rollout_generic(const DevProblem& P, const dou
             for (int a = 0; a < m; a++) Uc[(size_t)k * m + a] = u[a];
         }
         const int cid = P.cost_index[k];
-        J += cost_value(P.costs[cid], inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, !last);
+        J += cost_value(P.costs[cid], cost_data<INST>(P, b, cid), n, m, x, u, !last);
         J += al_knot_penalty<INST>(P, k + 1, x, u, lam_b, viol, b);
         if (!last) {
             // INST: the determinant form the shared kernel compiles to, written out (models.cuh det_sub_square)
@@ -697,11 +703,18 @@ __device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0,
         double J, viol = 0.0;
         double* prm = nullptr;
         double2* gbox = nullptr;
+        FwdCompactCost* gcost = nullptr;
         if constexpr (INST) {   // the instance's model parameters, one copy per group behind the rest of the CTA's shared memory
             prm = reinterpret_cast<double*>(fwd_smem + ls_smem_bytes<MODEL, G, PATH, LANES, LIE>()) + g * TO_NPARAM;
             if (l == 0) stage_model_params<INST>(P, b, prm);
-            if constexpr (PATH == FWD_COMPACT) {   // ... and its control box, behind the parameter rows of the CTA's groups
-                gbox = reinterpret_cast<double2*>(reinterpret_cast<double*>(fwd_smem + ls_smem_bytes<MODEL, G, PATH, LANES, LIE>()) + IPB * TO_NPARAM) + g * TO_MAXM;
+            if constexpr (PATH == FWD_COMPACT) {   // ... its control box, behind the parameter rows of the CTA's groups, and its two costs
+                double2* boxes = reinterpret_cast<double2*>(reinterpret_cast<double*>(fwd_smem + ls_smem_bytes<MODEL, G, PATH, LANES, LIE>()) + IPB * TO_NPARAM);
+                gbox = boxes + g * TO_MAXM;
+                gcost = reinterpret_cast<FwdCompactCost*>(boxes + IPB * TO_MAXM) + g;
+                const CostData c = cost_data<true>(P, b, tab->cid), ct = cost_data<true>(P, b, tab->tcid);
+                for (int i = l; i < n; i += G) { gcost->sx[i] = make_double2(c.Qd[i], c.q[i]); gcost->term.Qd[i] = ct.Qd[i]; gcost->term.q[i] = ct.q[i]; }
+                for (int i = l; i < m; i += G) gcost->su[i] = make_double2(c.Rd[i], c.r[i]);
+                if (l == 0) { gcost->sc = *c.c; gcost->term.c = *ct.c; }
                 if (tab->box_p != 0)
                     for (int ci = 0; ci < P.ncon; ci++)
                         if (P.cons[ci].kind == CON_BOUND) {
@@ -713,7 +726,7 @@ __device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0,
         }
         if constexpr (PATH == FWD_COMPACT) {
             double* ost = stage + FWD_STAGES * S::DOUBLES + (size_t)g * G * FWD_OKNOTS * (n + m);
-            J = rollout_compact<MODEL, IPB, G, LIE, INST>(P, *tab, stage, ost, prm, gbox, b, g, l, gmask, alpha, cbuf, ok, viol);
+            J = rollout_compact<MODEL, IPB, G, LIE, INST>(P, *tab, stage, ost, prm, gbox, gcost, b, g, l, gmask, alpha, cbuf, ok, viol);
         }
         else if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST>(P, *tab, stage, prm, b, g, l, gmask, alpha, cbuf, ok, viol);
         else J = rollout_generic<MODEL, LIE, INST>(P, prm, b, alpha, cbuf, ok, viol);
@@ -761,7 +774,7 @@ cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int f
     const int blocks = (P.B + IPB - 1) / IPB;
     static_assert(ls_smem_bytes<MODEL, G, PATH, LANES, LIE>() % 16 == 0, "the parameter rows and the staged boxes (double2) follow the tables");
     const size_t smem = ls_smem_bytes<MODEL, G, PATH, LANES, LIE>() + (INST ? (size_t)IPB * TO_NPARAM * sizeof(double) : 0)
-                      + (INST && PATH == FWD_COMPACT ? (size_t)IPB * TO_MAXM * sizeof(double2) : 0);
+                      + (INST && PATH == FWD_COMPACT ? (size_t)IPB * (TO_MAXM * sizeof(double2) + sizeof(FwdCompactCost)) : 0);
     auto kern = [] {
         if constexpr (PATH == FWD_COMPACT) return k_linesearch_compact<MODEL, G, LANES, LIE, INST>;
         else return k_linesearch<MODEL, G, PATH == FWD_FAST, LANES, LIE, INST>;
@@ -792,8 +805,8 @@ cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int f
     return launch_pass_l<MODEL, G, PATH, 32, false, INST>(P, trial0, first_pass, final_pass, s);
 }
 
-// per-instance linear cost terms / model parameters / constraint data: a kernel variant of its own, so that the shared one is the code it has
-// always been.  It serves every per-instance table; each accessor checks its own (inst_q, model_param, con_data).
+// per-instance cost weights / linear cost terms / model parameters / constraint data: a kernel variant of its own, so that the shared one is
+// the code it has always been.  It serves every per-instance table; each accessor checks its own (cost_data, model_param, con_data).
 template <int MODEL, int G, int PATH>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     if (inst_forward(P)) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);

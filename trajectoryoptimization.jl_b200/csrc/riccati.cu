@@ -259,13 +259,14 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         const int coff = (lane < n) ? (int)offsetof(DevCost, Qd) + 8 * lane : (int)offsetof(DevCost, Rd) + 8 * (lane < NM ? lane - n : 0);
         constexpr int GOFF = (int)(offsetof(DevCost, q) - offsetof(DevCost, Qd));
         static_assert(offsetof(DevCost, r) - offsetof(DevCost, Rd) == offsetof(DevCost, q) - offsetof(DevCost, Qd), "DevCost layout");
+        // INST: the instance's weights and linear terms through cost_data, with the same lane -> entry mapping
         auto cost_coeff_ptr = [&](int cid, bool hess) -> const double* {
+            if constexpr (INST) {
+                const CostData d = cost_data<true>(P, b, cid);
+                const int e = lane < NM ? lane : n;
+                return hess ? (e < n ? d.Qd + e : d.Rd + (e - n)) : (e < n ? d.q + e : d.r + (e - n));
+            }
             return reinterpret_cast<const double*>(reinterpret_cast<const char*>(P.costs) + (size_t)cid * sizeof(DevCost) + coff + (hess ? 0 : GOFF));
-        };
-        // cG of cost cid: the instance's own q | r row when INST (same lane -> entry mapping: q_i | r_a sit at i | n + a)
-        auto cost_g_ptr = [&](int cid) -> const double* {
-            if constexpr (INST) { if (P.qr) return inst_q<true>(P, b, cid) + (lane < NM ? lane : n); }
-            return cost_coeff_ptr(cid, false);
         };
         // act: bit t = term slot t is active at the knot, bit 4 + t = it is an equality (computed by load_lams one knot ahead)
         auto expand_fast = [&](double zi, const double (&lam)[MAXT], int act, double cH, double cG, double& gi, double& hi) {
@@ -365,7 +366,8 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
             {
                 const int cidN = P.cost_index[N - 1];
                 const DevCost& cost = P.costs[cidN];
-                const double* cq = inst_q<INST>(P, b, cidN);
+                const CostData cd = cost_data<INST>(P, b, cidN);
+                const double* cq = cd.q;
                 if (lane < n) {
                     const int i = lane;
                     const double xi = X[(size_t)(N - 1) * n + i];
@@ -373,13 +375,13 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     if (FASTAL && cost.diag) {
                         double lam[MAXT];
                         int act; load_lams(N - 1, lam, act);
-                        expand_fast(xi, lam, act, cost.Qd[lane], cq[lane], gi, hi);
+                        expand_fast(xi, lam, act, cd.Qd[lane], cq[lane], gi, hi);
                         sm.S[i * LDS_ + i] = hi;
                     } else {
                         gi = cq[i]; hi = 0.0;
-                        if (cost.diag) { gi = fma(cost.Qd[i], xi, gi); hi = cost.Qd[i]; }
+                        if (cost.diag) { gi = fma(cd.Qd[i], xi, gi); hi = cd.Qd[i]; }
                         else {
-                            for (int j = 0; j < n; j++) { gi = fma(cost.Q[j * n + i], X[(size_t)(N - 1) * n + j], gi); sm.S[j * LDS_ + i] = cost.Q[j * n + i]; }
+                            for (int j = 0; j < n; j++) { gi = fma(cd.Q[j * n + i], X[(size_t)(N - 1) * n + j], gi); sm.S[j * LDS_ + i] = cd.Q[j * n + i]; }
                         }
                         for (int ci = 0; ci < P.ncon; ci++) {
                             const DevCon& con = P.cons[ci];
@@ -412,7 +414,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
             // software pipeline of the cost coefficients: (cH,cG) of knot k are loaded during knot k+1, its index during knot k+2
             double cH_cur = 0.0, cG_cur = 0.0;
             int cid_next = (N >= 3) ? P.cost_index[N - 3] : 0;
-            if (FASTAL && P.all_diag_cost) { const int c0 = P.cost_index[N - 2]; cH_cur = *cost_coeff_ptr(c0, true); cG_cur = *cost_g_ptr(c0); }
+            if (FASTAL && P.all_diag_cost) { const int c0 = P.cost_index[N - 2]; cH_cur = *cost_coeff_ptr(c0, true); cG_cur = *cost_coeff_ptr(c0, false); }
             __syncwarp();
 
             double dV1 = 0.0, dV2 = 0.0;   // accumulated by lane n
@@ -430,7 +432,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                 double cH_nxt = 0.0, cG_nxt = 0.0;
                 int cid_next2 = 0;
                 if (FASTAL && P.all_diag_cost && k > 0) {
-                    cH_nxt = ldg_pinned(cost_coeff_ptr(cid_next, true)); cG_nxt = ldg_pinned(cost_g_ptr(cid_next));
+                    cH_nxt = ldg_pinned(cost_coeff_ptr(cid_next, true)); cG_nxt = ldg_pinned(cost_coeff_ptr(cid_next, false));
                     if (k > 1) cid_next2 = ldg_pinned(P.cost_index + (k - 2));
                 }
                 // ---- cost + AL expansion of knot k: lane i < NM handles z_i (diagonal terms) ------------
@@ -442,26 +444,27 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     } else if (lane < NM) {
                         const int cidk = P.cost_index[k];
                         const DevCost& cost = P.costs[cidk];
-                        const double* cq = inst_q<INST>(P, b, cidk);
-                        const double* cr = inst_r<INST>(P, b, cidk);
+                        const CostData cd = cost_data<INST>(P, b, cidk);
+                        const double* cq = cd.q;
+                        const double* cr = cd.r;
                         const int i = lane;
                         const double zi = z_cur;
                         if (FASTAL && cost.diag) {
-                            expand_fast(zi, lam_cur, act_cur, (i < n) ? cost.Qd[i] : cost.Rd[i - n], (i < n) ? cq[i] : cr[i - n], gi, hi);
+                            expand_fast(zi, lam_cur, act_cur, (i < n) ? cd.Qd[i] : cd.Rd[i - n], (i < n) ? cq[i] : cr[i - n], gi, hi);
                         } else {
                             if (cost.diag) {
-                                if (i < n) { gi = fma(cost.Qd[i], zi, cq[i]); hi = cost.Qd[i]; }
-                                else { gi = fma(cost.Rd[i - n], zi, cr[i - n]); hi = cost.Rd[i - n]; }
+                                if (i < n) { gi = fma(cd.Qd[i], zi, cq[i]); hi = cd.Qd[i]; }
+                                else { gi = fma(cd.Rd[i - n], zi, cr[i - n]); hi = cd.Rd[i - n]; }
                             } else {
                                 if (i < n) {
                                     gi = cq[i];
-                                    for (int j = 0; j < n; j++) gi = fma(cost.Q[j * n + i], X[(size_t)k * n + j], gi);
-                                    if (!cost.zeroH) for (int a = 0; a < m; a++) gi = fma(cost.H[i * m + a], U[(size_t)k * m + a], gi);
+                                    for (int j = 0; j < n; j++) gi = fma(cd.Q[j * n + i], X[(size_t)k * n + j], gi);
+                                    if (!cost.zeroH) for (int a = 0; a < m; a++) gi = fma(cd.H[i * m + a], U[(size_t)k * m + a], gi);
                                 } else {
                                     const int a = i - n;
                                     gi = cr[a];
-                                    for (int j = 0; j < m; j++) gi = fma(cost.R[j * m + a], U[(size_t)k * m + j], gi);
-                                    if (!cost.zeroH) for (int j = 0; j < n; j++) gi = fma(cost.H[j * m + a], X[(size_t)k * n + j], gi);
+                                    for (int j = 0; j < m; j++) gi = fma(cd.R[j * m + a], U[(size_t)k * m + j], gi);
+                                    if (!cost.zeroH) for (int j = 0; j < n; j++) gi = fma(cd.H[j * m + a], X[(size_t)k * n + j], gi);
                                 }
                             }
                             for (int ci = 0; ci < P.ncon; ci++) {
@@ -718,20 +721,22 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
 
                     // dense cost Hessian (QuadraticCost): add the off-diagonal entries of lzz to the upper part of Q
                     if (!P.all_diag_cost) {
-                        const DevCost& cost = P.costs[P.cost_index[k]];
+                        const int cidk = P.cost_index[k];
+                        const DevCost& cost = P.costs[cidk];
                         if (!cost.diag) {
+                            const CostData cd = cost_data<INST>(P, b, cidk);
                             for (int e = lane; e < NM * NM; e += 32) {
                                 const int i = e / NM, j = e % NM;     // need (i,j) with block(i) <= block(j)
                                 if (i == j || (i >> 1) > (j >> 1)) continue;
                                 double v;
-                                if (i < n && j < n) v = cost.Q[j * n + i];
-                                else if (i >= n && j >= n) v = cost.R[(j - n) * m + (i - n)];
-                                else if (i < n) v = cost.zeroH ? 0.0 : cost.H[i * m + (j - n)];   // (x_i, u_a): H[a][i]
-                                else v = cost.zeroH ? 0.0 : cost.H[j * m + (i - n)];
+                                if (i < n && j < n) v = cd.Q[j * n + i];
+                                else if (i >= n && j >= n) v = cd.R[(j - n) * m + (i - n)];
+                                else if (i < n) v = cost.zeroH ? 0.0 : cd.H[i * m + (j - n)];   // (x_i, u_a): H[a][i]
+                                else v = cost.zeroH ? 0.0 : cd.H[j * m + (i - n)];
                                 sm.Q[i * LDT + j] += v;
                             }
                             // diagonal: sm.h carried only the AL part for dense costs -> add Q_ii / R_aa
-                            if (lane < NM) sm.Q[lane * LDT + lane] += (lane < n) ? cost.Q[lane * n + lane] : cost.R[(lane - n) * m + (lane - n)];
+                            if (lane < NM) sm.Q[lane * LDT + lane] += (lane < n) ? cd.Q[lane * n + lane] : cd.R[(lane - n) * m + (lane - n)];
                             __syncwarp();
                         }
                     }
@@ -867,7 +872,7 @@ cudaError_t launch_riccati_v(const DevProblem& P, int* work_counter, cudaStream_
     return cudaGetLastError();
 }
 
-// INST: per-instance linear cost terms (P.qr) and constraint data (P.cdata), a kernel variant of its own so that the shared one stays as it is
+// INST: per-instance cost weights (P.cw), linear cost terms (P.qr) and constraint data (P.cdata), a kernel variant of its own so that the shared one stays as it is
 template <int N_, int M_, bool FASTAL, bool INST>
 cudaError_t launch_riccati_t(const DevProblem& P, const BackwardPlan& plan, int* work_counter, cudaStream_t s) {
     if constexpr (N_ >= 8 && M_ <= 4) {

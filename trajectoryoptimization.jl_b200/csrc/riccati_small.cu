@@ -34,8 +34,9 @@ __device__ __forceinline__ void expand_knot(const DevProblem& P, int b, int k0, 
     const DevCost& cost = P.costs[cid];
 #pragma unroll
     for (int i = 0; i < nm; i++) g[i] = 0.0;
-    cost_gradient_quadratic<false>(cost, inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, last, g);      // this kernel never sees user (program) costs: launch_backward routes them to lie.cu
-    cost_hessian_quadratic(cost, n, m, last, H);
+    const CostData cd = cost_data<INST>(P, b, cid);
+    cost_gradient_quadratic<false>(cost, cd, n, m, x, u, last, g);      // this kernel never sees user (program) costs: launch_backward routes them to lie.cu
+    cost_hessian_quadratic<INST>(cost, cd, n, m, last, H);
     double z[nm];
 #pragma unroll
     for (int i = 0; i < n; i++) z[i] = x[i];

@@ -163,16 +163,16 @@ __device__ __forceinline__ double exp_term_bound(const DevProblem& P, const ExpT
     if (P.cdata && j >= 0) return P.cdata[(size_t)b * P.ncdata + j];
     return shared;
 }
-// (INST: the linear cost terms and Goal / Bound bounds of instance b)
+// (INST: the cost weights, linear cost terms and Goal / Bound bounds of instance b)
 template <bool INST>
 __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, const ExpTab& tab, int b, int k, int i, double zi, const double* __restrict__ lam_b, double& g, double& h) {
     const int n = P.n;
     const bool last = (k == P.N - 1);
     const int cid = P.cost_index[k];
-    const DevCost& c = P.costs[cid];
-    if (i < n) { g = fma(c.Qd[i], zi, inst_q<INST>(P, b, cid)[i]); h = c.Qd[i]; }
+    const CostData c = cost_data<INST>(P, b, cid);
+    if (i < n) { g = fma(c.Qd[i], zi, c.q[i]); h = c.Qd[i]; }
     else if (last) { g = 0.0; h = 0.0; return; }
-    else { g = fma(c.Rd[i - n], zi, inst_r<INST>(P, b, cid)[i - n]); h = c.Rd[i - n]; }
+    else { g = fma(c.Rd[i - n], zi, c.r[i - n]); h = c.Rd[i - n]; }
 #pragma unroll
     for (int t = 0; t < TO_EXP_MAXT; t++) {
         const unsigned px = __ldg(&tab.pkx[t][i]);
@@ -458,7 +458,7 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
                 if (k0 + u >= nk) break;                                               // (uniform over the group)
                 const int cid = __shfl_sync(gm, mycid, k0 + u, 16);
                 if (i < n) {
-                    if (cid != ccid) { const DevCost& c = P.costs[cid]; ca = c.Qd[i]; cb = inst_q<INST>(P, b, cid)[i]; ccid = cid; }
+                    if (cid != ccid) { const CostData c = cost_data<INST>(P, b, cid); ca = c.Qd[i]; cb = c.q[i]; ccid = cid; }
                     double g = fma(ca, zi[u], cb), h = ca;
 #pragma unroll
                     for (int t = 0; t < TO_EXP_MAXT; t++) {
@@ -507,8 +507,8 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
             }
             // ---- phase C: the control entries of knot kb + i (coordinate 12 + a, physical slot 2a) ----------------------------------
             const int k = kb + i;
-            const DevCost& c = P.costs[mycid];
-            const double* cr = inst_r<INST>(P, b, mycid);
+            const CostData c = cost_data<INST>(P, b, mycid);
+            const double* cr = c.r;
             double zu[m], lu[m][TO_EXP_MAXT];
 #pragma unroll
             for (int a = 0; a < m; a++) {                                             // every load of the phase first

@@ -42,7 +42,7 @@ __global__ void __launch_bounds__(128) k_cost(const DevProblem P, double* __rest
         for (int i = 0; i < m; i++) zero_u[i] = 0.0;
         const double* u = last ? zero_u : U + (size_t)k * m;
         const int cid = P.cost_index[k];
-        double v = cost_value(P.costs[cid], inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, X + (size_t)k * n, u, !last);
+        double v = cost_value(P.costs[cid], cost_data<INST>(P, b, cid), n, m, X + (size_t)k * n, u, !last);
         if (Jk) Jk[(size_t)b * N + k] = v;
         if (WITH_AL) v += al_knot_penalty<INST>(P, k + 1, X + (size_t)k * n, u, lam, viol, b);
         acc += v;
@@ -73,10 +73,11 @@ __global__ void k_cost_gradient(const DevProblem P, double* __restrict__ grad) {
     double g[TO_MAXNM];
     for (int i = 0; i < nm; i++) g[i] = 0;
     const int cid = P.cost_index[k];
-    cost_gradient(P.costs[cid], inst_q<INST>(P, b, cid), inst_r<INST>(P, b, cid), n, m, x, u, last, g);
+    cost_gradient(P.costs[cid], cost_data<INST>(P, b, cid), n, m, x, u, last, g);
     for (int i = 0; i < nm; i++) grad[t * nm + i] = g[i];
 }
 
+template <bool INST>
 __global__ void k_cost_hessian(const DevProblem P, double* __restrict__ hess) {
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= (long long)P.B * P.N) return;
@@ -86,7 +87,8 @@ __global__ void k_cost_hessian(const DevProblem P, double* __restrict__ hess) {
     double zero_u[TO_MAXM] = {0};
     const double* x = traj_X(P, P.cur[b], b) + (size_t)k * P.n;
     const double* u = last ? zero_u : traj_U(P, P.cur[b], b) + (size_t)k * P.m;
-    cost_hessian(P.costs[P.cost_index[k]], P.n, P.m, x, u, last, hess + t * nm * nm);
+    const int cid = P.cost_index[k];
+    cost_hessian<INST>(P.costs[cid], cost_data<INST>(P, b, cid), P.n, P.m, x, u, last, hess + t * nm * nm);
 }
 
 template <bool INST>
@@ -251,7 +253,8 @@ cudaError_t launch_cost_gradient(const DevProblem& P, double* grad, cudaStream_t
     return cudaGetLastError();
 }
 cudaError_t launch_cost_hessian(const DevProblem& P, double* hess, cudaStream_t s) {
-    k_cost_hessian<<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, hess);
+    if (inst_backward(P)) k_cost_hessian<true><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, hess);
+    else k_cost_hessian<false><<<nblk((long long)P.B * P.N, 128), 128, 0, s>>>(P, hess);
     return cudaGetLastError();
 }
 cudaError_t launch_al_expansion(const DevProblem& P, double* grad, double* hess, cudaStream_t s) {

@@ -350,6 +350,22 @@ function constraint_data(p::BatchedProblem, con::Integer)
     check(p.h, ccall((:to_get_constraint_data, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}), p.h, con - 1, D))
     D
 end
+# per-instance cost weights: column b of W (len, B) is instance b's weights of distinct cost `cost` (1-based), in the layout of
+# to_set_cost_weights (DiagonalCost Qd | Rd | c, QuadraticCost Q | R | H | c column-major, DiagonalQuatCost Qd | Rd | c | w)
+function cost_weights_len(p::BatchedProblem, cost::Integer)
+    len = Ref{Int32}(0)
+    check(p.h, ccall((:to_cost_weights_len, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Int32}), p.h, cost - 1, len))
+    Int(len[])
+end
+function set_cost_weights!(p::BatchedProblem, cost::Integer, W::AbstractMatrix)
+    size(W) == (cost_weights_len(p, cost), p.B) || throw(DimensionMismatch("W must be (len, B)"))
+    check(p.h, ccall((:to_set_cost_weights, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}), p.h, cost - 1, Matrix{Float64}(W)))
+end
+function cost_weights(p::BatchedProblem, cost::Integer)
+    W = Matrix{Float64}(undef, cost_weights_len(p, cost), p.B)
+    check(p.h, ccall((:to_get_cost_weights, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}), p.h, cost - 1, W))
+    W
+end
 
 # ---- what Altro.jl's iLQR / AL loop does with the API above, fused on the device ------------------------------
 expand!(p::BatchedProblem) = check(p.h, ccall((:to_expand, libb200), Cint, (Ptr{Cvoid},), p.h))
