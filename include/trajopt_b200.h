@@ -7,7 +7,7 @@
  * to_update_trajectories, to_set_cost_terms), in the linear cost terms q, r and the Goal constraint values
  * (goal state / tracking reference per instance) -- and, after to_set_model_params, in the model parameters (mass,
  * inertia, lengths, motor constants, gravity) -- and, after to_set_constraint_data, in the constraint data (bounds, obstacles, collision
- * radii, norm values, linear right-hand sides) -- and, after to_set_cost_weights, in the cost weights Q, R, H, c, w.  Every function cites the reference interface it stands in for.  The
+ * radii, norm values, linear right-hand sides) -- and, after to_set_cost_weights, in the cost weights Q, R, H, c, w -- and, after to_set_penalties, in the AL penalties.  Every function cites the reference interface it stands in for.  The
  * Julia-side binding (ccall) that a maintainer adds is shown in INTEGRATION.md.
  *
  * Conventions
@@ -327,9 +327,15 @@ int to_get_gains(to_handle* h, double* K /*[B][N-1][n_e][m]: m x n_e col-major (
  *           update + penalty update + rho reset (to_al_update) and the next inner loop.  Inner loops use the *_intermediate tolerances except
  *           in the last allowed outer iteration (Altro set_tolerances!).
  *   no constraints: one plain iLQR loop with the final tolerances; SUCCEEDED, MAX_ITERATIONS, or UNSOLVED when it stalled (dJ_counter).
- * Penalties are per constraint, shared by the batch, so the outer loop is batch-synchronous: an instance whose inner loop has ended waits
- * (running no kernel) until no instance is in an inner loop; every instance in outer iteration j then sees mu_j = min(mu_0 phi^j, penalty_max),
- * exactly as when solved alone.  Converged instances are retired from every solver kernel: their X, U, lambda, K, d are those of the iteration
+ * Shared penalties (no to_set_penalties call): the penalties are per constraint, shared by the batch, so the outer loop is batch-synchronous:
+ * an instance whose inner loop has ended waits (running no kernel) until no instance is in an inner loop, and the host takes the outer step;
+ * every instance in outer iteration j then sees mu_j = min(mu_0 phi^j, penalty_max), exactly as when solved alone.  The shared penalties
+ * left behind are those of the batch's last outer iteration.
+ * Per-instance penalties (after to_set_penalties): each instance's outer step (decision, dual update, its own penalty update, rho reset,
+ * fresh merit) runs on the device in the iteration in which its inner loop ends, and it goes on without waiting for the rest of the batch.
+ * The statistics, X, U, lambda, K and d are those of the shared solve (bit for bit with equal rows); afterwards instance b holds its own
+ * penalties, min(mu_0 phi^(outer_b - 1), penalty_max), its own multipliers, and to_merit gives its merit at its own penalties.
+ * Converged instances are retired from every solver kernel: their X, U, lambda, K, d are those of the iteration
  * they stopped at, read with the getters above.
  * Altro's summary after solve! prints these statistics: examples/Cartpole.ipynb:216-223 (ALTRO), :378-382 (iLQR), examples/Quadrotor.ipynb:374-391. */
 enum to_solve_status { TO_SOLVE_UNSOLVED = 0, TO_SOLVE_SUCCEEDED = 1, TO_SOLVE_MAX_ITERATIONS = 2, TO_SOLVE_MAX_ITERATIONS_OUTER = 3,
@@ -387,8 +393,20 @@ int to_error_expansion(to_handle* h, double* grad, double* hess);
 int to_get_expansion_records(to_handle* h, double* out);
 int to_get_multipliers(to_handle* h, int32_t con, double* lambda /*[B][last-first+1][p]*/);
 int to_set_multipliers(to_handle* h, int32_t con, const double* lambda);
+/* The shared penalty of constraint con.  With per-instance penalties: to_get_penalty returns the common value while every instance holds the
+ * same one, else TO_ESTATE (read them with to_get_penalties); to_set_penalty writes through to every instance, the later call winning. */
 int to_get_penalty(to_handle* h, int32_t con, double* mu);
 int to_set_penalty(to_handle* h, int32_t con, double mu);
+/* ---- per-instance AL penalties ----------------------------------------------------------------------------------
+ * Instance b weighs constraint con with its own penalty mu[b] (Altro keeps one penalty per problem).  Until the first to_set_penalties there
+ * is no table and every kernel and to_solve run as before; the first call fills every instance with the shared penalty of every constraint,
+ * then applies its column.  From then on to_al_update scales every instance's penalties, mu <- min(mu phi, penalty_max), as it scales the
+ * shared ones, to_set_options with a new penalty_initial resets every instance's, and to_solve takes each instance's outer step on the device
+ * (see to_solve).  TO_EINVAL, naming the instance, with nothing changed: an entry that is non-finite or <= 0, a constraint index out of range,
+ * a hybrid problem.  A batch whose instance b holds mu_b computes, bit for bit, what instance b of a batch with to_set_penalty(mu_b) computes.
+ * Multi-GPU: each rank passes its shard's entries, as for x0. */
+int to_set_penalties(to_handle* h, int32_t con, const double* mu /*[B]*/);
+int to_get_penalties(to_handle* h, int32_t con, double* mu /*[B]*/);          /* the shared value broadcast when none are set */
 int to_get_solver_state(to_handle* h, double* rho /*[B]*/, double* dV /*[B][2]*/, double* alpha /*[B]*/, int32_t* ls_iters /*[B]*/, int32_t* bp_status /*[B]*/);
 
 /* ---- multi-GPU / measurement plumbing --------------------------------------------------------------- */

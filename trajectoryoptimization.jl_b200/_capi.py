@@ -196,6 +196,7 @@ def load_library():
         "to_backward": [H, c_int32_p], "to_forward": [H, c_double_p, c_double_p], "to_ilqr_step": [H, C.c_int32], "to_al_update": [H],
         "to_get_gains": [H, c_double_p, c_double_p], "to_get_multipliers": [H, C.c_int32, c_double_p],
         "to_set_multipliers": [H, C.c_int32, c_double_p], "to_get_penalty": [H, C.c_int32, c_double_p], "to_set_penalty": [H, C.c_int32, C.c_double],
+        "to_set_penalties": [H, C.c_int32, c_double_p], "to_get_penalties": [H, C.c_int32, c_double_p],
         "to_get_solver_state": [H, c_double_p, c_double_p, c_double_p, c_int32_p, c_int32_p],
         "to_reduce_merit": [H], "to_reduce_merit_async": [H, C.c_void_p], "to_merit_device_ptr": [H, C.POINTER(C.c_void_p)],
         "to_set_phase_timing": [H, C.c_int], "to_get_phase_times": [H, c_double_p, C.POINTER(C.c_int64), C.c_int],
@@ -224,7 +225,7 @@ EXPORTED_SYMBOLS = [
     "to_get_dynamics_jacobians", "to_cost", "to_cost_knots", "to_cost_gradient", "to_cost_hessian", "to_eval_constraints",
     "to_constraint_jacobians", "to_constraint_hessians", "to_max_violation", "to_merit", "to_al_expansion", "to_projection", "to_grad_projection",
     "to_hess_projection", "to_backward", "to_forward", "to_ilqr_step", "to_al_update", "to_get_gains", "to_get_multipliers",
-    "to_set_multipliers", "to_get_penalty", "to_set_penalty", "to_get_solver_state", "to_reduce_merit", "to_reduce_merit_async", "to_merit_device_ptr", "to_update_trajectory", "to_shift_trajectory",
+    "to_set_multipliers", "to_get_penalty", "to_set_penalty", "to_set_penalties", "to_get_penalties", "to_get_solver_state", "to_reduce_merit", "to_reduce_merit_async", "to_merit_device_ptr", "to_update_trajectory", "to_shift_trajectory",
     "to_set_goal_states", "to_update_trajectories", "to_get_cost_terms", "to_set_cost_terms", "to_get_goal_values", "to_set_goal_values",
     "to_set_model_params", "to_get_model_params", "to_constraint_data_len", "to_set_constraint_data", "to_get_constraint_data",
     "to_cost_weights_len", "to_set_cost_weights", "to_get_cost_weights",

@@ -1179,7 +1179,8 @@ class Problem:
         """The reference mutates a live problem's objective / constraint list in place.  The device tables are a copy taken at
         construction, so a change is re-uploaded here, before the next device call: the handle is rebuilt from the current host
         description with the live trajectory, initial state and solver options carried over (multipliers and penalties restart,
-        as they must when the constraint list changes shape)."""
+        as they must when the constraint list changes shape; per-instance penalties (``set_penalties``) restart with them, at the shared
+        ``penalty_initial``)."""
         if getattr(self, "_sig", None) is None or self._sig == self._signature():
             return
         X, U = np.empty((self.B, self.N, self.n)), np.empty((self.B, self.N - 1, self.m))
@@ -1967,7 +1968,44 @@ def penalty(prob, con):
 
 
 def set_penalty(prob, con, mu):
+    """The penalty of constraint ``con`` (index or object) for the whole batch; after ``set_penalties`` it replaces every instance's."""
     prob._call("to_set_penalty", _con_index(prob, con), float(mu))
+
+
+def _penalty_rows(prob, con, mu):
+    """(index, mu [B]) as to_set_penalties takes them; every check that needs no device happens here"""
+    if getattr(prob, "hybrid", False):
+        raise ArgumentError("per-instance penalties are not supported on hybrid problems")
+    i = _con_index(prob, con)
+    if not 0 <= i < len(prob.constraints):
+        raise ArgumentError(f"set_penalties: no constraint {i}")
+    mu = np.asarray(mu, dtype=np.float64)
+    if mu.ndim == 0:
+        mu = np.full(prob.B, float(mu))
+    if mu.shape != (prob.B,):
+        raise DimensionMismatch(f"set_penalties: expected [{prob.B}] penalties, got {mu.shape}")
+    bad = np.nonzero(~(np.isfinite(mu) & (mu > 0)))[0]
+    if bad.size:
+        raise ArgumentError(f"set_penalties: instance {bad[0]}: a penalty must be finite and positive")
+    return i, np.ascontiguousarray(mu)
+
+
+def set_penalties(prob, con, mu):
+    """Instance ``b`` weighs constraint ``con`` (index or object) with its own AL penalty ``mu[b]``; ``mu`` is ``[B]`` or a scalar for
+    every instance.  The first call gives every instance the shared penalty of every constraint, then sets this one.  From then on
+    ``al_update`` scales every instance's penalties, and ``solve`` runs each instance's outer (AL) step on the device when its inner loop
+    ends, so each instance keeps its own penalty schedule across calls.  A batch whose instance ``b`` holds ``mu_b`` computes, bit for bit,
+    what instance ``b`` of a batch built with ``set_penalty(mu_b)`` computes.  A handle rebuild restarts them, as it restarts the shared
+    penalties."""
+    i, mu = _penalty_rows(prob, con, mu)
+    prob._call("to_set_penalties", i, K._dp(mu))
+
+
+def penalties(prob, con):
+    """The penalty of constraint ``con`` for every instance, ``[B]`` (the shared penalty broadcast when none were set)."""
+    out = np.empty(prob.B)
+    prob._call("to_get_penalties", _con_index(prob, con), K._dp(out))
+    return out
 
 
 def backward_algebra(prob):

@@ -58,6 +58,8 @@ struct to_handle {
     std::vector<double> h_mparams;   // model parameters (DevProblem::mparams), [B][TO_NPARAM]
     std::vector<double> h_cdata;     // constraint data and Goal values (DevProblem::cdata), [B][ncdata]
     std::vector<double> h_cw;        // cost weights (DevProblem::cw), [B][ncw]
+    // AL penalties (DevProblem::mub), [B][ncon]: no host copy, the device scales the rows (k_al_update, to_solve's outer steps)
+    int* d_go = nullptr;             // SolveDev::go, allocated with the penalty table
     std::vector<double> stage;       // the rows a setter is building, committed by commit_rows (kept to reuse its allocation)
     int* d_fragerr = nullptr;     // sticky error word of that kernel (queue overflow / spin limit), read by to_synchronize
     double* d_fragpool = nullptr; // gains of its speculative regularisation candidates
@@ -119,7 +121,7 @@ int upload_exptab(to_handle* h) {
     const int nm = h->P.n + h->P.m, n = h->P.n;
     for (int i = 0; i < nm; i++) {
         int nterm = 0;
-        for (int k = 0; k < TO_EXP_MAXT; k++) { t.nms[k][i] = -1.0; t.pkx[k][i] = 4095u; t.inst[k][i] = -1; }      // empty knot range
+        for (int k = 0; k < TO_EXP_MAXT; k++) { t.nms[k][i] = -1.0; t.pkx[k][i] = 4095u; t.inst[k][i] = -1; t.con[k][i] = -1; }      // empty knot range
         for (size_t ci = 0; ci < h->h_cons.size(); ci++) {
             const DevCon& con = h->h_cons[ci];
             if (!con.diagonal) continue;
@@ -135,6 +137,7 @@ int upload_exptab(to_handle* h) {
                     t.pkx[nterm][i] = (unsigned)con.first | ((unsigned)(con.last - con.first) << 12) | ((unsigned)con.p << 24) | (eq ? 0x80000000u : 0u);
                     t.pky[nterm][i] = (unsigned)(con.offset + row - con.first * con.p);
                     t.inst[nterm][i] = con.cdoff + (eq ? row : (side ? nm : 0) + i);
+                    t.con[nterm][i] = (int)ci;
                 }
                 nterm++;
             }
@@ -163,6 +166,17 @@ int commit_rows(to_handle* h, std::vector<double>& host, const double*& dev) {
     CU(h, cudaStreamSynchronize(h->stream));   // the staged rows are the source of the copy
     host.swap(rows);
     dev = d;
+    return TO_OK;
+}
+
+// Every row of the penalty table `d` ([B][ncon] on the device) = the shared penalties
+int fill_penalty_rows(to_handle* h, double* d) {
+    const int B = h->P.B, nc = (int)h->h_mu.size();
+    std::vector<double>& rows = h->stage;
+    rows.resize((size_t)B * nc);
+    for (int b = 0; b < B; b++) std::memcpy(rows.data() + (size_t)b * nc, h->h_mu.data(), sizeof(double) * nc);
+    CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));   // the staged rows are the source of the copy
     return TO_OK;
 }
 
@@ -771,7 +785,10 @@ int to_set_options(to_handle* h, const to_options* o) {
     d.backward_kernel = o->backward_kernel;
     d.max_state_value = o->max_state_value; d.max_control_value = o->max_control_value;
     d.penalty_initial = o->penalty_initial; d.penalty_scaling = o->penalty_scaling; d.penalty_max = o->penalty_max; d.dual_max = o->dual_max;
-    if (reset_mu) for (auto& mu : h->h_mu) mu = d.penalty_initial;
+    if (reset_mu) {
+        for (auto& mu : h->h_mu) mu = d.penalty_initial;
+        if (h->P.mub) { int rc = fill_penalty_rows(h, h->P.mub); if (rc) return rc; }   // every instance restarts with them
+    }
     if (reset_rho) {
         std::vector<double> r(h->P.B, d.bp_reg_initial);
         CU(h, cudaMemcpyAsync(h->P.rho, r.data(), sizeof(double) * h->P.B, cudaMemcpyHostToDevice, h->stream));
@@ -1495,6 +1512,18 @@ static int record_active_count(to_handle* h, const SolveDev& sv, int slot, cudaS
     CU(h, cudaEventRecord(h->ev_count[slot], st));
     return TO_OK;
 }
+// Per-instance penalties: the outer step of the instances whose inner loop ended in half `half` of the iteration (SolveDev::go) and that go
+// on, on the stream of that half's check and before that half's next expansion.  k_al_update and k_cost run with go as DevProblem::active, so
+// each instance gets the dual update, the penalty update, the rho / drho reset and the merit those kernels give it in the host's outer step.
+static int solve_outer_step(to_handle* h, const SolveDev& sv, int half, cudaStream_t st) {
+    DevProblem Q = h->P;
+    Q.active = sv.go + (size_t)half * Q.B;
+    CU(h, launch_al_update(Q, st));
+    CU(h, launch_merit(Q, Q.J, h->d_viol, st));
+    CU(h, launch_solve_restart(h->P, sv, half, st));
+    h->launches += 3;
+    return TO_OK;
+}
 // One iteration of to_ilqr_step.  Per iteration: E (expansion) -> R (Riccati) -> F pass 1 (alpha = 1..1/8, ~90% of the instances) -> F pass 2 (the rest).
 // Pass 2 is latency-bound and touches few instances, so it runs on a high-priority side stream followed by the
 // expansion of ITS instances, concurrently with the next iteration's expansion of the instances pass 1 accepted
@@ -1503,7 +1532,8 @@ static int record_active_count(to_handle* h, const SolveDev& sv, int slot, cudaS
 // behind it, and the cost expansion (record path) then the dynamics expansion of the pass-1 instances on the main stream; without one,
 // the dynamics expansion of every instance on the main stream.
 // sv (to_solve): the stopping-rule check of every ACTIVE instance right after its line search -- for the two halves of an overlapped iteration
-// on their own streams, before the next iteration's expansion of each -- and the ACTIVE count behind it (record_active_count).
+// on their own streams, before the next iteration's expansion of each -- and the ACTIVE count behind it (record_active_count); with per-instance
+// penalties each check is followed on its stream by the outer step of the instances whose inner loop it ended (solve_outer_step).
 static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
     // (error state: only [A_e B_e] is needed by the solver kernels -- k_expand_lie; the full [A B] is produced by to_expand on request)
     auto expand = [&](cudaStream_t st, int mode) { return h->P.lie ? launch_expand_lie(h->P, st, mode) : launch_expand(h->P, st, mode); };
@@ -1537,8 +1567,10 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
         if (sv) { CU(h, launch_solve_check(h->P, *sv, 1, h->stream)); h->launches++; }
         CU(h, cudaEventRecord(h->ev_fork, h->stream));
         CU(h, cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));
+        if (sv && sv->go) { int rc2 = solve_outer_step(h, *sv, 0, h->stream); if (rc2) return rc2; }   // (an instance that goes on stays ACTIVE: the count holds)
         { PhaseScope ps(h, TO_PHASE_LADDER, h->stream2); CU(h, launch_ladder(h->P, h->stream2)); }
         if (sv) { CU(h, launch_solve_check(h->P, *sv, 2, h->stream2)); h->launches++; }      // ... the others, before their expansion on the side stream
+        if (sv && sv->go) { int rc2 = solve_outer_step(h, *sv, 1, h->stream2); if (rc2) return rc2; }
         if (sv) { int rc2 = record_active_count(h, *sv, slot, h->stream2); if (rc2) return rc2; }
         CU(h, cudaEventRecord(h->ev_join, h->stream2));
         h->side_pending = true;
@@ -1546,6 +1578,7 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
         { PhaseScope ps(h, TO_PHASE_LADDER); CU(h, launch_ladder(h->P, h->stream)); }
         if (sv) {
             CU(h, launch_solve_check(h->P, *sv, 0, h->stream)); h->launches++;
+            if (sv->go) { int rc2 = solve_outer_step(h, *sv, 0, h->stream); if (rc2) return rc2; }
             int rc2 = record_active_count(h, *sv, slot, h->stream); if (rc2) return rc2;
         }
     }
@@ -1565,7 +1598,7 @@ int to_ilqr_step(to_handle* h, int32_t iters) {
 int to_al_update(to_handle* h) {
     JOIN(h);
     if (!h) return TO_EINVAL;
-    if (h->P.ncon > 0) { CU(h, launch_al_update(h->P, h->stream)); h->launches++; }    // (k_al_update also restarts rho / drho)
+    if (h->P.ncon > 0) { CU(h, launch_al_update(h->P, h->stream)); h->launches++; }    // (k_al_update also restarts rho / drho, and scales the rows of P.mub)
     else {
         // no multipliers to update, but the regularisation restarts at bp_reg_initial all the same: Altro's inner solve resets it at
         // the start of every AL iteration, constrained or not
@@ -1597,7 +1630,9 @@ int to_default_solve_options(to_solve_options* o) {
     o->iterations = 300; o->iterations_inner = 300; o->iterations_outer = 30; o->dJ_counter_limit = 10;
     return TO_OK;
 }
-// the solve with P.active set (to_solve clears it on every exit)
+// the solve with P.active set (to_solve clears it on every exit).  With per-instance penalties (S.go set) every instance takes its outer steps
+// on the device (k_solve_check, solve_outer_step), so one loop of iterations runs until no instance is ACTIVE; with shared penalties the batch
+// takes each outer step together, on the host, once every inner loop has ended.
 static int solve_run(to_handle* h) {
     SolveDev& S = h->solve;
     DevProblem& P = h->P;
@@ -1622,7 +1657,7 @@ static int solve_run(to_handle* h) {
             if (it > S.opt.iterations + 1) return fail(h, TO_ESTATE, "to_solve: an inner loop outlived the iteration cap");
         }
         int rc = join_side(h); if (rc) return rc;
-        if (P.ncon == 0) break;                                       // no constraints: the iLQR loop decided every status
+        if (P.ncon == 0 || S.go) break;                               // no constraints: the iLQR loop decided every status; per-instance penalties: so did the device's outer steps
         // outer step: the WAITING instances are done or go on; the ones that go on get the dual update, the penalties of the next outer
         // iteration and a fresh merit
         CU(h, launch_solve_outer(P, S, h->stream)); h->launches++;
@@ -1653,6 +1688,7 @@ int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* 
     S.opt = SolveOpts{o->cost_tolerance, o->cost_tolerance_intermediate, o->gradient_tolerance, o->gradient_tolerance_intermediate, o->constraint_tolerance,
                       o->iterations, o->iterations_inner, o->iterations_outer, o->dJ_counter_limit};
     h->P.active = S.state;
+    S.go = h->P.mub ? h->d_go : nullptr;
     rc = solve_run(h);
     const int jrc = join_side(h);
     h->P.active = nullptr;                 // every other entry point works on every instance again
@@ -1766,9 +1802,25 @@ static int multipliers_copy(to_handle* h, int32_t con, double* host, bool to_hos
 }
 int to_get_multipliers(to_handle* h, int32_t con, double* lambda) { return multipliers_copy(h, con, lambda, true); }
 int to_set_multipliers(to_handle* h, int32_t con, const double* lambda) { return multipliers_copy(h, con, const_cast<double*>(lambda), false); }
+// Column con of the penalty table to / from host[B] (the table exists)
+static int penalty_column(to_handle* h, int32_t con, double* host, bool to_host) {
+    const size_t pitch = sizeof(double) * h->h_mu.size();
+    if (to_host) CU(h, cudaMemcpy2DAsync(host, sizeof(double), h->P.mub + con, pitch, sizeof(double), h->P.B, cudaMemcpyDeviceToHost, h->stream));
+    else CU(h, cudaMemcpy2DAsync(h->P.mub + con, pitch, host, sizeof(double), sizeof(double), h->P.B, cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return TO_OK;
+}
 int to_get_penalty(to_handle* h, int32_t con, double* mu) {
     JOIN(h);
     if (!h || !mu || con < 0 || con >= (int)h->h_mu.size()) return TO_EINVAL;
+    if (h->P.mub) {   // the common value of every instance's row, while they agree
+        std::vector<double> col(h->P.B);
+        int rc = penalty_column(h, con, col.data(), true); if (rc) return rc;
+        for (double v : col)
+            if (!(v == col[0])) return fail(h, TO_ESTATE, "to_get_penalty: the instances hold different penalties for constraint " + std::to_string(con) + "; read them with to_get_penalties");
+        *mu = col[0];
+        return TO_OK;
+    }
     *mu = h->h_mu[con];
     return TO_OK;
 }
@@ -1779,7 +1831,42 @@ int to_set_penalty(to_handle* h, int32_t con, double mu) {
     CU(h, cudaMemcpyAsync(h->d_mu, h->h_mu.data(), sizeof(double) * h->h_mu.size(), cudaMemcpyHostToDevice, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
     h->J_valid = false;
+    if (h->P.mub) {   // ... and every instance's
+        std::vector<double> col(h->P.B, mu);
+        int rc = penalty_column(h, con, col.data(), false); if (rc) return rc;
+    }
     return upload_exptab(h);
+}
+// mu [B]: constraint con's penalty of every instance.  The whole column is checked before anything changes: a refused call leaves the table
+// (or its absence) as it was.  The first call creates the table with the shared penalty of every constraint in every row.
+int to_set_penalties(to_handle* h, int32_t con, const double* mu) {
+    JOIN(h);
+    if (!h || !mu) return TO_EINVAL;
+    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance penalties are not supported on hybrid problems");
+    if (con < 0 || con >= (int)h->h_cons.size()) return fail(h, TO_EINVAL, "to_set_penalties: no constraint " + std::to_string(con));
+    const int B = h->P.B;
+    for (int b = 0; b < B; b++)
+        if (!(std::isfinite(mu[b]) && mu[b] > 0))
+            return fail(h, TO_EINVAL, "to_set_penalties: instance " + std::to_string(b) + ": a penalty must be finite and positive");
+    if (!h->P.mub) {
+        double* d = nullptr;
+        int rc = dalloc(h, &d, (size_t)B * h->h_mu.size()); if (rc) return rc;
+        if (!h->d_go) { rc = dalloc(h, &h->d_go, 2 * (size_t)B); if (rc) return rc; }
+        rc = fill_penalty_rows(h, d); if (rc) return rc;
+        h->P.mub = d;   // published once the device holds every row
+    }
+    int rc = penalty_column(h, con, const_cast<double*>(mu), false); if (rc) return rc;
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return TO_OK;
+}
+// mu [B]: constraint con's penalty of every instance (the shared penalty broadcast when none are set)
+int to_get_penalties(to_handle* h, int32_t con, double* mu) {
+    JOIN(h);
+    if (!h || !mu) return TO_EINVAL;
+    if (con < 0 || con >= (int)h->h_cons.size()) return fail(h, TO_EINVAL, "to_get_penalties: no constraint " + std::to_string(con));
+    if (h->P.mub) return penalty_column(h, con, mu, true);
+    for (int b = 0; b < h->P.B; b++) mu[b] = h->h_mu[con];
+    return TO_OK;
 }
 int to_get_solver_state(to_handle* h, double* rho, double* dV, double* alpha, int32_t* ls_iters, int32_t* bp_status) {
     JOIN(h);

@@ -84,6 +84,7 @@ struct ExpTab {
     unsigned pkx[TO_EXP_MAXT][TO_MAXNM];    // first knot (12 bits) | last - first (12) | rows p of the constraint (7) | equality (1)
     unsigned pky[TO_EXP_MAXT][TO_MAXNM];    // lambda index of the row at knot 0
     int inst[TO_EXP_MAXT][TO_MAXNM];        // index of the term's bound in an instance's row of DevProblem::cdata; -1: no term
+    int con[TO_EXP_MAXT][TO_MAXNM];         // the term's constraint (its penalty in an instance's row of DevProblem::mub); -1: no term
 };
 
 // one dynamics model of a hybrid problem (to_dynamics_spec): a recorded program, RK4-discretised or a discrete jump map
@@ -181,6 +182,10 @@ struct DevProblem {
     // nullptr until the first call; every kernel then reads the shared DevCost fields.
     int ncw;
     const double* cw;         // [B][ncw]
+    // Per-instance AL penalties (to_set_penalties): row b holds the penalty of every constraint for instance b (see penalty).  nullptr until
+    // the first call; every kernel then reads the shared `mu`.  Unlike the other tables the device also writes it: k_al_update scales the
+    // rows of the instances it updates, and to_solve runs each instance's outer step on the device.
+    double* mub;              // [B][ncon]
 };
 #define TO_NPARAM 16        // slots of DevProblem::params and of a row of DevProblem::mparams (one 128-byte line)
 
@@ -190,8 +195,8 @@ __host__ __device__ inline bool retired(const DevProblem& P, int b) { return P.a
 // Which variant of a kernel family runs: INST = true when a per-instance table the family reads exists.  The only place that decides; every
 // launcher and to_kernel_choice ask here.  The line search reads the linear cost terms, the model parameters and the constraint data; the
 // expansion, backward and sweep kernels the cost terms and the constraint data; the dynamics kernels the model parameters alone.
-__host__ __device__ inline bool inst_forward(const DevProblem& P) { return P.qr || P.mparams || P.cdata || P.cw; }
-__host__ __device__ inline bool inst_backward(const DevProblem& P) { return P.qr || P.cdata || P.cw; }
+__host__ __device__ inline bool inst_forward(const DevProblem& P) { return P.qr || P.mparams || P.cdata || P.cw || P.mub; }
+__host__ __device__ inline bool inst_backward(const DevProblem& P) { return P.qr || P.cdata || P.cw || P.mub; }
 __host__ __device__ inline bool inst_dynamics(const DevProblem& P) { return P.mparams; }
 
 // The weights and linear terms of cost cid for instance b: the only place that decides between an instance's rows (DevProblem::cw for the
@@ -236,6 +241,13 @@ template <bool INST>
 __device__ __forceinline__ double model_param(const DevProblem& P, int b, int i) {
     if constexpr (INST) { if (P.mparams) return P.mparams[(size_t)b * TO_NPARAM + i]; }
     return P.params[i];
+}
+// The AL penalty of constraint ci for instance b: the only place that decides between an instance's row of DevProblem::mub and the shared
+// DevProblem::mu, and the only way a kernel reads a penalty.
+template <bool INST>
+__device__ __forceinline__ double penalty(const DevProblem& P, int b, int ci) {
+    if constexpr (INST) { if (P.mub) return P.mub[(size_t)b * P.ncon + ci]; }
+    return P.mu[ci];
 }
 // The data of constraint ci for instance b, in the fields of DevCon it replaces: a (GOAL xf | BOUND z_max | CIRCLE / SPHERE xc), b (BOUND z_min |
 // LINEAR b | yc), c3 (zc), rad (CIRCLE / SPHERE r), val (NORM val | COLLISION radius).  LINEAR's A and every other field stay shared.  The only

@@ -486,7 +486,7 @@ __device__ inline double al_knot_penalty(const DevProblem& P, int k1, const doub
     for (int ci = 0; ci < P.ncon; ci++) {
         const DevCon& con = P.cons[ci];
         if (k1 < con.first || k1 > con.last) continue;
-        const double mu = P.mu[ci];
+        const double mu = penalty<INST>(P, b, ci);
         const double* lam = lam_b + con.offset + (size_t)(k1 - con.first) * con.p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
         con_evaluate(con, con_data<INST>(P, b, ci), P.n, P.m, x, u, c);
@@ -520,7 +520,7 @@ __device__ inline void al_knot_expansion(const DevProblem& P, int k0, const doub
         const DevCon& con = P.cons[ci];
         if (k0 + 1 < con.first || k0 + 1 > con.last) continue;
         const int p = con.p;
-        const double mu = P.mu[ci];
+        const double mu = penalty<INST>(P, b, ci);
         const double* lam = lam_b + con.offset + (size_t)(k0 + 1 - con.first) * p;
         double c[TO_MAXPV], lbar[TO_MAXPV], lp[TO_MAXPV];
         const ConData dd = con_data<INST>(P, b, ci);
@@ -610,7 +610,7 @@ __device__ __forceinline__ void compact_expansion(const DevProblem& P, int b, in
     for (int ci = 0; ci < P.ncon; ci++) {
         const DevCon& con = P.cons[ci];
         if (k + 1 < con.first || k + 1 > con.last) continue;
-        const double mu = P.mu[ci];
+        const double mu = penalty<INST>(P, b, ci);
         const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
         const bool eq = (con.kind == CON_GOAL);
         const ConData cd = con_data<INST>(P, b, ci);

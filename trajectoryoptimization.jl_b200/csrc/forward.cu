@@ -67,7 +67,7 @@ __device__ inline void load_tables(const DevProblem& P, FwdTab& tab) {
         FwdCon& f = tab.con[ci];
         if (t == 0) {
             f.kind = c.kind; f.first = c.first; f.last = c.last; f.p = c.p; f.offset = c.offset;
-            f.mu = P.mu[ci]; f.inv2mu = 1.0 / (2.0 * P.mu[ci]);
+            f.mu = penalty<false>(P, 0, ci); f.inv2mu = 1.0 / (2.0 * penalty<false>(P, 0, ci));   // the shared penalty (INST: rollout_fast reads each instance's)
             unsigned mx = 0, mn = 0;
             for (int j = 0; j < TO_MAXNM; j++) { if (c.row_max[j] >= 0) mx |= 1u << j; if (c.row_min[j] >= 0) mn |= 1u << j; }
             f.mask_max = mx; f.mask_min = mn;
@@ -119,6 +119,7 @@ struct alignas(16) FwdCompactCost {
     double2 sx[TO_MAXN], su[TO_MAXM];
     double sc, pad;
     FwdCost term;
+    double mu, inv2mu, gmu, ginv2mu;     // the instance's penalties of the box and of the Goal, and 1 / (2 mu), as load_compact_tables forms them
 };
 
 __device__ inline void load_compact_tables(const DevProblem& P, FwdCompactTab& tab) {
@@ -136,12 +137,12 @@ __device__ inline void load_compact_tables(const DevProblem& P, FwdCompactTab& t
         const DevCon& k = P.cons[ci];
         if (k.kind == CON_BOUND) {   // knots 1..N-1, rows 0..m-1 = upper, m..2m-1 = lower
             for (int j = t; j < P.m; j += T) tab.box[j] = make_double2(k.a[P.n + j], k.b[P.n + j]);
-            if (t == 0) { tab.box_off = k.offset; tab.box_p = k.p; tab.mu = P.mu[ci]; tab.inv2mu = 1.0 / (2.0 * P.mu[ci]); }
+            if (t == 0) { tab.box_off = k.offset; tab.box_p = k.p; tab.mu = penalty<false>(P, 0, ci); tab.inv2mu = 1.0 / (2.0 * penalty<false>(P, 0, ci)); }
         } else {                     // the Goal, knot N
             FwdCon& f = tab.goal;
             if (t == 0) {
                 tab.goal_ci = ci; tab.goal_off = k.offset; tab.goal_p = k.p;
-                f.mu = P.mu[ci]; f.inv2mu = 1.0 / (2.0 * P.mu[ci]);
+                f.mu = penalty<false>(P, 0, ci); f.inv2mu = 1.0 / (2.0 * penalty<false>(P, 0, ci));
                 unsigned mx = 0;
                 for (int j = 0; j < TO_MAXNM; j++) if (k.row_max[j] >= 0) mx |= 1u << j;
                 f.mask_max = mx;
@@ -331,7 +332,8 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
             for (int ci = 0; ci < tab.ncon; ci++) {
                 const FwdCon& c = tab.con[ci];
                 if (k + 1 < c.first || k + 1 > c.last) continue;
-                const double mu = c.mu;
+                const bool own = INST && P.mub != nullptr;                 // this instance's penalty, with load_tables' operations
+                const double mu = own ? penalty<INST>(P, b, ci) : c.mu;
                 const int lo = S::OFF_L + slot;
                 double a = 0.0, l2 = 0.0;
                 if (c.kind == CON_GOAL) {
@@ -374,7 +376,7 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
                         if (mn & (1u << (n + i))) { const double lm = st[S::sidx(lo + c.row_min[n + i], g)]; const double cv = cd.b[n + i] - u[i]; const double lp = fmin(0.0, fma(-mu, cv, lm)); a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, cv); }
                     }
                 }
-                J = fma(a - l2, c.inv2mu, J);
+                J = fma(a - l2, own ? 1.0 / (2.0 * mu) : c.inv2mu, J);
                 slot += c.p;
             }
         }
@@ -400,7 +402,7 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
 //     candidate stores ran pass 1 in about half the time);
 //   * RK4 writes the next state over the current one (rk4_step reads x_i for the last time where it writes xn_i), so the loop carries
 //     no x <- xn copies.  (Unrolled by two with x / xn swapping roles instead, the loop took 40 more registers and spilled.)
-// INST: gbox = the instance's control box {u_max_i, u_min_i} and gcost = its two costs, staged for the group by linesearch_pass
+// INST: gbox = the instance's control box {u_max_i, u_min_i} and gcost = its two costs and penalties, staged for the group by linesearch_pass
 template <int MODEL, int IPB, int G, bool LIE, bool INST>
 __device__ __forceinline__ double rollout_compact(const DevProblem& P, const FwdCompactTab& tab, double* stage, double* ost, const double* prm,
                                                   const double2* gbox, const FwdCompactCost* gcost, int b, int g, int l, unsigned gmask,
@@ -520,7 +522,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
             //     are finite, so cu and cl are both NaN (u is) or neither: both NaN -> t = NaN, and both forms keep viol.  Otherwise t is
             //     fmax(cu, cl) except for cu = +0, cl = -0, where t = -0: then fmax(viol, +0) = viol = the select, as viol >= +0.  For
             //     t != NaN, fmax(viol, t) and the select agree except at viol = +0, t = -0, where both give viol.
-            const double mu = tab.mu;
+            const double mu = INST ? gcost->mu : tab.mu;
             double a = 0.0, l2 = 0.0;
 #pragma unroll
             for (int i = 0; i < m; i++) {
@@ -533,7 +535,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
                 const double t = cu > cl ? cu : cl;
                 viol = t > viol ? t : viol;
             }
-            J = fma(a - l2, tab.inv2mu, J);
+            J = fma(a - l2, INST ? gcost->inv2mu : tab.inv2mu, J);
         }
         if constexpr (MODEL == MODEL_EXPR_42) {   // a discrete jump map writes its outputs while it reads its inputs
             double xn[n];
@@ -559,7 +561,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
         J += fma(0.5, a2, l1) + term.c;
         if (tab.goal_ci >= 0) {
             const FwdCon& c = tab.goal;
-            const double mu = c.mu;
+            const double mu = INST ? gcost->gmu : c.mu;
             double a = 0.0, l2 = 0.0;
             const unsigned mk = c.mask_max;
             const double* ga = con_data<INST>(P, b, tab.goal_ci, staged(c)).a;
@@ -573,7 +575,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
                     a = fma(lp, lp, a); l2 = fma(lm, lm, l2); viol = fmax(viol, fabs(cv));
                 }
             }
-            J = fma(a - l2, c.inv2mu, J);
+            J = fma(a - l2, INST ? gcost->ginv2mu : c.inv2mu, J);
         }
     }
     cp_async_wait<0>();
@@ -720,7 +722,9 @@ __device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0,
                         if (P.cons[ci].kind == CON_BOUND) {
                             const ConData cd = con_data<true>(P, b, ci);
                             for (int i = l; i < m; i += G) gbox[i] = make_double2(cd.a[n + i], cd.b[n + i]);
+                            if (l == 0) { gcost->mu = penalty<true>(P, b, ci); gcost->inv2mu = 1.0 / (2.0 * gcost->mu); }
                         }
+                if (l == 0 && tab->goal_ci >= 0) { gcost->gmu = penalty<true>(P, b, tab->goal_ci); gcost->ginv2mu = 1.0 / (2.0 * gcost->gmu); }
             }
             __syncwarp(gmask);
         }

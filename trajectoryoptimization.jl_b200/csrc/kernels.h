@@ -83,8 +83,13 @@ struct SolveDev {
     double* grad;      // [B] last gradient (Altro gradient_todorov)
     double* cmax;      // [B] max violation when the last inner loop ended
     int* n_active;     // [1] instances ACTIVE
+    // Per-instance penalties (DevProblem::mub): each instance's outer step runs on the device in the iteration in which its inner loop ends.
+    // go[half * B + b] == SOLVE_ACTIVE: instance b's inner loop ended in that half of the iteration (0: main stream, 1: side stream) and it
+    // goes on to another outer iteration; the outer-step kernels of that half see it as DevProblem::active.  nullptr: the host's outer step.
+    int* go;           // [2][B]
 };
 cudaError_t launch_solve_init(const DevProblem& P, const SolveDev& S, cudaStream_t s);
 cudaError_t launch_solve_begin(const DevProblem& P, const SolveDev& S, cudaStream_t s);
 cudaError_t launch_solve_check(const DevProblem& P, const SolveDev& S, int mode, cudaStream_t s);   // mode as launch_expand
 cudaError_t launch_solve_outer(const DevProblem& P, const SolveDev& S, cudaStream_t s);
+cudaError_t launch_solve_restart(const DevProblem& P, const SolveDev& S, int half, cudaStream_t s);

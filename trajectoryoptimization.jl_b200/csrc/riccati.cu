@@ -185,8 +185,9 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
 
     // ---- lane-resident AL terms of z_lane (Goal / Bound constraints) ----------------------------------------
     int tinst[MAXT];   // (INST) index of a term's bound in an instance's row of P.cdata, -1: none
+    int tcon[MAXT];    // (INST) the term's constraint, whose penalty in an instance's row of P.mub replaces mu in -mu * sign; -1: none
 #pragma unroll
-    for (int t = 0; t < MAXT; t++) tinst[t] = -1;
+    for (int t = 0; t < MAXT; t++) { tinst[t] = -1; tcon[t] = -1; }
     if (FASTAL) {
         if (lane < SM::NMT) {
 #pragma unroll
@@ -196,7 +197,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         if (lane < NM) {
             for (int ci = 0; ci < P.ncon; ci++) {
                 const DevCon& con = P.cons[ci];
-                const double mu = P.mu[ci];
+                const double mu = penalty<false>(P, 0, ci);   // the shared penalty; INST: each instance's replaces it below
                 for (int side = 0; side < 2; side++) {
                     int row = -1; double sign = 1.0, bound = 0.0; bool eq = false;
                     if (con.kind == CON_GOAL) { if (side == 0 && lane < n) { row = con.row_max[lane]; if (row >= 0) bound = con.a[row]; eq = true; } }
@@ -207,7 +208,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     if (INST && nterm < MAXT) {
                         const int src = con.cdoff + (eq ? row : (side ? n + m : 0) + lane);
 #pragma unroll
-                        for (int t = 0; t < MAXT; t++) if (t == nterm) tinst[t] = src;
+                        for (int t = 0; t < MAXT; t++) if (t == nterm) { tinst[t] = src; tcon[t] = ci; }
                     }
                     nterm++;
                 }
@@ -231,11 +232,13 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         b = __shfl_sync(0xffffffffu, b, 0);
         if (b >= P.B) break;
         if (retired(P, b)) continue;            // to_solve: not ACTIVE
-        if constexpr (INST && FASTAL) {         // this instance's Goal / Bound values into the lane-resident terms (read back by this lane only)
+        if constexpr (INST && FASTAL) {         // this instance's Goal / Bound values and penalties into the lane-resident terms (read back by this lane only)
             if (lane < NM) {
 #pragma unroll
-                for (int t = 0; t < MAXT; t++)
+                for (int t = 0; t < MAXT; t++) {
                     if (P.cdata && tinst[t] >= 0) sm.tbound[t][lane] = P.cdata[(size_t)b * P.ncdata + tinst[t]];
+                    if (P.mub && tcon[t] >= 0) { const double mu = penalty<INST>(P, b, tcon[t]); sm.tnms[t][lane] = sm.tnms[t][lane] < 0.0 ? -mu : mu; }   // sign = +-1: exact
+                }
             }
         }
 
@@ -304,7 +307,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                     const DevCon& con = P.cons[ci];
                     if (con.diagonal || k1 < con.first || k1 > con.last) continue;
                     const int p = con.p;
-                    const double mu = P.mu[ci];
+                    const double mu = penalty<INST>(P, b, ci);
                     const double* lam = lam_b + con.offset + (size_t)(k1 - con.first) * p;
                     const double* xk = X + (size_t)(k1 - 1) * n;
                     if (lane == 0) {
@@ -386,7 +389,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                         for (int ci = 0; ci < P.ncon; ci++) {
                             const DevCon& con = P.cons[ci];
                             if (N < con.first || N > con.last) continue;
-                            const double mu = P.mu[ci];
+                            const double mu = penalty<INST>(P, b, ci);
                             const double* lam = lam_b + con.offset + (size_t)(N - con.first) * con.p;
                             if (con.kind == CON_GOAL) {
                                 const int row = con.row_max[i];
@@ -470,7 +473,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
                             for (int ci = 0; ci < P.ncon; ci++) {
                                 const DevCon& con = P.cons[ci];
                                 if (k + 1 < con.first || k + 1 > con.last) continue;
-                                const double mu = P.mu[ci];
+                                const double mu = penalty<INST>(P, b, ci);
                                 const double* lam = lam_b + con.offset + (size_t)(k + 1 - con.first) * con.p;
                                 if (con.kind == CON_GOAL) {
                                     const int row = (i < n) ? con.row_max[i] : -1;

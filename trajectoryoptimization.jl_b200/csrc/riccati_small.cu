@@ -46,7 +46,7 @@ __device__ __forceinline__ void expand_knot(const DevProblem& P, int b, int k0, 
     for (int ci = 0; ci < P.ncon; ci++) {
         const DevCon& con = P.cons[ci];
         if (k0 + 1 < con.first || k0 + 1 > con.last) continue;
-        const double mu = P.mu[ci];
+        const double mu = penalty<INST>(P, b, ci);
         const double* lam = lam_b + con.offset + (size_t)(k0 + 1 - con.first) * con.p;
         const ConData cd = con_data<INST>(P, b, ci);
         if (con.kind == CON_GOAL) {

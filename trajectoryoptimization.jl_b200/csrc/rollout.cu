@@ -163,7 +163,14 @@ __device__ __forceinline__ double exp_term_bound(const DevProblem& P, const ExpT
     if (P.cdata && j >= 0) return P.cdata[(size_t)b * P.ncdata + j];
     return shared;
 }
-// (INST: the cost weights, linear cost terms and Goal / Bound bounds of instance b)
+// -mu sign of term t of z entry i for instance b: with its penalty from the instance's row of DevProblem::mub when the table exists (exact:
+// sign = +-1 and `shared` = -mu sign carries it), else `shared`
+__device__ __forceinline__ double exp_term_nms(const DevProblem& P, const ExpTab& tab, int b, int t, int i, double shared) {
+    const int ci = __ldg(&tab.con[t][i]);
+    if (P.mub && ci >= 0) { const double mu = penalty<true>(P, b, ci); return shared < 0.0 ? -mu : mu; }
+    return shared;
+}
+// (INST: the cost weights, linear cost terms, Goal / Bound bounds and penalties of instance b)
 template <bool INST>
 __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, const ExpTab& tab, int b, int k, int i, double zi, const double* __restrict__ lam_b, double& g, double& h) {
     const int n = P.n;
@@ -177,7 +184,8 @@ __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, con
     for (int t = 0; t < TO_EXP_MAXT; t++) {
         const unsigned px = __ldg(&tab.pkx[t][i]);
         if ((unsigned)(k + 1) - (px & 0xfffu) <= ((px >> 12) & 0xfffu)) {
-            const double nms = __ldg(&tab.nms[t][i]);
+            double nms = __ldg(&tab.nms[t][i]);
+            if constexpr (INST) nms = exp_term_nms(P, tab, b, t, i, nms);
             const double lam = lam_b[(int)(__ldg(&tab.pky[t][i]) + (unsigned)(k + 1) * ((px >> 24) & 0x7fu))];
             double bound = __ldg(&tab.bound[t][i]);
             if constexpr (INST) bound = exp_term_bound(P, tab, b, t, i, bound);
@@ -390,7 +398,7 @@ cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s) {
 #ifndef TO_CEXP2_THREADS
 #define TO_CEXP2_THREADS 64
 #endif
-// INST: the linear cost terms and Goal / Bound bounds of each instance (DevProblem::qr / cdata), a variant of its own so that the shared one stays as it is
+// INST: the linear cost terms, Goal / Bound bounds and penalties of each instance (DevProblem::qr / cdata / mub), a variant of its own so that the shared one stays as it is
 template <bool INST>
 __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_rec16b(const DevProblem P, int mode) {
     constexpr int qs = 3, n = 13, m = 4;
@@ -421,9 +429,9 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
         const double* __restrict__ Ub = traj_U(P, buf, b);
         const double* __restrict__ lam_b = P.lambda + (size_t)b * P.lambda_len;
         double* __restrict__ recb = P.REC + ((size_t)b * N + kb) * TO_REC_LEN + TO_REC_G;
-        if constexpr (INST) {                                                         // this instance's Goal / Bound bounds into the lane's terms
+        if constexpr (INST) {                                                         // this instance's Goal / Bound bounds and penalties into the lane's terms
 #pragma unroll
-            for (int t = 0; t < TO_EXP_MAXT; t++) bnd[t] = exp_term_bound(P, tab, b, t, i, tab.bound[t][i]);
+            for (int t = 0; t < TO_EXP_MAXT; t++) { bnd[t] = exp_term_bound(P, tab, b, t, i, tab.bound[t][i]); nms[t] = exp_term_nms(P, tab, b, t, i, tab.nms[t][i]); }
         }
         const int nk = (N - kb < 16) ? N - kb : 16;
         const int mycid = (i < nk) ? P.cost_index[kb + i] : 0;                        // lane j <-> knot kb + j (phases B, C; broadcast in phase A)
@@ -529,9 +537,9 @@ __global__ void __launch_bounds__(TO_CEXP2_THREADS, TO_CEXP2_MINB) k_expansion_r
                     for (int t = 0; t < TO_EXP_MAXT; t++) {
                         const unsigned rx = __ldg(&tab.pkx[t][n + a]);
                         if ((unsigned)(k + 1) - (rx & 0xfffu) <= ((rx >> 12) & 0xfffu)) {
-                            const double rn = __ldg(&tab.nms[t][n + a]);
+                            double rn = __ldg(&tab.nms[t][n + a]);
                             double bd = __ldg(&tab.bound[t][n + a]);
-                            if constexpr (INST) bd = exp_term_bound(P, tab, b, t, n + a, bd);
+                            if constexpr (INST) { bd = exp_term_bound(P, tab, b, t, n + a, bd); rn = exp_term_nms(P, tab, b, t, n + a, rn); }
                             const double lb = fma(rn, zu[a] - bd, lu[a][t]);
                             if ((rx >> 31) || lb <= 0.0) { g += (rn < 0.0) ? -lb : lb; h += fabs(rn); }
                         }

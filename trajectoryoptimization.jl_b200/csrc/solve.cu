@@ -1,9 +1,11 @@
 // solve.cu -- the per-instance stopping rules of to_solve (Altro's AL-iLQR `solve!`, restated in DESIGN.md 5d and include/trajopt_b200.h).
 //
 // The iteration itself is the one to_ilqr_step runs (expansion, backward pass, line search).  These kernels only DECIDE, one thread per
-// instance: after an instance's line search, whether its inner (iLQR) loop goes on; after every inner loop of the batch has ended, whether
-// an instance is done or goes on to another outer (AL) iteration.  An instance whose loop has ended is marked WAITING or DONE in
-// SolveDev::state, which is DevProblem::active while to_solve runs: every per-instance kernel of the iteration then skips it.
+// instance: after an instance's line search, whether its inner (iLQR) loop goes on; when its inner loop has ended, whether it is done or goes
+// on to another outer (AL) iteration.  With shared penalties that second decision waits until every inner loop of the batch has ended
+// (k_solve_outer), and an instance whose loop has ended is marked WAITING or DONE in SolveDev::state, which is DevProblem::active while
+// to_solve runs: every per-instance kernel of the iteration then skips it.  With per-instance penalties k_solve_check decides at once, and an
+// instance that goes on stays ACTIVE, flagged in SolveDev::go for the outer step that follows the check on its stream.
 #include "../../include/trajopt_b200.h"
 #include "kernels.h"
 
@@ -30,7 +32,18 @@ __global__ void k_solve_init(const DevProblem P, SolveDev S) {
     S.state[b] = SOLVE_ACTIVE; S.status[b] = TO_SOLVE_UNSOLVED;
     S.iter[b] = 0; S.outer[b] = 1; S.inner[b] = 0; S.dj_zero[b] = 0;
     S.dJ[b] = 0.0; S.grad[b] = 0.0; S.cmax[b] = 0.0;
+    if (S.go) { S.go[b] = SOLVE_DONE; S.go[P.B + b] = SOLVE_DONE; }
     P.rho[b] = P.opt.bp_reg_initial; P.drho[b] = 0.0;      // Altro initialize!: the regularisation restarts
+}
+
+// Altro's outer-loop rules for instance b, whose inner loop has ended with violation S.cmax[b]: its final status, or TO_SOLVE_UNSOLVED when
+// it goes on to another outer iteration
+__device__ int outer_decision(const SolveDev& S, int b) {
+    const SolveOpts& o = S.opt;
+    if (S.cmax[b] < o.constraint_tolerance) return TO_SOLVE_SUCCEEDED;
+    if (S.iter[b] >= o.iterations) return TO_SOLVE_MAX_ITERATIONS;
+    if (S.outer[b] >= o.iterations_outer) return TO_SOLVE_MAX_ITERATIONS_OUTER;
+    return TO_SOLVE_UNSOLVED;
 }
 
 // start of an inner loop of the ACTIVE instances: J_prev = the merit of the live trajectory (with the current multipliers and penalties)
@@ -68,7 +81,12 @@ __global__ void k_solve_check(const DevProblem P, SolveDev S, int mode) {
         const bool converged = stepped && dJ >= 0.0 && dJ < ctol && grad < gtol;
         const bool ended = converged || S.dj_zero[b] > o.dJ_counter_limit || iter >= o.iterations || (constrained && inner >= o.iterations_inner);
         if (ended) {
-            if (constrained) next = SOLVE_WAITING;          // the outer step (k_solve_outer) decides
+            if (constrained && S.go) {                      // per-instance penalties: the outer rules, now
+                S.cmax[b] = P.viol[b];
+                status = outer_decision(S, b);
+                if (status == TO_SOLVE_UNSOLVED) { S.go[(mode == 2 ? P.B : 0) + b] = SOLVE_ACTIVE; return; }   // the outer step of this half follows
+                next = SOLVE_DONE;
+            } else if (constrained) next = SOLVE_WAITING;   // the outer step (k_solve_outer) decides
             else { next = SOLVE_DONE; status = converged ? TO_SOLVE_SUCCEEDED : iter >= o.iterations ? TO_SOLVE_MAX_ITERATIONS : TO_SOLVE_UNSOLVED; }
         }
     }
@@ -85,15 +103,21 @@ __global__ void k_solve_check(const DevProblem P, SolveDev S, int mode) {
 __global__ void k_solve_outer(const DevProblem P, SolveDev S) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= P.B || S.state[b] != SOLVE_WAITING) return;
-    const SolveOpts& o = S.opt;
-    int status = TO_SOLVE_UNSOLVED;
-    if (S.cmax[b] < o.constraint_tolerance) status = TO_SOLVE_SUCCEEDED;
-    else if (S.iter[b] >= o.iterations) status = TO_SOLVE_MAX_ITERATIONS;
-    else if (S.outer[b] >= o.iterations_outer) status = TO_SOLVE_MAX_ITERATIONS_OUTER;
+    const int status = outer_decision(S, b);
     if (status != TO_SOLVE_UNSOLVED) { S.status[b] = status; S.state[b] = SOLVE_DONE; return; }
     S.outer[b]++;
     S.state[b] = SOLVE_ACTIVE;
     atomicAdd(S.n_active, 1);
+}
+
+// per-instance penalties: the end of the outer step of the instances flagged in half `half` of SolveDev::go, after their dual update, penalty
+// update and fresh merit (k_al_update and k_cost, launched with go as DevProblem::active): the next inner loop starts, as k_solve_begin starts it
+__global__ void k_solve_restart(const DevProblem P, SolveDev S, int half) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P.B || S.go[half * P.B + b] != SOLVE_ACTIVE) return;
+    S.J_prev[b] = P.J[b]; S.inner[b] = 0; S.dj_zero[b] = 0;
+    S.outer[b]++;
+    S.go[half * P.B + b] = SOLVE_DONE;
 }
 
 }  // namespace
@@ -112,5 +136,9 @@ cudaError_t launch_solve_check(const DevProblem& P, const SolveDev& S, int mode,
 }
 cudaError_t launch_solve_outer(const DevProblem& P, const SolveDev& S, cudaStream_t s) {
     k_solve_outer<<<nblk(P.B, 128), 128, 0, s>>>(P, S);
+    return cudaGetLastError();
+}
+cudaError_t launch_solve_restart(const DevProblem& P, const SolveDev& S, int half, cudaStream_t s) {
+    k_solve_restart<<<nblk(P.B, 128), 128, 0, s>>>(P, S, half);
     return cudaGetLastError();
 }

@@ -166,7 +166,8 @@ __global__ void k_hess_projection(int cone, int p, int count, const double* __re
     if (cone_hess_projection(cone, x + (size_t)t * p, b + (size_t)t * p, p, H + (size_t)t * p * p)) atomicExch(err, 1);
 }
 
-// dual update: lambda <- clamp(Pi_{K*}(lambda - mu c)); one thread per (instance, constraint, knot)
+// dual update: lambda <- clamp(Pi_{K*}(lambda - mu c)); one thread per (instance, constraint, knot).  With per-instance penalties it
+// also scales the instance's row, mu <- min(mu phi, mu_max): the host's operation on the shared penalties, so the bits match
 template <bool INST>
 __global__ void k_al_update(const DevProblem P) {
     const int b = blockIdx.x;
@@ -177,7 +178,7 @@ __global__ void k_al_update(const DevProblem P) {
     double zero_u[TO_MAXM] = {0};
     for (int ci = 0; ci < P.ncon; ci++) {
         const DevCon& con = P.cons[ci];
-        const double mu = P.mu[ci];
+        const double mu = penalty<INST>(P, b, ci);
         for (int k1 = con.first + threadIdx.x; k1 <= con.last; k1 += blockDim.x) {
             const double* x = X + (size_t)(k1 - 1) * P.n;
             const double* u = (k1 == P.N) ? zero_u : U + (size_t)(k1 - 1) * P.m;
@@ -190,6 +191,13 @@ __global__ void k_al_update(const DevProblem P) {
         }
     }
     if (threadIdx.x == 0) { P.rho[b] = P.opt.bp_reg_initial; P.drho[b] = 0.0; }
+    if constexpr (INST) {               // the instance's penalties for its next outer iteration, once every thread has read them
+        if (P.mub) {
+            __syncthreads();
+            double* mu = P.mub + (size_t)b * P.ncon;
+            for (int ci = threadIdx.x; ci < P.ncon; ci += blockDim.x) mu[ci] = fmin(mu[ci] * P.opt.penalty_scaling, P.opt.penalty_max);
+        }
+    }
 }
 
 // {sum_b J_b, max_b viol_b} for the cross-GPU merit all-reduce (SURVEY 8e)

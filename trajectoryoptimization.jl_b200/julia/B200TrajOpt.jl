@@ -366,6 +366,17 @@ function cost_weights(p::BatchedProblem, cost::Integer)
     check(p.h, ccall((:to_get_cost_weights, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}), p.h, cost - 1, W))
     W
 end
+# per-instance AL penalties: mu[b] is instance b's penalty of constraint `con` (1-based); a scalar sets every instance's
+function set_penalties!(p::BatchedProblem, con::Integer, mu::AbstractVector)
+    length(mu) == p.B || throw(DimensionMismatch("mu must have length B"))
+    check(p.h, ccall((:to_set_penalties, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}), p.h, con - 1, Vector{Float64}(mu)))
+end
+set_penalties!(p::BatchedProblem, con::Integer, mu::Real) = set_penalties!(p, con, fill(Float64(mu), p.B))
+function penalties(p::BatchedProblem, con::Integer)
+    mu = Vector{Float64}(undef, p.B)
+    check(p.h, ccall((:to_get_penalties, libb200), Cint, (Ptr{Cvoid}, Int32, Ptr{Float64}), p.h, con - 1, mu))
+    mu
+end
 
 # ---- what Altro.jl's iLQR / AL loop does with the API above, fused on the device ------------------------------
 expand!(p::BatchedProblem) = check(p.h, ccall((:to_expand, libb200), Cint, (Ptr{Cvoid},), p.h))
