@@ -7,7 +7,7 @@
  * to_update_trajectories, to_set_cost_terms), in the linear cost terms q, r and the Goal constraint values
  * (goal state / tracking reference per instance) -- and, after to_set_model_params, in the model parameters (mass,
  * inertia, lengths, motor constants, gravity) -- and, after to_set_constraint_data, in the constraint data (bounds, obstacles, collision
- * radii, norm values, linear right-hand sides) -- and, after to_set_cost_weights, in the cost weights Q, R, H, c, w -- and, after to_set_penalties, in the AL penalties.  Every function cites the reference interface it stands in for.  The
+ * radii, norm values, linear right-hand sides) -- and, after to_set_cost_weights, in the cost weights Q, R, H, c, w -- and, after to_set_penalties, in the AL penalties -- and, after to_set_time_steps, in the time steps and initial time.  Every function cites the reference interface it stands in for.  The
  * Julia-side binding (ccall) that a maintainer adds is shown in INTEGRATION.md.
  *
  * Conventions
@@ -239,6 +239,18 @@ int to_set_goal_values(to_handle* h, int32_t con, const double* vals);          
  * the instance and the entry, and the rows stay as they were.  Multi-GPU: each rank passes its shard's rows, as for x0. */
 int to_set_model_params(to_handle* h, const double* params /*[B][nparams]*/, int32_t nparams);
 int to_get_model_params(to_handle* h, double* params /*[B][nparams]*/);                             /* the shared values broadcast when none are set */
+
+/* ---- per-instance time steps -----------------------------------------------------------------------------------
+ * Instance b integrates knot k with its own step dt[b][k], and its clock starts at t0[b]: its knot times are t0_b, t0_b + dt_b[0], ...  This is
+ * what Problem(model, obj, x0_b, tf_b; t0 = t0_b, dt = dt_b) holds (src/problem.jl:16-29, 79-111).  Until the first call there is no table and
+ * every kernel runs as before; t0 = NULL keeps the clocks (the first call starts them at the shared t0).  A batch whose instance b holds
+ * (t0_b, dt_b) computes, bit for bit, what instance b of a batch created with that grid computes, on every solver path.  X is not rolled out
+ * again.  to_get_times keeps returning the shared grid (to_spec.t0 and dt), as to_bounds keeps the shared bounds.  to_set_initial_time sets
+ * the shared clock and every instance's; to_shift_trajectory advances each instance's clock by its own skipped steps and leaves the rows as
+ * they are.  TO_EINVAL: a hybrid problem, a step that is non-finite or <= 0, a non-finite t0; the message names the instance and the knot, and
+ * the table and clocks stay as they were.  Multi-GPU: each rank passes its shard's rows, as for x0. */
+int to_set_time_steps(to_handle* h, const double* dt /*[B][N-1]*/, const double* t0 /*[B] or NULL: keep the clocks*/);
+int to_get_time_steps(to_handle* h, double* dt /*[B][N-1]*/, double* t0 /*[B] or NULL*/);            /* the shared values broadcast when none are set */
 
 /* ---- per-instance constraint data ----------------------------------------------------------------------------
  * Instance b evaluates constraint con with its own data (a Problem owns its ConstraintList, src/problem.jl:36-73).  One instance's row, len doubles:

@@ -1217,6 +1217,10 @@ class Problem:
         if getattr(self, "_mparams", False):   # per-instance model parameters: carried over as they are
             mparams = np.empty((self.B, len(self.model.params)))
             self._raw_call("to_get_model_params", K._dp(mparams))
+        steps = None
+        if getattr(self, "_dtb", False):       # per-instance time steps and clocks: carried over as they are
+            steps = np.empty((self.B, self.N - 1)), np.empty(self.B)
+            self._raw_call("to_get_time_steps", K._dp(steps[0]), K._dp(steps[1]))
         self.close()
         self.spec = self._make_spec(self._dt, float(t[0]))
         self._open()
@@ -1239,6 +1243,8 @@ class Problem:
         self._con_snap = {cid: v for cid, v in snap.items() if cid in con_carry}
         if mparams is not None:
             self._raw_call("to_set_model_params", K._dp(mparams), int(mparams.shape[1]))
+        if steps is not None:
+            self._raw_call("to_set_time_steps", K._dp(steps[0]), K._dp(steps[1]))
         self._raw_call("to_set_initial_state", K._dp(self.x0))
         self._raw_call("to_set_controls", K._dp(U))
         if np.all(np.isfinite(X)):
@@ -1601,6 +1607,59 @@ def model_params(prob):
     out = np.empty((prob.B, len(prob.model.params)))
     prob._call("to_get_model_params", K._dp(out))
     return out
+
+
+def _time_step_rows(prob, dt, t0=None):
+    """``(dt[B, N-1], t0[B] or None)`` as ``to_set_time_steps`` takes them; every check that needs no device happens here"""
+    if getattr(prob, "hybrid", False):
+        raise ArgumentError("per-instance time steps are not supported on hybrid problems")
+    dt = np.asarray(dt, dtype=np.float64)
+    if dt.shape == (prob.B,):                  # one uniform step per instance: the reference's scalar dt
+        dt = np.repeat(dt[:, None], prob.N - 1, axis=1)
+    if dt.shape != (prob.B, prob.N - 1):
+        raise DimensionMismatch(f"set_time_steps: expected [{prob.B}, {prob.N - 1}] or [{prob.B}] time steps, got {dt.shape}")
+    bad = np.argwhere(~(np.isfinite(dt) & (dt > 0)))
+    if bad.size:
+        raise ArgumentError(f"set_time_steps: instance {bad[0][0]}, knot {bad[0][1]}: a time step must be finite and positive")
+    if t0 is not None:
+        t0 = np.asarray(t0, dtype=np.float64)
+        t0 = np.full(prob.B, float(t0)) if t0.ndim == 0 else t0
+        if t0.shape != (prob.B,):
+            raise DimensionMismatch(f"set_time_steps: expected [{prob.B}] initial times, got {t0.shape}")
+        bad = np.nonzero(~np.isfinite(t0))[0]
+        if bad.size:
+            raise ArgumentError(f"set_time_steps: instance {bad[0]}: the initial time must be finite")
+        t0 = np.ascontiguousarray(t0)
+    return np.ascontiguousarray(dt), t0
+
+
+def set_time_steps(prob, dt, t0=None):
+    """Instance ``b`` integrates knot ``k`` with its own step ``dt[b, k]``; ``dt`` is ``[B, N-1]``, or ``[B]`` for one uniform step per
+    instance (``np.full(N-1, dt_b)``: with ``dt_b = (tf_b - t0) / (N-1)`` the steps ``Problem(..., tf_b)`` builds).  ``t0`` (``[B]`` or a
+    scalar) starts each instance's clock; ``None`` keeps the clocks (the first call starts them at the shared initial time).  A batch whose
+    instance ``b`` holds ``(t0_b, dt_b)`` computes, bit for bit, what instance ``b`` of a batch built with ``Problem(..., t0=t0_b, dt=dt_b)``
+    computes.  The trajectory is not rolled out again.  ``gettimes`` keeps returning the shared grid; ``instance_times`` gives each
+    instance's."""
+    dt, t0 = _time_step_rows(prob, dt, t0)
+    prob._call("to_set_time_steps", K._dp(dt), K._dp(t0))
+    prob._dtb = True
+
+
+def time_steps(prob):
+    """``(dt[B, N-1], t0[B])``: every instance's time steps and initial time (the shared grid broadcast when none were set)."""
+    dt, t0 = np.empty((prob.B, prob.N - 1)), np.empty(prob.B)
+    prob._call("to_get_time_steps", K._dp(dt), K._dp(t0))
+    return dt, t0
+
+
+def instance_times(prob):
+    """``[B, N]``: the knot times of every instance, ``t0_b, t0_b + dt_b[0], ...``, summed in the order ``gettimes`` sums them."""
+    dt, t0 = time_steps(prob)
+    t = np.empty((prob.B, prob.N))
+    t[:, 0] = t0
+    for k in range(1, prob.N):
+        t[:, k] = t[:, k - 1] + dt[:, k - 1]
+    return t
 
 
 # which fields of a constraint's _spec are its per-instance data, in the order of an instance's row (include/trajopt_b200.h

@@ -58,6 +58,8 @@ struct to_handle {
     std::vector<double> h_mparams;   // model parameters (DevProblem::mparams), [B][TO_NPARAM]
     std::vector<double> h_cdata;     // constraint data and Goal values (DevProblem::cdata), [B][ncdata]
     std::vector<double> h_cw;        // cost weights (DevProblem::cw), [B][ncw]
+    std::vector<double> h_dtb;       // time steps (DevProblem::dtb), [B][N-1]
+    std::vector<double> t0b;         // ... and each instance's clock, [B]: host state only (every model is time-invariant), kept with the table
     // AL penalties (DevProblem::mub), [B][ncon]: no host copy, the device scales the rows (k_al_update, to_solve's outer steps)
     int* d_go = nullptr;             // SolveDev::go, allocated with the penalty table
     std::vector<double> stage;       // the rows a setter is building, committed by commit_rows (kept to reuse its allocation)
@@ -177,6 +179,16 @@ int fill_penalty_rows(to_handle* h, double* d) {
     for (int b = 0; b < B; b++) std::memcpy(rows.data() + (size_t)b * nc, h->h_mu.data(), sizeof(double) * nc);
     CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));   // the staged rows are the source of the copy
+    return TO_OK;
+}
+
+// The closed-form columns of [A B] (full-state Quadrotor) and of the materialised [A_e B_e] (error state outside the record path): functions of
+// the time steps alone, so no expansion kernel writes them.  Written when the problem is created and whenever its time steps change, through
+// the same view as the expansion kernels (each instance's own steps once DevProblem::dtb exists).
+int write_closed_form_columns(to_handle* h) {
+    CU(h, launch_trivial_columns_full(h->P, h->stream));
+    if (h->P.lie && h->P.model == MODEL_QUADROTOR) CU(h, launch_trivial_columns(h->P, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
     return TO_OK;
 }
 
@@ -742,10 +754,8 @@ int to_create(const to_spec* s, to_handle** out) {
     if (!okc) { h->err = std::string("device initialisation failed: ") + cudaGetErrorString(cudaGetLastError()); return bail(TO_ECUDA); }
     rc = upload_tables(h);
     if (rc) return bail(rc);
-    if (launch_trivial_columns_full(P, st) != cudaSuccess) { h->err = "k_trivial_columns_full failed"; return bail(TO_ECUDA); }   // closed-form columns of [A B] (rollout.cu SeedList)
-    if (P.lie && P.model == MODEL_QUADROTOR) {        // the position / velocity columns of [A_e B_e] are functions of the time steps alone (rollout.cu)
-        if (launch_trivial_columns(P, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess) { h->err = "k_trivial_columns failed"; return bail(TO_ECUDA); }
-    }
+    rc = write_closed_form_columns(h);     // closed-form columns of [A B] / [A_e B_e] (rollout.cu SeedList, lie_trivial)
+    if (rc) return bail(rc);
     *out = h;
     return TO_OK;
 }
@@ -907,6 +917,7 @@ int to_set_initial_time(to_handle* h, double t0, double* tf_out) {
     JOIN(h);
     if (!h) return TO_EINVAL;
     h->t0 = t0;
+    for (double& t : h->t0b) t = t0;      // ... and every instance's clock (tf_out stays the shared grid's)
     if (tf_out) { double t = t0; for (double d : h->h_dt) t += d; *tf_out = t; }
     return TO_OK;
 }
@@ -1233,6 +1244,43 @@ int to_get_cost_weights(to_handle* h, int32_t cost, double* w) {
     return TO_OK;
 }
 
+// ---- per-instance time steps (DevProblem::dtb) ----------------------------------------------------------
+// dt [B][N-1], t0 [B] or NULL (keep the clocks).  Instance b integrates knot k with dt[b][k] and its clock starts at t0[b]: what
+// Problem(model, obj, x0_b, tf_b; t0 = t0_b, dt = dt_b) holds.  The whole batch is checked before anything changes: a refused call leaves the
+// table (or its absence) and the clocks as they were.  The first call starts every clock at the shared t0 unless t0 is given.  The closed-form
+// Jacobian columns are rewritten from the new steps; X is not rolled out again.
+int to_set_time_steps(to_handle* h, const double* dt, const double* t0) {
+    JOIN(h);
+    if (!h || !dt) return TO_EINVAL;
+    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance time steps are not supported on hybrid problems");
+    const int B = h->P.B, K = h->P.N - 1;
+    for (int b = 0; b < B; b++) {
+        for (int k = 0; k < K; k++) {
+            const double v = dt[(size_t)b * K + k];
+            if (!(std::isfinite(v) && v > 0))
+                return fail(h, TO_EINVAL, "to_set_time_steps: instance " + std::to_string(b) + ", knot " + std::to_string(k) + ": a time step must be finite and positive");
+        }
+        if (t0 && !std::isfinite(t0[b])) return fail(h, TO_EINVAL, "to_set_time_steps: instance " + std::to_string(b) + ": the initial time must be finite");
+    }
+    h->stage.assign(dt, dt + (size_t)B * K);
+    int rc = commit_rows(h, h->h_dtb, h->P.dtb); if (rc) return rc;
+    if (t0) h->t0b.assign(t0, t0 + B);
+    else if (h->t0b.empty()) h->t0b.assign(B, h->t0);
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return write_closed_form_columns(h);
+}
+// dt [B][N-1], t0 [B] or NULL: every instance's time steps and clock (the shared grid broadcast when none are set)
+int to_get_time_steps(to_handle* h, double* dt, double* t0) {
+    JOIN(h);
+    if (!h || !dt) return TO_EINVAL;
+    const int B = h->P.B, K = h->P.N - 1;
+    for (int b = 0; b < B; b++) {
+        std::memcpy(dt + (size_t)b * K, h->P.dtb ? h->h_dtb.data() + (size_t)b * K : h->h_dt.data(), sizeof(double) * K);
+        if (t0) t0[b] = h->P.dtb ? h->t0b[b] : h->t0;
+    }
+    return TO_OK;
+}
+
 // ---- kernel 1 ---------------------------------------------------------------------------------------------
 int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, int32_t nref, int32_t start) {
     JOIN(h);
@@ -1267,6 +1315,9 @@ int to_shift_trajectory(to_handle* h, int32_t steps) {
     if (steps > h->P.N - 1) steps = h->P.N - 1;
     CU(h, launch_shift_traj(h->P, steps, h->stream)); h->launches++;
     for (int k = 0; k < steps; k++) h->t0 += h->h_dt[k];
+    const int K = h->P.N - 1;
+    for (size_t b = 0; b < h->t0b.size(); b++)            // each instance's clock by its own skipped steps, in the same order (the rows stay)
+        for (int k = 0; k < steps; k++) h->t0b[b] += h->h_dtb[b * K + k];
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }

@@ -186,6 +186,9 @@ struct DevProblem {
     // the first call; every kernel then reads the shared `mu`.  Unlike the other tables the device also writes it: k_al_update scales the
     // rows of the instances it updates, and to_solve runs each instance's outer step on the device.
     double* mub;              // [B][ncon]
+    // Per-instance time steps (to_set_time_steps): row b holds the N-1 steps of instance b (see time_step).  nullptr until the first call;
+    // every kernel then reads the shared `dt`.
+    const double* dtb;        // [B][N-1]
 };
 #define TO_NPARAM 16        // slots of DevProblem::params and of a row of DevProblem::mparams (one 128-byte line)
 
@@ -193,11 +196,12 @@ enum { SOLVE_ACTIVE = 0, SOLVE_WAITING = 1, SOLVE_DONE = 2 };
 __host__ __device__ inline bool retired(const DevProblem& P, int b) { return P.active != nullptr && P.active[b] != SOLVE_ACTIVE; }
 
 // Which variant of a kernel family runs: INST = true when a per-instance table the family reads exists.  The only place that decides; every
-// launcher and to_kernel_choice ask here.  The line search reads the linear cost terms, the model parameters and the constraint data; the
-// expansion, backward and sweep kernels the cost terms and the constraint data; the dynamics kernels the model parameters alone.
-__host__ __device__ inline bool inst_forward(const DevProblem& P) { return P.qr || P.mparams || P.cdata || P.cw || P.mub; }
+// launcher and to_kernel_choice ask here.  The line search reads the linear cost terms, the model parameters, the time steps and the
+// constraint data; the expansion, backward and sweep kernels the cost terms and the constraint data (none of them reads a time step); the
+// dynamics kernels, the closed-form Jacobian columns included, the model parameters and the time steps.
+__host__ __device__ inline bool inst_forward(const DevProblem& P) { return P.qr || P.mparams || P.cdata || P.cw || P.mub || P.dtb; }
 __host__ __device__ inline bool inst_backward(const DevProblem& P) { return P.qr || P.cdata || P.cw || P.mub; }
-__host__ __device__ inline bool inst_dynamics(const DevProblem& P) { return P.mparams; }
+__host__ __device__ inline bool inst_dynamics(const DevProblem& P) { return P.mparams || P.dtb; }
 
 // The weights and linear terms of cost cid for instance b: the only place that decides between an instance's rows (DevProblem::cw for the
 // weights, DevProblem::qr for the linear terms) and the descriptor, and the only way a kernel reads them.  The cost's structure (diag, zeroH,
@@ -242,6 +246,16 @@ __device__ __forceinline__ double model_param(const DevProblem& P, int b, int i)
     if constexpr (INST) { if (P.mparams) return P.mparams[(size_t)b * TO_NPARAM + i]; }
     return P.params[i];
 }
+// The time step of knot k (0-based, k < N-1) for instance b: the only place that decides between an instance's row of DevProblem::dtb and the
+// shared steps.  `shared`: P.dt, or a kernel's staged copy of it (the line search's table in shared memory), so that with INST = false a kernel
+// reads the address it always read.
+template <bool INST>
+__device__ __forceinline__ double time_step(const DevProblem& P, int b, int k, const double* shared) {
+    if constexpr (INST) { if (P.dtb) return P.dtb[(size_t)b * (P.N - 1) + k]; }
+    return shared[k];
+}
+template <bool INST>
+__device__ __forceinline__ double time_step(const DevProblem& P, int b, int k) { return time_step<INST>(P, b, k, P.dt); }
 // The AL penalty of constraint ci for instance b: the only place that decides between an instance's row of DevProblem::mub and the shared
 // DevProblem::mu, and the only way a kernel reads a penalty.
 template <bool INST>

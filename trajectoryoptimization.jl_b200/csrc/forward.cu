@@ -226,7 +226,8 @@ __device__ __forceinline__ void prefetch_knot(double* base, int g, int l, int k,
 
 // closed-loop rollout of instance b (group g of the CTA) with step size alpha, diagonal costs, Goal/Bound constraints.
 // The candidate trajectory goes to buffer `cbuf`.  Returns the merit; `ok` = no blow-up.
-// INST: the instance's own linear cost terms and Goal values (DevProblem::qr / goal, read from global memory instead of the CTA's table).
+// INST: the instance's own linear cost terms and Goal values (DevProblem::qr / goal, read from global memory instead of the CTA's table), and
+// time steps (DevProblem::dtb, loaded per knot instead of the table's).
 template <int MODEL, int IPB, int G, bool LIE, bool INST>
 __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab& tab, double* stage, const double* prm, int b, int g, int l,
                                                unsigned gmask, double alpha, int cbuf, bool& ok, double& viol) {
@@ -381,7 +382,7 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
             }
         }
         if (!last) {
-            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, tab.dt[k], xn);
+            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), xn);
 #pragma unroll
             for (int i = 0; i < n; i++) { x[i] = xn[i]; if (!(fabs(xn[i]) <= P.opt.max_state_value)) ok = false; }
             // a blown-up trial keeps integrating (the group stays in lock step); its result is rejected through `ok`
@@ -402,7 +403,8 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
 //     candidate stores ran pass 1 in about half the time);
 //   * RK4 writes the next state over the current one (rk4_step reads x_i for the last time where it writes xn_i), so the loop carries
 //     no x <- xn copies.  (Unrolled by two with x / xn swapping roles instead, the loop took 40 more registers and spilled.)
-// INST: gbox = the instance's control box {u_max_i, u_min_i} and gcost = its two costs and penalties, staged for the group by linesearch_pass
+// INST: gbox = the instance's control box {u_max_i, u_min_i} and gcost = its two costs and penalties, staged for the group by linesearch_pass;
+// its time steps are loaded per knot (time_step)
 template <int MODEL, int IPB, int G, bool LIE, bool INST>
 __device__ __forceinline__ double rollout_compact(const DevProblem& P, const FwdCompactTab& tab, double* stage, double* ost, const double* prm,
                                                   const double2* gbox, const FwdCompactCost* gcost, int b, int g, int l, unsigned gmask,
@@ -539,11 +541,11 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
         }
         if constexpr (MODEL == MODEL_EXPR_42) {   // a discrete jump map writes its outputs while it reads its inputs
             double xn[n];
-            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, tab.dt[k], xn);
+            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), xn);
 #pragma unroll
             for (int i = 0; i < n; i++) x[i] = xn[i];
         } else {
-            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, tab.dt[k], x);
+            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), x);
         }
 #pragma unroll
         for (int i = 0; i < n; i++) if (!(fabs(x[i]) <= P.opt.max_state_value)) ok = false;
@@ -631,7 +633,7 @@ __device__ __forceinline__ double rollout_generic(const DevProblem& P, const dou
         J += al_knot_penalty<INST>(P, k + 1, x, u, lam_b, viol, b);
         if (!last) {
             // INST: the determinant form the shared kernel compiles to, written out (models.cuh det_sub_square)
-            rk4_step<MODEL, double, INST>(model_params<MODEL, INST>(P, prm, k), x, u, P.dt[k], xn);
+            rk4_step<MODEL, double, INST>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k), xn);
 #pragma unroll
             for (int i = 0; i < n; i++) { x[i] = xn[i]; if (!(fabs(xn[i]) <= P.opt.max_state_value)) ok = false; }
             if (!ok) break;
@@ -809,8 +811,9 @@ cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int f
     return launch_pass_l<MODEL, G, PATH, 32, false, INST>(P, trial0, first_pass, final_pass, s);
 }
 
-// per-instance cost weights / linear cost terms / model parameters / constraint data: a kernel variant of its own, so that the shared one is
-// the code it has always been.  It serves every per-instance table; each accessor checks its own (cost_data, model_param, con_data).
+// per-instance cost weights / linear cost terms / model parameters / constraint data / penalties / time steps: a kernel variant of its own, so
+// that the shared one is the code it has always been.  It serves every per-instance table; each accessor checks its own (cost_data,
+// model_param, con_data, penalty, time_step).
 template <int MODEL, int G, int PATH>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     if (inst_forward(P)) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);

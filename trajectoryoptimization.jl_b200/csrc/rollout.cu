@@ -17,8 +17,9 @@
 
 // One thread integrates one instance; the warp writes its 32 states of a knot through a shared-memory transpose, so that the stores are runs of
 // n contiguous doubles per instance (full 32-byte sectors) instead of 32 scattered 8-byte words per instruction.
-// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per lane.  (Copied to registers instead, the
-// parameter-only subexpressions of the dynamics were hoisted out of the knot loop and lost FMA contractions the shared kernel has.)
+// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per lane, and time steps (DevProblem::dtb).
+// (Copied to registers instead, the parameter-only subexpressions of the dynamics were hoisted out of the knot loop and lost FMA contractions
+// the shared kernel has.)
 template <int MODEL, bool INST>
 __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m;
@@ -53,7 +54,7 @@ __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
         if (k == P.N - 1) break;
 #pragma unroll
         for (int i = 0; i < m; i++) u[i] = U[k * m + i];
-        rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, P.dt[k], xn);
+        rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, bc, k), xn);
 #pragma unroll
         for (int i = 0; i < n; i++) x[i] = xn[i];
     }
@@ -61,8 +62,8 @@ __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
 
 // Seed pruning (full state).  The position r and the world-frame linear velocity v of the Quadrotor (a RobotDynamics RigidBody) enter the
 // dynamics only through rdot = v, so their columns of [A B] are known in closed form -- d x+/d r = e_r, d x+/d v = h e_r + e_v (the RK4
-// weights sum to one) -- and are written once when the problem is created (k_trivial_columns_full); 11 seeds (quaternion, angular velocity,
-// controls) are pushed through the dual-number RK4 step instead of 17.  Other models: every seed.
+// weights sum to one) -- and are written when the problem is created and when its time steps change (k_trivial_columns_full); 11 seeds
+// (quaternion, angular velocity, controls) are pushed through the dual-number RK4 step instead of 17.  Other models: every seed.
 template <int MODEL> struct SeedList {
     static constexpr int count = ModelDims<MODEL>::n + ModelDims<MODEL>::m;
     __host__ __device__ static constexpr int seed(int s) { return s; }
@@ -76,7 +77,7 @@ template <> struct SeedList<MODEL_QUADROTOR> {
     __host__ __device__ static constexpr int trivial(int s) { return s < 3 ? s : 4 + s; }        // 0..2 (r), 7..9 (v)
 };
 
-// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per thread (see k_rollout)
+// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per thread (see k_rollout), and time steps
 template <int MODEL, int NP, bool INST>
 __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, nm = n + m;
@@ -118,7 +119,7 @@ __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
         stage_model_params<INST>(P, b, prm_s[threadIdx.x]);
         prm = prm_s[threadIdx.x];
     }
-    rk4_step<MODEL, D>(model_params<MODEL, INST>(P, prm, k), x, u, P.dt[k], xn);
+    rk4_step<MODEL, D>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k), xn);
 #pragma unroll
     for (int i = 0; i < n; i++) {
         if (NP == 2 && js[1] == js[0] + 1 && !(js[0] & 1)) *reinterpret_cast<double2*>(&AB[i * ld + js[0]]) = make_double2(xn[i].d[0], xn[i].d[1]);
@@ -129,8 +130,9 @@ __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
     }
 }
 
-// the closed-form columns of [A B] (SeedList<MODEL>::trivial): thread = (instance, knot, one of them); run once per problem
-template <int MODEL>
+// the closed-form columns of [A B] (SeedList<MODEL>::trivial): thread = (instance, knot, one of them); run when the problem is created and
+// whenever its time steps change (INST: each instance's own, DevProblem::dtb)
+template <int MODEL, bool INST>
 __global__ void __launch_bounds__(128) k_trivial_columns_full(const DevProblem P) {
     constexpr int n = ModelDims<MODEL>::n, NT = SeedList<MODEL>::ntrivial();
     if constexpr (NT > 0) {
@@ -140,7 +142,7 @@ __global__ void __launch_bounds__(128) k_trivial_columns_full(const DevProblem P
         const long long bk = t / NT;
         const int k = (int)(bk % (P.N - 1));
         double* AB = P.AB + (size_t)bk * n * P.ldab;
-        const double h = P.dt[k];
+        const double h = time_step<INST>(P, (int)(bk / (P.N - 1)), k);
         // x = [r(0..2); q(3..6); v(7..9); omega(10..12)]: d r+/d r = I, d r+/d v = h I, d v+/d v = I
         for (int i = 0; i < n; i++) AB[i * P.ldab + jt] = (i == jt) ? 1.0 : ((jt >= 7 && i == jt - 7) ? h : 0.0);
     }
@@ -148,7 +150,8 @@ __global__ void __launch_bounds__(128) k_trivial_columns_full(const DevProblem P
 cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s) {
     if (P.model == MODEL_QUADROTOR) {
         const long long total = (long long)P.B * (P.N - 1) * SeedList<MODEL_QUADROTOR>::ntrivial();
-        k_trivial_columns_full<MODEL_QUADROTOR><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+        if (inst_dynamics(P)) k_trivial_columns_full<MODEL_QUADROTOR, true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+        else k_trivial_columns_full<MODEL_QUADROTOR, false><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
     }
     return cudaGetLastError();
 }
@@ -199,18 +202,19 @@ __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, con
 // depend on r, and on v only in rdot.  Their columns of the discrete Jacobian are therefore known in closed form -- d x+/d r = e_r and
 // d x+/d v = h e_r + e_v (the RK4 weights sum to one) -- and need no dual-number sweep: 10 seeds (attitude, angular velocity, controls) are
 // pushed through the RK4 step instead of 16, one thread each; the six trivial columns depend on the time steps only.  The materialised P.ABe
-// gets them once, when the problem is created (k_trivial_columns); k_expand_lie_rec writes them into every record block it assembles.
+// gets them when the problem is created and when its time steps change (k_trivial_columns); k_expand_lie_rec writes them into every record
+// block it assembles, and the export of the records (launch_export_abe) carries them to P.ABe on the record path.
 __device__ __forceinline__ int lie_seed(int s) { return (int)((0xFEDCBA9543ULL >> (4 * s)) & 15); }       // 3,4,5,9,10,11,12,13,14,15
 __device__ __forceinline__ int lie_trivial(int s) { return (int)((0x876210ULL >> (4 * s)) & 15); }        // 0,1,2,6,7,8
 
 // column j of [A_e B_e]_k: the RK4 step of knot k pushed through Dual<1> with the seed of error-state coordinate j (attitude: a column of G(q_k)),
-// projected on the error state of knot k + 1 with G(q_{k+1})'  (INST: with the instance's parameters, staged in `prm`)
+// projected on the error state of knot k + 1 with G(q_{k+1})'  (INST: with instance b's parameters, staged in `prm`, and its time step)
 template <int MODEL, bool INST>
-__device__ __forceinline__ void expand_lie_column(const DevProblem& P, const double* prm, int k, int j, const double* __restrict__ X, const double* __restrict__ U,
-                                                  double (&col)[ModelDims<MODEL>::n - 1]) {
+__device__ __forceinline__ void expand_lie_column(const DevProblem& P, const double* prm, int b, int k, int j, const double* __restrict__ X,
+                                                  const double* __restrict__ U, double (&col)[ModelDims<MODEL>::n - 1]) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, qs = 3;
     using D = Dual<1>;
-    const double h = P.dt[k];
+    const double h = time_step<INST>(P, b, k);
     D x[n], u[m], xn[n];
 #pragma unroll
     for (int i = 0; i < n; i++) { x[i].v = X[i]; x[i].d[0] = 0.0; }
@@ -248,7 +252,7 @@ __device__ __forceinline__ void expand_lie_column(const DevProblem& P, const dou
 #ifndef TO_EXPAND_LIE_THREADS
 #define TO_EXPAND_LIE_THREADS 64
 #endif
-// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per thread (see k_rollout)
+// INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per thread (see k_rollout), and time steps
 template <int MODEL, bool INST>
 __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 128 / TO_EXPAND_LIE_THREADS) k_expand_lie(const DevProblem P, int mode) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, nme = ne + m, NS = 10;
@@ -271,7 +275,7 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
         prm = prm_s[threadIdx.x];
     }
     double col[ne];
-    expand_lie_column<MODEL, INST>(P, prm, k, j, X, U, col);
+    expand_lie_column<MODEL, INST>(P, prm, b, k, j, X, U, col);
     double* out = P.ABe + ((size_t)bk * nme + j) * ne;                 // column j of [A_e B_e]: 12 contiguous doubles
 #pragma unroll
     for (int e = 0; e < ne; e++) out[e] = col[e];
@@ -291,7 +295,7 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
 //   image     record order (frag_layout.cuh) with the 16-byte chunks of each 128-byte line permuted by fraglayout::stage_swz: the column
 //             stores of a warp spread over the banks, the line stores read every bank once.
 // tests/test_expand_staging.py restates the staging map and the write-out in NumPy.
-// INST: the instance's own model parameters (DevProblem::mparams), staged in shared memory once per CTA (the CTA's one instance)
+// INST: the instance's own model parameters (DevProblem::mparams), staged in shared memory once per CTA (the CTA's one instance), and time steps
 #define EXPB_KPB 6
 #define EXPB_T 64
 template <int MODEL, bool INST>
@@ -330,11 +334,11 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
             for (int e = 0; e < ne; e++) img[fraglayout::stage_swz(fraglayout::ab_index(e, 12) | cb, kk)] = col[e];
         };
         double col[ne];
-        expand_lie_column<MODEL, INST>(P, prm, k, lie_seed(sd), X, U, col);
+        expand_lie_column<MODEL, INST>(P, prm, b, k, lie_seed(sd), X, U, col);
         put(lie_seed(sd), col);
         if (sd < 6) {                                                                  // closed-form column jt: d x+/d r = I, d r+/d v = h I, d v+/d v = I
             const int jt = lie_trivial(sd);
-            const double h = P.dt[k];
+            const double h = time_step<INST>(P, b, k);
 #pragma unroll
             for (int e = 0; e < ne; e++) col[e] = (e == jt) ? 1.0 : ((jt >= 6 && e == jt - 6) ? h : 0.0);
             put(jt, col);
@@ -357,7 +361,8 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
     }
 }
 
-// the closed-form columns of [A_e B_e] (positions, velocities): thread = (instance, knot, one of the six)
+// the closed-form columns of [A_e B_e] (positions, velocities): thread = (instance, knot, one of the six); INST: each instance's time steps
+template <bool INST>
 __global__ void __launch_bounds__(128) k_trivial_columns(const DevProblem P) {
     constexpr int ne = 12, nme = 16;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -366,13 +371,14 @@ __global__ void __launch_bounds__(128) k_trivial_columns(const DevProblem P) {
     const long long bk = t / 6;
     const int k = (int)(bk % (P.N - 1));
     const int jt = lie_trivial(sd);
-    const double h = P.dt[k];
+    const double h = time_step<INST>(P, (int)(bk / (P.N - 1)), k);
     for (int e = 0; e < ne; e++) P.ABe[((size_t)bk * nme + jt) * ne + e] = (e == jt) ? 1.0 : ((jt >= 6 && e == jt - 6) ? h : 0.0);
 }
 cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s) {
     const long long total = (long long)P.B * (P.N - 1) * 6;
     if (P.frag) return cudaSuccess;       // k_expand_lie_rec writes the whole block, closed-form columns included, every time
-    k_trivial_columns<<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+    if (inst_dynamics(P)) k_trivial_columns<true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+    else k_trivial_columns<false><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }
 
@@ -587,7 +593,7 @@ cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
     return cudaGetLastError();
 }
 
-// the dynamics kernels read nothing per instance but the model parameters: their INST variant runs exactly when the rows exist
+// the dynamics kernels read nothing per instance but the model parameters and the time steps: their INST variant runs exactly when a table exists
 cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s) {
     const int threads = 32, blocks = (P.B + threads - 1) / threads;
     if (inst_dynamics(P)) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true><<<blocks, threads, 0, s>>>(P))); }

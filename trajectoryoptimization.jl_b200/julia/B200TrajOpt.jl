@@ -334,6 +334,20 @@ function model_params(p::BatchedProblem, nparams::Integer)
     check(p.h, ccall((:to_get_model_params, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}), p.h, P))
     P
 end
+# per-instance time steps: column b of dt (N-1, B) is instance b's steps, t0[b] its initial time (nothing: keep the clocks)
+function set_time_steps!(p::BatchedProblem, dt::AbstractMatrix, t0::Union{Nothing,AbstractVector}=nothing)
+    size(dt) == (p.prob.N - 1, p.B) || throw(DimensionMismatch("dt must be (N-1, B)"))
+    t0 === nothing || length(t0) == p.B || throw(DimensionMismatch("t0 must have length B"))
+    check(p.h, ccall((:to_set_time_steps, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}), p.h, Matrix{Float64}(dt),
+                     t0 === nothing ? C_NULL : Vector{Float64}(t0)))
+end
+set_time_steps!(p::BatchedProblem, dt::AbstractVector, t0=nothing) = set_time_steps!(p, repeat(permutedims(Vector{Float64}(dt)), p.prob.N - 1), t0)
+function time_steps(p::BatchedProblem)
+    dt = Matrix{Float64}(undef, p.prob.N - 1, p.B)
+    t0 = Vector{Float64}(undef, p.B)
+    check(p.h, ccall((:to_get_time_steps, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}), p.h, dt, t0))
+    dt, t0
+end
 # per-instance constraint data: column b of D (len, B) is instance b's data of constraint `con` (1-based), in the layout of
 # to_set_constraint_data (Bound z_max | z_min, Linear b, Circle xc | yc | r, Sphere xc | yc | zc | r, Norm val, Collision radius)
 function constraint_data_len(p::BatchedProblem, con::Integer)
