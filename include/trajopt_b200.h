@@ -49,6 +49,10 @@ enum to_model_id {
                                        test/hybrid_dynamics_model.jl): to_spec.dyn, dyn_index, nx, nu */
 };
 
+/* The explicit rule that discretises the dynamics (RobotDynamics' Euler, RK2, RK3, RK4 with zero-order hold on u; `Problem(...; integration)`,
+ * src/problem.jl:32, :119-123).  See to_set_integration. */
+enum to_integration { TO_EULER = 1, TO_RK2 = 2, TO_RK3 = 3, TO_RK4 = 4 };
+
 /* QuadraticCostFunction (src/cost_functions.jl:326-347 DiagonalCost, :417-454 QuadraticCost) */
 /* DiagonalQuatCost / QuatLQRCost (src/lie_costs.jl:33-95, :129-139): a DiagonalCost plus w * min(1 + q_ref'p, 1 - q_ref'p), p = x[q_ind] */
 /* Generic (user-defined) cost: the reference lets users subtype CostFunction and get gradient!/hessian! from ForwardDiff through
@@ -83,7 +87,7 @@ typedef struct {
 } to_cost_spec;
 
 /* One dynamics model of a hybrid problem: `RD.@autodiff struct M <: ContinuousDynamics` + `RD.dynamics(::M, x, u)` recorded as a program
- * (to_expr_op; inputs x[0..n_in), u[0..m_in); the LAST n_out instructions are the outputs), discretised with RK4 like every model of the path,
+ * (to_expr_op; inputs x[0..n_in), u[0..m_in); the LAST n_out instructions are the outputs), discretised with the problem's explicit rule (to_set_integration),
  * or -- `discrete` = 1 -- a jump map x+ = g(x, u) applied as is (n_out may differ from n_in: the state dimension changes there). */
 typedef struct {
     int32_t n_in, m_in, n_out, discrete;
@@ -293,7 +297,17 @@ int to_cost_weights_len(const to_handle* h, int32_t cost, int32_t* len);        
 int to_set_cost_weights(to_handle* h, int32_t cost, const double* w /*[B][len]*/);
 int to_get_cost_weights(to_handle* h, int32_t cost, double* w /*[B][len]*/);                       /* the shared values broadcast when none are set */
 
-/* ---- kernel 1: batched RK4 rollout (+ dual-number Jacobians) ---------------------------------------- */
+/* ---- integrator ------------------------------------------------------------------------------------------------
+ * The explicit rule every kernel that steps the dynamics uses (rollout, dynamics expansion, line search): TO_EULER x+ = x + h f(x,u);
+ * TO_RK2 (explicit midpoint); TO_RK3 (Kutta); TO_RK4, the default until the first call.  Each k_i is scaled by h before it is used, as
+ * RobotDynamics does.  One rule holds for the whole batch; in a hybrid problem it applies to every continuous model and a discrete jump map
+ * is still applied as it is.  The Jacobians, expansions and gains computed before the call are stale afterwards, as after to_set_time_steps;
+ * X is not rolled out again.  TO_EINVAL, naming the code, with nothing changed: any other code (the implicit rules, ImplicitMidpoint and
+ * HermiteSimpson, included: iLQR's rollout needs an explicit step). */
+int to_set_integration(to_handle* h, int32_t rule);
+int to_get_integration(const to_handle* h, int32_t* rule);
+
+/* ---- kernel 1: batched rollout (+ dual-number Jacobians) ------------------------------------------------- */
 int to_rollout(to_handle* h);                                                 /* rollout!           src/problem.jl:330-340 */
 int to_expand(to_handle* h);                                                  /* RD.jacobian!(ForwardAD) on the discretized dynamics at every knot */
 int to_get_dynamics_jacobians(to_handle* h, double* AB /*[B][N-1][n+m][n]: n x (n+m) col-major*/);

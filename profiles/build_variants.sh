@@ -13,6 +13,7 @@ done
 wait
 for o in _build/variants/riccati_*.o; do
   name=$(basename $o .o); name=${name#riccati_}
-  /usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -shared -ccbin /usr/bin/g++ -o ../variants/lib_$name.so _build/capi.o _build/rollout.o _build/sweep.o $o _build/riccati_small.o _build/lie.o _build/riccati_frag.o _build/forward.o _build/solve.o
+  /usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -shared -ccbin /usr/bin/g++ -o ../variants/lib_$name.so _build/capi.o _build/rollout.o _build/sweep.o $o _build/riccati_small.o _build/lie.o _build/riccati_frag.o _build/forward.o _build/solve.o \
+      _build/forward_r[0-9].o _build/rollout_r[0-9].o
   echo "$name: $(grep -A2 'k_riccatiILi13ELi4ELi2ELb1ELb1ELi' _build/variants/riccati_$name.log | grep -E 'Used|spill' | tr '\n' ' ')"
 done

@@ -182,6 +182,7 @@ def load_library():
         "to_get_goal_values": [H, C.c_int32, c_double_p], "to_set_goal_values": [H, C.c_int32, c_double_p],
         "to_set_model_params": [H, c_double_p, C.c_int32], "to_get_model_params": [H, c_double_p],
         "to_set_time_steps": [H, c_double_p, c_double_p], "to_get_time_steps": [H, c_double_p, c_double_p],
+        "to_set_integration": [H, C.c_int32], "to_get_integration": [H, c_int32_p],
         "to_constraint_data_len": [H, C.c_int32, C.POINTER(C.c_int32)], "to_set_constraint_data": [H, C.c_int32, c_double_p],
         "to_get_constraint_data": [H, C.c_int32, c_double_p],
         "to_cost_weights_len": [H, C.c_int32, C.POINTER(C.c_int32)], "to_set_cost_weights": [H, C.c_int32, c_double_p],
@@ -228,7 +229,7 @@ EXPORTED_SYMBOLS = [
     "to_hess_projection", "to_backward", "to_forward", "to_ilqr_step", "to_al_update", "to_get_gains", "to_get_multipliers",
     "to_set_multipliers", "to_get_penalty", "to_set_penalty", "to_set_penalties", "to_get_penalties", "to_get_solver_state", "to_reduce_merit", "to_reduce_merit_async", "to_merit_device_ptr", "to_update_trajectory", "to_shift_trajectory",
     "to_set_goal_states", "to_update_trajectories", "to_get_cost_terms", "to_set_cost_terms", "to_get_goal_values", "to_set_goal_values",
-    "to_set_model_params", "to_get_model_params", "to_set_time_steps", "to_get_time_steps", "to_constraint_data_len", "to_set_constraint_data", "to_get_constraint_data",
+    "to_set_model_params", "to_get_model_params", "to_set_time_steps", "to_get_time_steps", "to_set_integration", "to_get_integration", "to_constraint_data_len", "to_set_constraint_data", "to_get_constraint_data",
     "to_cost_weights_len", "to_set_cost_weights", "to_get_cost_weights",
     "to_set_phase_timing", "to_get_phase_times", "to_launch_count", "to_algorithmic_bytes",
     "to_backward_algebra", "to_kernel_choice", "to_error_state_dim", "to_state_diff", "to_get_error_dynamics", "to_error_expansion",

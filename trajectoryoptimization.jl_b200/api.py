@@ -178,8 +178,8 @@ class Acrobot(_Model):
 
 class AutodiffDynamics(_Model):
     """A user-defined dynamics model: the counterpart of ``RD.@autodiff struct M <: RD.ContinuousDynamics end`` + ``RD.state_dim`` /
-    ``RD.control_dim`` / ``RD.output_dim`` + ``RD.dynamics(::M, x, u)`` (test/hybrid_dynamics_model.jl:14-39), discretised with RK4 like every
-    model of the path (``RD.DiscretizedDynamics{RD.RK4}``).  ``fun(x, u)`` is called once with recording vectors (see ``Expr``) and returns
+    ``RD.control_dim`` / ``RD.output_dim`` + ``RD.dynamics(::M, x, u)`` (test/hybrid_dynamics_model.jl:14-39), discretised with the problem's
+    explicit rule like every model of the path (``RD.DiscretizedDynamics{RD.RK4}`` by default, see ``Problem(..., integration)``).  ``fun(x, u)`` is called once with recording vectors (see ``Expr``) and returns
     the ``output_dim`` entries of ``xdot``.  ``discrete=True``: ``fun`` is a jump map ``x+ = g(x, u)`` applied as is -- its output dimension
     may differ from its state dimension, which is how the state dimension changes along a hybrid trajectory.  Used through
     ``Problem([model_1, ..., model_{N-1}], obj, x0, tf)`` (src/problem.jl:36-73), or on its own as ``Problem(model, obj, x0, tf)``, which is
@@ -1022,17 +1022,75 @@ def num_constraints(cons_or_prob):
 # Problem (reference src/problem.jl)
 
 
-class Problem:
-    """``Problem(model, obj, x0, tf; xf, constraints, t0, X0, U0, dt)`` (src/problem.jl:79-123) for a batch.
+class _Integration:
+    """An explicit rule of RobotDynamics (``RD.Euler``, ``RD.RK2``, ``RD.RK3``, ``RD.RK4``) with zero-order hold on ``u``:
+    ``Problem(...; integration = RK3)`` or ``RK3(model)``, as the reference writes ``integration = RD.RK3(model)``."""
+    code = 0
 
-    ``x0`` is ``[n]`` (shared) or ``[B, n]``; ``batch`` gives ``B`` when ``x0`` is shared.  The integrator is RK4
-    (the reference's default, src/problem.jl:119-123).  States start as NaN and controls as zeros like the
+    def __init__(self, model=None):   # RD.RK4(model): the model is not needed to step it
+        pass
+
+    def __eq__(self, other):
+        return type(self) is type(other)
+
+    def __hash__(self):
+        return self.code
+
+    def __repr__(self):
+        return f"{type(self).__name__}()"
+
+
+class Euler(_Integration):
+    """``x+ = x + h f(x, u)``: one dynamics evaluation per knot"""
+    code = 1
+
+
+class RK2(_Integration):
+    """explicit midpoint: ``k1 = h f(x, u); k2 = h f(x + k1/2, u); x+ = x + k2``"""
+    code = 2
+
+
+class RK3(_Integration):
+    """Kutta's rule: ``k3 = h f(x - k1 + 2 k2, u); x+ = x + (k1 + 4 k2 + k3)/6``"""
+    code = 3
+
+
+class RK4(_Integration):
+    """the classical rule, the reference's default (src/problem.jl:119-123)"""
+    code = 4
+
+
+_INTEGRATIONS = {c.__name__: c for c in (Euler, RK2, RK3, RK4)}
+_RULE_OF_CODE = {c.code: c for c in _INTEGRATIONS.values()}
+
+
+def _integration_code(rule):
+    """the to_integration code of ``rule``: one of the rule types, an instance of one, or its name"""
+    if isinstance(rule, str):
+        cls = _INTEGRATIONS.get(rule)
+    elif isinstance(rule, type):
+        cls = rule if rule in _INTEGRATIONS.values() else None
+    else:
+        cls = type(rule) if type(rule) in _INTEGRATIONS.values() else None
+    if cls is None:
+        name = rule if isinstance(rule, str) else getattr(rule, "__name__", type(rule).__name__)
+        raise ArgumentError(f"unknown integration rule {name!r}: the explicit rules Euler, RK2, RK3 and RK4 are supported (iLQR's rollout "
+                            "needs an explicit step, so ImplicitMidpoint and HermiteSimpson are not)")
+    return cls.code
+
+
+class Problem:
+    """``Problem(model, obj, x0, tf; xf, constraints, t0, X0, U0, dt, integration)`` (src/problem.jl:79-123) for a batch.
+
+    ``x0`` is ``[n]`` (shared) or ``[B, n]``; ``batch`` gives ``B`` when ``x0`` is shared.  ``integration`` is the explicit rule that
+    discretises the dynamics: ``Euler``, ``RK2``, ``RK3`` or ``RK4`` (the reference's default, src/problem.jl:119-123), as a rule type, an
+    instance or its name; in a hybrid problem it applies to every continuous model.  States start as NaN and controls as zeros like the
     reference (src/problem.jl:83-84).  ``error_state=True`` makes the solver kernels (backward / forward pass) work on the
     Lie-group error state of the model (``RD.errstate_dim(model)`` dimensions, Quadrotor: 12) as Altro does for ``LieGroupModel``s.
     """
 
     def __init__(self, model, obj, *args, xf=None, constraints=None, t0=0.0, X0=None, U0=None, dt=None, batch=None, device=0,
-                 error_state=False, **kwargs):
+                 error_state=False, integration=RK4, **kwargs):
         if "x0" in kwargs:   # src/problem.jl:87-91
             raise ArgumentError("Cannot pass x0 as a keyword argument. It is now a positional argument, and xf is a keyword argument.")
         if kwargs:
@@ -1040,6 +1098,7 @@ class Problem:
         if len(args) != 2:
             raise ArgumentError("Problem(model, obj, x0, tf; xf, constraints, ...) takes x0 and tf positionally")
         x0, tf = args
+        self._integration = _integration_code(integration)
         N = len(obj)
         x0 = np.asarray(x0, dtype=float)
         if isinstance(model, AutodiffDynamics):
@@ -1113,6 +1172,7 @@ class Problem:
         self._dt = np.array(dtv, dtype=float)        # the time steps as given: a rebuild must not re-derive them from the knot times
         self.spec = self._make_spec(dtv, t0)
         self._open()
+        self._apply_integration()
         self._sig = self._signature()
         self._call("to_set_initial_state", K._dp(self.x0))
         if U0 is not None:
@@ -1167,6 +1227,11 @@ class Problem:
         self._h = C.c_void_p()
         rc = self._lib.to_create(C.byref(self.spec.c), C.byref(self._h))
         K.check(self._lib, None, rc)
+
+    def _apply_integration(self):
+        """the handle steps with the problem's rule; a new handle starts with RK4"""
+        if self._integration != RK4.code:
+            self._raw_call("to_set_integration", self._integration)
 
     def _signature(self):
         """what the device-side tables were built from: the cost object of every knot, the constraint list, and the version counters the
@@ -1224,6 +1289,7 @@ class Problem:
         self.close()
         self.spec = self._make_spec(self._dt, float(t[0]))
         self._open()
+        self._apply_integration()
         self._sig = self._signature()
         for j, c in enumerate(self._cost_objs):
             if id(c) in cw_carry:
@@ -1324,18 +1390,34 @@ def initial_trajectory(prob, X0, U0):   # initial_trajectory!(prob, Z0)  src/pro
 def copy_problem(prob, cls=None, **overrides):
     """``copy(prob)`` / ``Problem(p; model, obj, constraints, x0, xf, t0, tf)`` (src/problem.jl:125-128, :342-345): a new batch with copies of
     the objective and the constraint list (the constraint objects themselves are shared, as ``copy(::ConstraintList)`` does), the same x0, xf,
-    time grid and the current trajectory."""
+    time grid, integration rule and the current trajectory."""
     t = gettimes(prob)
     obj = overrides.pop("obj", prob.obj.copy())
     cons = overrides.pop("constraints", prob.constraints.copy())
     new = (cls or type(prob))(overrides.pop("model", prob.model), obj, overrides.pop("x0", prob.x0.copy()), float(t[-1]),
                               xf=overrides.pop("xf", prob.xf.copy()), constraints=cons, t0=float(t[0]), dt=np.diff(t),
-                              error_state=prob.error_state, **overrides)
+                              error_state=prob.error_state, integration=overrides.pop("integration", _RULE_OF_CODE[prob._integration]), **overrides)
     X, U = states(prob), controls(prob)
     if np.all(np.isfinite(X)):
         initial_states(new, X)
     initial_controls(new, U)
     return new
+
+
+def integration(prob):
+    """``RD.integration(prob.model[1])``: the explicit rule the problem's dynamics are discretised with, an instance of ``Euler``, ``RK2``,
+    ``RK3`` or ``RK4`` (``isinstance(integration(prob), RK3)`` reads as the reference's ``isa RD.RK3``)."""
+    code = np.zeros(1, dtype=np.int32)
+    prob._call("to_get_integration", code.ctypes.data_as(C.POINTER(C.c_int32)))
+    return _RULE_OF_CODE[int(code[0])]()
+
+
+def set_integration(prob, rule):
+    """Discretise the dynamics with ``rule`` from now on (``Euler``, ``RK2``, ``RK3`` or ``RK4``, as in ``Problem(..., integration)``).  The
+    trajectory is not rolled out again; the Jacobians, expansions and gains of the old rule are stale."""
+    code = _integration_code(rule)
+    prob._call("to_set_integration", code)
+    prob._integration = code
 
 
 def horizonlength(prob):

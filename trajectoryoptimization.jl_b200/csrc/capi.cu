@@ -608,6 +608,7 @@ int to_create(const to_spec* s, to_handle** out) {
     }
     DevProblem& P = h->P;
     P.model = s->model; P.n = mn; P.m = mm; P.N = s->N; P.B = s->B;
+    P.integration = TO_RK4;                     // the reference's default (src/problem.jl:119-123)
     // row stride of [A B]: even (16-byte rows); 20 (= 4 mod 16) for the tensor-MMA Riccati path (n >= 8), see riccati.cu
     P.ldab = (mn >= 8 && mn <= 16 && mn + mm + 1 <= 20) ? 20 : ((mn + mm + 1) & ~1);
     std::memcpy(P.params, params, sizeof(params));
@@ -1278,6 +1279,24 @@ int to_get_time_steps(to_handle* h, double* dt, double* t0) {
         std::memcpy(dt + (size_t)b * K, h->P.dtb ? h->h_dtb.data() + (size_t)b * K : h->h_dt.data(), sizeof(double) * K);
         if (t0) t0[b] = h->P.dtb ? h->t0b[b] : h->t0;
     }
+    return TO_OK;
+}
+
+// ---- integrator (DevProblem::integration) ------------------------------------------------------------------
+// Problem(...; integration = rule): the explicit rule every dynamics-stepping kernel dispatches on.  What was computed with the old rule (the
+// Jacobians, expansions, gains, the merit) is stale, as after to_set_time_steps; the closed-form Jacobian columns hold for every rule.
+int to_set_integration(to_handle* h, int32_t rule) {
+    JOIN(h);
+    if (!h) return TO_EINVAL;
+    if (rule < TO_EULER || rule > TO_RK4)
+        return fail(h, TO_EINVAL, "to_set_integration: unknown integration rule " + std::to_string(rule) + " (explicit rules: 1 Euler, 2 RK2, 3 RK3, 4 RK4)");
+    h->P.integration = rule;
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return TO_OK;
+}
+int to_get_integration(const to_handle* h, int32_t* rule) {
+    if (!h || !rule) return TO_EINVAL;
+    *rule = h->P.integration;
     return TO_OK;
 }
 

@@ -28,6 +28,7 @@
 // reference enums (mirrors include/trajopt_b200.h)
 enum { MODEL_DOUBLE_INTEGRATOR = 0, MODEL_CARTPOLE = 1, MODEL_QUADROTOR = 2, MODEL_ACROBOT = 3, MODEL_EXPR = 4 };
 enum { CONE_ZERO = 0, CONE_NEGATIVE_ORTHANT = 1, CONE_SECOND_ORDER = 2, CONE_IDENTITY = 3, CONE_POSITIVE_ORTHANT = 4 };
+enum { RULE_EULER = 1, RULE_RK2 = 2, RULE_RK3 = 3, RULE_RK4 = 4 };   // to_integration
 enum { CON_GOAL = 0, CON_BOUND = 1, CON_LINEAR = 2, CON_CIRCLE = 3, CON_SPHERE = 4, CON_NORM = 5, CON_COLLISION = 6, CON_QUATVEC = 7, CON_EXPR = 8 };
 
 // QuadraticCostFunction (reference src/cost_functions.jl:326-347, :417-454); dense storage + diagonal copy
@@ -87,7 +88,7 @@ struct ExpTab {
     int con[TO_EXP_MAXT][TO_MAXNM];         // the term's constraint (its penalty in an instance's row of DevProblem::mub); -1: no term
 };
 
-// one dynamics model of a hybrid problem (to_dynamics_spec): a recorded program, RK4-discretised or a discrete jump map
+// one dynamics model of a hybrid problem (to_dynamics_spec): a recorded program, discretised with the problem's rule, or a discrete jump map
 struct DevDyn {
     int n_in, m_in, n_out, discrete;
     int prog_len, pad[3];
@@ -170,6 +171,9 @@ struct DevProblem {
     // knot, at most one Bound with finite limits on every control and none on the state, on every stage knot, and at most one Goal, on the
     // terminal knot only.  Set at to_create (the structure of the costs and constraints never changes afterwards).
     int fwd_compact;
+    // The explicit rule of the discretised dynamics (to_set_integration): TO_EULER .. TO_RK4, TO_RK4 from to_create.  The launchers of every
+    // kernel that steps the dynamics dispatch on it (models.cuh TO_DISPATCH_RULE); it fills the padding in front of the next pointer.
+    int integration;
     // Per-instance model parameters (to_set_model_params): [B][TO_NPARAM] in the layout of `params`, the host-computed reciprocals included.
     // nullptr until the first per-instance call; every kernel then reads the shared `params`.
     const double* mparams;

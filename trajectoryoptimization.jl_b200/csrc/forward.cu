@@ -1,18 +1,18 @@
 #include <cstdlib>
 #include <type_traits>
-// forward.cu -- the forward pass of iLQR: closed-loop RK4 rollout fused with the cost + constraint + AL-penalty
+// forward.cu -- the forward pass of iLQR: closed-loop rollout fused with the cost + constraint + AL-penalty
 // sweep (kernel 1 without partials + kernel 2), and the per-instance backtracking line search.
 //
 // What it computes (Altro.jl forwardpass! / rollout!(solver, alpha), restated in oracle/oracle.hpp
 // `forward_rollout` / `forward_pass`; it drives the reference's rollout (src/problem.jl:334-340), cost
 // (src/objective.jl:89-106) and constraint evaluation (src/abstract_constraint.jl:200-225)):
-//     dx = xbar_k - x_k ; ubar_k = u_k + K_k dx + alpha d_k ; xbar_{k+1} = RK4(xbar_k, ubar_k)
+//     dx = xbar_k - x_k ; ubar_k = u_k + K_k dx + alpha d_k ; xbar_{k+1} = step(xbar_k, ubar_k)  (the problem's explicit rule, models.cuh)
 //     J(alpha) = sum_k l_k(xbar_k, ubar_k) + AL penalty ;  z = (J_prev - J) / -(alpha (dV1 + alpha dV2))
 //     accept the first alpha in 1, 1/2, ..., 2^-ls_iters with  lower < z <= upper  or  J < J_prev.
 // The line search is per instance (no communication, SURVEY.md 8e).
 //
 // Mapping.  The recursion is serial in k and one rollout has no parallelism worth a warp, so the kernel is
-// bound by the LATENCY of the per-knot dependency chain (feedback -> 4 dynamics evaluations -> next knot).  Two
+// bound by the LATENCY of the per-knot dependency chain (feedback -> 1 to 4 dynamics evaluations, by rule -> next knot).  Two
 // things follow:
 //   * backtracking trials are evaluated CONCURRENTLY: a group of G lanes owns one instance and lane j rolls out
 //     step size 2^-(trial0+j), writing its candidate into trajectory buffer (cur+1+j) % NBUF.  A ballot picks the
@@ -27,6 +27,12 @@
 #include "kernels.h"
 #include "models.cuh"
 #include "ptx.cuh"
+
+// The explicit rule this object instantiates the line search for (rollout.cu explains the one object per rule); the object of rule 4 (RK4)
+// also holds the host functions that do not depend on it and the launchers that dispatch on DevProblem::integration.
+#ifndef TO_RULE
+#define TO_RULE 4
+#endif
 
 namespace {
 
@@ -228,7 +234,7 @@ __device__ __forceinline__ void prefetch_knot(double* base, int g, int l, int k,
 // The candidate trajectory goes to buffer `cbuf`.  Returns the merit; `ok` = no blow-up.
 // INST: the instance's own linear cost terms and Goal values (DevProblem::qr / goal, read from global memory instead of the CTA's table), and
 // time steps (DevProblem::dtb, loaded per knot instead of the table's).
-template <int MODEL, int IPB, int G, bool LIE, bool INST>
+template <int MODEL, int IPB, int G, bool LIE, bool INST, int RULE>
 __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab& tab, double* stage, const double* prm, int b, int g, int l,
                                                unsigned gmask, double alpha, int cbuf, bool& ok, double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
@@ -382,7 +388,7 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
             }
         }
         if (!last) {
-            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), xn);
+            explicit_step<MODEL, double, RULE>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), xn);
 #pragma unroll
             for (int i = 0; i < n; i++) { x[i] = xn[i]; if (!(fabs(xn[i]) <= P.opt.max_state_value)) ok = false; }
             // a blown-up trial keeps integrating (the group stays in lock step); its result is rejected through `ok`
@@ -401,11 +407,11 @@ __device__ __forceinline__ double rollout_fast(const DevProblem& P, const FwdTab
 //     write each lane's runs together, G consecutive doubles per store instruction.  One lane storing its own 8-byte words sent one L2 write
 //     request per word from every lane, and those requests, not the arithmetic, set the pace of the pass (a timing-only build without the
 //     candidate stores ran pass 1 in about half the time);
-//   * RK4 writes the next state over the current one (rk4_step reads x_i for the last time where it writes xn_i), so the loop carries
+//   * the step writes the next state over the current one (every rule of explicit_step reads x_i for the last time where it writes xn_i), so the loop carries
 //     no x <- xn copies.  (Unrolled by two with x / xn swapping roles instead, the loop took 40 more registers and spilled.)
 // INST: gbox = the instance's control box {u_max_i, u_min_i} and gcost = its two costs and penalties, staged for the group by linesearch_pass;
 // its time steps are loaded per knot (time_step)
-template <int MODEL, int IPB, int G, bool LIE, bool INST>
+template <int MODEL, int IPB, int G, bool LIE, bool INST, int RULE>
 __device__ __forceinline__ double rollout_compact(const DevProblem& P, const FwdCompactTab& tab, double* stage, double* ost, const double* prm,
                                                   const double2* gbox, const FwdCompactCost* gcost, int b, int g, int l, unsigned gmask,
                                                   double alpha, int cbuf, bool& ok, double& viol) {
@@ -541,11 +547,11 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
         }
         if constexpr (MODEL == MODEL_EXPR_42) {   // a discrete jump map writes its outputs while it reads its inputs
             double xn[n];
-            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), xn);
+            explicit_step<MODEL, double, RULE>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), xn);
 #pragma unroll
             for (int i = 0; i < n; i++) x[i] = xn[i];
         } else {
-            rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), x);
+            explicit_step<MODEL, double, RULE>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), x);
         }
 #pragma unroll
         for (int i = 0; i < n; i++) if (!(fabs(x[i]) <= P.opt.max_state_value)) ok = false;
@@ -585,7 +591,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
 }
 
 // generic path (dense costs or general constraints): pointer-based evaluation, operands read directly from global
-template <int MODEL, bool LIE, bool INST>
+template <int MODEL, bool LIE, bool INST, int RULE>
 __device__ __forceinline__ double rollout_generic(const DevProblem& P, const double* prm, int b, double alpha, int cbuf, bool& ok, double& viol) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     const int N = P.N, buf = P.cur[b];
@@ -633,7 +639,7 @@ __device__ __forceinline__ double rollout_generic(const DevProblem& P, const dou
         J += al_knot_penalty<INST>(P, k + 1, x, u, lam_b, viol, b);
         if (!last) {
             // INST: the determinant form the shared kernel compiles to, written out (models.cuh det_sub_square)
-            rk4_step<MODEL, double, INST>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k), xn);
+            explicit_step<MODEL, double, RULE, INST>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k), xn);
 #pragma unroll
             for (int i = 0; i < n; i++) { x[i] = xn[i]; if (!(fabs(xn[i]) <= P.opt.max_state_value)) ok = false; }
             if (!ok) break;
@@ -671,7 +677,7 @@ __host__ __device__ constexpr size_t ls_smem_bytes() {
 
 // One line-search pass: lane l of group g evaluates trial (trial0 + l) of instance b.
 //   first_pass : ignore / reset accepted[b];   final_pass : commit failures (no acceptable step size).
-template <int MODEL, int G, int PATH, int LANES, bool LIE, bool INST>
+template <int MODEL, int G, int PATH, int LANES, bool LIE, bool INST, int RULE>
 __device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, NE = LIE ? n - 1 : n;
     constexpr bool FAST = PATH != FWD_GENERIC;
@@ -732,10 +738,10 @@ __device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0,
         }
         if constexpr (PATH == FWD_COMPACT) {
             double* ost = stage + FWD_STAGES * S::DOUBLES + (size_t)g * G * FWD_OKNOTS * (n + m);
-            J = rollout_compact<MODEL, IPB, G, LIE, INST>(P, *tab, stage, ost, prm, gbox, gcost, b, g, l, gmask, alpha, cbuf, ok, viol);
+            J = rollout_compact<MODEL, IPB, G, LIE, INST, RULE>(P, *tab, stage, ost, prm, gbox, gcost, b, g, l, gmask, alpha, cbuf, ok, viol);
         }
-        else if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST>(P, *tab, stage, prm, b, g, l, gmask, alpha, cbuf, ok, viol);
-        else J = rollout_generic<MODEL, LIE, INST>(P, prm, b, alpha, cbuf, ok, viol);
+        else if (FAST) J = rollout_fast<MODEL, IPB, G, LIE, INST, RULE>(P, *tab, stage, prm, b, g, l, gmask, alpha, cbuf, ok, viol);
+        else J = rollout_generic<MODEL, LIE, INST, RULE>(P, prm, b, alpha, cbuf, ok, viol);
         const bool good = (trial <= P.opt.ls_iters) && ls_accept(P, J, P.J[b], alpha, P.dV[2 * b], P.dV[2 * b + 1], ok);
         const unsigned votes = __ballot_sync(gmask, good) & gmask;
         if (votes) {
@@ -764,17 +770,17 @@ __device__ __forceinline__ void linesearch_pass(const DevProblem& P, int trial0,
     (void)sizeof(S);
 }
 
-template <int MODEL, int G, bool FAST, int LANES, bool LIE, bool INST>
+template <int MODEL, int G, bool FAST, int LANES, bool LIE, bool INST, int RULE>
 __global__ void __launch_bounds__(FWD_THREADS) k_linesearch(const DevProblem P, int trial0, int first_pass, int final_pass) {
-    linesearch_pass<MODEL, G, FAST ? FWD_FAST : FWD_GENERIC, LANES, LIE, INST>(P, trial0, first_pass, final_pass);
+    linesearch_pass<MODEL, G, FAST ? FWD_FAST : FWD_GENERIC, LANES, LIE, INST, RULE>(P, trial0, first_pass, final_pass);
 }
 
-template <int MODEL, int G, int LANES, bool LIE, bool INST>
+template <int MODEL, int G, int LANES, bool LIE, bool INST, int RULE>
 __global__ void __launch_bounds__(FWD_THREADS) k_linesearch_compact(const DevProblem P, int trial0, int first_pass, int final_pass) {
-    linesearch_pass<MODEL, G, FWD_COMPACT, LANES, LIE, INST>(P, trial0, first_pass, final_pass);
+    linesearch_pass<MODEL, G, FWD_COMPACT, LANES, LIE, INST, RULE>(P, trial0, first_pass, final_pass);
 }
 
-template <int MODEL, int G, int PATH, int LANES, bool LIE = false, bool INST = false>
+template <int MODEL, int G, int PATH, int LANES, bool LIE, bool INST, int RULE>
 cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     constexpr int IPB = LANES / G;
     const int blocks = (P.B + IPB - 1) / IPB;
@@ -782,8 +788,8 @@ cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int f
     const size_t smem = ls_smem_bytes<MODEL, G, PATH, LANES, LIE>() + (INST ? (size_t)IPB * TO_NPARAM * sizeof(double) : 0)
                       + (INST && PATH == FWD_COMPACT ? (size_t)IPB * (TO_MAXM * sizeof(double2) + sizeof(FwdCompactCost)) : 0);
     auto kern = [] {
-        if constexpr (PATH == FWD_COMPACT) return k_linesearch_compact<MODEL, G, LANES, LIE, INST>;
-        else return k_linesearch<MODEL, G, PATH == FWD_FAST, LANES, LIE, INST>;
+        if constexpr (PATH == FWD_COMPACT) return k_linesearch_compact<MODEL, G, LANES, LIE, INST, RULE>;
+        else return k_linesearch<MODEL, G, PATH == FWD_FAST, LANES, LIE, INST, RULE>;
     }();
     static bool configured[TO_MAXDEV] = {false};
     const int dev = current_device_slot();
@@ -796,42 +802,68 @@ cudaError_t launch_pass_l(const DevProblem& P, int trial0, int first_pass, int f
     return cudaGetLastError();
 }
 
-template <int MODEL, int G, int PATH, bool INST>
+template <int MODEL, int G, int PATH, bool INST, int RULE>
 cudaError_t launch_pass_i(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     // lanes of each warp that carry groups: 16 for the first pass (half-warp FP64 instructions take one pipe pass); the later passes
     // use 16 when they walk the compact late list (two-instance CTAs, see to_create) and 32 when they scan all instances.
     const int lanes = first_pass ? 16 : (P.late_list ? 16 : 32);
     if constexpr (MODEL == MODEL_QUADROTOR) {   // Lie-group error state: dx = state_diff(xbar, x), gains m x (n - 1)
         if (P.lie) {
-            if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, PATH, (G <= 16 ? 16 : 32), true, INST>(P, trial0, first_pass, final_pass, s);
-            return launch_pass_l<MODEL, G, PATH, 32, true, INST>(P, trial0, first_pass, final_pass, s);
+            if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, PATH, (G <= 16 ? 16 : 32), true, INST, RULE>(P, trial0, first_pass, final_pass, s);
+            return launch_pass_l<MODEL, G, PATH, 32, true, INST, RULE>(P, trial0, first_pass, final_pass, s);
         }
     }
-    if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, PATH, (G <= 16 ? 16 : 32), false, INST>(P, trial0, first_pass, final_pass, s);
-    return launch_pass_l<MODEL, G, PATH, 32, false, INST>(P, trial0, first_pass, final_pass, s);
+    if (G <= 16 && lanes == 16) return launch_pass_l<MODEL, G, PATH, (G <= 16 ? 16 : 32), false, INST, RULE>(P, trial0, first_pass, final_pass, s);
+    return launch_pass_l<MODEL, G, PATH, 32, false, INST, RULE>(P, trial0, first_pass, final_pass, s);
 }
 
 // per-instance cost weights / linear cost terms / model parameters / constraint data / penalties / time steps: a kernel variant of its own, so
 // that the shared one is the code it has always been.  It serves every per-instance table; each accessor checks its own (cost_data,
 // model_param, con_data, penalty, time_step).
-template <int MODEL, int G, int PATH>
+template <int MODEL, int G, int PATH, int RULE>
 cudaError_t launch_pass(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
-    if (inst_forward(P)) return launch_pass_i<MODEL, G, PATH, true>(P, trial0, first_pass, final_pass, s);
-    return launch_pass_i<MODEL, G, PATH, false>(P, trial0, first_pass, final_pass, s);
+    if (inst_forward(P)) return launch_pass_i<MODEL, G, PATH, true, RULE>(P, trial0, first_pass, final_pass, s);
+    return launch_pass_i<MODEL, G, PATH, false, RULE>(P, trial0, first_pass, final_pass, s);
 }
 
 static_assert(FWD_GENERIC == KC_LS_GENERIC && FWD_FAST == KC_LS_FAST && FWD_COMPACT == KC_LS_COMPACT, "kernels.h KC_LS_*");
 
-template <int MODEL, int G>
+template <int MODEL, int G, int RULE>
 cudaError_t launch_any(const DevProblem& P, int trial0, int first_pass, int final_pass, cudaStream_t s) {
     const int path = linesearch_path(P);
-    if constexpr (TO_FWD_COMPACT) { if (path == FWD_COMPACT) return launch_pass<MODEL, G, FWD_COMPACT>(P, trial0, first_pass, final_pass, s); }
-    if (path == FWD_FAST) return launch_pass<MODEL, G, FWD_FAST>(P, trial0, first_pass, final_pass, s);
-    return launch_pass<MODEL, G, FWD_GENERIC>(P, trial0, first_pass, final_pass, s);
+    if constexpr (TO_FWD_COMPACT) { if (path == FWD_COMPACT) return launch_pass<MODEL, G, FWD_COMPACT, RULE>(P, trial0, first_pass, final_pass, s); }
+    if (path == FWD_FAST) return launch_pass<MODEL, G, FWD_FAST, RULE>(P, trial0, first_pass, final_pass, s);
+    return launch_pass<MODEL, G, FWD_GENERIC, RULE>(P, trial0, first_pass, final_pass, s);
 }
 
 }  // namespace
 
+// pass 1: trials 0..3 (alpha = 1, 1/2, 1/4, 1/8), 4 lanes per instance.
+// (The alternative, the whole ladder in one 16-lane pass, computes 11x the FLOPs, and its uncoalesced candidate stores load the LSU.)
+template <int RULE>
+cudaError_t launch_forward_rule(const DevProblem& P, cudaStream_t s) {
+    cudaError_t e = cudaErrorNotSupported;
+    const int final_pass = P.opt.ls_iters < 4;
+    if (P.late_list) { e = cudaMemsetAsync(P.late_count, 0, sizeof(int), s); if (e != cudaSuccess) return e; e = cudaErrorNotSupported; }
+    TO_DISPATCH_MODEL(P.model, P.m, (e = launch_any<MODEL, 4, RULE>(P, 0, 1, final_pass, s)));
+    return e;
+}
+
+// pass 2 (+3 when ls_iters > 11): the remaining trials, 8 lanes per instance; commits failures
+template <int RULE>
+cudaError_t launch_ladder_rule(const DevProblem& P, cudaStream_t s) {
+    cudaError_t e = cudaSuccess;
+    for (int trial0 = 4; trial0 <= P.opt.ls_iters && e == cudaSuccess; trial0 += 8) {
+        const int final_pass = trial0 + 8 > P.opt.ls_iters;
+        TO_DISPATCH_MODEL(P.model, P.m, (e = launch_any<MODEL, 8, RULE>(P, trial0, 0, final_pass, s)));
+    }
+    return e;
+}
+
+template cudaError_t launch_forward_rule<TO_RULE>(const DevProblem&, cudaStream_t);
+template cudaError_t launch_ladder_rule<TO_RULE>(const DevProblem&, cudaStream_t);
+
+#if TO_RULE == 4
 // load_tables makes the same test on the device
 bool linesearch_costs_cached(const DevProblem& P) { return P.ncost <= FWD_MAX_COST; }
 
@@ -843,24 +875,17 @@ int linesearch_path(const DevProblem& P) {
     return fast ? FWD_FAST : FWD_GENERIC;
 }
 
-// pass 1: trials 0..3 (alpha = 1, 1/2, 1/4, 1/8), 4 lanes per instance.
-// (The alternative, the whole ladder in one 16-lane pass, computes 11x the FLOPs, and its uncoalesced candidate stores load the LSU.)
 cudaError_t launch_forward(const DevProblem& P, cudaStream_t s) {
     cudaError_t e = cudaErrorNotSupported;
-    const int final_pass = P.opt.ls_iters < 4;
-    if (P.late_list) { e = cudaMemsetAsync(P.late_count, 0, sizeof(int), s); if (e != cudaSuccess) return e; e = cudaErrorNotSupported; }
-    TO_DISPATCH_MODEL(P.model, P.m, (e = launch_any<MODEL, 4>(P, 0, 1, final_pass, s)));
+    TO_DISPATCH_RULE(P.integration, (e = launch_forward_rule<RULE>(P, s)));
     return e;
 }
 
-// pass 2 (+3 when ls_iters > 11): the remaining trials, 8 lanes per instance; commits failures
 cudaError_t launch_ladder(const DevProblem& P, cudaStream_t s) {
-    cudaError_t e = cudaSuccess;
-    for (int trial0 = 4; trial0 <= P.opt.ls_iters && e == cudaSuccess; trial0 += 8) {
-        const int final_pass = trial0 + 8 > P.opt.ls_iters;
-        TO_DISPATCH_MODEL(P.model, P.m, (e = launch_any<MODEL, 8>(P, trial0, 0, final_pass, s)));
-    }
+    cudaError_t e = cudaErrorNotSupported;
+    TO_DISPATCH_RULE(P.integration, (e = launch_ladder_rule<RULE>(P, s)));
     return e;
 }
 
 cudaError_t launch_accept(const DevProblem& P, cudaStream_t s) { return cudaSuccess; }   // acceptance is committed inside k_linesearch
+#endif

@@ -5,9 +5,28 @@
 // blocks of `threads` threads that cover `total` threads (the grid of a launcher)
 inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
-// kernel 1: batched RK4 rollout / dual-number dynamics expansion           (rollout.cu)
+// kernel 1: batched rollout / dual-number dynamics expansion with the problem's explicit rule           (rollout.cu)
 cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s);
 cudaError_t launch_expand(const DevProblem& P, cudaStream_t s, int mode = 0);   // mode 1 / 2: only instances with acc1 == 1 / == 0
+// The launchers of the kernels that step the dynamics, per explicit rule RULE (to_integration).  rollout.cu and forward.cu are compiled once
+// per rule; the object of rule R instantiates these for R alone, and the public launchers (launch_rollout, launch_expand, launch_expand_lie,
+// launch_forward, launch_ladder) dispatch on DevProblem::integration.
+template <int RULE> cudaError_t launch_rollout_rule(const DevProblem& P, cudaStream_t s);
+template <int RULE> cudaError_t launch_expand_rule(const DevProblem& P, cudaStream_t s, int mode);
+template <int RULE> cudaError_t launch_expand_lie_rule(const DevProblem& P, cudaStream_t s, int mode);
+template <int RULE> cudaError_t launch_forward_rule(const DevProblem& P, cudaStream_t s);
+template <int RULE> cudaError_t launch_ladder_rule(const DevProblem& P, cudaStream_t s);
+#define TO_RULE_EXTERN(R)                                                                                   \
+    extern template cudaError_t launch_rollout_rule<R>(const DevProblem&, cudaStream_t);                  \
+    extern template cudaError_t launch_expand_rule<R>(const DevProblem&, cudaStream_t, int);              \
+    extern template cudaError_t launch_expand_lie_rule<R>(const DevProblem&, cudaStream_t, int);          \
+    extern template cudaError_t launch_forward_rule<R>(const DevProblem&, cudaStream_t);                  \
+    extern template cudaError_t launch_ladder_rule<R>(const DevProblem&, cudaStream_t);
+TO_RULE_EXTERN(1)
+TO_RULE_EXTERN(2)
+TO_RULE_EXTERN(3)
+TO_RULE_EXTERN(4)
+#undef TO_RULE_EXTERN
 // kernel 2: cost + constraint + AL sweep                                     (sweep.cu)
 cudaError_t launch_cost(const DevProblem& P, double* J, double* Jk, cudaStream_t s);
 cudaError_t launch_merit(const DevProblem& P, double* J, double* viol, cudaStream_t s);
@@ -51,7 +70,7 @@ cudaError_t launch_error_dynamics(const DevProblem& P, cudaStream_t s);
 cudaError_t launch_error_expansion(const DevProblem& P, const double* gfull, const double* hfull, double* EG, double* EH, cudaStream_t s);
 cudaError_t launch_backward_dense(const DevProblem& P, const BackwardPlan& plan, cudaStream_t s);
 cudaError_t launch_expansion_compact(const DevProblem& P, cudaStream_t s);             // EC of every knot (P.compact)
-cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode = 0);     // [A_e B_e] straight from the dual-number RK4 step (rollout.cu)
+cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode = 0);     // [A_e B_e] straight from the dual-number explicit step (rollout.cu)
 // register-resident Riccati pass of the error-state Quadrotor + its record producers   (riccati_frag.cu)
 cudaError_t launch_expansion_rec(const DevProblem& P, cudaStream_t s);                 // compact expansion -> REC[192..240) of every knot
 cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode);               // ... 16-knot blocks per 16-lane group, from the host-built term table (rollout.cu)

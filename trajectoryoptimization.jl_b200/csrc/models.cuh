@@ -7,8 +7,8 @@
 //                     kinematics from RobotDynamics.jl `RigidBody` (world-frame velocity, scalar-first quaternion)
 //   DoubleIntegrator  examples/quickstart.jl:15-20
 //   Acrobot           RobotZoo.jl `Acrobot` (not present in the reference tree)
-// Discretisation: RobotDynamics.jl RK4 with zero-order hold, the integrator `Problem` selects by default
-// (src/problem.jl:119-123) and `rollout!` steps through (src/problem.jl:334-340).
+// Discretisation: RobotDynamics.jl's explicit rules with zero-order hold (explicit_step): Euler, RK2, RK3 or RK4, the
+// integrator `Problem` selects (src/problem.jl:119-123; RK4 by default) and `rollout!` steps through (src/problem.jl:334-340).
 #pragma once
 #include "common.cuh"
 
@@ -223,27 +223,63 @@ __device__ __forceinline__ void dynamics(const double* __restrict__ p, const S* 
     }
 }
 
-// RK4, zero-order hold:  k_i scaled by h as RobotDynamics does; x+ = x + (k1 + 2k2 + 2k3 + k4)/6
+// One step of the explicit rule RULE (include/trajopt_b200.h to_integration), zero-order hold on u, each k_i scaled by h as RobotDynamics
+// does before it is used:
+//   1 Euler  x+ = x + k1
+//   2 RK2    (explicit midpoint) k2 = h f(x + k1/2);  x+ = x + k2
+//   3 RK3    (Kutta) k2 = h f(x + k1/2);  k3 = h f(x - k1 + 2 k2);  x+ = x + (k1 + 4 k2 + k3)/6
+//   4 RK4    x+ = x + (k1 + 2k2 + 2k3 + k4)/6
+// with k1 = h f(x, u).  Every rule reads x_i for the last time where it writes xn_i, so xn may be x (rollout_compact steps in place).
+// The weights of every rule sum to one, which keeps the closed-form position / velocity Jacobian columns exact (rollout.cu SeedList).
+// The 1/6 of RK3 and RK4 is a product, as RK4 has always computed it: an FP64 division is a multi-instruction sequence on the line search's
+// dependency chain (RK3 written with / 6, as the oracle writes it, took the BASELINE line search's pass 1 to 0.49 ms, against 0.29 ms as a product).
 // DET_FMA: the Cartpole's determinant as one explicit fma (det_sub_square)
-template <int MODEL, class S, bool DET_FMA = false>
-__device__ __forceinline__ void rk4_step(const double* __restrict__ p, const S* x, const S* u, double h, S* xn) {
+template <int MODEL, class S, int RULE, bool DET_FMA = false>
+__device__ __forceinline__ void explicit_step(const double* __restrict__ p, const S* x, const S* u, double h, S* xn) {
+    static_assert(RULE >= 1 && RULE <= 4, "to_integration: TO_EULER .. TO_RK4");
     constexpr int n = ModelDims<MODEL>::n;
     if constexpr (MODEL == MODEL_EXPR_42) {     // a discrete jump map is applied as is
         if (reinterpret_cast<const DevDyn*>(p)->discrete) { dynamics<MODEL, S>(p, x, u, xn); return; }
     }
-    S k[n], acc[n], xt[n];
-    dynamics<MODEL, S, DET_FMA>(p, x, u, k);
+    if constexpr (RULE == 1) {
+        S k[n];
+        dynamics<MODEL, S, DET_FMA>(p, x, u, k);
 #pragma unroll
-    for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = k[i]; xt[i] = x[i] + k[i] * 0.5; }
-    dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
+        for (int i = 0; i < n; i++) xn[i] = x[i] + k[i] * h;
+    } else if constexpr (RULE == 2) {
+        S k[n], xt[n];
+        dynamics<MODEL, S, DET_FMA>(p, x, u, k);
 #pragma unroll
-    for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = acc[i] + 2.0 * k[i]; xt[i] = x[i] + k[i] * 0.5; }
-    dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
+        for (int i = 0; i < n; i++) { k[i] = k[i] * h; xt[i] = x[i] + k[i] * 0.5; }
+        dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
 #pragma unroll
-    for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = acc[i] + 2.0 * k[i]; xt[i] = x[i] + k[i]; }
-    dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
+        for (int i = 0; i < n; i++) xn[i] = x[i] + k[i] * h;
+    } else if constexpr (RULE == 3) {
+        S k1[n], k[n], xt[n];                   // k1 becomes k1 + 4 k2 once the third stage's point is formed
+        dynamics<MODEL, S, DET_FMA>(p, x, u, k1);
 #pragma unroll
-    for (int i = 0; i < n; i++) { k[i] = k[i] * h; xn[i] = x[i] + (acc[i] + k[i]) * (1.0 / 6.0); }
+        for (int i = 0; i < n; i++) { k1[i] = k1[i] * h; xt[i] = x[i] + k1[i] * 0.5; }
+        dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
+#pragma unroll
+        for (int i = 0; i < n; i++) { k[i] = k[i] * h; xt[i] = x[i] - k1[i] + 2.0 * k[i]; k1[i] = k1[i] + 4.0 * k[i]; }
+        dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
+#pragma unroll
+        for (int i = 0; i < n; i++) { k[i] = k[i] * h; xn[i] = x[i] + (k1[i] + k[i]) * (1.0 / 6.0); }
+    } else {
+        S k[n], acc[n], xt[n];
+        dynamics<MODEL, S, DET_FMA>(p, x, u, k);
+#pragma unroll
+        for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = k[i]; xt[i] = x[i] + k[i] * 0.5; }
+        dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
+#pragma unroll
+        for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = acc[i] + 2.0 * k[i]; xt[i] = x[i] + k[i] * 0.5; }
+        dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
+#pragma unroll
+        for (int i = 0; i < n; i++) { k[i] = k[i] * h; acc[i] = acc[i] + 2.0 * k[i]; xt[i] = x[i] + k[i]; }
+        dynamics<MODEL, S, DET_FMA>(p, xt, u, k);
+#pragma unroll
+        for (int i = 0; i < n; i++) { k[i] = k[i] * h; xn[i] = x[i] + (acc[i] + k[i]) * (1.0 / 6.0); }
+    }
 }
 
 // dispatch a templated launcher on the runtime model id / dimension
@@ -259,7 +295,16 @@ __device__ __forceinline__ void rk4_step(const double* __restrict__ p, const S* 
         case MODEL_EXPR: { constexpr int MODEL = MODEL_EXPR_42; CALL; } break;                     \
     }
 
-// what rk4_step / dynamics take as `p` at knot k: the shared parameter vector (INST = false); INST: `row`, the copy of instance b's parameters
+// dispatch on the problem's explicit rule (DevProblem::integration): RULE = RULE_EULER .. RULE_RK4
+#define TO_DISPATCH_RULE(rule, CALL)                                                               \
+    switch (rule) {                                                                                \
+        case RULE_EULER: { constexpr int RULE = RULE_EULER; CALL; } break;                         \
+        case RULE_RK2: { constexpr int RULE = RULE_RK2; CALL; } break;                             \
+        case RULE_RK3: { constexpr int RULE = RULE_RK3; CALL; } break;                             \
+        default: { constexpr int RULE = RULE_RK4; CALL; } break;                                   \
+    }
+
+// what explicit_step / dynamics take as `p` at knot k: the shared parameter vector (INST = false); INST: `row`, the copy of instance b's parameters
 // the kernel made with stage_model_params; recorded programs: the DevDyn of knot k (their constants are never per instance)
 template <int MODEL, bool INST = false>
 __device__ __forceinline__ const double* model_params(const DevProblem& P, const double* row, int k) {

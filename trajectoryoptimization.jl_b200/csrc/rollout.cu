@@ -1,11 +1,12 @@
-// rollout.cu -- kernel 1 of the hot path: batched RK4 rollout and dual-number dynamics expansion.
+// rollout.cu -- kernel 1 of the hot path: batched rollout and dual-number dynamics expansion.
 //
 //   k_rollout : rollout!(prob)                         reference src/problem.jl:330-340
-//               x_1 = x0 ; x_k = RK4(x_{k-1}, u_{k-1}, dt_{k-1}).  Serial in k, parallel over instances:
+//               x_1 = x0 ; x_k = step(x_{k-1}, u_{k-1}, dt_{k-1}) with the problem's explicit rule (models.cuh explicit_step).
+//               Serial in k, parallel over instances:
 //               one thread per instance (the recursion has no intra-instance parallelism worth a warp).
 //   k_expand  : RD.jacobian!(ForwardAD) on the discretised dynamics at every knot (no call site inside the
 //               reference; shape [A B] = n x (n+m) pinned by test/dynamics_constraints.jl:35,57-62).
-//               One thread per (instance, knot, seed direction j): the RK4 step is pushed through a
+//               One thread per (instance, knot, seed direction j): the explicit step is pushed through a
 //               Dual<1> whose tangent is the one-hot e_j, i.e. the thread computes column j of [A B] with the
 //               partial carried in registers.  Threads of one knot are adjacent, so row i of AB is written by
 //               adjacent lanes; the pad columns of a row (LDAB > n+m) are never touched and stay zero.
@@ -15,12 +16,19 @@
 #include "kernels.h"
 #include "models.cuh"
 
+// The kernels that step the dynamics take the explicit rule RULE (DevProblem::integration).  This file is compiled once per rule (Makefile):
+// the object built with TO_RULE = 4 (TO_RK4) holds the RK4 instantiations, every kernel that steps no dynamics and the launchers that dispatch on
+// the rule; the objects of the other rules hold only their rule's instantiations, so that they compile in parallel.
+#ifndef TO_RULE
+#define TO_RULE 4
+#endif
+
 // One thread integrates one instance; the warp writes its 32 states of a knot through a shared-memory transpose, so that the stores are runs of
 // n contiguous doubles per instance (full 32-byte sectors) instead of 32 scattered 8-byte words per instruction.
 // INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per lane, and time steps (DevProblem::dtb).
 // (Copied to registers instead, the parameter-only subexpressions of the dynamics were hoisted out of the knot loop and lost FMA contractions
 // the shared kernel has.)
-template <int MODEL, bool INST>
+template <int MODEL, bool INST, int RULE>
 __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m;
     __shared__ double stage[32 * n];
@@ -54,16 +62,17 @@ __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
         if (k == P.N - 1) break;
 #pragma unroll
         for (int i = 0; i < m; i++) u[i] = U[k * m + i];
-        rk4_step<MODEL, double>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, bc, k), xn);
+        explicit_step<MODEL, double, RULE>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, bc, k), xn);
 #pragma unroll
         for (int i = 0; i < n; i++) x[i] = xn[i];
     }
 }
 
 // Seed pruning (full state).  The position r and the world-frame linear velocity v of the Quadrotor (a RobotDynamics RigidBody) enter the
-// dynamics only through rdot = v, so their columns of [A B] are known in closed form -- d x+/d r = e_r, d x+/d v = h e_r + e_v (the RK4
-// weights sum to one) -- and are written when the problem is created and when its time steps change (k_trivial_columns_full); 11 seeds
-// (quaternion, angular velocity, controls) are pushed through the dual-number RK4 step instead of 17.  Other models: every seed.
+// dynamics only through rdot = v, so their columns of [A B] are known in closed form -- d x+/d r = e_r, d x+/d v = h e_r + e_v (the weights
+// of every explicit rule sum to one, so this holds for Euler, RK2, RK3 and RK4 alike) -- and are written when the problem is created and when
+// its time steps change (k_trivial_columns_full); 11 seeds (quaternion, angular velocity, controls) are pushed through the dual-number step
+// instead of 17.  Other models: every seed.
 template <int MODEL> struct SeedList {
     static constexpr int count = ModelDims<MODEL>::n + ModelDims<MODEL>::m;
     __host__ __device__ static constexpr int seed(int s) { return s; }
@@ -78,7 +87,7 @@ template <> struct SeedList<MODEL_QUADROTOR> {
 };
 
 // INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per thread (see k_rollout), and time steps
-template <int MODEL, int NP, bool INST>
+template <int MODEL, int NP, bool INST, int RULE>
 __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, nm = n + m;
     constexpr int NSEED = SeedList<MODEL>::count;
@@ -119,7 +128,7 @@ __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
         stage_model_params<INST>(P, b, prm_s[threadIdx.x]);
         prm = prm_s[threadIdx.x];
     }
-    rk4_step<MODEL, D>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k), xn);
+    explicit_step<MODEL, D, RULE>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k), xn);
 #pragma unroll
     for (int i = 0; i < n; i++) {
         if (NP == 2 && js[1] == js[0] + 1 && !(js[0] & 1)) *reinterpret_cast<double2*>(&AB[i * ld + js[0]]) = make_double2(xn[i].d[0], xn[i].d[1]);
@@ -130,6 +139,7 @@ __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
     }
 }
 
+#if TO_RULE == 4
 // the closed-form columns of [A B] (SeedList<MODEL>::trivial): thread = (instance, knot, one of them); run when the problem is created and
 // whenever its time steps change (INST: each instance's own, DevProblem::dtb)
 template <int MODEL, bool INST>
@@ -198,18 +208,20 @@ __device__ __forceinline__ void compact_entry_expansion(const DevProblem& P, con
     }
 }
 
+#endif  // TO_RULE == 4
+
 // Seed pruning.  The position r and the (world-frame) linear velocity v of a RigidBody enter the dynamics only through rdot = v: f does not
 // depend on r, and on v only in rdot.  Their columns of the discrete Jacobian are therefore known in closed form -- d x+/d r = e_r and
-// d x+/d v = h e_r + e_v (the RK4 weights sum to one) -- and need no dual-number sweep: 10 seeds (attitude, angular velocity, controls) are
-// pushed through the RK4 step instead of 16, one thread each; the six trivial columns depend on the time steps only.  The materialised P.ABe
+// d x+/d v = h e_r + e_v (the weights of every explicit rule sum to one) -- and need no dual-number sweep: 10 seeds (attitude, angular
+// velocity, controls) are pushed through the step instead of 16, one thread each; the six trivial columns depend on the time steps only.  The materialised P.ABe
 // gets them when the problem is created and when its time steps change (k_trivial_columns); k_expand_lie_rec writes them into every record
 // block it assembles, and the export of the records (launch_export_abe) carries them to P.ABe on the record path.
 __device__ __forceinline__ int lie_seed(int s) { return (int)((0xFEDCBA9543ULL >> (4 * s)) & 15); }       // 3,4,5,9,10,11,12,13,14,15
 __device__ __forceinline__ int lie_trivial(int s) { return (int)((0x876210ULL >> (4 * s)) & 15); }        // 0,1,2,6,7,8
 
-// column j of [A_e B_e]_k: the RK4 step of knot k pushed through Dual<1> with the seed of error-state coordinate j (attitude: a column of G(q_k)),
+// column j of [A_e B_e]_k: the explicit step of knot k pushed through Dual<1> with the seed of error-state coordinate j (attitude: a column of G(q_k)),
 // projected on the error state of knot k + 1 with G(q_{k+1})'  (INST: with instance b's parameters, staged in `prm`, and its time step)
-template <int MODEL, bool INST>
+template <int MODEL, bool INST, int RULE>
 __device__ __forceinline__ void expand_lie_column(const DevProblem& P, const double* prm, int b, int k, int j, const double* __restrict__ X,
                                                   const double* __restrict__ U, double (&col)[ModelDims<MODEL>::n - 1]) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, qs = 3;
@@ -231,7 +243,7 @@ __device__ __forceinline__ void expand_lie_column(const DevProblem& P, const dou
 #pragma unroll
         for (int i = qs + 4; i < n; i++) x[i].d[0] = (i == j + 1) ? 1.0 : 0.0;
     }
-    rk4_step<MODEL, D>(model_params<MODEL, INST>(P, prm, k), x, u, h, xn);
+    explicit_step<MODEL, D, RULE>(model_params<MODEL, INST>(P, prm, k), x, u, h, xn);
     const double* q1 = X + n + qs;                                     // attitude of knot k + 1
     const double w1 = q1[0], x1 = q1[1], y1 = q1[2], z1 = q1[3];
 #pragma unroll
@@ -253,7 +265,7 @@ __device__ __forceinline__ void expand_lie_column(const DevProblem& P, const dou
 #define TO_EXPAND_LIE_THREADS 64
 #endif
 // INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per thread (see k_rollout), and time steps
-template <int MODEL, bool INST>
+template <int MODEL, bool INST, int RULE>
 __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 128 / TO_EXPAND_LIE_THREADS) k_expand_lie(const DevProblem P, int mode) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, nme = ne + m, NS = 10;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -275,7 +287,7 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
         prm = prm_s[threadIdx.x];
     }
     double col[ne];
-    expand_lie_column<MODEL, INST>(P, prm, b, k, j, X, U, col);
+    expand_lie_column<MODEL, INST, RULE>(P, prm, b, k, j, X, U, col);
     double* out = P.ABe + ((size_t)bk * nme + j) * ne;                 // column j of [A_e B_e]: 12 contiguous doubles
 #pragma unroll
     for (int e = 0; e < ne; e++) out[e] = col[e];
@@ -298,7 +310,7 @@ __global__ void __launch_bounds__(TO_EXPAND_LIE_THREADS, TO_EXPAND_LIE_MINB * 12
 // INST: the instance's own model parameters (DevProblem::mparams), staged in shared memory once per CTA (the CTA's one instance), and time steps
 #define EXPB_KPB 6
 #define EXPB_T 64
-template <int MODEL, bool INST>
+template <int MODEL, bool INST, int RULE>
 __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_expand_lie_rec(const DevProblem P, int mode, int nkb) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m, ne = n - 1, NS = 10;
     static_assert(ne == 12 && m == 4 && EXPB_KPB * NS <= EXPB_T, "record layout of the error-state Quadrotor");
@@ -334,7 +346,7 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
             for (int e = 0; e < ne; e++) img[fraglayout::stage_swz(fraglayout::ab_index(e, 12) | cb, kk)] = col[e];
         };
         double col[ne];
-        expand_lie_column<MODEL, INST>(P, prm, b, k, lie_seed(sd), X, U, col);
+        expand_lie_column<MODEL, INST, RULE>(P, prm, b, k, lie_seed(sd), X, U, col);
         put(lie_seed(sd), col);
         if (sd < 6) {                                                                  // closed-form column jt: d x+/d r = I, d r+/d v = h I, d v+/d v = I
             const int jt = lie_trivial(sd);
@@ -361,6 +373,7 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
     }
 }
 
+#if TO_RULE == 4
 // the closed-form columns of [A_e B_e] (positions, velocities): thread = (instance, knot, one of the six); INST: each instance's time steps
 template <bool INST>
 __global__ void __launch_bounds__(128) k_trivial_columns(const DevProblem P) {
@@ -577,7 +590,10 @@ cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode
     return cudaGetLastError();
 }
 
-cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
+#endif  // TO_RULE == 4
+
+template <int RULE>
+cudaError_t launch_expand_lie_rule(const DevProblem& P, cudaStream_t s, int mode) {
     if (P.model != MODEL_QUADROTOR) return cudaErrorNotSupported;
     const long long total = (long long)P.B * (P.N - 1) * 10;      // 10 dual-number seeds per knot (k_expand_lie: seed pruning)
     static_assert(fraglayout::phys_z(0) == 1 && fraglayout::phys_z(5) == 12 && fraglayout::phys_z(11) == 15 && fraglayout::phys_z(12) == 0 && fraglayout::phys_z(15) == 6, "nibble table of k_expand_lie_rec and k_expansion_rec16b");
@@ -586,38 +602,62 @@ cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
         // one CTA per (instance, block of EXPB_KPB knots); mode 2 with the late list: the first *late_count instance slots carry work
         const int nkb = (P.N - 1 + EXPB_KPB - 1) / EXPB_KPB;
         const unsigned blocks = (unsigned)((long long)P.B * nkb);
-        if (inst_dynamics(P)) k_expand_lie_rec<MODEL_QUADROTOR, true><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
-        else k_expand_lie_rec<MODEL_QUADROTOR, false><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
-    } else if (inst_dynamics(P)) k_expand_lie<MODEL_QUADROTOR, true><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
-    else k_expand_lie<MODEL_QUADROTOR, false><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
+        if (inst_dynamics(P)) k_expand_lie_rec<MODEL_QUADROTOR, true, RULE><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
+        else k_expand_lie_rec<MODEL_QUADROTOR, false, RULE><<<blocks, EXPB_T, 0, s>>>(P, mode, nkb);
+    } else if (inst_dynamics(P)) k_expand_lie<MODEL_QUADROTOR, true, RULE><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
+    else k_expand_lie<MODEL_QUADROTOR, false, RULE><<<(unsigned)((total + T - 1) / T), T, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
 
 // the dynamics kernels read nothing per instance but the model parameters and the time steps: their INST variant runs exactly when a table exists
-cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s) {
+template <int RULE>
+cudaError_t launch_rollout_rule(const DevProblem& P, cudaStream_t s) {
     const int threads = 32, blocks = (P.B + threads - 1) / threads;
-    if (inst_dynamics(P)) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true><<<blocks, threads, 0, s>>>(P))); }
-    else { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, false><<<blocks, threads, 0, s>>>(P))); }
+    if (inst_dynamics(P)) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true, RULE><<<blocks, threads, 0, s>>>(P))); }
+    else { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, false, RULE><<<blocks, threads, 0, s>>>(P))); }
     return cudaGetLastError();
 }
 
-template <int MODEL, int NP>
+template <int MODEL, int NP, int RULE>
 static cudaError_t launch_expand_t(const DevProblem& P, cudaStream_t s, int mode) {
     constexpr int TPK = (SeedList<MODEL>::count + NP - 1) / NP;
     const long long total = (long long)P.B * (P.N - 1) * TPK;
     const int threads = 128;
     const unsigned blocks = (unsigned)((total + threads - 1) / threads);
-    if (inst_dynamics(P)) k_expand<MODEL, NP, true><<<blocks, threads, 0, s>>>(P, mode);
-    else k_expand<MODEL, NP, false><<<blocks, threads, 0, s>>>(P, mode);
+    if (inst_dynamics(P)) k_expand<MODEL, NP, true, RULE><<<blocks, threads, 0, s>>>(P, mode);
+    else k_expand<MODEL, NP, false, RULE><<<blocks, threads, 0, s>>>(P, mode);
     return cudaGetLastError();
 }
 
-cudaError_t launch_expand(const DevProblem& P, cudaStream_t s, int mode) {
+template <int RULE>
+cudaError_t launch_expand_rule(const DevProblem& P, cudaStream_t s, int mode) {
     // seeds per thread: 1 (value recomputed per seed) or 2 (value shared by two seeds, more registers)
     static int np = -1;
     if (np < 0) { const char* v = getenv("TO_EXPAND_SEEDS"); np = v ? atoi(v) : 1; }
     cudaError_t e = cudaErrorNotSupported;
-    if (np == 2) { TO_DISPATCH_MODEL(P.model, P.m, (e = launch_expand_t<MODEL, 2>(P, s, mode))); }
-    else { TO_DISPATCH_MODEL(P.model, P.m, (e = launch_expand_t<MODEL, 1>(P, s, mode))); }
+    if (np == 2) { TO_DISPATCH_MODEL(P.model, P.m, (e = launch_expand_t<MODEL, 2, RULE>(P, s, mode))); }
+    else { TO_DISPATCH_MODEL(P.model, P.m, (e = launch_expand_t<MODEL, 1, RULE>(P, s, mode))); }
     return e;
 }
+
+template cudaError_t launch_expand_lie_rule<TO_RULE>(const DevProblem&, cudaStream_t, int);
+template cudaError_t launch_rollout_rule<TO_RULE>(const DevProblem&, cudaStream_t);
+template cudaError_t launch_expand_rule<TO_RULE>(const DevProblem&, cudaStream_t, int);
+
+#if TO_RULE == 4
+cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
+    cudaError_t e = cudaErrorNotSupported;
+    TO_DISPATCH_RULE(P.integration, (e = launch_expand_lie_rule<RULE>(P, s, mode)));
+    return e;
+}
+cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s) {
+    cudaError_t e = cudaErrorNotSupported;
+    TO_DISPATCH_RULE(P.integration, (e = launch_rollout_rule<RULE>(P, s)));
+    return e;
+}
+cudaError_t launch_expand(const DevProblem& P, cudaStream_t s, int mode) {
+    cudaError_t e = cudaErrorNotSupported;
+    TO_DISPATCH_RULE(P.integration, (e = launch_expand_rule<RULE>(P, s, mode)));
+    return e;
+}
+#endif

@@ -131,14 +131,24 @@ function constraint_spec(con::TO.StageConstraint, f, l, n, m, root)             
     ToConstraintSpec(8, f, l, sense_code(TO.sense(con)), P, length(tape.consts), length(tape.prog), pointer(tape.prog), pointer(tape.consts), NULLD, NULLD, NULLD, 0.0)
 end
 
+# the to_integration code of an explicit RobotDynamics rule; the implicit rules are refused (iLQR's rollout needs an explicit step)
+integration_code(::RD.Euler) = Int32(1)
+integration_code(::RD.RK2) = Int32(2)
+integration_code(::RD.RK3) = Int32(3)
+integration_code(::RD.RK4) = Int32(4)
+integration_code(rule) = throw(ArgumentError("integration $(typeof(rule)) is not supported: the explicit rules RD.Euler, RD.RK2, RD.RK3 and RD.RK4 are"))
+
 """
-    BatchedProblem(prob::TO.Problem, model_id, B; device=0, params=Float64[])
+    BatchedProblem(prob::TO.Problem, model_id, B; device=0, params=Float64[], integration=RD.integration(prob.model[1]))
 
 Describe `prob` (objective = vector of QuadraticCostFunctions, ConstraintList of Goal/Bound/Linear/Circle/Sphere/Norm)
-to the library and allocate a batch of `B` instances on `device`.
+to the library and allocate a batch of `B` instances on `device`.  `integration` is the explicit rule the dynamics are discretised
+with (to_set_integration): `prob`'s own by default.
 """
 function BatchedProblem(prob::TO.Problem, mid::Integer, B::Integer; device::Integer=0, params::Vector{Float64}=Float64[],
-                        error_state::Bool=(RD.errstate_dim(TO.get_model(prob)[1]) != RD.state_dim(TO.get_model(prob)[1])))
+                        error_state::Bool=(RD.errstate_dim(TO.get_model(prob)[1]) != RD.state_dim(TO.get_model(prob)[1])),
+                        integration=RD.integration(TO.get_model(prob)[1]))
+    rule = integration_code(integration)
     n, m, N = RD.dims(prob, 1)
     keep = Any[]
     root(x) = (push!(keep, x); x)
@@ -183,6 +193,7 @@ function BatchedProblem(prob::TO.Problem, mid::Integer, B::Integer; device::Inte
     check(C_NULL, rc)
     bp = BatchedProblem(h[], prob, B, keep)
     finalizer(p -> ccall((:to_destroy, libb200), Cint, (Ptr{Cvoid},), p.h), bp)
+    check(bp.h, ccall((:to_set_integration, libb200), Cint, (Ptr{Cvoid}, Int32), bp.h, rule))
     return bp
 end
 
@@ -342,6 +353,13 @@ function set_time_steps!(p::BatchedProblem, dt::AbstractMatrix, t0::Union{Nothin
                      t0 === nothing ? C_NULL : Vector{Float64}(t0)))
 end
 set_time_steps!(p::BatchedProblem, dt::AbstractVector, t0=nothing) = set_time_steps!(p, repeat(permutedims(Vector{Float64}(dt)), p.prob.N - 1), t0)
+# RD.integration(prob.model[1]) of the batch: the code of its explicit rule (1 Euler, 2 RK2, 3 RK3, 4 RK4)
+function integration(p::BatchedProblem)
+    rule = Ref{Int32}(0)
+    check(p.h, ccall((:to_get_integration, libb200), Cint, (Ptr{Cvoid}, Ref{Int32}), p.h, rule))
+    return rule[]
+end
+
 function time_steps(p::BatchedProblem)
     dt = Matrix{Float64}(undef, p.prob.N - 1, p.B)
     t0 = Vector{Float64}(undef, p.B)
