@@ -307,6 +307,44 @@ int to_get_cost_weights(to_handle* h, int32_t cost, double* w /*[B][len]*/);    
 int to_set_integration(to_handle* h, int32_t rule);
 int to_get_integration(const to_handle* h, int32_t* rule);
 
+/* ---- closed-loop MPC on the device -------------------------------------------------------------------------------
+ * A receding-horizon simulation of every instance without a host round trip per step.  MPC step j (j counts from the last setup) runs, bit
+ * for bit, what this host-scripted loop of entry points computes:
+ *   1. with a reference: to_update_trajectories(Xref, Uref, nref, start + j);
+ *   2. to_rollout;  3. to_ilqr_step(iterations);
+ *   4. record u_j = U[b][0] (to_get_controls) and the plan's merit J_j (to_merit);
+ *   5. the plant: xp <- step(xp, u_j) (+) w_j, recorded as Xcl[j+1];
+ *   6. to_shift_trajectory(1), then to_set_initial_state(xp).
+ * The plant is the problem's model stepped once with the problem's integration rule over the instance's knot-0 time step (its own row after
+ * to_set_time_steps), with the plant's parameter rows when the setup gave them, else the planner's (per instance when set).  (+) is the
+ * inverse of to_state_diff: addition for vector-space states, the Cayley-map composition q (x) (1, phi) / sqrt(1 + phi'phi) on the
+ * error-state Quadrotor's quaternion; w_j has n_e entries.  A run starts from xp = x0, so runs of T1 and T2 steps leave what one run of
+ * T1 + T2 leaves.  Multipliers and penalties are shifted by step 6 and not otherwise updated; to_al_update or any setter may run between runs.
+ * Not on hybrid problems; a problem whose every knot steps one continuous recorded model is a plant like any other, without a reference window
+ * or plant parameters (it has no per-instance goals or parameters). */
+typedef struct {
+    int32_t nsteps;              /* the steps the setup holds room for (>= 1) */
+    int32_t nparams;             /* entries of a plant row, as to_set_model_params takes them */
+    const double* plant_params;  /* [B][nparams] or NULL: the planner's parameters */
+    const double* W;             /* [B][nsteps][n_e] disturbances or NULL: none */
+    const double* Xref;          /* [B][nref][n] or NULL: no reference window */
+    const double* Uref;          /* [B][nref][m] (with Xref) */
+    int32_t nref, start;         /* step j tracks rows start - 1 + j .. start - 2 + j + N (1-based start) */
+} to_mpc_spec;
+/* Synchronous: checks the inputs and copies them to device buffers of the handle, allocates the history and resets the step counter; with a
+ * reference it creates the per-instance linear terms as to_update_trajectories does.  TO_EDIM: start - 1 + (nsteps - 1) + N > nref, or a
+ * plant row of the wrong length.  TO_EINVAL, naming the instance: a non-finite entry, a plant row to_set_model_params would refuse; nsteps
+ * < 1, a hybrid problem.  A refused setup leaves the previous one as it was. */
+int to_mpc_setup(to_handle* h, const to_mpc_spec* spec);
+/* Asynchronous, like to_ilqr_step: enqueues `steps` MPC steps of `iterations` iLQR iterations each on the handle's stream(s) and returns.
+ * TO_ESTATE before any setup; TO_EDIM when the steps done since the setup + steps > nsteps; TO_EINVAL when steps or iterations < 1; the
+ * checks of to_ilqr_step.  The host clocks advance as to_shift_trajectory(1) advances them; to_get_cost_terms reads the rows the last window
+ * wrote. */
+int to_mpc_run(to_handle* h, int32_t steps, int32_t iterations);
+/* The history of the s steps run since the setup, and synchronises: Xcl [B][s+1][n] (row j: the state step j started from; row s: where the
+ * last step ended, x0 when s = 0), Ucl [B][s][m], J [B][s].  Any output may be NULL.  TO_ESTATE before any setup. */
+int to_mpc_history(to_handle* h, double* Xcl, double* Ucl, double* J);
+
 /* ---- kernel 1: batched rollout (+ dual-number Jacobians) ------------------------------------------------- */
 int to_rollout(to_handle* h);                                                 /* rollout!           src/problem.jl:330-340 */
 int to_expand(to_handle* h);                                                  /* RD.jacobian!(ForwardAD) on the discretized dynamics at every knot */

@@ -79,6 +79,11 @@ class to_solve_options(C.Structure):
                 ("iterations", C.c_int32), ("iterations_inner", C.c_int32), ("iterations_outer", C.c_int32), ("dJ_counter_limit", C.c_int32)]
 
 
+class to_mpc_spec(C.Structure):
+    _fields_ = [("nsteps", C.c_int32), ("nparams", C.c_int32), ("plant_params", c_double_p), ("W", c_double_p), ("Xref", c_double_p),
+                ("Uref", c_double_p), ("nref", C.c_int32), ("start", C.c_int32)]
+
+
 def _dp(a):
     return None if a is None else a.ctypes.data_as(c_double_p)
 
@@ -207,6 +212,7 @@ def load_library():
         "to_error_expansion": [H, c_double_p, c_double_p], "to_get_expansion_records": [H, c_double_p],
         "to_default_solve_options": [C.POINTER(to_solve_options)],
         "to_solve": [H, C.POINTER(to_solve_options), c_int32_p, c_int32_p, c_int32_p, c_double_p, c_double_p, c_double_p, c_double_p],
+        "to_mpc_setup": [H, C.POINTER(to_mpc_spec)], "to_mpc_run": [H, C.c_int32, C.c_int32], "to_mpc_history": [H, c_double_p, c_double_p, c_double_p],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)
@@ -233,7 +239,7 @@ EXPORTED_SYMBOLS = [
     "to_cost_weights_len", "to_set_cost_weights", "to_get_cost_weights",
     "to_set_phase_timing", "to_get_phase_times", "to_launch_count", "to_algorithmic_bytes",
     "to_backward_algebra", "to_kernel_choice", "to_error_state_dim", "to_state_diff", "to_get_error_dynamics", "to_error_expansion",
-    "to_get_expansion_records", "to_default_solve_options", "to_solve",
+    "to_get_expansion_records", "to_default_solve_options", "to_solve", "to_mpc_setup", "to_mpc_run", "to_mpc_history",
 ]
 
 

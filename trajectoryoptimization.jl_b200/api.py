@@ -1287,6 +1287,7 @@ class Problem:
             steps = np.empty((self.B, self.N - 1)), np.empty(self.B)
             self._raw_call("to_get_time_steps", K._dp(steps[0]), K._dp(steps[1]))
         self.close()
+        self._mpc = None          # a new handle holds no MPC setup
         self.spec = self._make_spec(self._dt, float(t[0]))
         self._open()
         self._apply_integration()
@@ -1653,22 +1654,22 @@ def cost_weights(prob, cost):
     return out
 
 
-def _model_param_rows(prob, params):
+def _model_param_rows(prob, params, what="set_model_params"):
     """``params`` as the ``[B, nparams]`` rows ``to_set_model_params`` takes; every check that needs no device happens here"""
     if getattr(prob, "hybrid", False):
         raise ArgumentError("per-instance model parameters are not supported on hybrid problems (their constants live in the recorded programs)")
     nparams = len(prob.model.params)
     if isinstance(params, (list, tuple)) and any(isinstance(x, _Model) for x in params):
         if len(params) != prob.B:
-            raise DimensionMismatch(f"set_model_params: {len(params)} models for a batch of {prob.B} instances")
+            raise DimensionMismatch(f"{what}: {len(params)} models for a batch of {prob.B} instances")
         for b, x in enumerate(params):
             if type(x) is not type(prob.model) or x.dims() != prob.model.dims():
-                raise ArgumentError(f"set_model_params: instance {b} holds a {type(x).__name__} {getattr(x, 'dims', lambda: '')()}, the problem's model is "
+                raise ArgumentError(f"{what}: instance {b} holds a {type(x).__name__} {getattr(x, 'dims', lambda: '')()}, the problem's model is "
                                     f"a {type(prob.model).__name__} {prob.model.dims()}")
         params = [x.params for x in params]
     rows = np.ascontiguousarray(np.asarray(params, dtype=np.float64))
     if rows.shape != (prob.B, nparams):
-        raise DimensionMismatch(f"set_model_params: expected [{prob.B}, {nparams}] parameters, got {rows.shape}")
+        raise DimensionMismatch(f"{what}: expected [{prob.B}, {nparams}] parameters, got {rows.shape}")
     return rows
 
 
@@ -1861,6 +1862,103 @@ def shift_trajectory(prob, steps=1):
     ``X_k <- X_{k+steps}``, ``U_k <- U_{k+steps}`` with the tail repeated, multipliers moved with their knots,
     ``x0 <- X_{1+steps}``, ``t0`` advanced.  Follow with ``set_initial_state`` (measured state) and ``rollout``."""
     prob._call("to_shift_trajectory", int(steps))
+
+
+# the parameters the device dynamics divide by or build a determinant from, by model (capi.cu positive_param_name): they must be positive
+_POSITIVE_PARAMS = {K.MODEL_DOUBLE_INTEGRATOR: ("mass",), K.MODEL_CARTPOLE: ("mc", "mp", "l"), K.MODEL_QUADROTOR: ("mass", "J1", "J2", "J3"),
+                    K.MODEL_ACROBOT: ("l1", "l2", "m1", "m2")}
+
+
+def _mpc_inputs(prob, nsteps, plant_params, disturbances, Xref, Uref, start):
+    """the arrays ``to_mpc_setup`` takes; every check that needs no device happens here"""
+    expr = getattr(prob, "hybrid", False)
+    if expr:   # one recorded model stepping every knot (Problem(AutodiffDynamics(...), ...)) is a plant like any other; a hybrid problem is not
+        mdl = prob.model[0]
+        if any(x is not mdl for x in prob.model) or mdl.discrete or mdl.n_out != mdl.n:
+            raise ArgumentError("mpc_setup: closed-loop MPC is not supported on hybrid problems")
+        if plant_params is not None or Xref is not None or Uref is not None:
+            raise ArgumentError("mpc_setup: a recorded-program model takes no reference window and no plant parameters (per-instance goals and "
+                                "parameters are not supported on it)")
+    if int(nsteps) != nsteps or nsteps < 1:
+        raise ArgumentError(f"mpc_setup: nsteps must be a positive integer, got {nsteps}")
+    nsteps = int(nsteps)
+    plant = None
+    if plant_params is not None:
+        plant = _model_param_rows(prob, plant_params, what="mpc_setup (plant parameters)")
+        pos = _POSITIVE_PARAMS.get(prob.model.model_id, ())
+        for b, row in enumerate(plant):
+            for i, v in enumerate(row):
+                if not np.isfinite(v):
+                    raise ArgumentError(f"mpc_setup (plant parameters): instance {b}, parameter {i} is not finite")
+                if i < len(pos) and not v > 0:
+                    raise ArgumentError(f"mpc_setup (plant parameters): instance {b}, parameter {i} ({pos[i]}) must be positive")
+    W = None
+    if disturbances is not None:
+        W = np.ascontiguousarray(np.asarray(disturbances, dtype=np.float64))
+        if W.shape != (prob.B, nsteps, prob.ne):
+            raise DimensionMismatch(f"mpc_setup: disturbances must be [{prob.B}, {nsteps}, {prob.ne}], got {W.shape}")
+        bad = np.argwhere(~np.isfinite(W))
+        if bad.size:
+            raise ArgumentError(f"mpc_setup: instance {bad[0][0]}: a disturbance is not finite")
+    if (Xref is None) != (Uref is None):
+        raise ArgumentError("mpc_setup: Xref and Uref are given together")
+    if Xref is not None:
+        Xref = np.ascontiguousarray(np.asarray(Xref, dtype=np.float64)); Uref = np.ascontiguousarray(np.asarray(Uref, dtype=np.float64))
+        if (Xref.ndim != 3 or Uref.ndim != 3 or Xref.shape[0] != prob.B or Uref.shape[0] != prob.B or Xref.shape[2] != prob.n
+                or Uref.shape[2] != prob.m or Uref.shape[1] != Xref.shape[1]):
+            raise DimensionMismatch("mpc_setup: Xref must be [B, nref, n] and Uref [B, nref, m]")
+        if int(start) != start or start < 1 or start - 1 + (nsteps - 1) + prob.N > Xref.shape[1]:
+            raise DimensionMismatch("mpc_setup: the reference is shorter than start - 1 + (nsteps - 1) + N")
+        for what, a in (("state", Xref), ("control", Uref)):
+            bad = np.argwhere(~np.isfinite(a))
+            if bad.size:
+                raise ArgumentError(f"mpc_setup: instance {bad[0][0]}: the {what} reference is not finite")
+        if not all(isinstance(c, QuadraticCostFunction) for c in prob.obj):
+            raise ArgumentError("update_trajectory! is defined for objectives of QuadraticCostFunctions (src/objective.jl:207)")
+    return nsteps, plant, W, Xref, Uref, int(start)
+
+
+def mpc_setup(prob, nsteps, plant_params=None, disturbances=None, Xref=None, Uref=None, start=1):
+    """Prepares a closed-loop MPC simulation of every instance on the device (``mpc_run``): room for ``nsteps`` steps, the plant's model
+    parameters ``plant_params[B, nparams]`` (as ``set_model_params`` takes them; ``None``: the planner's), the disturbances
+    ``disturbances[B, nsteps, n_e]`` added to the plant state after each step (``None``: none) and a long tracking reference
+    ``Xref[B, nref, n]``, ``Uref[B, nref, m]`` whose window ``start + j`` step ``j`` tracks (``None``: the objective stays as it is).
+    Synchronous; resets the step counter.  A refused setup leaves the previous one as it was."""
+    nsteps, plant, W, Xref, Uref, start = _mpc_inputs(prob, nsteps, plant_params, disturbances, Xref, Uref, start)
+    spec = K.to_mpc_spec(nsteps, 0 if plant is None else plant.shape[1], K._dp(plant), K._dp(W), K._dp(Xref), K._dp(Uref),
+                         0 if Xref is None else Xref.shape[1], start)
+    prob._call("to_mpc_setup", C.byref(spec))
+    if Xref is not None:
+        prob._inst = True
+    prob._mpc = {"nsteps": nsteps, "done": 0}
+
+
+def mpc_run(prob, steps, iterations=1):
+    """Enqueues ``steps`` MPC steps and returns without waiting for them.  Step ``j`` (counted from ``mpc_setup``) of every instance: the
+    reference window (``update_trajectory`` with ``start + j``), ``rollout``, ``ilqr_step(iterations)``, then the plan's first control
+    drives the plant one knot-0 time step, ``x+ = step(x0, u_j) (+) w_j``, and the plan is shifted (``shift_trajectory(1)``) and restarted
+    from the plant (``set_initial_state(x+)``).  Bit for bit what that loop of calls computes, with no host round trip per step."""
+    mpc = getattr(prob, "_mpc", None)
+    if mpc is None:
+        raise ArgumentError("mpc_run before mpc_setup")
+    if int(steps) != steps or steps < 1 or int(iterations) != iterations or iterations < 1:
+        raise ArgumentError(f"mpc_run: steps and iterations must be positive integers, got {steps} and {iterations}")
+    if mpc["done"] + steps > mpc["nsteps"]:
+        raise DimensionMismatch(f"mpc_run: {mpc['done']} steps done + {steps} exceed the setup's nsteps = {mpc['nsteps']}")
+    prob._call("to_mpc_run", int(steps), int(iterations))
+    mpc["done"] += int(steps)
+
+
+def mpc_history(prob):
+    """``(X[B, s+1, n], U[B, s, m], J[B, s])`` of the ``s`` steps run since ``mpc_setup``: ``X[:, j]`` is the plant state step ``j``
+    started from and ``X[:, s]`` where the last step ended, ``U[:, j]`` the control it applied, ``J[:, j]`` the merit of its plan."""
+    mpc = getattr(prob, "_mpc", None)
+    if mpc is None:
+        raise ArgumentError("mpc_history before mpc_setup")
+    s = mpc["done"]
+    X, U, J = np.empty((prob.B, s + 1, prob.n)), np.empty((prob.B, s, prob.m)), np.empty((prob.B, s))
+    prob._call("to_mpc_history", K._dp(X), K._dp(U), K._dp(J))
+    return X, U, J
 
 
 def states(prob, k=None):   # states(prob)  src/problem.jl:175

@@ -63,6 +63,13 @@ struct to_handle {
     // AL penalties (DevProblem::mub), [B][ncon]: no host copy, the device scales the rows (k_al_update, to_solve's outer steps)
     int* d_go = nullptr;             // SolveDev::go, allocated with the penalty table
     std::vector<double> stage;       // the rows a setter is building, committed by commit_rows (kept to reuse its allocation)
+    bool qr_stale = false;           // to_mpc_run wrote DevProblem::qr on the device: h_qr is copied back before it is read (refresh_qr)
+    // closed-loop MPC (to_mpc_setup / to_mpc_run): the device copies of the inputs and the history live in one allocation, replaced by the
+    // next setup; mpc_done counts the steps enqueued since the setup
+    MpcDev mpc{};
+    void* mpc_buf = nullptr;
+    bool mpc_ready = false;
+    int mpc_done = 0, mpc_start = 1;
     int* d_fragerr = nullptr;     // sticky error word of that kernel (queue overflow / spin limit), read by to_synchronize
     double* d_fragpool = nullptr; // gains of its speculative regularisation candidates
     int* d_fragq = nullptr;       // work queue of the register-resident Riccati kernel (riccati_frag.cu)
@@ -767,6 +774,7 @@ int to_destroy(to_handle* h) {
     if (h->stream) cudaStreamSynchronize(h->stream);
     for (void* p : h->allocs) cudaFree(p);
     if (h->scratch.ptr) cudaFree(h->scratch.ptr);
+    if (h->mpc_buf) cudaFree(h->mpc_buf);
     for (auto& e : h->pending) { cudaEventDestroy(e.a); cudaEventDestroy(e.b); }
     for (auto e : h->pool) cudaEventDestroy(e);
     if (h->stream2) { cudaStreamSynchronize(h->stream2); cudaStreamDestroy(h->stream2); }
@@ -928,9 +936,22 @@ int to_set_initial_time(to_handle* h, double t0, double* tf_out) {
 static int hybrid_goals(to_handle* h) { return fail(h, TO_EINVAL, "per-instance goals are not supported on hybrid problems"); }
 static size_t q_off(const to_handle* h, int b, int cid) { return ((size_t)b * h->P.ncost + cid) * (h->P.n + h->P.m); }
 static size_t cd_off(const to_handle* h, int b, const DevCon& c) { return (size_t)b * h->P.ncdata + c.cdoff; }
+// h->h_qr := the device's rows when to_mpc_run has written them since the host copy was last current.  The only way h_qr is brought up to
+// date: every reader of it (to_get_cost_terms, stage_qr) calls this first.
+static int refresh_qr(to_handle* h) {
+    if (!h->qr_stale) return TO_OK;
+    CU(h, cudaMemcpyAsync(h->h_qr.data(), h->P.qr, sizeof(double) * h->h_qr.size(), cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    h->qr_stale = false;
+    return TO_OK;
+}
 // h->stage := the rows of the cost-term table, or every instance's shared terms when it does not exist yet
-static void stage_qr(to_handle* h) {
-    if (h->P.qr) { h->stage = h->h_qr; return; }
+static int stage_qr(to_handle* h) {
+    if (h->P.qr) {
+        int rc = refresh_qr(h); if (rc) return rc;
+        h->stage = h->h_qr;
+        return TO_OK;
+    }
     const int B = h->P.B, ncost = h->P.ncost, n = h->P.n, m = h->P.m;
     h->stage.resize((size_t)B * ncost * (n + m));
     for (int b = 0; b < B; b++)
@@ -938,6 +959,7 @@ static void stage_qr(to_handle* h) {
             std::memcpy(h->stage.data() + q_off(h, b, ci), h->h_costs[ci].q, sizeof(double) * n);
             std::memcpy(h->stage.data() + q_off(h, b, ci) + n, h->h_costs[ci].r, sizeof(double) * m);
         }
+    return TO_OK;
 }
 static size_t cw_off(const to_handle* h, int b, const DevCost& c) { return (size_t)b * h->P.ncw + c.cwoff; }
 // q | r of cost ci for instance b from the goal xf and, when uf is given, the control reference uf: with the instance's own Q and R once the
@@ -983,7 +1005,7 @@ int to_set_goal_state(to_handle* h, const double* xf, int objective, int constra
     int rc = upload_tables(h); if (rc) return rc;
     // the later call wins: every instance takes the shared goal, through its own weights once they are per instance
     if (objective && (h->P.qr || h->P.cw)) {
-        stage_qr(h);
+        rc = stage_qr(h); if (rc) return rc;
         for (int b = 0; b < h->P.B; b++)
             for (int ci = 0; ci < h->P.ncost; ci++) {
                 double* row = h->stage.data() + q_off(h, b, ci);
@@ -1008,10 +1030,10 @@ int to_set_goal_states(to_handle* h, const double* xf, int objective, int constr
     if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
     const int n = h->P.n;
     if (objective) {
-        stage_qr(h);
+        int rc = stage_qr(h); if (rc) return rc;
         for (int b = 0; b < h->P.B; b++)
             for (int ci = 0; ci < h->P.ncost; ci++) instance_linear_term(h, b, ci, xf + (size_t)b * n, nullptr, h->stage.data() + q_off(h, b, ci));
-        int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
+        rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
         h->J_valid = false;
     }
     if (constraint) {
@@ -1031,14 +1053,14 @@ int to_update_trajectories(to_handle* h, const double* Xref, const double* Uref,
     const int n = h->P.n, m = h->P.m, N = h->P.N;
     if (start < 1 || start - 1 + N > nref) return fail(h, TO_EDIM, "update_trajectory!: the reference is shorter than start + N - 1");
     if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
-    stage_qr(h);
+    int rc = stage_qr(h); if (rc) return rc;
     for (int b = 0; b < h->P.B; b++)
         for (int i = 0; i < N; i++) {                   // set_LQR_goal!(obj[i], state(Z[k]), control(Z[k])) of instance b
             const int cid = h->h_cost_index[i];
             instance_linear_term(h, b, cid, Xref + ((size_t)b * nref + start - 1 + i) * n, Uref + ((size_t)b * nref + start - 1 + i) * m,
                                  h->stage.data() + q_off(h, b, cid));
         }
-    int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
+    rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1046,6 +1068,7 @@ int to_update_trajectories(to_handle* h, const double* Xref, const double* Uref,
 int to_get_cost_terms(to_handle* h, double* q, double* r) {
     JOIN(h);
     if (!h || !q || !r) return TO_EINVAL;
+    int rc = refresh_qr(h); if (rc) return rc;
     const int n = h->P.n, m = h->P.m, ncost = h->P.ncost;
     for (int b = 0; b < h->P.B; b++)
         for (int ci = 0; ci < ncost; ci++) {
@@ -1091,23 +1114,19 @@ int to_set_cost_terms(to_handle* h, const double* q, const double* r) {
             std::memcpy(h->stage.data() + q_off(h, b, ci) + n, r + ((size_t)b * ncost + ci) * m, sizeof(double) * m);
         }
     int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
+    h->qr_stale = false;                                  // every row was written
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
 
 // ---- per-instance model parameters (DevProblem::mparams) ----------------------------------------------------------
-// params [B][nparams] in the order of to_spec.params.  The whole batch is checked before anything changes: a refused call leaves the rows
-// (or their absence) as they were.  X is not rolled out again (set_initial_state! does not either); the next rollout, expansion, line
-// search or solve integrates with the new values.
-int to_set_model_params(to_handle* h, const double* params, int32_t nparams) {
-    JOIN(h);
-    if (!h || !params) return TO_EINVAL;
+// rows := params [B][nparams] checked and completed into the layout of DevProblem::mparams ([B][TO_NPARAM]); `what` names the caller in
+// the messages.  The checks of every per-instance parameter row: to_set_model_params and to_mpc_setup's plant rows.
+static int model_param_rows(to_handle* h, const double* params, int32_t nparams, const char* what, std::vector<double>& rows) {
     const int model = h->P.model, B = h->P.B;
-    if (model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance model parameters are not supported on hybrid problems (their constants live in the recorded programs)");
     const int np = model_nparams(model);
     if (nparams != np)
-        return fail(h, TO_EDIM, "to_set_model_params: the model takes " + std::to_string(np) + " parameters per instance, got " + std::to_string(nparams));
-    std::vector<double>& rows = h->stage;
+        return fail(h, TO_EDIM, std::string(what) + ": the model takes " + std::to_string(np) + " parameters per instance, got " + std::to_string(nparams));
     rows.assign((size_t)B * TO_NPARAM, 0.0);
     for (int b = 0; b < B; b++) {
         double* row = rows.data() + (size_t)b * TO_NPARAM;
@@ -1115,14 +1134,24 @@ int to_set_model_params(to_handle* h, const double* params, int32_t nparams) {
             const double v = params[(size_t)b * np + i];
             const char* pos = positive_param_name(model, i);
             if (!std::isfinite(v))
-                return fail(h, TO_EINVAL, "to_set_model_params: instance " + std::to_string(b) + ", parameter " + std::to_string(i) + " is not finite");
+                return fail(h, TO_EINVAL, std::string(what) + ": instance " + std::to_string(b) + ", parameter " + std::to_string(i) + " is not finite");
             if (pos && !(v > 0))
-                return fail(h, TO_EINVAL, "to_set_model_params: instance " + std::to_string(b) + ", parameter " + std::to_string(i) + " (" + pos + ") must be positive");
+                return fail(h, TO_EINVAL, std::string(what) + ": instance " + std::to_string(b) + ", parameter " + std::to_string(i) + " (" + pos + ") must be positive");
             row[i] = v;
         }
         complete_model_params(model, row);
     }
-    int rc = commit_rows(h, h->h_mparams, h->P.mparams); if (rc) return rc;
+    return TO_OK;
+}
+// params [B][nparams] in the order of to_spec.params.  The whole batch is checked before anything changes: a refused call leaves the rows
+// (or their absence) as they were.  X is not rolled out again (set_initial_state! does not either); the next rollout, expansion, line
+// search or solve integrates with the new values.
+int to_set_model_params(to_handle* h, const double* params, int32_t nparams) {
+    JOIN(h);
+    if (!h || !params) return TO_EINVAL;
+    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance model parameters are not supported on hybrid problems (their constants live in the recorded programs)");
+    int rc = model_param_rows(h, params, nparams, "to_set_model_params", h->stage); if (rc) return rc;
+    rc = commit_rows(h, h->h_mparams, h->P.mparams); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1314,7 +1343,7 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     int rc = upload_tables(h); if (rc) return rc;
     if (!h->P.qr && !h->P.cw) return TO_OK;
-    stage_qr(h);
+    rc = stage_qr(h); if (rc) return rc;
     for (int b = 0; b < h->P.B; b++)                    // the later call wins: every instance takes the shared reference, through its own weights
         for (int i = 0; i < N; i++) {
             const int cid = h->h_cost_index[i];
@@ -1327,16 +1356,21 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
         }
     return commit_rows(h, h->h_qr, h->P.qr);
 }
+// the host's clocks after a shift by `steps` knots (to_shift_trajectory, each step of to_mpc_run): the shared one by the shared steps, each
+// instance's by its own skipped steps, in the same order (the rows stay)
+static void advance_clocks(to_handle* h, int steps) {
+    for (int k = 0; k < steps; k++) h->t0 += h->h_dt[k];
+    const int K = h->P.N - 1;
+    for (size_t b = 0; b < h->t0b.size(); b++)
+        for (int k = 0; k < steps; k++) h->t0b[b] += h->h_dtb[b * K + k];
+}
 int to_shift_trajectory(to_handle* h, int32_t steps) {
     JOIN(h);
     if (!h || steps < 0) return TO_EINVAL;
     if (steps == 0) return TO_OK;
     if (steps > h->P.N - 1) steps = h->P.N - 1;
     CU(h, launch_shift_traj(h->P, steps, h->stream)); h->launches++;
-    for (int k = 0; k < steps; k++) h->t0 += h->h_dt[k];
-    const int K = h->P.N - 1;
-    for (size_t b = 0; b < h->t0b.size(); b++)            // each instance's clock by its own skipped steps, in the same order (the rows stay)
-        for (int k = 0; k < steps; k++) h->t0b[b] += h->h_dtb[b * K + k];
+    advance_clocks(h, steps);
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1776,6 +1810,121 @@ int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* 
     CU(h, cudaStreamSynchronize(h->stream));
     return TO_OK;
 }
+// ---- closed-loop MPC (include/trajopt_b200.h, DESIGN.md 5l) ---------------------------------------------------------------------
+static std::string inst_msg(const char* what, int b, const char* rest) { return std::string(what) + ": instance " + std::to_string(b) + rest; }
+int to_mpc_setup(to_handle* h, const to_mpc_spec* s) {
+    JOIN(h);
+    if (!h || !s) return TO_EINVAL;
+    const int B = h->P.B, n = h->P.n, m = h->P.m, N = h->P.N, ne = h->P.ne, ncost = h->P.ncost;
+    // one recorded model stepping every knot (a single AutodiffDynamics model) is a plant like any other; a hybrid problem is not
+    if (h->P.model == MODEL_EXPR && (h->h_dyn.size() != 1 || h->h_dyn[0].discrete || h->h_dyn[0].n_out != h->h_dyn[0].n_in))
+        return fail(h, TO_EINVAL, "to_mpc_setup: closed-loop MPC is not supported on hybrid problems");
+    if (s->nsteps < 1) return fail(h, TO_EINVAL, "to_mpc_setup: nsteps must be >= 1");
+    const bool ref = s->Xref || s->Uref;
+    const int nref = ref ? s->nref : 0;
+    if (h->P.model == MODEL_EXPR && (ref || s->plant_params))
+        return fail(h, TO_EINVAL, "to_mpc_setup: a recorded-program model takes no reference window and no plant parameters (per-instance goals and "
+                                  "parameters are not supported on it)");
+    if (ref) {
+        if (!s->Xref || !s->Uref) return fail(h, TO_EINVAL, "to_mpc_setup: Xref and Uref are given together");
+        if (s->start < 1 || (long long)s->start - 1 + (s->nsteps - 1) + N > s->nref)
+            return fail(h, TO_EDIM, "to_mpc_setup: the reference is shorter than start - 1 + (nsteps - 1) + N");
+    }
+    // every check before anything changes: a refused setup leaves the previous one as it was
+    std::vector<double> plant;
+    if (s->plant_params) { int rc = model_param_rows(h, s->plant_params, s->nparams, "to_mpc_setup (plant parameters)", plant); if (rc) return rc; }
+    auto finite_rows = [&](const double* a, size_t per, const char* what, const char* rest) {
+        for (int b = 0; b < B; b++)
+            for (size_t i = 0; i < per; i++)
+                if (!std::isfinite(a[(size_t)b * per + i])) return fail(h, TO_EINVAL, inst_msg(what, b, rest));
+        return TO_OK;
+    };
+    int rc = TO_OK;
+    if (s->W) rc = finite_rows(s->W, (size_t)s->nsteps * ne, "to_mpc_setup", ": a disturbance is not finite");
+    if (!rc && ref) rc = finite_rows(s->Xref, (size_t)nref * n, "to_mpc_setup", ": the state reference is not finite");
+    if (!rc && ref) rc = finite_rows(s->Uref, (size_t)nref * m, "to_mpc_setup", ": the control reference is not finite");
+    if (rc) return rc;
+    // one allocation: Xref | Uref | W | plant | Xcl | Ucl | Jcl (doubles), then last_knot (ints)
+    const size_t S = s->nsteps;
+    const size_t nX = ref ? (size_t)B * nref * n : 0, nU = ref ? (size_t)B * nref * m : 0, nW = s->W ? (size_t)B * S * ne : 0;
+    const size_t nP = plant.size(), nXc = (size_t)B * (S + 1) * n, nUc = (size_t)B * S * m, nJ = (size_t)B * S;
+    const size_t nd = nX + nU + nW + nP + nXc + nUc + nJ;
+    void* buf = nullptr;
+    cudaError_t e = cudaMalloc(&buf, nd * sizeof(double) + (size_t)ncost * sizeof(int));
+    if (e != cudaSuccess) return cuda_fail(h, e, "cudaMalloc(mpc)");
+    MpcDev M{};
+    double* d = static_cast<double*>(buf);
+    auto take = [&](size_t cnt) { double* p = cnt ? d : nullptr; d += cnt; return p; };
+    M.Xref = take(nX); M.Uref = take(nU); M.W = take(nW); M.plant = take(nP);
+    M.Xcl = take(nXc); M.Ucl = take(nUc); M.Jcl = take(nJ);
+    M.last_knot = reinterpret_cast<int*>(d);
+    M.nref = nref; M.nsteps = s->nsteps;
+    std::vector<int> last(ncost, -1);
+    for (int k = 0; k < N; k++) last[h->h_cost_index[k]] = k;      // the host's update_trajectory! writes knot k's cost row k-th: the last knot wins
+    auto up = [&](const void* dst, const void* src, size_t bytes) {
+        return bytes ? cudaMemcpyAsync(const_cast<void*>(dst), src, bytes, cudaMemcpyHostToDevice, h->stream) : cudaSuccess;
+    };
+    e = up(M.Xref, s->Xref, nX * sizeof(double));
+    if (e == cudaSuccess) e = up(M.Uref, s->Uref, nU * sizeof(double));
+    if (e == cudaSuccess) e = up(M.W, s->W, nW * sizeof(double));
+    if (e == cudaSuccess) e = up(M.plant, plant.data(), nP * sizeof(double));
+    if (e == cudaSuccess) e = up(M.last_knot, last.data(), (size_t)ncost * sizeof(int));
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);     // the host arrays are the sources of the copies
+    if (e != cudaSuccess) { cudaFree(buf); return cuda_fail(h, e, "to_mpc_setup: upload"); }
+    if (ref && !h->P.qr) {   // the per-instance linear terms the window writes: created as to_update_trajectories creates them
+        rc = stage_qr(h);
+        if (!rc) rc = commit_rows(h, h->h_qr, h->P.qr);
+        if (rc) { cudaFree(buf); return rc; }
+    }
+    if (h->mpc_buf) cudaFree(h->mpc_buf);     // (the stream was synchronised above: no kernel of an earlier run reads it)
+    h->mpc_buf = buf; h->mpc = M; h->mpc_ready = true; h->mpc_done = 0; h->mpc_start = ref ? s->start : 1;
+    return TO_OK;
+}
+// Enqueues `steps` MPC steps and returns.  Step j runs what the host-scripted loop of entry points runs, launch for launch: the window (with a
+// reference), to_rollout, to_ilqr_step(iterations) (the merit, then the iterations), and one advance kernel in place of to_get_controls /
+// to_merit, the plant and to_shift_trajectory(1) + to_set_initial_state.  No host synchronisation: the advance waits for the side stream's
+// late line-search trials through join_side, a stream wait on an event.
+int to_mpc_run(to_handle* h, int32_t steps, int32_t iterations) {
+    JOIN(h);
+    if (!h) return TO_EINVAL;
+    if (!h->mpc_ready) return fail(h, TO_ESTATE, "to_mpc_run before to_mpc_setup");
+    if (steps < 1 || iterations < 1) return fail(h, TO_EINVAL, "to_mpc_run: steps and iterations must be >= 1");
+    if ((long long)h->mpc_done + steps > h->mpc.nsteps)
+        return fail(h, TO_EDIM, "to_mpc_run: " + std::to_string(h->mpc_done) + " steps done + " + std::to_string(steps) + " exceed the setup's nsteps = " +
+                                    std::to_string(h->mpc.nsteps));
+    int rc = solver_supported(h); if (rc) return rc;
+    for (int st = 0; st < steps; st++) {
+        const int j = h->mpc_done;
+        if (h->mpc.Xref) {   // 1. the reference window of step j (to_update_trajectories(Xref, Uref, nref, start + j))
+            CU(h, launch_mpc_window(h->P, h->mpc, h->mpc_start - 1 + j, h->stream)); h->launches++;
+            h->qr_stale = true;
+        }
+        CU(h, launch_rollout(h->P, h->stream)); h->launches++;       // 2. to_rollout
+        h->J_valid = false; h->expanded = false; h->backward_done = false;
+        rc = ensure_merit(h); if (rc) return rc;                     // 3. to_ilqr_step(iterations)
+        for (int it = 0; it < iterations; it++) { rc = ilqr_iteration(h, nullptr, 0); if (rc) return rc; }
+        rc = join_side(h); if (rc) return rc;                        // the late trials write U and J of their instances
+        CU(h, launch_mpc_advance(h->P, h->mpc, j, h->stream)); h->launches++;    // 4.-6. record, plant, shift, x0
+        advance_clocks(h, 1);
+        h->mpc_done++;
+        h->J_valid = false; h->expanded = false; h->backward_done = false;
+    }
+    return TO_OK;
+}
+int to_mpc_history(to_handle* h, double* Xcl, double* Ucl, double* J) {
+    JOIN(h);
+    if (!h) return TO_EINVAL;
+    if (!h->mpc_ready) return fail(h, TO_ESTATE, "to_mpc_history before to_mpc_setup");
+    const int B = h->P.B, n = h->P.n, m = h->P.m, s = h->mpc_done, S = h->mpc.nsteps;
+    const size_t w = sizeof(double);
+    if (Xcl && s == 0) CU(h, cudaMemcpyAsync(Xcl, h->P.x0, (size_t)B * n * w, cudaMemcpyDeviceToHost, h->stream));   // no step yet: where the next starts
+    else if (Xcl) CU(h, cudaMemcpy2DAsync(Xcl, (size_t)(s + 1) * n * w, h->mpc.Xcl, (size_t)(S + 1) * n * w, (size_t)(s + 1) * n * w, B, cudaMemcpyDeviceToHost, h->stream));
+    if (Ucl && s) CU(h, cudaMemcpy2DAsync(Ucl, (size_t)s * m * w, h->mpc.Ucl, (size_t)S * m * w, (size_t)s * m * w, B, cudaMemcpyDeviceToHost, h->stream));
+    if (J && s) CU(h, cudaMemcpy2DAsync(J, (size_t)s * w, h->mpc.Jcl, (size_t)S * w, (size_t)s * w, B, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return TO_OK;
+}
+
 // ---- Lie-group error state (lie.cu) ---------------------------------------------------------------------------
 int to_backward_algebra(const to_handle* h, int32_t* variant) {
     if (!h || !variant) return TO_EINVAL;

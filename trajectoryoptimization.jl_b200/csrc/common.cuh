@@ -305,6 +305,28 @@ __host__ __device__ inline const double* traj_U(const DevProblem& P, int buf, in
 __host__ __device__ inline double* traj_Xw(const DevProblem& P, int buf, int b) { return P.X + buf * P.strideX + (size_t)b * P.N * P.n; }
 __host__ __device__ inline double* traj_Uw(const DevProblem& P, int buf, int b) { return P.U + buf * P.strideU + (size_t)b * (P.N - 1) * P.m; }
 
+// The receding-horizon shift of instance b by `steps` knots, run by the whole CTA (sweep.cu k_shift_traj, rollout.cu k_mpc_advance): the
+// trajectory goes to the next ring buffer, the multipliers shift in place (thread = one row of one constraint, ascending knots: reads
+// k+steps, writes k), x0 <- X[steps] (thread i writes x0[i]).  Ends with a barrier and the move of cur[b].
+__device__ __forceinline__ void shift_traj_cta(const DevProblem& P, int b, int steps) {
+    const int n = P.n, m = P.m, N = P.N;
+    const int src = P.cur[b], dst = (src + 1) % TO_NBUF;
+    const double* X = traj_X(P, src, b); const double* U = traj_U(P, src, b);
+    double* Xn = traj_Xw(P, dst, b); double* Un = traj_Uw(P, dst, b);
+    for (int i = threadIdx.x; i < N * n; i += blockDim.x) { int k = i / n + steps; if (k > N - 1) k = N - 1; Xn[i] = X[k * n + i % n]; }
+    for (int i = threadIdx.x; i < (N - 1) * m; i += blockDim.x) { int k = i / m + steps; if (k > N - 2) k = N - 2; Un[i] = U[k * m + i % m]; }
+    for (int i = threadIdx.x; i < n; i += blockDim.x) { int k = steps < N - 1 ? steps : N - 1; P.x0[(size_t)b * n + i] = X[k * n + i]; }
+    double* lam = P.lambda + (size_t)b * P.lambda_len;
+    for (int ci = 0; ci < P.ncon; ci++) {
+        const DevCon& c = P.cons[ci];
+        const int nk = c.last - c.first + 1;
+        for (int r = threadIdx.x; r < c.p; r += blockDim.x)
+            for (int k = 0; k + steps < nk; k++) lam[c.offset + k * c.p + r] = lam[c.offset + (k + steps) * c.p + r];
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) P.cur[b] = dst;
+}
+
 // One process may hold handles on several GPUs (to_spec.device): function attributes and occupancy are per device, so the
 // launchers cache their one-time configuration per device ordinal.
 #define TO_MAXDEV 64

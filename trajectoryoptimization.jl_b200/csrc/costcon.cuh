@@ -584,6 +584,21 @@ __device__ __forceinline__ void state_diff(bool lie, int n, int qs, const double
     quat_diff(x + qs, xbar + qs, dx + qs);
     for (int i = qs + 4; i < n; i++) dx[i - 1] = xbar[i] - x[i];
 }
+// x <- x (+) w in place, w[ne]: the inverse of state_diff, state_diff(x (+) w, x) = w.  Vector-space states add; the quaternion composes
+// with the Cayley map of its three entries, q (x) (1, phi) / sqrt(1 + phi'phi), whose inverse quat_diff is
+__device__ __forceinline__ void state_add(bool lie, int n, int qs, double* x, const double* w) {
+    if (!lie) { for (int i = 0; i < n; i++) x[i] = x[i] + w[i]; return; }
+    for (int i = 0; i < qs; i++) x[i] = x[i] + w[i];
+    for (int i = qs + 4; i < n; i++) x[i] = x[i] + w[i - 1];
+    const double p1 = w[qs], p2 = w[qs + 1], p3 = w[qs + 2];
+    const double s = 1.0 / sqrt(1.0 + (p1 * p1 + p2 * p2 + p3 * p3));
+    const double c0 = s, c1 = p1 * s, c2 = p2 * s, c3 = p3 * s;
+    const double q0 = x[qs], q1 = x[qs + 1], q2 = x[qs + 2], q3 = x[qs + 3];
+    x[qs] = q0 * c0 - q1 * c1 - q2 * c2 - q3 * c3;
+    x[qs + 1] = q0 * c1 + q1 * c0 + q2 * c3 - q3 * c2;
+    x[qs + 2] = q0 * c2 - q1 * c3 + q2 * c0 + q3 * c1;
+    x[qs + 3] = q0 * c3 + q1 * c2 - q2 * c1 + q3 * c0;
+}
 
 // Compact error-state expansion of knot k of instance b (P.compact: DiagonalCost objective, Goal / Bound constraints, n_e + m = 16 -- the
 // BASELINE problem class).  The full-state expansion is a gradient g and a DIAGONAL h, so the error-state one is G'g, the same diagonal

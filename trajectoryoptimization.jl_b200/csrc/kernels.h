@@ -16,12 +16,28 @@ template <int RULE> cudaError_t launch_expand_rule(const DevProblem& P, cudaStre
 template <int RULE> cudaError_t launch_expand_lie_rule(const DevProblem& P, cudaStream_t s, int mode);
 template <int RULE> cudaError_t launch_forward_rule(const DevProblem& P, cudaStream_t s);
 template <int RULE> cudaError_t launch_ladder_rule(const DevProblem& P, cudaStream_t s);
+// Closed-loop MPC (to_mpc_run): the device copies of the run's inputs, made by to_mpc_setup, and the history the run writes.
+struct MpcDev {
+    const double* Xref;        // [B][nref][n] or nullptr: no reference window
+    const double* Uref;        // [B][nref][m]
+    const int* last_knot;      // [ncost]: the last knot that uses each cost (-1: none), the row the host's update_trajectory! writes last
+    const double* W;           // [B][nsteps][ne] or nullptr: no disturbance
+    const double* plant;       // [B][TO_NPARAM] (the layout of DevProblem::mparams) or nullptr: the planner's parameters
+    double* Xcl;               // [B][nsteps+1][n]: row j = the state step j started from, row j+1 = where it ended
+    double* Ucl;               // [B][nsteps][m]
+    double* Jcl;               // [B][nsteps]: the merit of the plan step j applied
+    int nref, nsteps;
+};
+cudaError_t launch_mpc_window(const DevProblem& P, const MpcDev& M, int row, cudaStream_t s);   // sweep.cu: the linear terms of reference row `row`
+cudaError_t launch_mpc_advance(const DevProblem& P, const MpcDev& M, int j, cudaStream_t s);    // rollout.cu: record, plant step, shift of step j
+template <int RULE> cudaError_t launch_mpc_advance_rule(const DevProblem& P, const MpcDev& M, int j, cudaStream_t s);
 #define TO_RULE_EXTERN(R)                                                                                   \
     extern template cudaError_t launch_rollout_rule<R>(const DevProblem&, cudaStream_t);                  \
     extern template cudaError_t launch_expand_rule<R>(const DevProblem&, cudaStream_t, int);              \
     extern template cudaError_t launch_expand_lie_rule<R>(const DevProblem&, cudaStream_t, int);          \
     extern template cudaError_t launch_forward_rule<R>(const DevProblem&, cudaStream_t);                  \
-    extern template cudaError_t launch_ladder_rule<R>(const DevProblem&, cudaStream_t);
+    extern template cudaError_t launch_ladder_rule<R>(const DevProblem&, cudaStream_t);                   \
+    extern template cudaError_t launch_mpc_advance_rule<R>(const DevProblem&, const MpcDev&, int, cudaStream_t);
 TO_RULE_EXTERN(1)
 TO_RULE_EXTERN(2)
 TO_RULE_EXTERN(3)

@@ -12,6 +12,7 @@
 //               adjacent lanes; the pad columns of a row (LDAB > n+m) are never touched and stay zero.
 #include <cstdlib>
 
+#include "costcon.cuh"
 #include "frag_layout.cuh"
 #include "kernels.h"
 #include "models.cuh"
@@ -66,6 +67,58 @@ __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
 #pragma unroll
         for (int i = 0; i < n; i++) x[i] = xn[i];
     }
+}
+
+// to_mpc_run, steps 4-6 of MPC step j, CTA = instance b.  Warp 0 steps the plant: k_rollout's loop over a trajectory of `knots` = 2 knots
+// (x0, x+), written as k_rollout writes it -- the parameters staged per lane, the knot count read at run time, the state staged in shared
+// memory behind a warp barrier every knot -- so that the compiler hoists and contracts the step's arithmetic as it does in k_rollout, and
+// the plant computes k_rollout's bits: explicit_step<MODEL, double, RULE> on model_params<MODEL, INST> (the launcher's view carries the plant's
+// rows as DevProblem::mparams) over knot 0's time step.  Every lane steps instance b; lane 0 applies the disturbance, x+ = step(x0, u_j) (+) w_j
+// (costcon.cuh state_add), and records x0, x+, u_j = U[0] and the plan's merit J_j.  Then the CTA shifts the plan by one knot
+// (shift_traj_cta, k_shift_traj's body), and x+ overwrites the x0 the shift wrote (each thread its own entry): the next step starts from the
+// plant.
+template <int MODEL, bool INST, int RULE>
+__global__ void __launch_bounds__(128) k_mpc_advance(const DevProblem P, const MpcDev M, int j, int knots) {
+    constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m;
+    __shared__ double xp[n];
+    const int b = blockIdx.x;
+    if (threadIdx.x < 32) {
+        __shared__ double stage[32 * n];
+        const int lane = threadIdx.x;
+        const double* U = traj_U(P, P.cur[b], b);
+        const double* prm = nullptr;
+        if constexpr (INST) {
+            __shared__ double prm_s[32][TO_NPARAM];
+            stage_model_params<INST>(P, b, prm_s[lane]);
+            prm = prm_s[lane];
+        }
+        double x[n], u[m], xn[n];
+#pragma unroll
+        for (int i = 0; i < n; i++) x[i] = P.x0[(size_t)b * n + i];
+        for (int k = 0; k < knots; k++) {
+#pragma unroll
+            for (int i = 0; i < n; i++) stage[lane * n + i] = x[i];
+            __syncwarp();
+            if (k == knots - 1) break;
+#pragma unroll
+            for (int i = 0; i < m; i++) u[i] = U[k * m + i];
+            explicit_step<MODEL, double, RULE>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k), xn);
+#pragma unroll
+            for (int i = 0; i < n; i++) x[i] = xn[i];
+        }
+        if (lane == 0) {
+            if (M.W) state_add(P.lie != 0, n, P.qs, x, M.W + ((size_t)b * M.nsteps + j) * P.ne);
+            double* Xh = M.Xcl + ((size_t)b * (M.nsteps + 1) + j) * n;
+#pragma unroll
+            for (int i = 0; i < n; i++) { Xh[i] = P.x0[(size_t)b * n + i]; Xh[n + i] = x[i]; xp[i] = x[i]; }
+#pragma unroll
+            for (int i = 0; i < m; i++) M.Ucl[((size_t)b * M.nsteps + j) * m + i] = U[i];
+            M.Jcl[(size_t)b * M.nsteps + j] = P.J[b];
+        }
+    }
+    __syncthreads();
+    shift_traj_cta(P, b, 1);
+    if (threadIdx.x < n) P.x0[(size_t)b * n + threadIdx.x] = xp[threadIdx.x];
 }
 
 // Seed pruning (full state).  The position r and the world-frame linear velocity v of the Quadrotor (a RobotDynamics RigidBody) enter the
@@ -640,9 +693,21 @@ cudaError_t launch_expand_rule(const DevProblem& P, cudaStream_t s, int mode) {
     return e;
 }
 
+// the plant's parameters: its own rows when to_mpc_setup was given them, else the planner's (per instance when set); the INST variant runs
+// exactly when k_rollout's would on a problem holding those rows and the planner's time steps
+template <int RULE>
+cudaError_t launch_mpc_advance_rule(const DevProblem& P, const MpcDev& M, int j, cudaStream_t s) {
+    DevProblem Q = P;
+    if (M.plant) Q.mparams = M.plant;
+    if (inst_dynamics(Q)) { TO_DISPATCH_MODEL(Q.model, Q.m, (k_mpc_advance<MODEL, true, RULE><<<Q.B, 128, 0, s>>>(Q, M, j, 2))); }
+    else { TO_DISPATCH_MODEL(Q.model, Q.m, (k_mpc_advance<MODEL, false, RULE><<<Q.B, 128, 0, s>>>(Q, M, j, 2))); }
+    return cudaGetLastError();
+}
+
 template cudaError_t launch_expand_lie_rule<TO_RULE>(const DevProblem&, cudaStream_t, int);
 template cudaError_t launch_rollout_rule<TO_RULE>(const DevProblem&, cudaStream_t);
 template cudaError_t launch_expand_rule<TO_RULE>(const DevProblem&, cudaStream_t, int);
+template cudaError_t launch_mpc_advance_rule<TO_RULE>(const DevProblem&, const MpcDev&, int, cudaStream_t);
 
 #if TO_RULE == 4
 cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
@@ -658,6 +723,11 @@ cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s) {
 cudaError_t launch_expand(const DevProblem& P, cudaStream_t s, int mode) {
     cudaError_t e = cudaErrorNotSupported;
     TO_DISPATCH_RULE(P.integration, (e = launch_expand_rule<RULE>(P, s, mode)));
+    return e;
+}
+cudaError_t launch_mpc_advance(const DevProblem& P, const MpcDev& M, int j, cudaStream_t s) {
+    cudaError_t e = cudaErrorNotSupported;
+    TO_DISPATCH_RULE(P.integration, (e = launch_mpc_advance_rule<RULE>(P, M, j, s)));
     return e;
 }
 #endif

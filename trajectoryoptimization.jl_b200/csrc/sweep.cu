@@ -307,28 +307,42 @@ cudaError_t launch_reduce_merit(const DevProblem& P, const double* viol, double*
     k_reduce_merit<<<1, 1024, 0, s>>>(P.B, P.J, viol, out2);
     return cudaGetLastError();
 }
-// receding-horizon shift (to_shift_trajectory): CTA = instance; the trajectory goes to the next ring buffer, the
-// multipliers shift in place (thread = one row of one constraint, ascending knots: reads k+steps, writes k)
-__global__ void k_shift_traj(const DevProblem P, int steps) {
-    const int b = blockIdx.x, n = P.n, m = P.m, N = P.N;
-    const int src = P.cur[b], dst = (src + 1) % TO_NBUF;
-    const double* X = traj_X(P, src, b); const double* U = traj_U(P, src, b);
-    double* Xn = traj_Xw(P, dst, b); double* Un = traj_Uw(P, dst, b);
-    for (int i = threadIdx.x; i < N * n; i += blockDim.x) { int k = i / n + steps; if (k > N - 1) k = N - 1; Xn[i] = X[k * n + i % n]; }
-    for (int i = threadIdx.x; i < (N - 1) * m; i += blockDim.x) { int k = i / m + steps; if (k > N - 2) k = N - 2; Un[i] = U[k * m + i % m]; }
-    for (int i = threadIdx.x; i < n; i += blockDim.x) { int k = steps < N - 1 ? steps : N - 1; P.x0[(size_t)b * n + i] = X[k * n + i]; }
-    double* lam = P.lambda + (size_t)b * P.lambda_len;
-    for (int ci = 0; ci < P.ncon; ci++) {
-        const DevCon& c = P.cons[ci];
-        const int nk = c.last - c.first + 1;
-        for (int r = threadIdx.x; r < c.p; r += blockDim.x)
-            for (int k = 0; k + steps < nk; k++) lam[c.offset + k * c.p + r] = lam[c.offset + (k + steps) * c.p + r];
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) P.cur[b] = dst;
-}
+// receding-horizon shift (to_shift_trajectory): CTA = instance (common.cuh shift_traj_cta)
+__global__ void k_shift_traj(const DevProblem P, int steps) { shift_traj_cta(P, blockIdx.x, steps); }
 cudaError_t launch_shift_traj(const DevProblem& P, int steps, cudaStream_t s) {
     k_shift_traj<<<P.B, 128, 0, s>>>(P, steps);
+    return cudaGetLastError();
+}
+
+// to_mpc_run's reference window of step j: the linear terms to_update_trajectories(Xref, Uref, nref, row + 1) writes on the host (capi.cu
+// instance_linear_term).  Cost ci tracks the last knot i that uses it (M.last_knot): q = -Q xref[row + i], r = -R uref[row + i], with the
+// instance's own Q and R when it has a weight row (the dense matrices capi.cu cost_row_QR builds from it).  Thread = one entry of one
+// (instance, cost) row; the products and the sum in the host's order, each rounded on its own (the host code is compiled without FMA).
+__global__ void k_mpc_window(const DevProblem P, const MpcDev M, int row) {
+    const int n = P.n, m = P.m, nm = n + m;
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= (long long)P.B * P.ncost * nm) return;
+    const int e = (int)(t % nm), ci = (int)((t / nm) % P.ncost), b = (int)(t / ((long long)nm * P.ncost));
+    const int i = M.last_knot[ci];
+    if (i < 0) return;                                   // no knot uses the cost: its row stays
+    const DevCost& c = P.costs[ci];
+    const bool st = e < n;
+    const int dim = st ? n : m, r = st ? e : e - n;
+    const double* ref = st ? M.Xref + ((size_t)b * M.nref + row + i) * n : M.Uref + ((size_t)b * M.nref + row + i) * m;
+    const double* w = (P.cw && c.cwoff >= 0) ? P.cw + (size_t)b * P.ncw + c.cwoff : nullptr;
+    double acc = 0.0;
+    for (int jj = 0; jj < dim; jj++) {
+        double a;                                        // column-major entry (r, jj) of Q or R
+        if (!w) a = st ? c.Q[jj * dim + r] : c.R[jj * dim + r];
+        else if (c.diag) a = jj == r ? w[st ? r : n + r] : 0.0;
+        else a = st ? w[jj * dim + r] : w[n * n + jj * dim + r];
+        acc = __dadd_rn(acc, __dmul_rn(a, ref[jj]));
+    }
+    const_cast<double*>(P.qr)[((size_t)b * P.ncost + ci) * nm + e] = -acc;
+}
+cudaError_t launch_mpc_window(const DevProblem& P, const MpcDev& M, int row, cudaStream_t s) {
+    if (!P.qr) return cudaErrorInvalidValue;             // to_mpc_setup creates the table
+    k_mpc_window<<<nblk((long long)P.B * P.ncost * (P.n + P.m), 128), 128, 0, s>>>(P, M, row);
     return cudaGetLastError();
 }
 

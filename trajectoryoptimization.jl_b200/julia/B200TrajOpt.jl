@@ -464,6 +464,48 @@ function TO.update_trajectory!(p::BatchedProblem, Xref::Array{Float64,3}, Uref::
 end
 shift_trajectory!(p::BatchedProblem, steps::Integer=1) = check(p.h, ccall((:to_shift_trajectory, libb200), Cint, (Ptr{Cvoid}, Int32), p.h, steps))
 
+# closed-loop MPC on the device (to_mpc_spec field for field): a receding-horizon simulation of every instance, no host round trip per step
+struct ToMpcSpec
+    nsteps::Int32; nparams::Int32
+    plant_params::Ptr{Float64}; W::Ptr{Float64}; Xref::Ptr{Float64}; Uref::Ptr{Float64}
+    nref::Int32; start::Int32
+end
+const MPC_STEPS = WeakKeyDict{BatchedProblem,Vector{Int}}()    # [steps done, nsteps] since the last mpc_setup!
+# plant_params (nparams, B) or nothing; W (n_e, nsteps, B) or nothing; Xref (n, nref, B) and Uref (m, nref, B) or nothing
+function mpc_setup!(p::BatchedProblem, nsteps::Integer; plant_params=nothing, W=nothing, Xref=nothing, Uref=nothing, start::Integer=1)
+    P = plant_params === nothing ? nothing : Matrix{Float64}(plant_params)
+    Wd = W === nothing ? nothing : Array{Float64,3}(W)
+    Xr = Xref === nothing ? nothing : Array{Float64,3}(Xref)
+    Ur = Uref === nothing ? nothing : Array{Float64,3}(Uref)
+    P === nothing || size(P, 2) == p.B || throw(DimensionMismatch("plant_params must be (nparams, B)"))
+    Wd === nothing || (size(Wd, 2) == nsteps && size(Wd, 3) == p.B) || throw(DimensionMismatch("W must be (n_e, nsteps, B)"))
+    (Xr === nothing) == (Ur === nothing) || throw(ArgumentError("Xref and Uref are given together"))
+    Xr === nothing || (size(Xr, 3) == p.B && size(Ur, 3) == p.B && size(Ur, 2) == size(Xr, 2)) || throw(DimensionMismatch("Xref (n, nref, B), Uref (m, nref, B)"))
+    ptr(a) = a === nothing ? Ptr{Float64}(C_NULL) : pointer(a)
+    GC.@preserve P Wd Xr Ur begin
+        spec = ToMpcSpec(nsteps, P === nothing ? 0 : size(P, 1), ptr(P), ptr(Wd), ptr(Xr), ptr(Ur), Xr === nothing ? 0 : size(Xr, 2), start)
+        check(p.h, ccall((:to_mpc_setup, libb200), Cint, (Ptr{Cvoid}, Ref{ToMpcSpec}), p.h, spec))
+    end
+    MPC_STEPS[p] = [0, Int(nsteps)]
+    nothing
+end
+# enqueues `steps` MPC steps of `iterations` iLQR iterations each and returns without waiting for them
+function mpc_run!(p::BatchedProblem, steps::Integer; iterations::Integer=1)
+    haskey(MPC_STEPS, p) || throw(ArgumentError("mpc_run! before mpc_setup!"))
+    check(p.h, ccall((:to_mpc_run, libb200), Cint, (Ptr{Cvoid}, Int32, Int32), p.h, steps, iterations))
+    MPC_STEPS[p][1] += steps
+    nothing
+end
+# (X (n, s+1, B), U (m, s, B), J (s, B)) of the s steps run since mpc_setup!
+function mpc_history(p::BatchedProblem)
+    haskey(MPC_STEPS, p) || throw(ArgumentError("mpc_history before mpc_setup!"))
+    s = MPC_STEPS[p][1]
+    n, m, _ = RD.dims(p.prob, 1)
+    X = Array{Float64,3}(undef, n, s + 1, p.B); U = Array{Float64,3}(undef, m, s, p.B); J = Matrix{Float64}(undef, s, p.B)
+    check(p.h, ccall((:to_mpc_history, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}), p.h, X, U, J))
+    X, U, J
+end
+
 # multi-GPU (one process per GPU, e.g. under MPI.jl + NCCL.jl): the only collective is the {sum J, max violation} all-reduce.
 # `to_reduce_merit_async` queues the per-GPU reduction behind the iteration in flight and makes `stream` (the CUDA.jl
 # stream the NCCL call is issued on) wait for it; `merit_device_ptr` is the 2-double buffer to all-reduce in place.
