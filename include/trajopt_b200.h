@@ -321,7 +321,16 @@ int to_get_integration(const to_handle* h, int32_t* rule);
  * error-state Quadrotor's quaternion; w_j has n_e entries.  A run starts from xp = x0, so runs of T1 and T2 steps leave what one run of
  * T1 + T2 leaves.  Multipliers and penalties are shifted by step 6 and not otherwise updated; to_al_update or any setter may run between runs.
  * Not on hybrid problems; a problem whose every knot steps one continuous recorded model is a plant like any other, without a reference window
- * or plant parameters (it has no per-instance goals or parameters). */
+ * or plant parameters (it has no per-instance goals or parameters).
+ * to_mpc_solve replaces steps 2-3 by a solve: step j runs, bit for bit,
+ *   2. to_solve(o) (roll out from x0, merit, inner loops and outer steps; multipliers and penalties kept, as to_solve keeps them);
+ *   3. record J_j = to_merit after the solve, and the step's status, iterations, iterations_outer and c_max as to_solve returns them;
+ * with steps 1 and 4-6 as above.  Each step runs exactly o->iterations iterations with the stopping-rule checks and reads nothing back: every
+ * instance is done within that budget, and the iterations after an instance stops leave it as it is (to_solve's own last iteration, in which
+ * no instance is ACTIVE, is one of them).  The device takes each outer step only when every instance holds its own penalties: on a
+ * constrained problem without a per-instance penalty table the first to_mpc_solve creates it, every row holding the shared penalties, as the
+ * first to_set_penalties does (synchronous, once; bit for bit the shared penalties' results).  So the scripted equivalent is
+ * to_set_penalties(con, shared mu) for every constraint, then the loop.  to_mpc_run and to_mpc_solve steps may alternate within one setup. */
 typedef struct {
     int32_t nsteps;              /* the steps the setup holds room for (>= 1) */
     int32_t nparams;             /* entries of a plant row, as to_set_model_params takes them */
@@ -344,6 +353,16 @@ int to_mpc_run(to_handle* h, int32_t steps, int32_t iterations);
 /* The history of the s steps run since the setup, and synchronises: Xcl [B][s+1][n] (row j: the state step j started from; row s: where the
  * last step ended, x0 when s = 0), Ucl [B][s][m], J [B][s].  Any output may be NULL.  TO_ESTATE before any setup. */
 int to_mpc_history(to_handle* h, double* Xcl, double* Ucl, double* J);
+struct to_solve_options;   /* (declared with to_solve below) */
+/* Asynchronous, like to_mpc_run: enqueues `steps` MPC steps whose plan is to_solve(o) (above) and returns.  TO_ESTATE before any setup;
+ * TO_EDIM when the steps done since the setup + steps > nsteps; TO_EINVAL when steps < 1, for the options to_solve refuses (with its
+ * messages), and for a constrained problem of a recorded-program model (it has no per-instance penalties); the checks of to_solve.  Every
+ * check comes before anything is enqueued or changed. */
+int to_mpc_solve(to_handle* h, int32_t steps, const struct to_solve_options* o);
+/* The solve statistics of the s steps run since the setup, and synchronises: status, iterations, iterations_outer, c_max [B][s] each, as
+ * to_solve returns them.  A step to_mpc_run took holds status -1, iterations 0, iterations_outer 0, c_max NaN.  Any output may be NULL.
+ * TO_ESTATE before any setup. */
+int to_mpc_solve_history(to_handle* h, int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* c_max);
 
 /* ---- kernel 1: batched rollout (+ dual-number Jacobians) ------------------------------------------------- */
 int to_rollout(to_handle* h);                                                 /* rollout!           src/problem.jl:330-340 */
@@ -405,7 +424,7 @@ int to_get_gains(to_handle* h, double* K /*[B][N-1][n_e][m]: m x n_e col-major (
 enum to_solve_status { TO_SOLVE_UNSOLVED = 0, TO_SOLVE_SUCCEEDED = 1, TO_SOLVE_MAX_ITERATIONS = 2, TO_SOLVE_MAX_ITERATIONS_OUTER = 3,
                        TO_SOLVE_MAX_REGULARIZATION = 4 };
 /* Altro 0.3 SolverOptions names; defaults (to_default_solve_options) restated from Altro, pinned by the notebooks only where noted */
-typedef struct {
+typedef struct to_solve_options {
     double cost_tolerance;                  /* 1e-4 (pinned: the notebook's iLQR run stops at dJ 6.9e-5) */
     double cost_tolerance_intermediate;     /* 1e-3 (unpinned; the notebook's ALTRO run sets 1e-2) */
     double gradient_tolerance;              /* 10   (unpinned) */

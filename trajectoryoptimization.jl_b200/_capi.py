@@ -213,6 +213,7 @@ def load_library():
         "to_default_solve_options": [C.POINTER(to_solve_options)],
         "to_solve": [H, C.POINTER(to_solve_options), c_int32_p, c_int32_p, c_int32_p, c_double_p, c_double_p, c_double_p, c_double_p],
         "to_mpc_setup": [H, C.POINTER(to_mpc_spec)], "to_mpc_run": [H, C.c_int32, C.c_int32], "to_mpc_history": [H, c_double_p, c_double_p, c_double_p],
+        "to_mpc_solve": [H, C.c_int32, C.POINTER(to_solve_options)], "to_mpc_solve_history": [H, c_int32_p, c_int32_p, c_int32_p, c_double_p],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)
@@ -240,6 +241,7 @@ EXPORTED_SYMBOLS = [
     "to_set_phase_timing", "to_get_phase_times", "to_launch_count", "to_algorithmic_bytes",
     "to_backward_algebra", "to_kernel_choice", "to_error_state_dim", "to_state_diff", "to_get_error_dynamics", "to_error_expansion",
     "to_get_expansion_records", "to_default_solve_options", "to_solve", "to_mpc_setup", "to_mpc_run", "to_mpc_history",
+    "to_mpc_solve", "to_mpc_solve_history",
 ]
 
 

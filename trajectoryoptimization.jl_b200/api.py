@@ -1869,13 +1869,20 @@ _POSITIVE_PARAMS = {K.MODEL_DOUBLE_INTEGRATOR: ("mass",), K.MODEL_CARTPOLE: ("mc
                     K.MODEL_ACROBOT: ("l1", "l2", "m1", "m2")}
 
 
+def _mpc_recorded_model(prob, what):
+    """True for a problem of one recorded model stepping every knot (Problem(AutodiffDynamics(...), ...)), a plant like any other;
+    ArgumentError for a hybrid problem"""
+    if not getattr(prob, "hybrid", False):
+        return False
+    mdl = prob.model[0]
+    if any(x is not mdl for x in prob.model) or mdl.discrete or mdl.n_out != mdl.n:
+        raise ArgumentError(f"{what}: closed-loop MPC is not supported on hybrid problems")
+    return True
+
+
 def _mpc_inputs(prob, nsteps, plant_params, disturbances, Xref, Uref, start):
     """the arrays ``to_mpc_setup`` takes; every check that needs no device happens here"""
-    expr = getattr(prob, "hybrid", False)
-    if expr:   # one recorded model stepping every knot (Problem(AutodiffDynamics(...), ...)) is a plant like any other; a hybrid problem is not
-        mdl = prob.model[0]
-        if any(x is not mdl for x in prob.model) or mdl.discrete or mdl.n_out != mdl.n:
-            raise ArgumentError("mpc_setup: closed-loop MPC is not supported on hybrid problems")
+    if _mpc_recorded_model(prob, "mpc_setup"):
         if plant_params is not None or Xref is not None or Uref is not None:
             raise ArgumentError("mpc_setup: a recorded-program model takes no reference window and no plant parameters (per-instance goals and "
                                 "parameters are not supported on it)")
@@ -1947,6 +1954,61 @@ def mpc_run(prob, steps, iterations=1):
         raise DimensionMismatch(f"mpc_run: {mpc['done']} steps done + {steps} exceed the setup's nsteps = {mpc['nsteps']}")
     prob._call("to_mpc_run", int(steps), int(iterations))
     mpc["done"] += int(steps)
+
+
+def _mpc_solve_steps(prob, steps):
+    """the checks of ``mpc_solve`` that need no device"""
+    mpc = getattr(prob, "_mpc", None)
+    if mpc is None:
+        raise ArgumentError("mpc_solve before mpc_setup")
+    if int(steps) != steps or steps < 1:
+        raise ArgumentError(f"mpc_solve: steps must be a positive integer, got {steps}")
+    if mpc["done"] + steps > mpc["nsteps"]:
+        raise DimensionMismatch(f"mpc_solve: {mpc['done']} steps done + {steps} exceed the setup's nsteps = {mpc['nsteps']}")
+    if _mpc_recorded_model(prob, "mpc_solve") and len(prob.constraints):
+        raise ArgumentError("mpc_solve: a constrained problem needs per-instance penalties, which a recorded-program model does not support")
+    return mpc
+
+
+def mpc_solve(prob, steps, **options):
+    """Enqueues ``steps`` MPC steps whose plan is a ``solve`` (Altro's ``solve!``, with the options ``solve`` takes) and returns without
+    waiting for them.  Step ``j`` computes, bit for bit, what ``mpc_run``'s step computes with ``rollout`` + ``ilqr_step`` replaced by
+    ``solve(prob, **options)``: each instance stops by Altro's rules, takes its own AL outer steps on the device, and keeps its multipliers
+    and penalties from step to step.  Each step runs ``iterations`` iterations (every instance has stopped by then).  On a constrained
+    problem the first call gives every instance its own copy of the shared penalties, as the first ``set_penalties`` does, so the scripted
+    equivalent is ``set_penalties(prob, con, penalty(prob, con))`` for every constraint, then the loop.  The statistics of each step:
+    ``mpc_solve_history``."""
+    mpc = _mpc_solve_steps(prob, steps)
+    o = solve_options(**options)
+    prob._call("to_mpc_solve", int(steps), C.byref(o))
+    mpc["done"] += int(steps)
+
+
+class MpcSolveHistory:
+    """per-step solve statistics of the ``s`` steps run since ``mpc_setup``, arrays ``[B, s]``: ``status``, ``iterations``,
+    ``iterations_outer``, ``c_max``, as ``solve`` returns them (``SolveStats``).  A step ``mpc_run`` took holds status -1, iterations 0,
+    iterations_outer 0 and c_max NaN."""
+
+    FIELDS = ("status", "iterations", "iterations_outer", "c_max")
+
+    def __init__(self, B, s):
+        self.status = np.empty((B, s), dtype=np.int32)
+        self.iterations = np.empty((B, s), dtype=np.int32)
+        self.iterations_outer = np.empty((B, s), dtype=np.int32)
+        self.c_max = np.empty((B, s))
+
+    def __repr__(self):
+        return f"MpcSolveHistory(B={self.status.shape[0]}, steps={self.status.shape[1]})"
+
+
+def mpc_solve_history(prob):
+    """the ``MpcSolveHistory`` of the steps run since ``mpc_setup``"""
+    mpc = getattr(prob, "_mpc", None)
+    if mpc is None:
+        raise ArgumentError("mpc_solve_history before mpc_setup")
+    h = MpcSolveHistory(prob.B, mpc["done"])
+    prob._call("to_mpc_solve_history", K._ip(h.status), K._ip(h.iterations), K._ip(h.iterations_outer), K._dp(h.c_max))
+    return h
 
 
 def mpc_history(prob):

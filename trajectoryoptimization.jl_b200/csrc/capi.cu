@@ -5,6 +5,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -186,6 +187,17 @@ int fill_penalty_rows(to_handle* h, double* d) {
     for (int b = 0; b < B; b++) std::memcpy(rows.data() + (size_t)b * nc, h->h_mu.data(), sizeof(double) * nc);
     CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));   // the staged rows are the source of the copy
+    return TO_OK;
+}
+// The per-instance penalty table (DevProblem::mub) and SolveDev::go, created once with the shared penalties in every row: by the first
+// to_set_penalties, and by the first to_mpc_solve of a constrained problem
+int ensure_penalty_table(to_handle* h) {
+    if (h->P.mub) return TO_OK;
+    double* d = nullptr;
+    int rc = dalloc(h, &d, (size_t)h->P.B * h->h_mu.size()); if (rc) return rc;
+    if (!h->d_go) { rc = dalloc(h, &h->d_go, 2 * (size_t)h->P.B); if (rc) return rc; }
+    rc = fill_penalty_rows(h, d); if (rc) return rc;
+    h->P.mub = d;   // published once the device holds every row
     return TO_OK;
 }
 
@@ -1637,7 +1649,8 @@ static int solve_outer_step(to_handle* h, const SolveDev& sv, int half, cudaStre
 // the dynamics expansion of every instance on the main stream.
 // sv (to_solve): the stopping-rule check of every ACTIVE instance right after its line search -- for the two halves of an overlapped iteration
 // on their own streams, before the next iteration's expansion of each -- and the ACTIVE count behind it (record_active_count); with per-instance
-// penalties each check is followed on its stream by the outer step of the instances whose inner loop it ended (solve_outer_step).
+// penalties each check is followed on its stream by the outer step of the instances whose inner loop it ended (solve_outer_step).  slot < 0
+// (to_mpc_solve, which runs a fixed budget of iterations): no ACTIVE count, so nothing waits on the host.
 static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
     // (error state: only [A_e B_e] is needed by the solver kernels -- k_expand_lie; the full [A B] is produced by to_expand on request)
     auto expand = [&](cudaStream_t st, int mode) { return h->P.lie ? launch_expand_lie(h->P, st, mode) : launch_expand(h->P, st, mode); };
@@ -1675,7 +1688,7 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
         { PhaseScope ps(h, TO_PHASE_LADDER, h->stream2); CU(h, launch_ladder(h->P, h->stream2)); }
         if (sv) { CU(h, launch_solve_check(h->P, *sv, 2, h->stream2)); h->launches++; }      // ... the others, before their expansion on the side stream
         if (sv && sv->go) { int rc2 = solve_outer_step(h, *sv, 1, h->stream2); if (rc2) return rc2; }
-        if (sv) { int rc2 = record_active_count(h, *sv, slot, h->stream2); if (rc2) return rc2; }
+        if (sv && slot >= 0) { int rc2 = record_active_count(h, *sv, slot, h->stream2); if (rc2) return rc2; }
         CU(h, cudaEventRecord(h->ev_join, h->stream2));
         h->side_pending = true;
     } else {
@@ -1683,7 +1696,7 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
         if (sv) {
             CU(h, launch_solve_check(h->P, *sv, 0, h->stream)); h->launches++;
             if (sv->go) { int rc2 = solve_outer_step(h, *sv, 0, h->stream); if (rc2) return rc2; }
-            int rc2 = record_active_count(h, *sv, slot, h->stream); if (rc2) return rc2;
+            if (slot >= 0) { int rc2 = record_active_count(h, *sv, slot, h->stream); if (rc2) return rc2; }
         }
     }
     h->launches++; h->phase_launches[TO_PHASE_LADDER]++;
@@ -1734,10 +1747,8 @@ int to_default_solve_options(to_solve_options* o) {
     o->iterations = 300; o->iterations_inner = 300; o->iterations_outer = 30; o->dJ_counter_limit = 10;
     return TO_OK;
 }
-// the solve with P.active set (to_solve clears it on every exit).  With per-instance penalties (S.go set) every instance takes its outer steps
-// on the device (k_solve_check, solve_outer_step), so one loop of iterations runs until no instance is ACTIVE; with shared penalties the batch
-// takes each outer step together, on the host, once every inner loop has ended.
-static int solve_run(to_handle* h) {
+// the start of a solve (to_solve, each to_mpc_solve step), with P.active set
+static int solve_start(to_handle* h) {
     SolveDev& S = h->solve;
     DevProblem& P = h->P;
     CU(h, launch_solve_init(P, S, h->stream)); h->launches++;      // every instance ACTIVE, rho = bp_reg_initial, counters zero
@@ -1745,6 +1756,15 @@ static int solve_run(to_handle* h) {
     CU(h, launch_merit(P, P.J, h->d_viol, h->stream)); h->launches++;
     h->J_valid = true;
     CU(h, launch_solve_begin(P, S, h->stream)); h->launches++;
+    return TO_OK;
+}
+// the solve with P.active set (to_solve clears it on every exit).  With per-instance penalties (S.go set) every instance takes its outer steps
+// on the device (k_solve_check, solve_outer_step), so one loop of iterations runs until no instance is ACTIVE; with shared penalties the batch
+// takes each outer step together, on the host, once every inner loop has ended.
+static int solve_run(to_handle* h) {
+    SolveDev& S = h->solve;
+    DevProblem& P = h->P;
+    int rc0 = solve_start(h); if (rc0) return rc0;
     for (;;) {
         // inner loops: iterations are queued without waiting for each other; the ACTIVE count of iteration i - 1 (ordered after both of its
         // checks) is read while iteration i is in the queue, so one iteration in which no instance is ACTIVE (every kernel exits at once)
@@ -1778,21 +1798,31 @@ static int solve_run(to_handle* h) {
     }
     return TO_OK;
 }
-int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* cost, double* dJ,
-             double* gradient, double* c_max) {
-    JOIN(h);
-    if (!h || !o) return TO_EINVAL;
+// the option checks of to_solve and to_mpc_solve
+static int check_solve_options(to_handle* h, const to_solve_options* o) {
     if (!(o->cost_tolerance > 0) || !(o->cost_tolerance_intermediate > 0) || !(o->gradient_tolerance > 0) || !(o->gradient_tolerance_intermediate > 0) ||
         !(o->constraint_tolerance > 0))
         return fail(h, TO_EINVAL, "to_solve: tolerances must be positive");
     if (o->iterations < 1 || o->iterations_inner < 1 || o->iterations_outer < 1 || o->dJ_counter_limit < 0)
         return fail(h, TO_EINVAL, "to_solve: iterations, iterations_inner and iterations_outer must be positive, dJ_counter_limit non-negative");
-    int rc = solver_supported(h); if (rc) return rc;
+    return TO_OK;
+}
+// h->solve for a solve with the checked options `o`: the options, and SolveDev::go when the instances hold their own penalties
+static void prepare_solve(to_handle* h, const to_solve_options* o) {
     SolveDev& S = h->solve;
     S.opt = SolveOpts{o->cost_tolerance, o->cost_tolerance_intermediate, o->gradient_tolerance, o->gradient_tolerance_intermediate, o->constraint_tolerance,
                       o->iterations, o->iterations_inner, o->iterations_outer, o->dJ_counter_limit};
-    h->P.active = S.state;
     S.go = h->P.mub ? h->d_go : nullptr;
+}
+int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* cost, double* dJ,
+             double* gradient, double* c_max) {
+    JOIN(h);
+    if (!h || !o) return TO_EINVAL;
+    int rc = check_solve_options(h, o); if (rc) return rc;
+    rc = solver_supported(h); if (rc) return rc;
+    SolveDev& S = h->solve;
+    prepare_solve(h, o);
+    h->P.active = S.state;
     rc = solve_run(h);
     const int jrc = join_side(h);
     h->P.active = nullptr;                 // every other entry point works on every instance again
@@ -1844,20 +1874,22 @@ int to_mpc_setup(to_handle* h, const to_mpc_spec* s) {
     if (!rc && ref) rc = finite_rows(s->Xref, (size_t)nref * n, "to_mpc_setup", ": the state reference is not finite");
     if (!rc && ref) rc = finite_rows(s->Uref, (size_t)nref * m, "to_mpc_setup", ": the control reference is not finite");
     if (rc) return rc;
-    // one allocation: Xref | Uref | W | plant | Xcl | Ucl | Jcl (doubles), then last_knot (ints)
+    // one allocation: Xref | Uref | W | plant | Xcl | Ucl | Jcl | c_max (doubles), then last_knot | status | iterations | iterations_outer (ints)
     const size_t S = s->nsteps;
     const size_t nX = ref ? (size_t)B * nref * n : 0, nU = ref ? (size_t)B * nref * m : 0, nW = s->W ? (size_t)B * S * ne : 0;
     const size_t nP = plant.size(), nXc = (size_t)B * (S + 1) * n, nUc = (size_t)B * S * m, nJ = (size_t)B * S;
-    const size_t nd = nX + nU + nW + nP + nXc + nUc + nJ;
+    const size_t nd = nX + nU + nW + nP + nXc + nUc + 2 * nJ;
     void* buf = nullptr;
-    cudaError_t e = cudaMalloc(&buf, nd * sizeof(double) + (size_t)ncost * sizeof(int));
+    cudaError_t e = cudaMalloc(&buf, nd * sizeof(double) + ((size_t)ncost + 3 * nJ) * sizeof(int));
     if (e != cudaSuccess) return cuda_fail(h, e, "cudaMalloc(mpc)");
     MpcDev M{};
     double* d = static_cast<double*>(buf);
     auto take = [&](size_t cnt) { double* p = cnt ? d : nullptr; d += cnt; return p; };
     M.Xref = take(nX); M.Uref = take(nU); M.W = take(nW); M.plant = take(nP);
-    M.Xcl = take(nXc); M.Ucl = take(nUc); M.Jcl = take(nJ);
-    M.last_knot = reinterpret_cast<int*>(d);
+    M.Xcl = take(nXc); M.Ucl = take(nUc); M.Jcl = take(nJ); M.c_max = take(nJ);
+    int* ip = reinterpret_cast<int*>(d);
+    M.last_knot = ip; ip += ncost;
+    M.status = ip; M.iterations = ip + nJ; M.iterations_outer = ip + 2 * nJ;
     M.nref = nref; M.nsteps = s->nsteps;
     std::vector<int> last(ncost, -1);
     for (int k = 0; k < N; k++) last[h->h_cost_index[k]] = k;      // the host's update_trajectory! writes knot k's cost row k-th: the last knot wins
@@ -1869,6 +1901,11 @@ int to_mpc_setup(to_handle* h, const to_mpc_spec* s) {
     if (e == cudaSuccess) e = up(M.W, s->W, nW * sizeof(double));
     if (e == cudaSuccess) e = up(M.plant, plant.data(), nP * sizeof(double));
     if (e == cudaSuccess) e = up(M.last_knot, last.data(), (size_t)ncost * sizeof(int));
+    // the solve statistics' marker, which no solve produces (a step to_mpc_run takes keeps it): status -1 (every byte 0xff), iterations 0,
+    // iterations_outer 0, c_max NaN (every byte 0xff)
+    if (e == cudaSuccess) e = cudaMemsetAsync(M.status, 0xff, nJ * sizeof(int), h->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(M.iterations, 0, 2 * nJ * sizeof(int), h->stream);
+    if (e == cudaSuccess) e = cudaMemsetAsync(M.c_max, 0xff, nJ * sizeof(double), h->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);     // the host arrays are the sources of the copies
     if (e != cudaSuccess) { cudaFree(buf); return cuda_fail(h, e, "to_mpc_setup: upload"); }
     if (ref && !h->P.qr) {   // the per-instance linear terms the window writes: created as to_update_trajectories creates them
@@ -1880,35 +1917,81 @@ int to_mpc_setup(to_handle* h, const to_mpc_spec* s) {
     h->mpc_buf = buf; h->mpc = M; h->mpc_ready = true; h->mpc_done = 0; h->mpc_start = ref ? s->start : 1;
     return TO_OK;
 }
+// TO_EDIM when the setup holds no room for `steps` more steps
+static int mpc_room(to_handle* h, int32_t steps, const char* what) {
+    if ((long long)h->mpc_done + steps > h->mpc.nsteps)
+        return fail(h, TO_EDIM, std::string(what) + ": " + std::to_string(h->mpc_done) + " steps done + " + std::to_string(steps) +
+                                    " exceed the setup's nsteps = " + std::to_string(h->mpc.nsteps));
+    return TO_OK;
+}
+// MPC step j = h->mpc_done: the reference window, the plan of step j (plan(j), which leaves the plan's merit in P.J), then one advance kernel
+// in place of to_get_controls / to_merit, the plant and to_shift_trajectory(1) + to_set_initial_state.  No host synchronisation: the
+// advance waits for the side stream's late line-search trials through join_side, a stream wait on an event.
+static int mpc_step(to_handle* h, const std::function<int(int)>& plan) {
+    const int j = h->mpc_done;
+    if (h->mpc.Xref) {   // 1. the reference window of step j (to_update_trajectories(Xref, Uref, nref, start + j))
+        CU(h, launch_mpc_window(h->P, h->mpc, h->mpc_start - 1 + j, h->stream)); h->launches++;
+        h->qr_stale = true;
+    }
+    int rc = plan(j); if (rc) return rc;                         // 2.-3.
+    rc = join_side(h); if (rc) return rc;                        // the late trials write U and J of their instances
+    CU(h, launch_mpc_advance(h->P, h->mpc, j, h->stream)); h->launches++;    // 4.-6. record, plant, shift, x0
+    advance_clocks(h, 1);
+    h->mpc_done++;
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    return TO_OK;
+}
 // Enqueues `steps` MPC steps and returns.  Step j runs what the host-scripted loop of entry points runs, launch for launch: the window (with a
-// reference), to_rollout, to_ilqr_step(iterations) (the merit, then the iterations), and one advance kernel in place of to_get_controls /
-// to_merit, the plant and to_shift_trajectory(1) + to_set_initial_state.  No host synchronisation: the advance waits for the side stream's
-// late line-search trials through join_side, a stream wait on an event.
+// reference), to_rollout, to_ilqr_step(iterations) (the merit, then the iterations), and the advance (mpc_step).
 int to_mpc_run(to_handle* h, int32_t steps, int32_t iterations) {
     JOIN(h);
     if (!h) return TO_EINVAL;
     if (!h->mpc_ready) return fail(h, TO_ESTATE, "to_mpc_run before to_mpc_setup");
     if (steps < 1 || iterations < 1) return fail(h, TO_EINVAL, "to_mpc_run: steps and iterations must be >= 1");
-    if ((long long)h->mpc_done + steps > h->mpc.nsteps)
-        return fail(h, TO_EDIM, "to_mpc_run: " + std::to_string(h->mpc_done) + " steps done + " + std::to_string(steps) + " exceed the setup's nsteps = " +
-                                    std::to_string(h->mpc.nsteps));
-    int rc = solver_supported(h); if (rc) return rc;
-    for (int st = 0; st < steps; st++) {
-        const int j = h->mpc_done;
-        if (h->mpc.Xref) {   // 1. the reference window of step j (to_update_trajectories(Xref, Uref, nref, start + j))
-            CU(h, launch_mpc_window(h->P, h->mpc, h->mpc_start - 1 + j, h->stream)); h->launches++;
-            h->qr_stale = true;
-        }
+    int rc = mpc_room(h, steps, "to_mpc_run"); if (rc) return rc;
+    rc = solver_supported(h); if (rc) return rc;
+    auto ilqr = [&](int) {
         CU(h, launch_rollout(h->P, h->stream)); h->launches++;       // 2. to_rollout
         h->J_valid = false; h->expanded = false; h->backward_done = false;
-        rc = ensure_merit(h); if (rc) return rc;                     // 3. to_ilqr_step(iterations)
-        for (int it = 0; it < iterations; it++) { rc = ilqr_iteration(h, nullptr, 0); if (rc) return rc; }
-        rc = join_side(h); if (rc) return rc;                        // the late trials write U and J of their instances
-        CU(h, launch_mpc_advance(h->P, h->mpc, j, h->stream)); h->launches++;    // 4.-6. record, plant, shift, x0
-        advance_clocks(h, 1);
-        h->mpc_done++;
-        h->J_valid = false; h->expanded = false; h->backward_done = false;
-    }
+        int rc2 = ensure_merit(h); if (rc2) return rc2;              // 3. to_ilqr_step(iterations)
+        for (int it = 0; it < iterations; it++) { rc2 = ilqr_iteration(h, nullptr, 0); if (rc2) return rc2; }
+        return TO_OK;
+    };
+    for (int st = 0; st < steps; st++) { rc = mpc_step(h, ilqr); if (rc) return rc; }
+    return TO_OK;
+}
+// The plan of a to_mpc_solve step: to_solve's start, then the budget of S.opt.iterations iterations with the stopping-rule checks and the
+// device's outer steps, and no ACTIVE count read back.  Every instance is DONE within the budget (each ACTIVE one is checked once per
+// iteration, and at iter >= iterations both the inner rule and outer_decision end it), and an iteration leaves a DONE instance as it is,
+// so the step leaves what to_solve leaves (DESIGN.md 5m).  Then, with P.active cleared as to_solve clears it, the merit of every instance
+// (to_merit's value) and the step's statistics into row j.
+static int mpc_solve_plan(to_handle* h, int j) {
+    SolveDev& S = h->solve;
+    h->P.active = S.state;
+    int rc = solve_start(h);
+    for (int it = 0; !rc && it < S.opt.iterations; it++) rc = ilqr_iteration(h, &S, -1);
+    h->P.active = nullptr;
+    if (rc) return rc;
+    rc = join_side(h); if (rc) return rc;
+    CU(h, launch_merit(h->P, h->P.J, h->d_viol, h->stream)); h->launches++;
+    CU(h, launch_mpc_solve_record(h->P, S, h->mpc, j, h->stream)); h->launches++;
+    return TO_OK;
+}
+// Enqueues `steps` MPC steps whose plan is a to_solve with the options `o` and a budget of o->iterations iterations, and returns.  A
+// constrained problem without per-instance penalties gets the table first (synchronous, once), so that every outer step runs on the device.
+int to_mpc_solve(to_handle* h, int32_t steps, const to_solve_options* o) {
+    JOIN(h);
+    if (!h || !o) return TO_EINVAL;
+    if (!h->mpc_ready) return fail(h, TO_ESTATE, "to_mpc_solve before to_mpc_setup");
+    if (steps < 1) return fail(h, TO_EINVAL, "to_mpc_solve: steps must be >= 1");
+    int rc = mpc_room(h, steps, "to_mpc_solve"); if (rc) return rc;
+    rc = check_solve_options(h, o); if (rc) return rc;
+    if (h->P.model == MODEL_EXPR && h->P.ncon > 0)
+        return fail(h, TO_EINVAL, "to_mpc_solve: a constrained problem needs per-instance penalties, which a recorded-program model does not support");
+    rc = solver_supported(h); if (rc) return rc;
+    if (h->P.ncon > 0) { rc = ensure_penalty_table(h); if (rc) return rc; }
+    prepare_solve(h, o);
+    for (int st = 0; st < steps; st++) { rc = mpc_step(h, [&](int j) { return mpc_solve_plan(h, j); }); if (rc) return rc; }
     return TO_OK;
 }
 int to_mpc_history(to_handle* h, double* Xcl, double* Ucl, double* J) {
@@ -1921,6 +2004,21 @@ int to_mpc_history(to_handle* h, double* Xcl, double* Ucl, double* J) {
     else if (Xcl) CU(h, cudaMemcpy2DAsync(Xcl, (size_t)(s + 1) * n * w, h->mpc.Xcl, (size_t)(S + 1) * n * w, (size_t)(s + 1) * n * w, B, cudaMemcpyDeviceToHost, h->stream));
     if (Ucl && s) CU(h, cudaMemcpy2DAsync(Ucl, (size_t)s * m * w, h->mpc.Ucl, (size_t)S * m * w, (size_t)s * m * w, B, cudaMemcpyDeviceToHost, h->stream));
     if (J && s) CU(h, cudaMemcpy2DAsync(J, (size_t)s * w, h->mpc.Jcl, (size_t)S * w, (size_t)s * w, B, cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    return TO_OK;
+}
+int to_mpc_solve_history(to_handle* h, int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* c_max) {
+    JOIN(h);
+    if (!h) return TO_EINVAL;
+    if (!h->mpc_ready) return fail(h, TO_ESTATE, "to_mpc_solve_history before to_mpc_setup");
+    const int B = h->P.B, s = h->mpc_done, S = h->mpc.nsteps;
+    auto rows = [&](void* dst, const void* src, size_t w) {   // [B][s] of the [B][nsteps] rows
+        return dst && s ? cudaMemcpy2DAsync(dst, (size_t)s * w, src, (size_t)S * w, (size_t)s * w, B, cudaMemcpyDeviceToHost, h->stream) : cudaSuccess;
+    };
+    CU(h, rows(status, h->mpc.status, sizeof(int32_t)));
+    CU(h, rows(iterations, h->mpc.iterations, sizeof(int32_t)));
+    CU(h, rows(iterations_outer, h->mpc.iterations_outer, sizeof(int32_t)));
+    CU(h, rows(c_max, h->mpc.c_max, sizeof(double)));
     CU(h, cudaStreamSynchronize(h->stream));
     return TO_OK;
 }
@@ -2067,14 +2165,8 @@ int to_set_penalties(to_handle* h, int32_t con, const double* mu) {
     for (int b = 0; b < B; b++)
         if (!(std::isfinite(mu[b]) && mu[b] > 0))
             return fail(h, TO_EINVAL, "to_set_penalties: instance " + std::to_string(b) + ": a penalty must be finite and positive");
-    if (!h->P.mub) {
-        double* d = nullptr;
-        int rc = dalloc(h, &d, (size_t)B * h->h_mu.size()); if (rc) return rc;
-        if (!h->d_go) { rc = dalloc(h, &h->d_go, 2 * (size_t)B); if (rc) return rc; }
-        rc = fill_penalty_rows(h, d); if (rc) return rc;
-        h->P.mub = d;   // published once the device holds every row
-    }
-    int rc = penalty_column(h, con, const_cast<double*>(mu), false); if (rc) return rc;
+    int rc = ensure_penalty_table(h); if (rc) return rc;
+    rc = penalty_column(h, con, const_cast<double*>(mu), false); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }

@@ -27,6 +27,11 @@ struct MpcDev {
     double* Ucl;               // [B][nsteps][m]
     double* Jcl;               // [B][nsteps]: the merit of the plan step j applied
     int nref, nsteps;
+    // to_mpc_solve: the solve statistics of step j, [B][nsteps] each (to_mpc_setup writes status -1, 0, 0, NaN: a step to_mpc_run took)
+    int* status;
+    int* iterations;
+    int* iterations_outer;
+    double* c_max;
 };
 cudaError_t launch_mpc_window(const DevProblem& P, const MpcDev& M, int row, cudaStream_t s);   // sweep.cu: the linear terms of reference row `row`
 cudaError_t launch_mpc_advance(const DevProblem& P, const MpcDev& M, int j, cudaStream_t s);    // rollout.cu: record, plant step, shift of step j
@@ -128,3 +133,4 @@ cudaError_t launch_solve_begin(const DevProblem& P, const SolveDev& S, cudaStrea
 cudaError_t launch_solve_check(const DevProblem& P, const SolveDev& S, int mode, cudaStream_t s);   // mode as launch_expand
 cudaError_t launch_solve_outer(const DevProblem& P, const SolveDev& S, cudaStream_t s);
 cudaError_t launch_solve_restart(const DevProblem& P, const SolveDev& S, int half, cudaStream_t s);
+cudaError_t launch_mpc_solve_record(const DevProblem& P, const SolveDev& S, const MpcDev& M, int j, cudaStream_t s);   // row j of the statistics

@@ -120,6 +120,15 @@ __global__ void k_solve_restart(const DevProblem P, SolveDev S, int half) {
     S.go[half * P.B + b] = SOLVE_DONE;
 }
 
+// to_mpc_solve: step j's solve statistics of instance b, as to_solve returns them, into row j of the history.  A launch of its own:
+// k_mpc_advance's plant step is kept as it is compiled (DESIGN.md 5l)
+__global__ void k_mpc_solve_record(const DevProblem P, const SolveDev S, const MpcDev M, int j) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P.B) return;
+    const size_t r = (size_t)b * M.nsteps + j;
+    M.status[r] = S.status[b]; M.iterations[r] = S.iter[b]; M.iterations_outer[r] = S.outer[b]; M.c_max[r] = S.cmax[b];
+}
+
 }  // namespace
 
 cudaError_t launch_solve_init(const DevProblem& P, const SolveDev& S, cudaStream_t s) {
@@ -140,5 +149,9 @@ cudaError_t launch_solve_outer(const DevProblem& P, const SolveDev& S, cudaStrea
 }
 cudaError_t launch_solve_restart(const DevProblem& P, const SolveDev& S, int half, cudaStream_t s) {
     k_solve_restart<<<nblk(P.B, 128), 128, 0, s>>>(P, S, half);
+    return cudaGetLastError();
+}
+cudaError_t launch_mpc_solve_record(const DevProblem& P, const SolveDev& S, const MpcDev& M, int j, cudaStream_t s) {
+    k_mpc_solve_record<<<nblk(P.B, 128), 128, 0, s>>>(P, S, M, j);
     return cudaGetLastError();
 }

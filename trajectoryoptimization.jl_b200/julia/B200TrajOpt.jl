@@ -437,7 +437,8 @@ struct ToSolveOptions
     dJ_counter_limit::Int32
 end
 const SOLVE_STATUS = (:UNSOLVED, :SOLVE_SUCCEEDED, :MAX_ITERATIONS, :MAX_ITERATIONS_OUTER, :MAX_REGULARIZATION)   # to_solve_status 0..4
-function solve!(p::BatchedProblem; kw...)
+# Altro's defaults (to_default_solve_options) with the keyword overrides
+function solve_options(kw)
     d = Ref{ToSolveOptions}()
     ccall((:to_default_solve_options, libb200), Cint, (Ref{ToSolveOptions},), d)
     vals = Dict{Symbol,Any}(f => getfield(d[], f) for f in fieldnames(ToSolveOptions))
@@ -445,7 +446,10 @@ function solve!(p::BatchedProblem; kw...)
         haskey(vals, k) || throw(ArgumentError("unknown solve option $k"))
         vals[k] = v
     end
-    o = Ref(ToSolveOptions((convert(fieldtype(ToSolveOptions, f), vals[f]) for f in fieldnames(ToSolveOptions))...))
+    Ref(ToSolveOptions((convert(fieldtype(ToSolveOptions, f), vals[f]) for f in fieldnames(ToSolveOptions))...))
+end
+function solve!(p::BatchedProblem; kw...)
+    o = solve_options(kw)
     status, iters, outer = Vector{Int32}(undef, p.B), Vector{Int32}(undef, p.B), Vector{Int32}(undef, p.B)
     cost, dJ, grad, cmax = (Vector{Float64}(undef, p.B) for _ in 1:4)
     check(p.h, ccall((:to_solve, libb200), Cint,
@@ -504,6 +508,26 @@ function mpc_history(p::BatchedProblem)
     X = Array{Float64,3}(undef, n, s + 1, p.B); U = Array{Float64,3}(undef, m, s, p.B); J = Matrix{Float64}(undef, s, p.B)
     check(p.h, ccall((:to_mpc_history, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}), p.h, X, U, J))
     X, U, J
+end
+# enqueues `steps` MPC steps whose plan is solve!(p; kw...) (a budget of `iterations` iterations per step, the options solve! takes) and
+# returns without waiting for them; a constrained problem gets per-instance penalties first, so each instance takes its own outer steps
+function mpc_solve!(p::BatchedProblem, steps::Integer; kw...)
+    haskey(MPC_STEPS, p) || throw(ArgumentError("mpc_solve! before mpc_setup!"))
+    o = solve_options(kw)
+    check(p.h, ccall((:to_mpc_solve, libb200), Cint, (Ptr{Cvoid}, Int32, Ref{ToSolveOptions}), p.h, steps, o))
+    MPC_STEPS[p][1] += steps
+    nothing
+end
+# the solve statistics of the s steps run since mpc_setup!, (s, B) each; a step mpc_run! took holds status -1 (:NOT_SOLVED here), iterations 0,
+# iterations_outer 0, c_max NaN
+function mpc_solve_history(p::BatchedProblem)
+    haskey(MPC_STEPS, p) || throw(ArgumentError("mpc_solve_history before mpc_setup!"))
+    s = MPC_STEPS[p][1]
+    status, iters, outer = (Matrix{Int32}(undef, s, p.B) for _ in 1:3)
+    cmax = Matrix{Float64}(undef, s, p.B)
+    check(p.h, ccall((:to_mpc_solve_history, libb200), Cint, (Ptr{Cvoid}, Ptr{Int32}, Ptr{Int32}, Ptr{Int32}, Ptr{Float64}),
+                     p.h, status, iters, outer, cmax))
+    (status = [st < 0 ? :NOT_SOLVED : SOLVE_STATUS[st + 1] for st in status], iterations = iters, iterations_outer = outer, c_max = cmax)
 end
 
 # multi-GPU (one process per GPU, e.g. under MPI.jl + NCCL.jl): the only collective is the {sum J, max violation} all-reduce.
