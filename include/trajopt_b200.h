@@ -441,6 +441,35 @@ int to_default_solve_options(to_solve_options* o);
  * tolerance or cap (dJ_counter_limit may be 0). */
 int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* cost, double* dJ,
              double* gradient, double* c_max);
+/* ---- a queue of problems through the batch's slots: Altro's solve! of each problem of a list longer than the batch (DESIGN.md 5n) ------
+ * Every problem shares the handle's structure (model, N, costs, constraints, time steps, solver options) and brings its own x0 and initial
+ * controls, and optionally its own goal state and model parameters.  The B instances of the handle are slots: a slot whose solve stops hands
+ * its results back and takes the next problem at once, on the device.  Problem p's outputs are, bit for bit, what to_solve returns for an
+ * instance that starts with x0 = x0[p], controls U0[p], lambda = 0, the handle's shared penalties (to_get_penalty), the goal rows
+ * to_set_goal_states(xf, goal_objective, goal_constraint) would give it and the parameter row to_set_model_params would give it; they depend
+ * neither on the slot nor on the problems beside it, nor on M or B (as long as B does not change an automatic kernel choice). */
+typedef struct to_queue_spec {
+    int32_t M;                 /* problems, >= 1 */
+    int32_t U0_shared;         /* 1: U0 is one [N-1][m] for every problem */
+    const double* x0;          /* [M][n] */
+    const double* U0;          /* [M][N-1][m], or [N-1][m] when U0_shared = 1 */
+    const double* xf;          /* [M][n] or NULL: each problem's goal, as to_set_goal_states(xf, goal_objective, goal_constraint) */
+    int32_t goal_objective;
+    int32_t goal_constraint;
+    const double* params;      /* [M][nparams] or NULL: each problem's model parameters, as to_set_model_params */
+    int32_t nparams;
+    int32_t pad;
+} to_queue_spec;
+/* Synchronous.  Outputs [M] each, any may be NULL: to_solve's outputs, per problem; X [M][N][n] and U [M][N-1][m] or NULL: each problem's final
+ * trajectory.  On return the handle is as it was: x0, trajectories, multipliers, shared and per-instance penalties and every per-instance table.
+ * The solver scratch (gains, rho, to_get_solver_state) is left unspecified, and the merit is stale, as after to_solve.  Refused before any device
+ * work (TO_EINVAL / TO_EDIM, with nothing changed): M < 1; a non-finite x0, U0, xf or params entry; a parameter row to_set_model_params refuses;
+ * a hybrid problem; a constrained recorded-program model, or one given xf or params; the options to_solve refuses; a per-instance table the
+ * queue does not replace whose rows differ between instances (cost weights, time steps, constraint data other than the Goal values xf
+ * replaces, linear cost terms other than the q that xf replaces), since the results would then depend on the slot.  TO_ENOMEM, naming the
+ * size, when the device cannot hold the staged problems and their outputs: the queue is never split silently. */
+int to_solve_queue(to_handle* h, const to_queue_spec* q, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer,
+                   double* cost, double* dJ, double* gradient, double* c_max, double* X, double* U);
 /* ---- Lie-group error state (SURVEY 8 f2) ------------------------------------------------------------------- */
 int to_backward_algebra(const to_handle* h, int32_t* variant);             /* which arithmetic the next to_backward will use: 0 = pivot-by-pivot LDL' solve
                                                                              (riccati.cu, riccati_small.cu, lie.cu), 1 = 2 x 2 block inverse + W'K update

@@ -2402,3 +2402,86 @@ def solve(prob, **options):
     prob._call("to_solve", C.byref(o), K._ip(st.status), K._ip(st.iterations), K._ip(st.iterations_outer), K._dp(st.cost), K._dp(st.dJ),
                K._dp(st.gradient), K._dp(st.c_max))
     return st
+
+
+# ---- a queue of problems through the batch's slots (C ABI to_solve_queue; DESIGN.md 5n) ----
+class QueueResult(SolveStats):
+    """per-problem results of ``solve_queue``: the ``SolveStats`` fields as arrays of length M, and ``X [M, N, n]``, ``U [M, N-1, m]`` (the
+    final trajectories; None when ``trajectories=False``)"""
+
+    def __init__(self, M, N=None, n=None, m=None):
+        super().__init__(M)
+        self.X = None if N is None else np.empty((M, N, n))
+        self.U = None if N is None else np.empty((M, N - 1, m))
+
+    def __repr__(self):
+        return "Queue" + super().__repr__().replace("B=", "M=")
+
+
+def _queue_inputs(prob, x0, U0, xf, params):
+    """the arrays ``to_solve_queue`` takes; every check that needs no device happens here"""
+    recorded = False
+    if getattr(prob, "hybrid", False):   # one recorded model stepping every knot runs; a hybrid problem does not
+        mdl = prob.model[0]
+        if any(x is not mdl for x in prob.model) or mdl.discrete or mdl.n_out != mdl.n:
+            raise ArgumentError("solve_queue: not supported on hybrid problems")
+        recorded = True
+    if recorded and (len(prob.constraints) or xf is not None or params is not None):
+        raise ArgumentError("solve_queue: a recorded-program model takes no constraints (they need per-instance penalties), no xf and no params "
+                            "(per-instance goals and parameters are not supported on it)")
+    x0 = np.ascontiguousarray(np.asarray(x0, dtype=np.float64))
+    if x0.ndim != 2 or x0.shape[1] != prob.n:
+        raise DimensionMismatch(f"solve_queue: x0 must be [M, {prob.n}], got {x0.shape}")
+    M = x0.shape[0]
+    if M < 1:
+        raise ArgumentError("solve_queue: at least one problem (M >= 1)")
+    U0 = np.ascontiguousarray(np.asarray(U0, dtype=np.float64))
+    if U0.shape == (prob.N - 1, prob.m):
+        shared = True
+    elif U0.shape == (M, prob.N - 1, prob.m):
+        shared = False
+    else:
+        raise DimensionMismatch(f"solve_queue: U0 must be [{prob.N - 1}, {prob.m}] or [M, {prob.N - 1}, {prob.m}], got {U0.shape}")
+    checks = [("x0", x0), ("U0", U0)]
+    if xf is not None:
+        xf = np.ascontiguousarray(np.asarray(xf, dtype=np.float64))
+        if xf.shape != (M, prob.n):
+            raise DimensionMismatch(f"solve_queue: xf must be [{M}, {prob.n}], got {xf.shape}")
+        checks.append(("xf", xf))
+    if params is not None:
+        params = np.ascontiguousarray(np.asarray(params, dtype=np.float64))
+        nparams = len(prob.model.params)
+        if params.shape != (M, nparams):
+            raise DimensionMismatch(f"solve_queue: params must be [{M}, {nparams}], got {params.shape}")
+        checks.append(("params", params))
+    for what, a in checks:
+        bad = np.argwhere(~np.isfinite(a))
+        if bad.size:
+            p = 0 if (what == "U0" and shared) else int(bad[0][0])
+            raise ArgumentError(f"solve_queue: problem {p}: {what} is not finite")
+    if params is not None:
+        pos = _POSITIVE_PARAMS.get(prob.model.model_id, ())
+        for p, row in enumerate(params):
+            for i, v in enumerate(row[:len(pos)]):
+                if not v > 0:
+                    raise ArgumentError(f"solve_queue: problem {p}, parameter {i} ({pos[i]}) must be positive")
+    return M, x0, U0, shared, xf, params
+
+
+def solve_queue(prob, x0, U0, xf=None, objective=True, constraint=True, params=None, trajectories=True, **options):
+    """Altro's ``solve!`` of M problems through the batch's B instances, which act as slots: a slot whose solve stops takes the next problem
+    at once, on the device, so the batch stays full until the queue runs dry.  Every problem shares the problem's structure (model, N, costs,
+    constraints, time steps, solver options) and brings its own ``x0[M, n]`` and initial controls ``U0`` (``[M, N-1, m]``, or ``[N-1, m]`` for
+    every problem), and optionally its own goal ``xf[M, n]`` (as ``set_goal_state(xf, objective, constraint)`` per instance) and model
+    parameters ``params[M, nparams]`` (as ``set_model_params``).  Problem p's results are, bit for bit, those ``solve`` gives an instance that
+    starts from x0[p], U0[p], zero multipliers, the shared penalties and those goal and parameter rows, whichever slot it ran in.  The
+    problem is left as it was (trajectories, multipliers, penalties, per-instance tables).  Per-instance cost weights, time steps, constraint
+    data and cost terms must be equal in every instance (xf replaces the Goal values and the q terms).  Returns a ``QueueResult``."""
+    M, x0, U0, shared, xf, params = _queue_inputs(prob, x0, U0, xf, params)
+    o = solve_options(**options)
+    r = QueueResult(M, prob.N, prob.n, prob.m) if trajectories else QueueResult(M)
+    spec = K.to_queue_spec(M, int(shared), K._dp(x0), K._dp(U0), K._dp(xf), int(bool(objective)), int(bool(constraint)), K._dp(params),
+                           0 if params is None else int(params.shape[1]), 0)
+    prob._call("to_solve_queue", C.byref(spec), C.byref(o), K._ip(r.status), K._ip(r.iterations), K._ip(r.iterations_outer), K._dp(r.cost),
+               K._dp(r.dJ), K._dp(r.gradient), K._dp(r.c_max), K._dp(r.X), K._dp(r.U))
+    return r

@@ -37,6 +37,7 @@ struct to_handle {
     SolveDev solve{};
     int* pin_count = nullptr;           // [2] (pinned)
     cudaEvent_t ev_count[2] = {nullptr, nullptr};
+    cudaEvent_t ev_refill = nullptr;    // to_solve_queue: the main stream's refill of an iteration, which the side stream's ACTIVE count waits for
     std::string err;
     std::vector<void*> allocs;
     std::vector<DevCost> h_costs;
@@ -622,7 +623,8 @@ int to_create(const to_spec* s, to_handle** out) {
             cudaEventCreateWithFlags(&h->ev_merit, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_cons, cudaEventDisableTiming) != cudaSuccess ||
             cudaEventCreateWithFlags(&h->ev_count[0], cudaEventDisableTiming) != cudaSuccess ||
-            cudaEventCreateWithFlags(&h->ev_count[1], cudaEventDisableTiming) != cudaSuccess) { h->err = "side stream creation failed"; return bail(TO_ECUDA); }
+            cudaEventCreateWithFlags(&h->ev_count[1], cudaEventDisableTiming) != cudaSuccess ||
+            cudaEventCreateWithFlags(&h->ev_refill, cudaEventDisableTiming) != cudaSuccess) { h->err = "side stream creation failed"; return bail(TO_ECUDA); }
         if (cudaHostAlloc((void**)&h->pin_count, 2 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) { h->err = "cudaHostAlloc failed"; return bail(TO_ENOMEM); }
     }
     DevProblem& P = h->P;
@@ -795,6 +797,7 @@ int to_destroy(to_handle* h) {
     if (h->ev_merit) cudaEventDestroy(h->ev_merit);
     if (h->ev_cons) cudaEventDestroy(h->ev_cons);
     for (auto e : h->ev_count) if (e) cudaEventDestroy(e);
+    if (h->ev_refill) cudaEventDestroy(h->ev_refill);
     if (h->pin_count) cudaFreeHost(h->pin_count);
     if (h->own_stream && h->stream) cudaStreamDestroy(h->stream);
     delete h;
@@ -1134,8 +1137,9 @@ int to_set_cost_terms(to_handle* h, const double* q, const double* r) {
 // ---- per-instance model parameters (DevProblem::mparams) ----------------------------------------------------------
 // rows := params [B][nparams] checked and completed into the layout of DevProblem::mparams ([B][TO_NPARAM]); `what` names the caller in
 // the messages.  The checks of every per-instance parameter row: to_set_model_params and to_mpc_setup's plant rows.
-static int model_param_rows(to_handle* h, const double* params, int32_t nparams, const char* what, std::vector<double>& rows) {
-    const int model = h->P.model, B = h->P.B;
+static int model_param_rows(to_handle* h, const double* params, int32_t nparams, const char* what, std::vector<double>& rows, int B = -1) {
+    const int model = h->P.model;
+    if (B < 0) B = h->P.B;
     const int np = model_nparams(model);
     if (nparams != np)
         return fail(h, TO_EDIM, std::string(what) + ": the model takes " + std::to_string(np) + " parameters per instance, got " + std::to_string(nparams));
@@ -1651,7 +1655,8 @@ static int solve_outer_step(to_handle* h, const SolveDev& sv, int half, cudaStre
 // on their own streams, before the next iteration's expansion of each -- and the ACTIVE count behind it (record_active_count); with per-instance
 // penalties each check is followed on its stream by the outer step of the instances whose inner loop it ended (solve_outer_step).  slot < 0
 // (to_mpc_solve, which runs a fixed budget of iterations): no ACTIVE count, so nothing waits on the host.
-static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
+static int queue_refill(to_handle* h, const QueueDev& q, int half, int mode, cudaStream_t st);
+static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot, const QueueDev* q = nullptr) {
     // (error state: only [A_e B_e] is needed by the solver kernels -- k_expand_lie; the full [A B] is produced by to_expand on request)
     auto expand = [&](cudaStream_t st, int mode) { return h->P.lie ? launch_expand_lie(h->P, st, mode) : launch_expand(h->P, st, mode); };
     bool costexp_done = false;
@@ -1685,9 +1690,17 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
         CU(h, cudaEventRecord(h->ev_fork, h->stream));
         CU(h, cudaStreamWaitEvent(h->stream2, h->ev_fork, 0));
         if (sv && sv->go) { int rc2 = solve_outer_step(h, *sv, 0, h->stream); if (rc2) return rc2; }   // (an instance that goes on stays ACTIVE: the count holds)
+        if (q) {   // to_solve_queue: this half's refill; the side stream's ACTIVE count below waits for it
+            int rc2 = queue_refill(h, *q, 0, 1, h->stream); if (rc2) return rc2;
+            CU(h, cudaEventRecord(h->ev_refill, h->stream));
+        }
         { PhaseScope ps(h, TO_PHASE_LADDER, h->stream2); CU(h, launch_ladder(h->P, h->stream2)); }
         if (sv) { CU(h, launch_solve_check(h->P, *sv, 2, h->stream2)); h->launches++; }      // ... the others, before their expansion on the side stream
         if (sv && sv->go) { int rc2 = solve_outer_step(h, *sv, 1, h->stream2); if (rc2) return rc2; }
+        if (q) {
+            int rc2 = queue_refill(h, *q, 1, 2, h->stream2); if (rc2) return rc2;
+            CU(h, cudaStreamWaitEvent(h->stream2, h->ev_refill, 0));
+        }
         if (sv && slot >= 0) { int rc2 = record_active_count(h, *sv, slot, h->stream2); if (rc2) return rc2; }
         CU(h, cudaEventRecord(h->ev_join, h->stream2));
         h->side_pending = true;
@@ -1696,6 +1709,7 @@ static int ilqr_iteration(to_handle* h, const SolveDev* sv, int slot) {
         if (sv) {
             CU(h, launch_solve_check(h->P, *sv, 0, h->stream)); h->launches++;
             if (sv->go) { int rc2 = solve_outer_step(h, *sv, 0, h->stream); if (rc2) return rc2; }
+            if (q) { int rc2 = queue_refill(h, *q, 0, 0, h->stream); if (rc2) return rc2; }
             if (slot >= 0) { int rc2 = record_active_count(h, *sv, slot, h->stream); if (rc2) return rc2; }
         }
     }
@@ -1838,6 +1852,211 @@ int to_solve(to_handle* h, const to_solve_options* o, int32_t* status, int32_t* 
     if (gradient) CU(h, cudaMemcpyAsync(gradient, S.grad, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
     if (c_max) CU(h, cudaMemcpyAsync(c_max, S.cmax, sizeof(double) * B, cudaMemcpyDeviceToHost, h->stream));
     CU(h, cudaStreamSynchronize(h->stream));
+    return TO_OK;
+}
+// ---- a queue of problems through the slots (include/trajopt_b200.h, DESIGN.md 5n) ------------------------------------------------------------
+// The harvest and refill of half `half` of an iteration (mode as launch_solve_check), on that half's stream right after its check and outer
+// step: the slots whose problem stopped hand back their results (k_cost gives the objective, as to_solve computes it), then every DONE slot of
+// the half claims the next problem, which is rolled out, gets its merit and starts its first inner loop.  A refilled slot keeps its acc1, so
+// its next expansion runs on the same stream.
+static int queue_refill(to_handle* h, const QueueDev& q, int half, int mode, cudaStream_t st) {
+    DevProblem M = h->P;
+    M.active = q.mask + (size_t)half * M.B;
+    CU(h, launch_queue_harvest(h->P, h->solve, q, half, mode, st));
+    CU(h, launch_cost(M, q.cost_slot, nullptr, st));
+    CU(h, launch_queue_refill(h->P, h->solve, q, half, mode, st));
+    CU(h, launch_rollout(M, st, true));
+    CU(h, launch_merit(M, M.J, h->d_viol, st));
+    CU(h, launch_queue_begin(h->P, h->solve, q, half, st));
+    h->launches += 6;
+    return TO_OK;
+}
+// the first B problems go into the slots through the refill; then iterations, each ACTIVE count read one iteration later as solve_run reads
+// it, until no slot is ACTIVE: a refill raises the count, so zero means the queue is drained and every result is harvested
+static int queue_run(to_handle* h, const QueueDev& q) {
+    SolveDev& S = h->solve;
+    CU(h, launch_queue_init(h->P, S, q, h->stream)); h->launches++;
+    int rc = queue_refill(h, q, 0, 0, h->stream); if (rc) return rc;
+    const long long cap = ((long long)S.opt.iterations + 1) * q.M;
+    int prev = -1;
+    for (long long it = 0;; it++) {
+        const int slot = (int)(it & 1);
+        rc = ilqr_iteration(h, &S, slot, &q); if (rc) return rc;
+        if (prev >= 0) {
+            CU(h, cudaEventSynchronize(h->ev_count[prev]));
+            if (h->pin_count[prev] == 0) break;
+        }
+        prev = slot;
+        if (it > cap) return fail(h, TO_ESTATE, "to_solve_queue: the queue outlived (iterations + 1) x M iterations");
+    }
+    return join_side(h);
+}
+// TO_EINVAL when the rows [B][w] of a per-instance table differ between instances (in the entries keep[j] != 0, all when keep is empty)
+static int uniform_rows(to_handle* h, const std::vector<double>& rows, size_t w, const std::vector<char>& keep, const char* what) {
+    for (int b = 1; b < h->P.B; b++)
+        for (size_t j = 0; j < w; j++)
+            if ((keep.empty() || keep[j]) && std::memcmp(&rows[j], &rows[(size_t)b * w + j], sizeof(double)) != 0)
+                return fail(h, TO_EINVAL, std::string("to_solve_queue: the per-instance ") + what + " differ between instances (instance " + std::to_string(b) +
+                                              "), so a problem's result would depend on its slot; the queue needs them equal in every row");
+    return TO_OK;
+}
+int to_solve_queue(to_handle* h, const to_queue_spec* qs, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer,
+                   double* cost, double* dJ, double* gradient, double* c_max, double* X, double* U) {
+    JOIN(h);
+    if (!h || !qs || !o) return TO_EINVAL;
+    const int B = h->P.B, n = h->P.n, m = h->P.m, N = h->P.N, M = qs->M, ncost = h->P.ncost, ncd = h->P.ncdata, nc = h->P.ncon;
+    // ---- every check before any device work
+    if (M < 1) return fail(h, TO_EINVAL, "to_solve_queue: M must be >= 1");
+    if (!qs->x0 || !qs->U0) return fail(h, TO_EINVAL, "to_solve_queue: x0 and U0 are required");
+    int rc = check_solve_options(h, o); if (rc) return rc;
+    if (h->P.model == MODEL_EXPR) {
+        if (h->h_dyn.size() != 1 || h->h_dyn[0].discrete || h->h_dyn[0].n_out != h->h_dyn[0].n_in)
+            return fail(h, TO_EINVAL, "to_solve_queue: not supported on hybrid problems");
+        if (nc > 0 || qs->xf || qs->params)
+            return fail(h, TO_EINVAL, "to_solve_queue: a recorded-program model takes no constraints (they need per-instance penalties), no xf and no params "
+                                      "(per-instance goals and parameters are not supported on it)");
+    }
+    rc = solver_supported(h); if (rc) return rc;
+    const size_t wu = (size_t)(N - 1) * m, mu0 = qs->U0_shared ? 1 : (size_t)M;
+    auto finite = [&](const double* a, size_t rows, size_t w, const char* what) {
+        for (size_t p = 0; p < rows; p++)
+            for (size_t i = 0; i < w; i++)
+                if (!std::isfinite(a[p * w + i]))
+                    return fail(h, TO_EINVAL, std::string("to_solve_queue: problem ") + std::to_string(p) + ": " + what + " is not finite");
+        return TO_OK;
+    };
+    rc = finite(qs->x0, M, n, "x0"); if (rc) return rc;
+    rc = finite(qs->U0, mu0, wu, "U0"); if (rc) return rc;
+    if (qs->xf) { rc = finite(qs->xf, M, n, "xf"); if (rc) return rc; }
+    std::vector<double> mp_rows;
+    if (qs->params) { rc = model_param_rows(h, qs->params, qs->nparams, "to_solve_queue", mp_rows, M); if (rc) return rc; }
+    const bool objective = qs->xf && qs->goal_objective, goal_con = qs->xf && qs->goal_constraint && ncd > 0;
+    // the tables the queue keeps must not depend on the slot
+    if (h->P.cw) { rc = uniform_rows(h, h->h_cw, h->P.ncw, {}, "cost weights"); if (rc) return rc; }
+    if (h->P.dtb) { rc = uniform_rows(h, h->h_dtb, N - 1, {}, "time steps"); if (rc) return rc; }
+    if (h->P.mparams && !qs->params) { rc = uniform_rows(h, h->h_mparams, TO_NPARAM, {}, "model parameters"); if (rc) return rc; }
+    if (h->P.cdata) {
+        std::vector<char> keep(ncd, 1);     // the Goal values xf replaces need not agree
+        if (goal_con) for (const auto& c : h->h_cons) if (c.kind == CON_GOAL) std::fill(keep.begin() + c.cdoff, keep.begin() + c.cdoff + c.p, 0);
+        rc = uniform_rows(h, h->h_cdata, ncd, keep, "constraint data"); if (rc) return rc;
+    }
+    const size_t wq = (size_t)ncost * (n + m);
+    if (h->P.qr) {
+        rc = refresh_qr(h); if (rc) return rc;
+        std::vector<char> keep(wq, 1);      // the q that xf replaces need not agree
+        if (objective) for (int ci = 0; ci < ncost; ci++) std::fill(keep.begin() + ci * (n + m), keep.begin() + ci * (n + m) + n, 0);
+        rc = uniform_rows(h, h->h_qr, wq, keep, "linear cost terms"); if (rc) return rc;
+    }
+    // ---- each problem's rows, built as the setters build them (to_set_goal_states, to_set_model_params)
+    std::vector<double> qr_rows, cd_rows;
+    if (objective) {
+        rc = stage_qr(h); if (rc) return rc;
+        qr_rows.resize((size_t)M * wq);
+        for (int p = 0; p < M; p++) {
+            double* row = qr_rows.data() + (size_t)p * wq;
+            std::memcpy(row, h->stage.data(), sizeof(double) * wq);
+            for (int ci = 0; ci < ncost; ci++) instance_linear_term(h, 0, ci, qs->xf + (size_t)p * n, nullptr, row + (size_t)ci * (n + m));
+        }
+    }
+    if (goal_con) {
+        stage_cdata(h);
+        cd_rows.resize((size_t)M * ncd);
+        for (int p = 0; p < M; p++) {
+            double* row = cd_rows.data() + (size_t)p * ncd;
+            std::memcpy(row, h->stage.data(), sizeof(double) * ncd);
+            for (const auto& c : h->h_cons)
+                if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) row[c.cdoff + i] = qs->xf[(size_t)p * n + c.inds[i]];
+        }
+    }
+    // ---- one allocation: the staged problems, the slot tables, the outputs and the handle's state the refills overwrite
+    const bool traj = X || U;
+    const size_t nX = (size_t)N * n, ll = (size_t)h->P.lambda_len;
+    const size_t d_in = (size_t)M * n + mu0 * wu + qr_rows.size() + cd_rows.size() + mp_rows.size();
+    const size_t d_slot = (objective ? B * wq : 0) + (goal_con ? (size_t)B * ncd : 0) + (qs->params ? (size_t)B * TO_NPARAM : 0) + (size_t)B * nc + B;
+    const size_t d_out = 4 * (size_t)M + (traj ? (size_t)M * (nX + wu) : 0);
+    const size_t d_save = (size_t)B * n + (size_t)B * ll;
+    const size_t n_int = 3 * (size_t)M + 1 + 3 * (size_t)B + 2 * (size_t)B;
+    const size_t bytes = (d_in + d_slot + d_out + d_save) * sizeof(double) + n_int * sizeof(int);
+    void* buf = nullptr;
+    cudaError_t e = cudaMalloc(&buf, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        char msg[256];
+        std::snprintf(msg, sizeof msg, "to_solve_queue: %.1f MB of device memory for %d staged problems and their outputs: %s", bytes / 1048576.0, M,
+                      cudaGetErrorString(e));
+        return fail(h, e == cudaErrorMemoryAllocation ? TO_ENOMEM : TO_ECUDA, msg);
+    }
+    double* d = static_cast<double*>(buf);
+    auto take = [&](size_t cnt) { double* p = cnt ? d : nullptr; d += cnt; return p; };
+    QueueDev q{};
+    q.M = M; q.U0_shared = qs->U0_shared ? 1 : 0;
+    double* x0_in = take((size_t)M * n); double* U0_in = take(mu0 * wu);
+    double* qr_in = take(qr_rows.size()); double* cd_in = take(cd_rows.size()); double* mp_in = take(mp_rows.size());
+    q.x0 = x0_in; q.U0 = U0_in; q.qr_src = qr_in; q.cd_src = cd_in; q.mp_src = mp_in;
+    q.qr = take(objective ? B * wq : 0); q.cd = take(goal_con ? (size_t)B * ncd : 0); q.mp = take(qs->params ? (size_t)B * TO_NPARAM : 0);
+    q.mub = take((size_t)B * nc); q.cost_slot = take(B);
+    q.cost = take(M); q.dJ = take(M); q.grad = take(M); q.cmax = take(M);
+    q.X = traj ? take((size_t)M * nX) : nullptr; q.U = traj ? take((size_t)M * wu) : nullptr;
+    double* save_x0 = take((size_t)B * n); double* save_lam = take((size_t)B * ll);
+    int* ip = reinterpret_cast<int*>(d);
+    q.status = ip; q.iter = ip + M; q.outer = ip + 2 * (size_t)M; ip += 3 * (size_t)M;
+    q.next = ip++; q.slot = ip; ip += B; q.mask = ip; ip += 2 * (size_t)B;
+    int* go = ip;
+    auto up = [&](double* dst, const double* src, size_t cnt) {
+        return cnt ? cudaMemcpyAsync(dst, src, cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream) : cudaSuccess;
+    };
+    e = up(x0_in, qs->x0, (size_t)M * n);
+    if (e == cudaSuccess) e = up(U0_in, qs->U0, mu0 * wu);
+    if (e == cudaSuccess) e = up(qr_in, qr_rows.data(), qr_rows.size());
+    if (e == cudaSuccess) e = up(cd_in, cd_rows.data(), cd_rows.size());
+    if (e == cudaSuccess) e = up(mp_in, mp_rows.data(), mp_rows.size());
+    // the handle's state the refills overwrite: x0, the live trajectories (in the get / set staging buffers), the multipliers
+    if (e == cudaSuccess) e = cudaMemcpyAsync(save_x0, h->P.x0, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, h->stream);
+    if (e == cudaSuccess && ll) e = cudaMemcpyAsync(save_lam, h->P.lambda, (size_t)B * ll * sizeof(double), cudaMemcpyDeviceToDevice, h->stream);
+    if (e == cudaSuccess) e = launch_gather_traj(h->P, h->d_stageX, h->d_stageU, h->stream);
+    if (e != cudaSuccess) { cudaStreamSynchronize(h->stream); cudaFree(buf); return cuda_fail(h, e, "to_solve_queue: upload"); }
+    h->launches++;
+    // ---- the run, on the slot tables; the handle's own tables (or their absence) come back afterwards
+    const DevProblem saved = h->P;
+    SolveDev& S = h->solve;
+    if (q.qr) h->P.qr = q.qr;
+    if (q.cd) h->P.cdata = q.cd;
+    if (q.mp) h->P.mparams = q.mp;
+    h->P.mub = q.mub;                          // (nullptr without constraints)
+    prepare_solve(h, o);
+    S.go = nc > 0 ? go : nullptr;              // a constrained problem takes every outer step on the device
+    h->P.active = S.state;
+    rc = queue_run(h, q);
+    const int jrc = join_side(h);
+    h->P.active = nullptr;
+    h->P.qr = saved.qr; h->P.cdata = saved.cdata; h->P.mparams = saved.mparams; h->P.mub = saved.mub;
+    S.go = h->P.mub ? h->d_go : nullptr;
+    h->J_valid = false; h->expanded = false; h->backward_done = false;
+    if (!rc) rc = jrc;
+    auto down = [&](void* dst, const void* src, size_t bytes_) {
+        return dst ? cudaMemcpyAsync(dst, src, bytes_, cudaMemcpyDeviceToHost, h->stream) : cudaSuccess;
+    };
+    e = cudaSuccess;
+    if (!rc) {
+        e = down(status, q.status, M * sizeof(int));
+        if (e == cudaSuccess) e = down(iterations, q.iter, M * sizeof(int));
+        if (e == cudaSuccess) e = down(iterations_outer, q.outer, M * sizeof(int));
+        if (e == cudaSuccess) e = down(cost, q.cost, M * sizeof(double));
+        if (e == cudaSuccess) e = down(dJ, q.dJ, M * sizeof(double));
+        if (e == cudaSuccess) e = down(gradient, q.grad, M * sizeof(double));
+        if (e == cudaSuccess) e = down(c_max, q.cmax, M * sizeof(double));
+        if (e == cudaSuccess) e = down(X, q.X, (size_t)M * nX * sizeof(double));
+        if (e == cudaSuccess) e = down(U, q.U, (size_t)M * wu * sizeof(double));
+    }
+    // restore the handle's state
+    if (e == cudaSuccess) e = cudaMemcpyAsync(h->P.x0, save_x0, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, h->stream);
+    if (e == cudaSuccess && ll) e = cudaMemcpyAsync(h->P.lambda, save_lam, (size_t)B * ll * sizeof(double), cudaMemcpyDeviceToDevice, h->stream);
+    if (e == cudaSuccess) { e = launch_scatter_traj(h->P, h->d_stageX, h->d_stageU, h->stream); h->launches++; }
+    const cudaError_t se = cudaStreamSynchronize(h->stream);
+    cudaFree(buf);
+    if (rc) return rc;
+    if (e != cudaSuccess) return cuda_fail(h, e, "to_solve_queue: results");
+    if (se != cudaSuccess) return cuda_fail(h, se, "to_solve_queue");
     return TO_OK;
 }
 // ---- closed-loop MPC (include/trajopt_b200.h, DESIGN.md 5l) ---------------------------------------------------------------------

@@ -6,12 +6,12 @@
 inline unsigned nblk(long long total, int threads) { return (unsigned)((total + threads - 1) / threads); }
 
 // kernel 1: batched rollout / dual-number dynamics expansion with the problem's explicit rule           (rollout.cu)
-cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s);
+cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s, bool masked = false);   // masked: only the instances P.active marks ACTIVE
 cudaError_t launch_expand(const DevProblem& P, cudaStream_t s, int mode = 0);   // mode 1 / 2: only instances with acc1 == 1 / == 0
 // The launchers of the kernels that step the dynamics, per explicit rule RULE (to_integration).  rollout.cu and forward.cu are compiled once
 // per rule; the object of rule R instantiates these for R alone, and the public launchers (launch_rollout, launch_expand, launch_expand_lie,
 // launch_forward, launch_ladder) dispatch on DevProblem::integration.
-template <int RULE> cudaError_t launch_rollout_rule(const DevProblem& P, cudaStream_t s);
+template <int RULE> cudaError_t launch_rollout_rule(const DevProblem& P, cudaStream_t s, bool masked);
 template <int RULE> cudaError_t launch_expand_rule(const DevProblem& P, cudaStream_t s, int mode);
 template <int RULE> cudaError_t launch_expand_lie_rule(const DevProblem& P, cudaStream_t s, int mode);
 template <int RULE> cudaError_t launch_forward_rule(const DevProblem& P, cudaStream_t s);
@@ -37,7 +37,7 @@ cudaError_t launch_mpc_window(const DevProblem& P, const MpcDev& M, int row, cud
 cudaError_t launch_mpc_advance(const DevProblem& P, const MpcDev& M, int j, cudaStream_t s);    // rollout.cu: record, plant step, shift of step j
 template <int RULE> cudaError_t launch_mpc_advance_rule(const DevProblem& P, const MpcDev& M, int j, cudaStream_t s);
 #define TO_RULE_EXTERN(R)                                                                                   \
-    extern template cudaError_t launch_rollout_rule<R>(const DevProblem&, cudaStream_t);                  \
+    extern template cudaError_t launch_rollout_rule<R>(const DevProblem&, cudaStream_t, bool);            \
     extern template cudaError_t launch_expand_rule<R>(const DevProblem&, cudaStream_t, int);              \
     extern template cudaError_t launch_expand_lie_rule<R>(const DevProblem&, cudaStream_t, int);          \
     extern template cudaError_t launch_forward_rule<R>(const DevProblem&, cudaStream_t);                  \
@@ -134,3 +134,29 @@ cudaError_t launch_solve_check(const DevProblem& P, const SolveDev& S, int mode,
 cudaError_t launch_solve_outer(const DevProblem& P, const SolveDev& S, cudaStream_t s);
 cudaError_t launch_solve_restart(const DevProblem& P, const SolveDev& S, int half, cudaStream_t s);
 cudaError_t launch_mpc_solve_record(const DevProblem& P, const SolveDev& S, const MpcDev& M, int j, cudaStream_t s);   // row j of the statistics
+// to_solve_queue (capi.cu, DESIGN.md 5n): M problems through the B slots of the batch.  A slot whose instance is DONE hands its results to row p
+// of the outputs (harvest) and takes the next problem (refill), in the half of the iteration whose check stopped it.
+struct QueueDev {
+    int M, U0_shared;
+    int* next;               // [1] the next problem to claim
+    int* slot;               // [B] the problem in slot b, -1: none
+    int* mask;               // [2][B] per half: the slots harvested, then the slots refilled (SOLVE_ACTIVE), as DevProblem::active of the launches after
+    double* cost_slot;       // [B] the objective of the harvested slots (k_cost)
+    const double* x0;        // [M][n]
+    const double* U0;        // [M][N-1][m], or [N-1][m] when U0_shared
+    // each problem's rows, src [M][w], and the slot tables the refill writes them into, [B][w] (nullptr: the table is not replaced)
+    const double* qr_src;    // w = ncost (n + m): DevProblem::qr
+    double* qr;
+    const double* cd_src;    // w = ncdata: DevProblem::cdata
+    double* cd;
+    const double* mp_src;    // w = TO_NPARAM: DevProblem::mparams
+    double* mp;
+    double* mub;             // [B][ncon] or nullptr: DevProblem::mub, refilled with the shared penalties
+    // outputs [M]: to_solve's statistics, and X [M][N][n], U [M][N-1][m] or nullptr
+    int *status, *iter, *outer;
+    double *cost, *dJ, *grad, *cmax, *X, *U;
+};
+cudaError_t launch_queue_init(const DevProblem& P, const SolveDev& S, const QueueDev& Q, cudaStream_t s);
+cudaError_t launch_queue_harvest(const DevProblem& P, const SolveDev& S, const QueueDev& Q, int half, int mode, cudaStream_t s);   // mode as launch_solve_check
+cudaError_t launch_queue_refill(const DevProblem& P, const SolveDev& S, const QueueDev& Q, int half, int mode, cudaStream_t s);
+cudaError_t launch_queue_begin(const DevProblem& P, const SolveDev& S, const QueueDev& Q, int half, cudaStream_t s);

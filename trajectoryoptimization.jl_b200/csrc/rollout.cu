@@ -29,15 +29,18 @@
 // INST: the instance's own model parameters (DevProblem::mparams), one shared-memory copy per lane, and time steps (DevProblem::dtb).
 // (Copied to registers instead, the parameter-only subexpressions of the dynamics were hoisted out of the knot loop and lost FMA contractions
 // the shared kernel has.)
-template <int MODEL, bool INST, int RULE>
+// MASK (to_solve_queue's refill): only the instances P.active marks ACTIVE are written; the others compute a rollout of their own that is not
+// stored, so that the knot loop is the one the unmasked kernel runs.  A warp with no instance to write exits.
+template <int MODEL, bool INST, int RULE, bool MASK = false>
 __global__ void __launch_bounds__(32) k_rollout(const DevProblem P) {
     constexpr int n = ModelDims<MODEL>::n, m = ModelDims<MODEL>::m;
     __shared__ double stage[32 * n];
     __shared__ double* base[32];
     const int lane = threadIdx.x;
     const int b = blockIdx.x * 32 + lane;
-    const bool valid = b < P.B;
-    const int bc = valid ? b : P.B - 1;                     // (idle lanes of the last warp shadow a real instance and store nothing)
+    const bool valid = b < P.B && (!MASK || !retired(P, b));
+    if constexpr (MASK) { if (!__any_sync(0xffffffffu, valid)) return; }
+    const int bc = b < P.B ? b : P.B - 1;                   // (idle lanes of the last warp shadow a real instance and store nothing)
     base[lane] = valid ? traj_Xw(P, P.cur[bc], bc) : nullptr;
     const double* U = traj_U(P, P.cur[bc], bc);
     const double* prm = nullptr;
@@ -664,9 +667,12 @@ cudaError_t launch_expand_lie_rule(const DevProblem& P, cudaStream_t s, int mode
 
 // the dynamics kernels read nothing per instance but the model parameters and the time steps: their INST variant runs exactly when a table exists
 template <int RULE>
-cudaError_t launch_rollout_rule(const DevProblem& P, cudaStream_t s) {
+cudaError_t launch_rollout_rule(const DevProblem& P, cudaStream_t s, bool masked) {
     const int threads = 32, blocks = (P.B + threads - 1) / threads;
-    if (inst_dynamics(P)) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true, RULE><<<blocks, threads, 0, s>>>(P))); }
+    if (masked) {
+        if (inst_dynamics(P)) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true, RULE, true><<<blocks, threads, 0, s>>>(P))); }
+        else { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, false, RULE, true><<<blocks, threads, 0, s>>>(P))); }
+    } else if (inst_dynamics(P)) { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, true, RULE><<<blocks, threads, 0, s>>>(P))); }
     else { TO_DISPATCH_MODEL(P.model, P.m, (k_rollout<MODEL, false, RULE><<<blocks, threads, 0, s>>>(P))); }
     return cudaGetLastError();
 }
@@ -705,7 +711,7 @@ cudaError_t launch_mpc_advance_rule(const DevProblem& P, const MpcDev& M, int j,
 }
 
 template cudaError_t launch_expand_lie_rule<TO_RULE>(const DevProblem&, cudaStream_t, int);
-template cudaError_t launch_rollout_rule<TO_RULE>(const DevProblem&, cudaStream_t);
+template cudaError_t launch_rollout_rule<TO_RULE>(const DevProblem&, cudaStream_t, bool);
 template cudaError_t launch_expand_rule<TO_RULE>(const DevProblem&, cudaStream_t, int);
 template cudaError_t launch_mpc_advance_rule<TO_RULE>(const DevProblem&, const MpcDev&, int, cudaStream_t);
 
@@ -715,9 +721,9 @@ cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode) {
     TO_DISPATCH_RULE(P.integration, (e = launch_expand_lie_rule<RULE>(P, s, mode)));
     return e;
 }
-cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s) {
+cudaError_t launch_rollout(const DevProblem& P, cudaStream_t s, bool masked) {
     cudaError_t e = cudaErrorNotSupported;
-    TO_DISPATCH_RULE(P.integration, (e = launch_rollout_rule<RULE>(P, s)));
+    TO_DISPATCH_RULE(P.integration, (e = launch_rollout_rule<RULE>(P, s, masked)));
     return e;
 }
 cudaError_t launch_expand(const DevProblem& P, cudaStream_t s, int mode) {

@@ -25,15 +25,20 @@ __device__ double todorov_gradient(const DevProblem& P, int b) {
     return acc / (N - 1);
 }
 
-__global__ void k_solve_init(const DevProblem P, SolveDev S) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b == 0) *S.n_active = P.B;
-    if (b >= P.B) return;
+// the start of instance b's solve: ACTIVE, counters zero, rho restarted (k_solve_init, and k_queue_refill for a slot's new problem)
+__device__ __forceinline__ void solve_init_instance(const DevProblem& P, const SolveDev& S, int b) {
     S.state[b] = SOLVE_ACTIVE; S.status[b] = TO_SOLVE_UNSOLVED;
     S.iter[b] = 0; S.outer[b] = 1; S.inner[b] = 0; S.dj_zero[b] = 0;
     S.dJ[b] = 0.0; S.grad[b] = 0.0; S.cmax[b] = 0.0;
     if (S.go) { S.go[b] = SOLVE_DONE; S.go[P.B + b] = SOLVE_DONE; }
     P.rho[b] = P.opt.bp_reg_initial; P.drho[b] = 0.0;      // Altro initialize!: the regularisation restarts
+}
+
+__global__ void k_solve_init(const DevProblem P, SolveDev S) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b == 0) *S.n_active = P.B;
+    if (b >= P.B) return;
+    solve_init_instance(P, S, b);
 }
 
 // Altro's outer-loop rules for instance b, whose inner loop has ended with violation S.cmax[b]: its final status, or TO_SOLVE_UNSOLVED when
@@ -120,6 +125,75 @@ __global__ void k_solve_restart(const DevProblem P, SolveDev S, int half) {
     S.go[half * P.B + b] = SOLVE_DONE;
 }
 
+// ---- to_solve_queue (DESIGN.md 5n): one thread per slot ----
+// mode as k_solve_check: the slots of that half of the iteration (1: accepted by the first line-search pass, 2: the others, 0: every slot)
+__device__ __forceinline__ bool in_half(const DevProblem& P, int b, int mode) { return mode == 0 || (P.acc1[b] != 0) == (mode == 1); }
+
+// every slot empty and DONE, nothing claimed yet
+__global__ void k_queue_init(const DevProblem P, SolveDev S, QueueDev Q) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b == 0) { *S.n_active = 0; *Q.next = 0; }
+    if (b >= P.B) return;
+    S.state[b] = SOLVE_DONE;
+    Q.slot[b] = -1;
+    Q.mask[b] = SOLVE_DONE; Q.mask[P.B + b] = SOLVE_DONE;
+    if (S.go) { S.go[b] = SOLVE_DONE; S.go[P.B + b] = SOLVE_DONE; }
+}
+
+// mask of half `half` := the slots of the half whose problem stopped in this half's check (its objective, k_cost, follows with this mask)
+__global__ void k_queue_harvest(const DevProblem P, SolveDev S, QueueDev Q, int half, int mode) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P.B) return;
+    Q.mask[half * P.B + b] = in_half(P, b, mode) && Q.slot[b] >= 0 && S.state[b] == SOLVE_DONE ? SOLVE_ACTIVE : SOLVE_DONE;
+}
+
+// The harvested slots hand their statistics, objective and trajectory to their problem's row of the outputs; then every DONE slot of the half
+// claims the next problem.  A claimed problem starts as to_solve starts an instance that holds it: x0, U0 in the live buffer, lambda = 0, the
+// shared penalties, its rows of the slot tables, k_solve_init's state.  The mask then marks the refilled slots, for their rollout, merit and
+// k_queue_begin.
+__global__ void k_queue_refill(const DevProblem P, SolveDev S, QueueDev Q, int half, int mode) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P.B || !in_half(P, b, mode)) return;
+    const int n = P.n, m = P.m, N = P.N;
+    int* mask = Q.mask + (size_t)half * P.B + b;
+    if (*mask == SOLVE_ACTIVE) {
+        const int p = Q.slot[b];
+        Q.status[p] = S.status[b]; Q.iter[p] = S.iter[b]; Q.outer[p] = S.outer[b];
+        Q.cost[p] = Q.cost_slot[b]; Q.dJ[p] = S.dJ[b]; Q.grad[p] = S.grad[b]; Q.cmax[p] = S.cmax[b];
+        if (Q.X) { const double* X = traj_X(P, P.cur[b], b); for (int i = 0; i < N * n; i++) Q.X[(size_t)p * N * n + i] = X[i]; }
+        if (Q.U) { const double* U = traj_U(P, P.cur[b], b); for (int i = 0; i < (N - 1) * m; i++) Q.U[(size_t)p * (N - 1) * m + i] = U[i]; }
+        Q.slot[b] = -1;
+    }
+    *mask = SOLVE_DONE;
+    if (S.state[b] != SOLVE_DONE || *(volatile int*)Q.next >= Q.M) return;
+    const int p = atomicAdd(Q.next, 1);
+    if (p >= Q.M) return;
+    Q.slot[b] = p;
+    for (int i = 0; i < n; i++) P.x0[(size_t)b * n + i] = Q.x0[(size_t)p * n + i];
+    const double* U0 = Q.U0 + (Q.U0_shared ? 0 : (size_t)p * (N - 1) * m);
+    double* U = traj_Uw(P, P.cur[b], b);
+    for (int i = 0; i < (N - 1) * m; i++) U[i] = U0[i];
+    for (int i = 0; i < P.lambda_len; i++) P.lambda[(size_t)b * P.lambda_len + i] = 0.0;
+    if (Q.mub) for (int i = 0; i < P.ncon; i++) Q.mub[(size_t)b * P.ncon + i] = P.mu[i];
+    auto rows = [&](const double* src, double* dst, int w) {
+        if (dst) for (int i = 0; i < w; i++) dst[(size_t)b * w + i] = src[(size_t)p * w + i];
+    };
+    rows(Q.qr_src, Q.qr, P.ncost * (n + m));
+    rows(Q.cd_src, Q.cd, P.ncdata);
+    rows(Q.mp_src, Q.mp, TO_NPARAM);
+    solve_init_instance(P, S, b);
+    *mask = SOLVE_ACTIVE;
+    __threadfence();
+    atomicAdd(S.n_active, 1);
+}
+
+// the refilled slots of half `half`, after their rollout and merit: their first inner loop starts, as k_solve_begin starts it
+__global__ void k_queue_begin(const DevProblem P, SolveDev S, QueueDev Q, int half) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= P.B || Q.mask[half * P.B + b] != SOLVE_ACTIVE) return;
+    S.J_prev[b] = P.J[b]; S.inner[b] = 0; S.dj_zero[b] = 0;
+}
+
 // to_mpc_solve: step j's solve statistics of instance b, as to_solve returns them, into row j of the history.  A launch of its own:
 // k_mpc_advance's plant step is kept as it is compiled (DESIGN.md 5l)
 __global__ void k_mpc_solve_record(const DevProblem P, const SolveDev S, const MpcDev M, int j) {
@@ -153,5 +227,21 @@ cudaError_t launch_solve_restart(const DevProblem& P, const SolveDev& S, int hal
 }
 cudaError_t launch_mpc_solve_record(const DevProblem& P, const SolveDev& S, const MpcDev& M, int j, cudaStream_t s) {
     k_mpc_solve_record<<<nblk(P.B, 128), 128, 0, s>>>(P, S, M, j);
+    return cudaGetLastError();
+}
+cudaError_t launch_queue_init(const DevProblem& P, const SolveDev& S, const QueueDev& Q, cudaStream_t s) {
+    k_queue_init<<<nblk(P.B, 128), 128, 0, s>>>(P, S, Q);
+    return cudaGetLastError();
+}
+cudaError_t launch_queue_harvest(const DevProblem& P, const SolveDev& S, const QueueDev& Q, int half, int mode, cudaStream_t s) {
+    k_queue_harvest<<<nblk(P.B, 128), 128, 0, s>>>(P, S, Q, half, mode);
+    return cudaGetLastError();
+}
+cudaError_t launch_queue_refill(const DevProblem& P, const SolveDev& S, const QueueDev& Q, int half, int mode, cudaStream_t s) {
+    k_queue_refill<<<nblk(P.B, 128), 128, 0, s>>>(P, S, Q, half, mode);
+    return cudaGetLastError();
+}
+cudaError_t launch_queue_begin(const DevProblem& P, const SolveDev& S, const QueueDev& Q, int half, cudaStream_t s) {
+    k_queue_begin<<<nblk(P.B, 128), 128, 0, s>>>(P, S, Q, half);
     return cudaGetLastError();
 }

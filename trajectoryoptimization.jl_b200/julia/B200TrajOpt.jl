@@ -458,6 +458,41 @@ function solve!(p::BatchedProblem; kw...)
     (status = [SOLVE_STATUS[s + 1] for s in status], iterations = iters, iterations_outer = outer, cost = cost, dJ = dJ, gradient = grad, c_max = cmax)
 end
 
+# a queue of M problems through the batch's slots (to_solve_queue, DESIGN.md 5n): Altro's loop of solve! over many Problems, on the device.
+# x0s (n, M); U0s (m, N-1, M) or (m, N-1) for every problem; xf (n, M) or nothing (objective / constraint as set_goal_state!); params
+# (nparams, M) or nothing.  A named tuple of [M] vectors as solve! returns, plus X (n, N, M) and U (m, N-1, M).
+struct ToQueueSpec
+    M::Int32; U0_shared::Int32
+    x0::Ptr{Float64}; U0::Ptr{Float64}; xf::Ptr{Float64}
+    goal_objective::Int32; goal_constraint::Int32
+    params::Ptr{Float64}
+    nparams::Int32; pad::Int32
+end
+function solve_queue!(p::BatchedProblem, x0s, U0s; xf = nothing, params = nothing, objective::Bool = true, constraint::Bool = true, kw...)
+    X0 = Matrix{Float64}(x0s); M = size(X0, 2)
+    U0 = Array{Float64}(U0s); shared = ndims(U0) == 2
+    (shared || size(U0, 3) == M) || throw(DimensionMismatch("U0s must be (m, N-1, M) or (m, N-1)"))
+    XF = xf === nothing ? nothing : Matrix{Float64}(xf)
+    XF === nothing || size(XF, 2) == M || throw(DimensionMismatch("xf must be (n, M)"))
+    P = params === nothing ? nothing : Matrix{Float64}(params)
+    P === nothing || size(P, 2) == M || throw(DimensionMismatch("params must be (nparams, M)"))
+    o = solve_options(kw)
+    n, N = size(X0, 1), size(U0, 2) + 1; m = size(U0, 1)
+    status, iters, outer = Vector{Int32}(undef, M), Vector{Int32}(undef, M), Vector{Int32}(undef, M)
+    cost, dJ, grad, cmax = (Vector{Float64}(undef, M) for _ in 1:4)
+    X, U = Array{Float64,3}(undef, n, N, M), Array{Float64,3}(undef, m, N - 1, M)
+    GC.@preserve X0 U0 XF P begin
+        spec = Ref(ToQueueSpec(M, shared, pointer(X0), pointer(U0), XF === nothing ? C_NULL : pointer(XF), objective, constraint,
+                               P === nothing ? C_NULL : pointer(P), P === nothing ? 0 : size(P, 1), 0))
+        check(p.h, ccall((:to_solve_queue, libb200), Cint,
+                         (Ptr{Cvoid}, Ref{ToQueueSpec}, Ref{ToSolveOptions}, Ptr{Int32}, Ptr{Int32}, Ptr{Int32}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+                          Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                         p.h, spec, o, status, iters, outer, cost, dJ, grad, cmax, X, U))
+    end
+    (status = [SOLVE_STATUS[s + 1] for s in status], iterations = iters, iterations_outer = outer, cost = cost, dJ = dJ, gradient = grad,
+     c_max = cmax, X = X, U = U)
+end
+
 # MPC plumbing: update_trajectory!(obj, Z, start) src/objective.jl:198-212 on the batched problem; Xref (n, nref), Uref (m, nref)
 TO.update_trajectory!(p::BatchedProblem, Xref::Matrix{Float64}, Uref::Matrix{Float64}, start::Integer=1) =
     check(p.h, ccall((:to_update_trajectory, libb200), Cint, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Float64}, Int32, Int32), p.h, Xref, Uref, size(Xref, 2), start))
