@@ -153,8 +153,8 @@ typedef struct {
                                 cost expansion G'lxx G + grad^2-differential, dx = state_diff(xbar, x) with the Cayley map.  The reference's hooks for
                                 it: src/abstract_constraint.jl:282-303 (error_expansion! of constraint Jacobians), src/lie_costs.jl.  0: full state. */
     /* TO_MODEL_EXPR only (else 0 / NULL): `Problem(models::Vector{<:DiscreteDynamics}, ...)`, src/problem.jl:36-73 with RD.dims(models), src/dynamics.jl:15-31.
-       n, m are the LARGEST state / control dimensions; knot k has nx[k] <= n states and nu[k] <= m controls, stored in the first entries of the
-       n- / m-sized slots (the rest stays zero: costs and constraints are described on the padded [x(n); u(m)] layout, with unit weights on the
+       n, m are the padded size class to_recorded_dims gives for the LARGEST per-knot state / control dimensions (any other n, m is refused
+       with TO_EDIM); knot k has nx[k] <= n states and nu[k] <= m controls, stored in the first entries of the n- / m-sized slots (the rest stays zero: costs and constraints are described on the padded [x(n); u(m)] layout, with unit weights on the
        unused controls so that Quu stays positive definite).  Model dyn[dyn_index[k]] maps knot k to k+1: n_in = nx[k], m_in = nu[k], n_out = nx[k+1]
        (checked: the reference's DimensionMismatch "Model mismatch at time step k"). */
     int32_t ndyn;
@@ -182,6 +182,10 @@ typedef struct to_handle to_handle;
 
 /* ---- lifecycle -------------------------------------------------------------------------------------- */
 int to_create(const to_spec* spec, to_handle** out);                 /* Problem(...)           src/problem.jl:79-111 */
+/* The padded size class (n, m) of a recorded-program problem (TO_MODEL_EXPR) whose largest per-knot state dimension is nx_max and largest
+ * per-knot control dimension is nu_max: the smallest of (4, 2), (8, 4) and (16, 8) that holds both.  TO_EDIM past (16, 8); TO_EINVAL for
+ * nx_max < 1, nu_max < 0 or a NULL output.  to_spec.n, m of such a problem must be this class. */
+int to_recorded_dims(int32_t nx_max, int32_t nu_max, int32_t* n, int32_t* m);
 int to_destroy(to_handle* h);
 const char* to_last_error(const to_handle* h);                       /* h may be NULL: error of the last failed to_create */
 int to_default_options(to_options* o);

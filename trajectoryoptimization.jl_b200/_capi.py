@@ -178,6 +178,7 @@ def load_library():
     H = C.c_void_p
     sig = {
         "to_create": [C.POINTER(to_spec), C.POINTER(H)],
+        "to_recorded_dims": [C.c_int32, C.c_int32, c_int32_p, c_int32_p],
         "to_destroy": [H], "to_default_options": [C.POINTER(to_options)], "to_set_options": [H, C.POINTER(to_options)],
         "to_set_stream": [H, C.c_void_p], "to_synchronize": [H],
         "to_dims": [H, c_int32_p, c_int32_p, c_int32_p, c_int32_p], "to_num_constraints": [H, c_int32_p],
@@ -235,7 +236,7 @@ def load_library():
 
 
 EXPORTED_SYMBOLS = [
-    "to_create", "to_destroy", "to_last_error", "to_default_options", "to_set_options", "to_set_stream", "to_synchronize", "to_dims",
+    "to_create", "to_recorded_dims", "to_destroy", "to_last_error", "to_default_options", "to_set_options", "to_set_stream", "to_synchronize", "to_dims",
     "to_num_constraints", "to_constraint_info", "to_bounds", "to_set_initial_state", "to_set_controls", "to_set_states",
     "to_set_goal_state", "to_set_initial_time", "to_get_states", "to_get_controls", "to_get_times", "to_rollout", "to_expand",
     "to_get_dynamics_jacobians", "to_cost", "to_cost_knots", "to_cost_gradient", "to_cost_hessian", "to_eval_constraints",
@@ -254,6 +255,19 @@ EXPORTED_SYMBOLS = [
 
 class TrajOptError(RuntimeError):
     pass
+
+
+def recorded_dims(nx_max, nu_max):
+    """to_recorded_dims: the padded size class ``(n, m)`` -- (4, 2), (8, 4) or (16, 8) -- a recorded-program problem runs on when its largest
+    per-knot state dimension is ``nx_max`` and its largest per-knot control dimension ``nu_max``.  Raises ``DimensionMismatch`` past (16, 8)."""
+    lib = load_library()
+    n, m = C.c_int32(), C.c_int32()
+    rc = lib.to_recorded_dims(int(nx_max), int(nu_max), C.byref(n), C.byref(m))
+    if rc == TO_EDIM:
+        raise DimensionMismatch(f"recorded-program models: at most 16 states and 8 controls per knot, the largest has ({nx_max}, {nu_max})")
+    if rc != TO_OK:
+        raise ArgumentError(f"recorded-program models: no size class for ({nx_max}, {nu_max})")
+    return n.value, m.value
 
 
 class DimensionMismatch(TrajOptError):   # Julia DimensionMismatch (reference src/problem.jl:64-68)

@@ -1103,23 +1103,24 @@ class Problem:
         x0 = np.asarray(x0, dtype=float)
         if isinstance(model, AutodiffDynamics):
             # one user model (RD.@autodiff struct M <: ContinuousDynamics + Problem(model, obj, x0, tf)) steps every knot: it is the model
-            # vector [model] * (N - 1), on the padded (4, 2) layout the recorded-program kernels exist for
+            # vector [model] * (N - 1), on the padded size class of its dimensions
             model = [model] * (N - 1)
         self.hybrid = isinstance(model, (list, tuple))
         if self.hybrid:
             # Problem(models::Vector{<:DiscreteDynamics}, obj, x0, tf)  src/problem.jl:36-73: per-knot dimensions from RD.dims(models); the
-            # device works on the padded dimensions (n, m) = (4, 2) with the knot's own entries first (include/trajopt_b200.h to_spec.nx)
+            # device works on the padded size class (n, m) of the largest -- (4, 2), (8, 4) or (16, 8), to_recorded_dims -- with the knot's own
+            # entries first (include/trajopt_b200.h to_spec.nx)
             models = list(model)
             nxv, nuv = model_dims(models)                       # DimensionMismatch "Model mismatch at time step k"
             if len(models) != N - 1:
                 raise DimensionMismatch("need one model per time step (N - 1 models)")     # @assert length(models) == N-1
             if any(not isinstance(mdl, AutodiffDynamics) for mdl in models):
                 raise ArgumentError("a model vector holds AutodiffDynamics models")
-            if max(nxv) > 4 or max(nuv) > 2:
-                raise ArgumentError("hybrid problems: at most 4 states and 2 controls per knot (the padded kernel instance)")
-            n, m = 4, 2
+            n, m = K.recorded_dims(max(nxv), max(nuv))          # DimensionMismatch past 16 states or 8 controls
             if error_state:
                 raise ArgumentError("error_state=True needs a Lie-group model (RD.errstate_dim(model) != state_dim)")
+            if x0.shape[-1] == n and n != nxv[0] and not np.any(x0[..., nxv[0]:]):
+                x0 = x0[..., :nxv[0]]                           # x0 on the padded layout, as prob.x0 holds it
             if x0.shape[-1] != nxv[0]:
                 raise DimensionMismatch("x0 does not match the first model's state dimension")   # @assert length(x0) == nx[1]
             cons = constraints if constraints is not None else ConstraintList(nxv, nuv)
@@ -1171,7 +1172,15 @@ class Problem:
         self._device = device
         self._dt = np.array(dtv, dtype=float)        # the time steps as given: a rebuild must not re-derive them from the knot times
         self.spec = self._make_spec(dtv, t0)
-        self._open()
+        try:
+            self._open()
+        except DimensionMismatch as e:
+            # the spec carries the class to_recorded_dims gives, so a dimension refusal of a larger class comes from a library that opens
+            # recorded programs on the (4, 2) layout only (one built before the size classes)
+            if self.hybrid and (n, m) != (4, 2):
+                raise ArgumentError(f"recorded-program models: this library does not open the padded size class ({n}, {m}) ({e}); it takes "
+                                    "at most 4 states and 2 controls per knot") from e
+            raise
         self._apply_integration()
         self._sig = self._signature()
         self._call("to_set_initial_state", K._dp(self.x0))
@@ -1189,7 +1198,7 @@ class Problem:
             con_specs = [c._spec(f, l) for (f, l), c in zip(cons.inds, cons.constraints)]
             return K.Spec(self.model.model_id, self.n, self.m, self.N, self.B, dtv, [c._spec() for c in uniq], index, con_specs,
                           params=self.model.params, t0=t0, device=self._device, error_state=self.error_state)
-        # hybrid: every cost / constraint is re-expressed on the padded [x(4); u(2)] layout (change_dimension, src/cost_functions.jl:391-401,
+        # hybrid: every cost / constraint is re-expressed on the padded [x(n); u(m)] layout (change_dimension, src/cost_functions.jl:391-401,
         # src/constraints.jl:934-936); the unused controls get a unit weight so that Quu stays positive definite -- they stay exactly zero
         n, m = self.n, self.m
         padded, uniq, index, seen = {}, [], [], {}

@@ -257,7 +257,7 @@ void model_defaults(int model, int m, int& n_out, int& m_out, double* p) {
             p[7] = 0.1750; p[8] = 1.0; p[9] = 0.0245; break;
         case TO_MODEL_ACROBOT:
             n_out = 4; m_out = 1; p[0] = 1; p[1] = 1; p[2] = 1; p[3] = 1; p[4] = 1.0 / 12; p[5] = 1.0 / 12; p[6] = 1.0; p[7] = 9.81; break;
-        case TO_MODEL_EXPR: n_out = 4; m_out = 2; break;       // recorded programs on the padded dimensions the kernels are instantiated for
+        case TO_MODEL_EXPR: n_out = 0; m_out = 0; break;       // recorded programs: the size class of the per-knot dimensions (to_create)
         default: n_out = -1; m_out = -1;
     }
 }
@@ -544,6 +544,16 @@ int to_default_options(to_options* o) {
     return TO_OK;
 }
 
+// The recorded-program kernels exist for three padded size classes (models.cuh MODEL_EXPR_42 / _84 / _168): a problem takes the smallest that
+// holds its largest per-knot dimensions, so that problems which fit (4, 2) keep the kernels they have always run.
+int to_recorded_dims(int32_t nx_max, int32_t nu_max, int32_t* n, int32_t* m) {
+    if (!n || !m || nx_max < 1 || nu_max < 0) return TO_EINVAL;
+    static const int32_t cls[3][2] = {{4, 2}, {8, 4}, {16, 8}};
+    for (const auto& c : cls)
+        if (nx_max <= c[0] && nu_max <= c[1]) { *n = c[0]; *m = c[1]; return TO_OK; }
+    return TO_EDIM;
+}
+
 int to_create(const to_spec* s, to_handle** out) {
     if (!s || !out) return fail(nullptr, TO_EINVAL, "null argument");
     *out = nullptr;
@@ -558,13 +568,24 @@ int to_create(const to_spec* s, to_handle** out) {
     if (s->model == TO_MODEL_DOUBLE_INTEGRATOR && s->m != 1 && s->m != 2) return fail(nullptr, TO_EDIM, "DoubleIntegrator: supported dimensions are 1 and 2");
     std::vector<DevDyn> dyn_tab; std::vector<int> dyn_idx;
     if (s->model == TO_MODEL_EXPR) {
-        // Problem(models::Vector, ...) with RD.dims(models) (src/dynamics.jl:15-31): per-knot dimensions, padded to the (n, m) = (4, 2) the kernels exist for
-        if (s->n != 4 || s->m != 2) return fail(nullptr, TO_EDIM, "recorded-program models: the padded dimensions must be n = 4, m = 2 (largest per-knot dimensions <= that)");
+        // Problem(models::Vector, ...) with RD.dims(models) (src/dynamics.jl:15-31): per-knot dimensions, padded to the size class of the largest
         if (s->N < 2 || !s->dyn || s->ndyn < 1 || !s->dyn_index || !s->nx || !s->nu) return fail(nullptr, TO_EINVAL, "recorded-program models: null dyn / dyn_index / nx / nu");
+        int nx_max = 0, nu_max = 0;
+        for (int k = 0; k < s->N; k++) {
+            if (s->nx[k] < 1 || s->nu[k] < 0) return fail(nullptr, TO_EINVAL, "recorded-program models: a knot has fewer than 1 state or 0 controls");
+            nx_max = std::max(nx_max, (int)s->nx[k]); nu_max = std::max(nu_max, (int)s->nu[k]);
+        }
+        if (to_recorded_dims(nx_max, nu_max, &mn, &mm) != TO_OK)
+            return fail(nullptr, TO_EDIM, "recorded-program models: at most 16 states and 8 controls per knot, the largest has (" + std::to_string(nx_max) + ", " +
+                        std::to_string(nu_max) + ")");
+        if (s->n != mn || s->m != mm)
+            return fail(nullptr, TO_EDIM, "recorded-program models: largest per-knot dimensions (" + std::to_string(nx_max) + ", " + std::to_string(nu_max) +
+                        ") run on the padded size class n = " + std::to_string(mn) + ", m = " + std::to_string(mm) + " (to_recorded_dims), not n = " +
+                        std::to_string(s->n) + ", m = " + std::to_string(s->m));
         for (int i = 0; i < s->ndyn; i++) {
             const to_dynamics_spec& d = s->dyn[i];
             if (!d.prog || d.prog_len < 1 || d.prog_len > TO_EXPR_LEN || d.nconst < 0 || d.nconst > TO_EXPR_CONST || (d.nconst > 0 && !d.consts) ||
-                d.n_in < 1 || d.n_in > 4 || d.m_in < 0 || d.m_in > 2 || d.n_out < 1 || d.n_out > 4 || d.n_out > d.prog_len)
+                d.n_in < 1 || d.n_in > mn || d.m_in < 0 || d.m_in > mm || d.n_out < 1 || d.n_out > mn || d.n_out > d.prog_len)
                 return fail(nullptr, TO_EINVAL, "recorded-program model: bad program size or dimensions");
             DevDyn dd; std::memset(&dd, 0, sizeof(dd));
             dd.n_in = d.n_in; dd.m_in = d.m_in; dd.n_out = d.n_out; dd.discrete = d.discrete != 0; dd.prog_len = d.prog_len;

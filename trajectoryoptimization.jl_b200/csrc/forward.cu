@@ -545,7 +545,7 @@ __device__ __forceinline__ double rollout_compact(const DevProblem& P, const Fwd
             }
             J = fma(a - l2, INST ? gcost->inv2mu : tab.inv2mu, J);
         }
-        if constexpr (MODEL == MODEL_EXPR_42) {   // a discrete jump map writes its outputs while it reads its inputs
+        if constexpr (is_recorded<MODEL>) {   // a discrete jump map writes its outputs while it reads its inputs
             double xn[n];
             explicit_step<MODEL, double, RULE>(model_params<MODEL, INST>(P, prm, k), x, u, time_step<INST>(P, b, k, tab.dt), xn);
 #pragma unroll

@@ -92,10 +92,14 @@ template <> struct ModelDims<MODEL_ACROBOT> { static constexpr int n = 4, m = 1;
 constexpr int MODEL_DOUBLE_INTEGRATOR_2D = 16;
 template <> struct ModelDims<MODEL_DOUBLE_INTEGRATOR> { static constexpr int n = 2, m = 1; };
 template <> struct ModelDims<MODEL_DOUBLE_INTEGRATOR_2D> { static constexpr int n = 4, m = 2; };
-// user dynamics recorded as programs (TO_MODEL_EXPR), hybrid / variable-dimension models: instantiated for the padded dimensions (4, 2)
-// of the reference's example (test/hybrid_dynamics_model.jl:15-54)
-constexpr int MODEL_EXPR_42 = 20;
+// user dynamics recorded as programs (TO_MODEL_EXPR), single or hybrid / variable-dimension models: instantiated for three padded size
+// classes, (4, 2) -- the reference's hybrid example (test/hybrid_dynamics_model.jl:15-54) --, (8, 4) and (16, 8).  A problem runs on the
+// smallest class that holds its largest per-knot dimensions (capi.cu to_recorded_dims); the padded m (2, 4 or 8) names the class.
+constexpr int MODEL_EXPR_42 = 20, MODEL_EXPR_84 = 21, MODEL_EXPR_168 = 22;
 template <> struct ModelDims<MODEL_EXPR_42> { static constexpr int n = 4, m = 2; };
+template <> struct ModelDims<MODEL_EXPR_84> { static constexpr int n = 8, m = 4; };
+template <> struct ModelDims<MODEL_EXPR_168> { static constexpr int n = 16, m = 8; };
+template <int MODEL> constexpr bool is_recorded = MODEL == MODEL_EXPR_42 || MODEL == MODEL_EXPR_84 || MODEL == MODEL_EXPR_168;
 
 // a b - c c (the Cartpole's mass-matrix determinant).  With dual numbers the value is written as the one rounding fma(a, b, -(c c)): the
 // compiler is free to contract either product, and it chose differently when the parameters came from shared memory (per-instance
@@ -121,7 +125,7 @@ __device__ __forceinline__ Dual<P> det_sub_square(const Dual<P>& a, const Dual<P
 
 template <int MODEL, class S, bool DET_FMA = false>
 __device__ __forceinline__ void dynamics(const double* __restrict__ p, const S* x, const S* u, S* xd) {
-    if constexpr (MODEL == MODEL_EXPR_42) {
+    if constexpr (is_recorded<MODEL>) {
         // `p` is the knot's DevDyn (model_params): interpret the recorded program with the scalar type S (double or dual numbers); the
         // outputs are the last n_out instructions, the unused state slots of the next knot stay zero
         constexpr int n = ModelDims<MODEL>::n;
@@ -238,7 +242,7 @@ template <int MODEL, class S, int RULE, bool DET_FMA = false>
 __device__ __forceinline__ void explicit_step(const double* __restrict__ p, const S* x, const S* u, double h, S* xn) {
     static_assert(RULE >= 1 && RULE <= 4, "to_integration: TO_EULER .. TO_RK4");
     constexpr int n = ModelDims<MODEL>::n;
-    if constexpr (MODEL == MODEL_EXPR_42) {     // a discrete jump map is applied as is
+    if constexpr (is_recorded<MODEL>) {     // a discrete jump map is applied as is
         if (reinterpret_cast<const DevDyn*>(p)->discrete) { dynamics<MODEL, S>(p, x, u, xn); return; }
     }
     if constexpr (RULE == 1) {
@@ -292,7 +296,11 @@ __device__ __forceinline__ void explicit_step(const double* __restrict__ p, cons
         case MODEL_CARTPOLE: { constexpr int MODEL = MODEL_CARTPOLE; CALL; } break;                \
         case MODEL_QUADROTOR: { constexpr int MODEL = MODEL_QUADROTOR; CALL; } break;              \
         case MODEL_ACROBOT: { constexpr int MODEL = MODEL_ACROBOT; CALL; } break;                  \
-        case MODEL_EXPR: { constexpr int MODEL = MODEL_EXPR_42; CALL; } break;                     \
+        case MODEL_EXPR:                                                                           \
+            if ((m_dim) == 2) { constexpr int MODEL = MODEL_EXPR_42; CALL; }                       \
+            else if ((m_dim) == 4) { constexpr int MODEL = MODEL_EXPR_84; CALL; }                  \
+            else { constexpr int MODEL = MODEL_EXPR_168; CALL; }                                   \
+            break;                                                                                 \
     }
 
 // dispatch on the problem's explicit rule (DevProblem::integration): RULE = RULE_EULER .. RULE_RK4
@@ -308,7 +316,7 @@ __device__ __forceinline__ void explicit_step(const double* __restrict__ p, cons
 // the kernel made with stage_model_params; recorded programs: the DevDyn of knot k (their constants are never per instance)
 template <int MODEL, bool INST = false>
 __device__ __forceinline__ const double* model_params(const DevProblem& P, const double* row, int k) {
-    if constexpr (MODEL == MODEL_EXPR_42) return reinterpret_cast<const double*>(&P.dyn[P.dyn_index[k]]);
+    if constexpr (is_recorded<MODEL>) return reinterpret_cast<const double*>(&P.dyn[P.dyn_index[k]]);
     else if constexpr (INST) return row;
     else return P.params;
 }

@@ -102,7 +102,7 @@ struct RiccatiSmem {
     double Q[MMA ? 2 : even_up(NM) * LDT + 8];   // full Q only on the DFMA path
     // u / Qz strip of Q, gains K|d and W = Qux - rho K.  MMA path: they overlay T, which is dead once Q sits in the
     // accumulator registers and is rewritten only by the next knot (2.2 KB per warp -> room for 18-20 warps per SM)
-    static constexpr int QS_SIZE = (NM + 1) * LDQS, KW_SIZE = 4 * LDK + 8;
+    static constexpr int QS_SIZE = (NM + 1) * LDQS, KW_SIZE = (M_ > 4 ? M_ : 4) * LDK + 8;   // m rows of K|d (W): 4 at least
     static_assert(!MMA || QS_SIZE + 2 * KW_SIZE <= TROWS * LDT + 8, "overlay does not fit T");
     double QKW[MMA ? 2 : QS_SIZE + 2 * KW_SIZE];
     __device__ __forceinline__ double* qs() { return MMA ? T : QKW; }
@@ -217,7 +217,7 @@ __global__ void TO_RICCATI_BOUNDS(MINB) k_riccati(const DevProblem P, int* __res
         (void)nterm;   // NSLOT (template) >= the largest per-lane count: launch_riccati_nm picks it from P.max_terms_per_z
     }
 
-    for (int e = lane; e < 4 * LDK + 8; e += 32) { K_[e] = 0.0; W_[e] = 0.0; }   // padding columns stay finite
+    for (int e = lane; e < SM::KW_SIZE; e += 32) { K_[e] = 0.0; W_[e] = 0.0; }   // padding columns stay finite
     if (lane == 0) {
 #pragma unroll
         for (int s = 0; s < STAGES; s++) mbar_init(&sm.bar[s], 1);
@@ -885,7 +885,10 @@ cudaError_t launch_riccati_t(const DevProblem& P, const BackwardPlan& plan, int*
         }
         return launch_riccati_v<N_, M_, FASTAL, 2, 12, false, MAXT, INST>(P, work_counter, s);   // dense costs: DFMA micro-block kernel
     } else {
-        return launch_riccati_v<N_, M_, FASTAL, 3, 16, false, MAXT, INST>(P, work_counter, s);
+        // m > 4 (the recorded class (16, 8)): its shared memory holds at most 6 one-warp CTAs per SM, so the register cap of 16 CTAs per SM
+        // (128) only made it spill; 8 CTAs lift the cap to 255
+        constexpr int MINB = M_ > 4 ? 8 : 16;
+        return launch_riccati_v<N_, M_, FASTAL, 3, MINB, false, MAXT, INST>(P, work_counter, s);
     }
 }
 
@@ -924,5 +927,8 @@ cudaError_t launch_backward(const DevProblem& P, const BackwardPlan& plan, int* 
     if (P.n == 4 && P.m == 1) return launch_riccati_nm<4, 1>(P, plan, work_counter, s);
     if (P.n == 4 && P.m == 2) return launch_riccati_nm<4, 2>(P, plan, work_counter, s);
     if (P.n == 2 && P.m == 1) return launch_riccati_nm<2, 1>(P, plan, work_counter, s);
+    // the recorded-program size classes (8, 4) and (16, 8) (models.cuh); (4, 2) is above
+    if (P.n == 8 && P.m == 4) return launch_riccati_nm<8, 4>(P, plan, work_counter, s);
+    if (P.n == 16 && P.m == 8) return launch_riccati_nm<16, 8>(P, plan, work_counter, s);
     return cudaErrorNotSupported;
 }

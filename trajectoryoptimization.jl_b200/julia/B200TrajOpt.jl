@@ -52,6 +52,21 @@ function check(h::Ptr{Cvoid}, rc::Cint)
     error("libtrajopt_b200 [$rc]: $msg")
 end
 
+"""
+    recorded_dims(nx_max, nu_max) -> (n, m)
+
+The padded size class a problem of recorded dynamics programs (`TO_MODEL_EXPR`) runs on: the smallest of (4, 2), (8, 4) and (16, 8) that
+holds its largest per-knot state dimension `nx_max` and control dimension `nu_max` (`RD.dims(models)`).  `ToSpec.n, m` of such a problem
+must be this class; `DimensionMismatch` past 16 states or 8 controls.
+"""
+function recorded_dims(nx_max::Integer, nu_max::Integer)
+    n = Ref{Int32}(0); m = Ref{Int32}(0)
+    rc = ccall((:to_recorded_dims, libb200), Cint, (Int32, Int32, Ref{Int32}, Ref{Int32}), nx_max, nu_max, n, m)
+    rc == TO_EDIM && throw(DimensionMismatch("recorded-program models: at most 16 states and 8 controls per knot, the largest has ($nx_max, $nu_max)"))
+    rc == 0 || throw(ArgumentError("recorded-program models: no size class for ($nx_max, $nu_max)"))
+    (Int(n[]), Int(m[]))
+end
+
 model_id(::Any) = error("model not available on the device; supported: DoubleIntegrator, Cartpole, Quadrotor, Acrobot")
 
 mutable struct BatchedProblem
