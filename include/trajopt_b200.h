@@ -474,6 +474,36 @@ typedef struct to_queue_spec {
  * size, when the device cannot hold the staged problems and their outputs: the queue is never split silently. */
 int to_solve_queue(to_handle* h, const to_queue_spec* q, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer,
                    double* cost, double* dJ, double* gradient, double* c_max, double* X, double* U);
+/* ---- the queue with per-problem tables (DESIGN.md 5p): time steps, cost weights, constraint data, AL penalties, tracking references ------
+ * Each table gives every problem its own row of one per-instance table.  Problem p's rows are what the setters write, applied in this order to
+ * an instance of the handle: to_set_time_steps (the dt row; the clock is left alone), to_set_cost_weights for each cost given,
+ * to_set_constraint_data for each constraint given, to_update_trajectories (Xref, Uref, start), to_set_goal_states (xf, goal_objective,
+ * goal_constraint), to_set_model_params, to_set_penalties per constraint given (its entry replaces the shared penalty; the others
+ * keep the shared penalties, as without a table).  Its outputs are, bit for bit, what to_solve
+ * returns for an instance that starts from those rows, whatever slot it ran in, as for to_solve_queue.  So with weights and xf (or a reference),
+ * each problem's q | r are derived from its own weights; weights without xf or a reference leave the linear terms as they are, as
+ * to_set_cost_weights does.  Not supported: a per-problem initial time (host state no result reads), per-problem initial multipliers (problems
+ * start at lambda = 0), hybrid and recorded-program models (the setters refuse these tables there). */
+enum to_queue_table_kind { TO_QT_TIME_STEPS = 0, TO_QT_COST_WEIGHTS = 1, TO_QT_CONSTRAINT_DATA = 2, TO_QT_PENALTIES = 3, TO_QT_REFERENCE = 4 };
+typedef struct to_queue_table {
+    int32_t kind;              /* to_queue_table_kind */
+    int32_t index;             /* COST_WEIGHTS: the distinct cost; CONSTRAINT_DATA, PENALTIES: the constraint; REFERENCE: start; else 0 */
+    int32_t len;               /* doubles per problem (N-1, to_cost_weights_len, to_constraint_data_len, 1); REFERENCE: nref */
+    int32_t pad;
+    const double* rows;        /* [M][len]; REFERENCE: Xref [M][nref][n] */
+    const double* rows2;       /* REFERENCE: Uref [M][nref][m]; NULL otherwise */
+} to_queue_table;
+/* to_solve_queue with ntables tables; to_solve_queue is this call with ntables = 0.  The handle is left as to_solve_queue leaves it, its
+ * per-instance tables, clocks and closed-form Jacobian columns included.  Refused before any device work, with nothing changed (TO_EINVAL /
+ * TO_EDIM, naming the table, the problem and the entry): what to_solve_queue refuses; a row the table's setter refuses (a non-finite entry,
+ * dt <= 0, a non-zero H where the shared H is zero, a changed +-Inf pattern of a Bound or z_max < z_min, a NORM value < 0, a penalty <= 0,
+ * nref < start + N - 1, and the costs and constraints the setters keep shared, Goal constraints included: their values come from xf); a len
+ * other than the table's; an unknown kind; the same table twice; a reference together with xf and goal_objective = 1.  When the run
+ * fails, the handle is restored as far as the device allows, its closed-form Jacobian columns included.  The check that per-instance tables
+ * agree in every instance applies to every table the call does not replace, and not to the entries it does.  TO_ENOMEM as to_solve_queue, the staged rows and slot tables counted. */
+int to_solve_queue_tables(to_handle* h, const to_queue_spec* q, const to_queue_table* tables, int32_t ntables, const to_solve_options* o,
+                          int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* cost, double* dJ, double* gradient, double* c_max,
+                          double* X, double* U);
 /* ---- Lie-group error state (SURVEY 8 f2) ------------------------------------------------------------------- */
 int to_backward_algebra(const to_handle* h, int32_t* variant);             /* which arithmetic the next to_backward will use: 0 = pivot-by-pivot LDL' solve
                                                                              (riccati.cu, riccati_small.cu, lie.cu), 1 = 2 x 2 block inverse + W'K update

@@ -84,6 +84,13 @@ class to_queue_spec(C.Structure):
                 ("goal_objective", C.c_int32), ("goal_constraint", C.c_int32), ("params", c_double_p), ("nparams", C.c_int32), ("pad", C.c_int32)]
 
 
+class to_queue_table(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("index", C.c_int32), ("len", C.c_int32), ("pad", C.c_int32), ("rows", c_double_p), ("rows2", c_double_p)]
+
+
+QT_TIME_STEPS, QT_COST_WEIGHTS, QT_CONSTRAINT_DATA, QT_PENALTIES, QT_REFERENCE = 0, 1, 2, 3, 4
+
+
 class to_mpc_spec(C.Structure):
     _fields_ = [("nsteps", C.c_int32), ("nparams", C.c_int32), ("plant_params", c_double_p), ("W", c_double_p), ("Xref", c_double_p),
                 ("Uref", c_double_p), ("nref", C.c_int32), ("start", C.c_int32)]
@@ -222,6 +229,8 @@ def load_library():
         "to_mpc_solve": [H, C.c_int32, C.POINTER(to_solve_options)], "to_mpc_solve_history": [H, c_int32_p, c_int32_p, c_int32_p, c_double_p],
         "to_solve_queue": [H, C.POINTER(to_queue_spec), C.POINTER(to_solve_options), c_int32_p, c_int32_p, c_int32_p, c_double_p, c_double_p,
                            c_double_p, c_double_p, c_double_p, c_double_p],
+        "to_solve_queue_tables": [H, C.POINTER(to_queue_spec), C.POINTER(to_queue_table), C.c_int32, C.POINTER(to_solve_options), c_int32_p,
+                                  c_int32_p, c_int32_p, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p, c_double_p],
     }
     for name, args in sig.items():
         fn = getattr(lib, name)
@@ -249,7 +258,7 @@ EXPORTED_SYMBOLS = [
     "to_set_phase_timing", "to_get_phase_times", "to_launch_count", "to_algorithmic_bytes",
     "to_backward_algebra", "to_kernel_choice", "to_error_state_dim", "to_state_diff", "to_get_error_dynamics", "to_error_expansion",
     "to_get_expansion_records", "to_default_solve_options", "to_solve", "to_mpc_setup", "to_mpc_run", "to_mpc_history",
-    "to_mpc_solve", "to_mpc_solve_history", "to_solve_queue",
+    "to_mpc_solve", "to_mpc_solve_history", "to_solve_queue", "to_solve_queue_tables",
 ]
 
 

@@ -1594,45 +1594,47 @@ def _cost_and_index(prob, cost):
     return j, prob._cost_objs[j]
 
 
-def _cost_weight_rows(prob, cost, rows):
+def _cost_weight_rows(prob, cost, rows, M=None):
     """(index, cost, rows [B, len], linear terms or None) as ``to_set_cost_weights`` takes them; every check that needs no device happens
-    here.  Given cost objects, their q and r come back as ``(q [B, n], r [B, m])``, the cost's linear terms of every instance."""
+    here.  Given cost objects, their q and r come back as ``(q [B, n], r [B, m])``, the cost's linear terms of every instance.  ``M``: the
+    rows of M queued problems instead (``solve_queue``), named so in the messages."""
+    B, what, unit = (prob.B, "set_cost_weights", "instance") if M is None else (M, "solve_queue", "problem")
     if getattr(prob, "hybrid", False):
         raise ArgumentError("per-instance cost weights are not supported on hybrid problems")
     j, cost = _cost_and_index(prob, cost)
     shared = _cost_weight_row(cost)
     lin = None
     if isinstance(rows, (list, tuple)) and any(isinstance(x, CostFunction) for x in rows):
-        if len(rows) != prob.B:
-            raise DimensionMismatch(f"set_cost_weights: {len(rows)} costs for a batch of {prob.B} instances")
+        if len(rows) != B:
+            raise DimensionMismatch(f"{what}: {len(rows)} costs for " + (f"a batch of {B} instances" if M is None else f"{B} problems"))
         for b, x in enumerate(rows):
             if type(x) is not type(cost):
-                raise ArgumentError(f"set_cost_weights: instance {b} holds a {type(x).__name__}, the cost is a {type(cost).__name__}")
+                raise ArgumentError(f"{what}: {unit} {b} holds a {type(x).__name__}, the cost is a {type(cost).__name__}")
             if (x.state_dim, x.control_dim) != (cost.state_dim, cost.control_dim):
-                raise DimensionMismatch(f"set_cost_weights: instance {b}'s cost has dimensions {(x.state_dim, x.control_dim)}, "
+                raise DimensionMismatch(f"{what}: {unit} {b}'s cost has dimensions {(x.state_dim, x.control_dim)}, "
                                         f"the problem's {(cost.state_dim, cost.control_dim)}")
             if x.terminal != cost.terminal:
-                raise ArgumentError(f"set_cost_weights: instance {b}'s cost differs in its terminal flag")
+                raise ArgumentError(f"{what}: {unit} {b}'s cost differs in its terminal flag")
             if isinstance(cost, DiagonalQuatCost) and not (np.array_equal(x.q_ind, cost.q_ind) and np.array_equal(x.q_ref, cost.q_ref)):
-                raise ArgumentError(f"set_cost_weights: instance {b}'s DiagonalQuatCost differs in q_ind / q_ref")
+                raise ArgumentError(f"{what}: {unit} {b}'s DiagonalQuatCost differs in q_ind / q_ref")
             if not cost.is_diag and x.is_blockdiag() != cost.is_blockdiag():
-                raise ArgumentError(f"set_cost_weights: instance {b}'s QuadraticCost has another H-zero pattern (H == 0 selects kernel code)")
+                raise ArgumentError(f"{what}: {unit} {b}'s QuadraticCost has another H-zero pattern (H == 0 selects kernel code)")
         lin = (np.array([x.q for x in rows], dtype=np.float64), np.array([x.r for x in rows], dtype=np.float64))
         rows = [_cost_weight_row(x) for x in rows]
     out = np.ascontiguousarray(np.asarray(rows, dtype=np.float64))
-    if out.shape != (prob.B, shared.size):
-        raise DimensionMismatch(f"set_cost_weights: expected [{prob.B}, {shared.size}] rows, got {out.shape}")
-    for b in range(prob.B):
+    if out.shape != (B, shared.size):
+        raise DimensionMismatch(f"{what}: expected [{B}, {shared.size}] rows, got {out.shape}")
+    for b in range(B):
         bad = np.nonzero(~np.isfinite(out[b]))[0]
         if bad.size:
-            raise ArgumentError(f"set_cost_weights: instance {b}, entry {bad[0]} is not finite")
+            raise ArgumentError(f"{what}: {unit} {b}, entry {bad[0]} is not finite")
     if not cost.is_diag and cost.is_blockdiag():   # QuadraticCost with H == 0: every row keeps H zero
         n, m = cost.state_dim, cost.control_dim
         h0 = n * n + m * m
-        for b in range(prob.B):
+        for b in range(B):
             bad = np.nonzero(out[b, h0:h0 + m * n] != 0.0)[0]
             if bad.size:
-                raise ArgumentError(f"set_cost_weights: instance {b}, entry {h0 + bad[0]}: H must stay zero where the shared H is zero")
+                raise ArgumentError(f"{what}: {unit} {b}, entry {h0 + bad[0]}: H must stay zero where the shared H is zero")
     return j, cost, out, lin
 
 
@@ -1701,26 +1703,28 @@ def model_params(prob):
     return out
 
 
-def _time_step_rows(prob, dt, t0=None):
-    """``(dt[B, N-1], t0[B] or None)`` as ``to_set_time_steps`` takes them; every check that needs no device happens here"""
+def _time_step_rows(prob, dt, t0=None, M=None):
+    """``(dt[B, N-1], t0[B] or None)`` as ``to_set_time_steps`` takes them; every check that needs no device happens here (``M``: the rows of M
+    queued problems, as ``_cost_weight_rows``)"""
+    B, what, unit = (prob.B, "set_time_steps", "instance") if M is None else (M, "solve_queue", "problem")
     if getattr(prob, "hybrid", False):
         raise ArgumentError("per-instance time steps are not supported on hybrid problems")
     dt = np.asarray(dt, dtype=np.float64)
-    if dt.shape == (prob.B,):                  # one uniform step per instance: the reference's scalar dt
+    if dt.shape == (B,):                  # one uniform step per instance: the reference's scalar dt
         dt = np.repeat(dt[:, None], prob.N - 1, axis=1)
-    if dt.shape != (prob.B, prob.N - 1):
-        raise DimensionMismatch(f"set_time_steps: expected [{prob.B}, {prob.N - 1}] or [{prob.B}] time steps, got {dt.shape}")
+    if dt.shape != (B, prob.N - 1):
+        raise DimensionMismatch(f"{what}: expected [{B}, {prob.N - 1}] or [{B}] time steps, got {dt.shape}")
     bad = np.argwhere(~(np.isfinite(dt) & (dt > 0)))
     if bad.size:
-        raise ArgumentError(f"set_time_steps: instance {bad[0][0]}, knot {bad[0][1]}: a time step must be finite and positive")
+        raise ArgumentError(f"{what}: {unit} {bad[0][0]}, knot {bad[0][1]}: a time step must be finite and positive")
     if t0 is not None:
         t0 = np.asarray(t0, dtype=np.float64)
-        t0 = np.full(prob.B, float(t0)) if t0.ndim == 0 else t0
-        if t0.shape != (prob.B,):
-            raise DimensionMismatch(f"set_time_steps: expected [{prob.B}] initial times, got {t0.shape}")
+        t0 = np.full(B, float(t0)) if t0.ndim == 0 else t0
+        if t0.shape != (B,):
+            raise DimensionMismatch(f"{what}: expected [{B}] initial times, got {t0.shape}")
         bad = np.nonzero(~np.isfinite(t0))[0]
         if bad.size:
-            raise ArgumentError(f"set_time_steps: instance {bad[0]}: the initial time must be finite")
+            raise ArgumentError(f"{what}: {unit} {bad[0]}: the initial time must be finite")
         t0 = np.ascontiguousarray(t0)
     return np.ascontiguousarray(dt), t0
 
@@ -1789,59 +1793,63 @@ def _con_and_index(prob, con):
     return j, prob.constraints[j]
 
 
-def _constraint_data_rows(prob, con, rows):
-    """(index, constraint, rows [B, len]) as to_set_constraint_data / to_set_goal_values take them; every check that needs no device happens here"""
+def _constraint_data_rows(prob, con, rows, M=None):
+    """(index, constraint, rows [B, len]) as to_set_constraint_data / to_set_goal_values take them; every check that needs no
+    device happens here (``M``: the rows of M queued problems, as ``_cost_weight_rows``; a Goal constraint's values then come from xf)"""
+    B, what, unit = (prob.B, "set_constraint_data", "instance") if M is None else (M, "solve_queue", "problem")
     if getattr(prob, "hybrid", False):
         raise ArgumentError("per-instance constraint data is not supported on hybrid problems")
     j, con = _con_and_index(prob, con)
     objs = isinstance(rows, (list, tuple)) and any(isinstance(x, AbstractConstraint) for x in rows)
     if isinstance(con, GoalConstraint):
+        if M is not None:
+            raise ArgumentError(f"{what}: a Goal constraint's values come from xf")
         if objs:
-            if len(rows) != prob.B:
-                raise DimensionMismatch(f"set_constraint_data: {len(rows)} constraints for a batch of {prob.B} instances")
+            if len(rows) != B:
+                raise DimensionMismatch(f"{what}: {len(rows)} constraints for " + (f"a batch of {B} instances" if M is None else f"{B} problems"))
             if any(type(x) is not GoalConstraint or not np.array_equal(x.inds, con.inds) for x in rows):
                 raise ArgumentError("set_constraint_data: every instance's constraint must be a GoalConstraint on the same indices")
             rows = [x.xf for x in rows]
         out = np.ascontiguousarray(np.asarray(rows, dtype=np.float64))
-        if out.shape != (prob.B, con.p):
-            raise DimensionMismatch(f"set_constraint_data: expected [{prob.B}, {con.p}] Goal values, got {out.shape}")
+        if out.shape != (B, con.p):
+            raise DimensionMismatch(f"{what}: expected [{B}, {con.p}] Goal values, got {out.shape}")
         return j, con, out
     spec, shared = _con_row(con)
     if objs:
-        if len(rows) != prob.B:
-            raise DimensionMismatch(f"set_constraint_data: {len(rows)} constraints for a batch of {prob.B} instances")
+        if len(rows) != B:
+            raise DimensionMismatch(f"{what}: {len(rows)} constraints for " + (f"a batch of {B} instances" if M is None else f"{B} problems"))
         fields = _CON_DATA_FIELDS[spec["kind"]]
         packed = []
         for b, x in enumerate(rows):
             if type(x) is not type(con):
-                raise ArgumentError(f"set_constraint_data: instance {b} holds a {type(x).__name__}, the constraint is a {type(con).__name__}")
+                raise ArgumentError(f"{what}: {unit} {b} holds a {type(x).__name__}, the constraint is a {type(con).__name__}")
             xs, xr = _con_row(x)
             same = all(np.array_equal(np.asarray(xs[k]), np.asarray(spec[k])) for k in spec if k not in fields and k in xs) and set(xs) == set(spec)
             if xr.shape != shared.shape or not same:
-                raise DimensionMismatch(f"set_constraint_data: instance {b}'s {type(x).__name__} differs from the problem's in more than its data")
+                raise DimensionMismatch(f"{what}: {unit} {b}'s {type(x).__name__} differs from the problem's in more than its data")
             packed.append(xr)
         rows = packed
     out = np.ascontiguousarray(np.asarray(rows, dtype=np.float64))
-    if out.shape != (prob.B, shared.size):
-        raise DimensionMismatch(f"set_constraint_data: expected [{prob.B}, {shared.size}] rows, got {out.shape}")
-    for b in range(prob.B):
+    if out.shape != (B, shared.size):
+        raise DimensionMismatch(f"{what}: expected [{B}, {shared.size}] rows, got {out.shape}")
+    for b in range(B):
         r = out[b]
         if spec["kind"] == K.CON_BOUND:
             nm = shared.size // 2
             fin = np.isfinite(shared)
             bad = np.nonzero(np.where(fin, ~np.isfinite(r), r != shared))[0]
             if bad.size:
-                raise ArgumentError(f"set_constraint_data: instance {b}, entry {bad[0]}: BoundConstraint entries must be finite exactly where the "
+                raise ArgumentError(f"{what}: {unit} {b}, entry {bad[0]}: BoundConstraint entries must be finite exactly where the "
                                     "shared bound is, with the same infinities")
             bad = np.nonzero(~(r[:nm] >= r[nm:]))[0]
             if bad.size:
-                raise ArgumentError(f"set_constraint_data: instance {b}, entry {bad[0]}: Upper bounds must be greater than or equal to lower bounds")
+                raise ArgumentError(f"{what}: {unit} {b}, entry {bad[0]}: Upper bounds must be greater than or equal to lower bounds")
         else:
             bad = np.nonzero(~np.isfinite(r))[0]
             if bad.size:
-                raise ArgumentError(f"set_constraint_data: instance {b}, entry {bad[0]} is not finite")
+                raise ArgumentError(f"{what}: {unit} {b}, entry {bad[0]} is not finite")
             if spec["kind"] == K.CON_NORM and not r[0] >= 0:
-                raise ArgumentError(f"set_constraint_data: instance {b}: NormConstraint value must be non-negative")
+                raise ArgumentError(f"{what}: {unit} {b}: NormConstraint value must be non-negative")
     return j, con, out
 
 
@@ -2282,21 +2290,23 @@ def set_penalty(prob, con, mu):
     prob._call("to_set_penalty", _con_index(prob, con), float(mu))
 
 
-def _penalty_rows(prob, con, mu):
-    """(index, mu [B]) as to_set_penalties takes them; every check that needs no device happens here"""
+def _penalty_rows(prob, con, mu, M=None):
+    """(index, mu [B]) as to_set_penalties takes them; every check that needs no device happens here (``M``: the rows of
+    M queued problems, as ``_cost_weight_rows``)"""
+    B, what, unit = (prob.B, "set_penalties", "instance") if M is None else (M, "solve_queue", "problem")
     if getattr(prob, "hybrid", False):
         raise ArgumentError("per-instance penalties are not supported on hybrid problems")
     i = _con_index(prob, con)
     if not 0 <= i < len(prob.constraints):
-        raise ArgumentError(f"set_penalties: no constraint {i}")
+        raise ArgumentError(f"{what}: no constraint {i}")
     mu = np.asarray(mu, dtype=np.float64)
     if mu.ndim == 0:
-        mu = np.full(prob.B, float(mu))
-    if mu.shape != (prob.B,):
-        raise DimensionMismatch(f"set_penalties: expected [{prob.B}] penalties, got {mu.shape}")
+        mu = np.full(B, float(mu))
+    if mu.shape != (B,):
+        raise DimensionMismatch(f"{what}: expected [{B}] penalties, got {mu.shape}")
     bad = np.nonzero(~(np.isfinite(mu) & (mu > 0)))[0]
     if bad.size:
-        raise ArgumentError(f"set_penalties: instance {bad[0]}: a penalty must be finite and positive")
+        raise ArgumentError(f"{what}: {unit} {bad[0]}: a penalty must be finite and positive")
     return i, np.ascontiguousarray(mu)
 
 
@@ -2477,7 +2487,66 @@ def _queue_inputs(prob, x0, U0, xf, params):
     return M, x0, U0, shared, xf, params
 
 
-def solve_queue(prob, x0, U0, xf=None, objective=True, constraint=True, params=None, trajectories=True, **options):
+def _queue_tables(prob, M, xf, objective, dt, cost_weights, constraint_data, penalties, Xref, Uref, start):
+    """the per-problem tables ``to_solve_queue_tables`` takes, as ``(kind, index, len, rows, rows2)``; every check that needs no device
+    happens here, and the one device call (the problem's linear terms, when cost objects are given) comes after them"""
+    tables, lins = [], {}
+    if dt is not None:
+        rows = _time_step_rows(prob, dt, M=M)[0]
+        tables.append((K.QT_TIME_STEPS, 0, prob.N - 1, rows, None))
+    for kind, given, build in ((K.QT_COST_WEIGHTS, cost_weights, _cost_weight_rows), (K.QT_CONSTRAINT_DATA, constraint_data, _constraint_data_rows)):
+        seen = set()
+        for key, rows in (given or {}).items():
+            j, _, out, *lin = build(prob, key, rows, M=M)
+            if j in seen:
+                raise ArgumentError(f"solve_queue: the same table is given twice ({'cost' if kind == K.QT_COST_WEIGHTS else 'constraint'} {j})")
+            seen.add(j)
+            tables.append((kind, j, out.shape[1], out, None))
+            if lin and lin[0] is not None:
+                lins[j] = lin[0]
+    seen = set()
+    for key, v in (penalties or {}).items():
+        i, col = _penalty_rows(prob, key, v, M=M)
+        if i in seen:
+            raise ArgumentError(f"solve_queue: the same table is given twice (penalties of constraint {i})")
+        seen.add(i)
+        tables.append((K.QT_PENALTIES, i, 1, col, None))
+    if (Xref is None) != (Uref is None):
+        raise ArgumentError("solve_queue: Xref and Uref come together")
+    if Xref is not None:
+        if getattr(prob, "hybrid", False):
+            raise ArgumentError("per-instance goals are not supported on hybrid problems")
+        Xref = np.ascontiguousarray(np.asarray(Xref, dtype=np.float64)); Uref = np.ascontiguousarray(np.asarray(Uref, dtype=np.float64))
+        if (Xref.ndim != 3 or Uref.ndim != 3 or Xref.shape[0] != M or Uref.shape[0] != M or Xref.shape[2] != prob.n or Uref.shape[2] != prob.m
+                or Uref.shape[1] != Xref.shape[1]):
+            raise DimensionMismatch(f"solve_queue: Xref must be [{M}, nref, {prob.n}] and Uref [{M}, nref, {prob.m}]")
+        if start < 1 or start - 1 + prob.N > Xref.shape[1]:
+            raise DimensionMismatch("update_trajectory!: the reference is shorter than start + N - 1")
+        if not all(isinstance(c, QuadraticCostFunction) for c in prob.obj):
+            raise ArgumentError("update_trajectory! is defined for objectives of QuadraticCostFunctions (src/objective.jl:207)")
+        for what, a in (("Xref", Xref), ("Uref", Uref)):
+            bad = np.argwhere(~np.isfinite(a))
+            if bad.size:
+                raise ArgumentError(f"solve_queue: problem {bad[0][0]}, row {bad[0][1]}, entry {bad[0][2]}: {what} is not finite")
+        if xf is not None and objective:
+            raise ArgumentError("solve_queue: a reference and xf with objective=True would both set the linear cost terms")
+        tables.append((K.QT_REFERENCE, int(start), Xref.shape[1], Xref, Uref))
+    # Cost objects bring their q and r as well (set_cost_weights writes them).  The queue derives no linear term from them, so every q | r
+    # the later steps do not replace (a reference replaces both, xf with objective=True the q) must be the problem's own, bit for bit.
+    if lins and Xref is None:
+        q, r = cost_terms(prob)
+        same = lambda a, b: np.array_equal(np.asarray(a, dtype=np.float64).view(np.int64), np.asarray(b, dtype=np.float64).view(np.int64))
+        for j, (lq, lr) in lins.items():
+            for p in range(M):
+                for what, mine, theirs in (("r", lr[p], r[0, j]),) + ((("q", lq[p], q[0, j]),) if xf is None or not objective else ()):
+                    if not same(mine, theirs):
+                        raise ArgumentError(f"solve_queue: problem {p}: cost {j}'s {what} differs from the problem's linear terms; the queue takes "
+                                            "the weights of cost objects, not their linear terms: give weight rows, or xf / a reference that sets them")
+    return tables
+
+
+def solve_queue(prob, x0, U0, xf=None, objective=True, constraint=True, params=None, trajectories=True, *, dt=None, cost_weights=None,
+                constraint_data=None, penalties=None, Xref=None, Uref=None, start=1, **options):
     """Altro's ``solve!`` of M problems through the batch's B instances, which act as slots: a slot whose solve stops takes the next problem
     at once, on the device, so the batch stays full until the queue runs dry.  Every problem shares the problem's structure (model, N, costs,
     constraints, time steps, solver options) and brings its own ``x0[M, n]`` and initial controls ``U0`` (``[M, N-1, m]``, or ``[N-1, m]`` for
@@ -2485,12 +2554,28 @@ def solve_queue(prob, x0, U0, xf=None, objective=True, constraint=True, params=N
     parameters ``params[M, nparams]`` (as ``set_model_params``).  Problem p's results are, bit for bit, those ``solve`` gives an instance that
     starts from x0[p], U0[p], zero multipliers, the shared penalties and those goal and parameter rows, whichever slot it ran in.  The
     problem is left as it was (trajectories, multipliers, penalties, per-instance tables).  Per-instance cost weights, time steps, constraint
-    data and cost terms must be equal in every instance (xf replaces the Goal values and the q terms).  Returns a ``QueueResult``."""
+    data and cost terms must be equal in every instance (xf replaces the Goal values and the q terms).  Returns a ``QueueResult``.
+
+    Each problem can also bring its own rows of the per-instance tables (DESIGN.md 5p), each as its setter takes them with M rows:
+    ``dt`` (``[M, N-1]`` or ``[M]``, as ``set_time_steps``; the clocks stay), ``cost_weights`` (``{cost: rows[M, len] or [cost] * M}``, as
+    ``set_cost_weights``; cost objects give their weights, and their q and r must be the problem's wherever xf or a reference does not
+    replace them), ``constraint_data`` (``{con: rows[M, len] or [con] * M}``, as
+    ``set_constraint_data``; a Goal constraint's values come from xf), ``penalties`` (``{con: mu[M] or scalar}``, as ``set_penalties``;
+    the constraints not named keep the shared penalties, as without a table) and a tracking reference ``Xref[M, nref, n]``, ``Uref[M, nref, m]`` from
+    ``start`` (as ``update_trajectory``; not together with xf and ``objective=True``).  Problem p's rows are what the setters write in the
+    order time steps, weights, constraint data, reference, goal, parameters, penalties: with weights and xf or a reference its linear terms
+    come from its own weights.  The tables it gives need not agree between the problem's instances."""
     M, x0, U0, shared, xf, params = _queue_inputs(prob, x0, U0, xf, params)
     o = solve_options(**options)
+    tables = _queue_tables(prob, M, xf, objective, dt, cost_weights, constraint_data, penalties, Xref, Uref, start)
     r = QueueResult(M, prob.N, prob.n, prob.m) if trajectories else QueueResult(M)
     spec = K.to_queue_spec(M, int(shared), K._dp(x0), K._dp(U0), K._dp(xf), int(bool(objective)), int(bool(constraint)), K._dp(params),
                            0 if params is None else int(params.shape[1]), 0)
-    prob._call("to_solve_queue", C.byref(spec), C.byref(o), K._ip(r.status), K._ip(r.iterations), K._ip(r.iterations_outer), K._dp(r.cost),
-               K._dp(r.dJ), K._dp(r.gradient), K._dp(r.c_max), K._dp(r.X), K._dp(r.U))
+    outs = (K._ip(r.status), K._ip(r.iterations), K._ip(r.iterations_outer), K._dp(r.cost), K._dp(r.dJ), K._dp(r.gradient), K._dp(r.c_max),
+            K._dp(r.X), K._dp(r.U))
+    if not tables:
+        prob._call("to_solve_queue", C.byref(spec), C.byref(o), *outs)
+        return r
+    arr = (K.to_queue_table * len(tables))(*(K.to_queue_table(kind, index, ln, 0, K._dp(a), K._dp(a2)) for kind, index, ln, a, a2 in tables))
+    prob._call("to_solve_queue_tables", C.byref(spec), arr, len(tables), C.byref(o), *outs)
     return r

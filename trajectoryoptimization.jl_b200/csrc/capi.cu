@@ -998,16 +998,20 @@ static int stage_qr(to_handle* h) {
     return TO_OK;
 }
 static size_t cw_off(const to_handle* h, int b, const DevCost& c) { return (size_t)b * h->P.ncw + c.cwoff; }
-// q | r of cost ci for instance b from the goal xf and, when uf is given, the control reference uf: with the instance's own Q and R once the
-// weight table exists, else with the shared ones (the bits every instance had before)
-static void instance_linear_term(const to_handle* h, int b, int ci, const double* xf, const double* uf, double* row) {
+// q | r of cost ci from the goal xf and, when uf is given, the control reference uf: with the Q and R of the weights row w (one row of
+// DevProblem::cw, [ncw]) when it is given, else with the shared ones (the bits every instance had before)
+static void weights_linear_term(const to_handle* h, const double* w, int ci, const double* xf, const double* uf, double* row) {
     const DevCost& c = h->h_costs[ci];
     const int n = h->P.n, m = h->P.m;
     const double* Q = c.Q; const double* R = c.R;
     double Qb[TO_MAXN * TO_MAXN], Rb[TO_MAXM * TO_MAXM];
-    if (h->P.cw && c.cwoff >= 0) { cost_row_QR(c, h->h_cw.data() + cw_off(h, b, c), n, m, Qb, Rb); Q = Qb; R = Rb; }
+    if (w && c.cwoff >= 0) { cost_row_QR(c, w + c.cwoff, n, m, Qb, Rb); Q = Qb; R = Rb; }
     lqr_linear_term(Q, n, xf, row);
     if (uf) lqr_linear_term(R, m, uf, row + n);
+}
+// ... of instance b: with its own Q and R once the weight table exists
+static void instance_linear_term(const to_handle* h, int b, int ci, const double* xf, const double* uf, double* row) {
+    weights_linear_term(h, h->P.cw ? h->h_cw.data() + (size_t)b * h->P.ncw : nullptr, ci, xf, uf, row);
 }
 // h->stage := the rows of the cost-weight table, or every instance's shared weights of every cost when it does not exist yet
 static void stage_cw(to_handle* h) {
@@ -1082,12 +1086,17 @@ int to_set_goal_states(to_handle* h, const double* xf, int objective, int constr
     }
     return TO_OK;
 }
+// the reference window of update_trajectory! (to_update_trajectory, to_update_trajectories, to_solve_queue_tables)
+static int reference_window(to_handle* h, int32_t nref, int32_t start) {
+    if (start < 1 || start - 1 + h->P.N > nref) return fail(h, TO_EDIM, "update_trajectory!: the reference is shorter than start + N - 1");
+    return TO_OK;
+}
 // update_trajectory! per instance: Xref [B][nref][n], Uref [B][nref][m], one start for the batch
 int to_update_trajectories(to_handle* h, const double* Xref, const double* Uref, int32_t nref, int32_t start) {
     JOIN(h);
     if (!h || !Xref || !Uref) return TO_EINVAL;
     const int n = h->P.n, m = h->P.m, N = h->P.N;
-    if (start < 1 || start - 1 + N > nref) return fail(h, TO_EDIM, "update_trajectory!: the reference is shorter than start + N - 1");
+    if (reference_window(h, nref, start)) return TO_EDIM;
     if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
     int rc = stage_qr(h); if (rc) return rc;
     for (int b = 0; b < h->P.B; b++)
@@ -1210,40 +1219,49 @@ int to_constraint_data_len(const to_handle* h, int32_t con, int32_t* len) {
     *len = con_data_len(h->h_cons[con], h->P.n + h->P.m);
     return TO_OK;
 }
-// data [B][len] of constraint con (the layout of con_shared_row).  The whole batch is checked before anything changes: a refused call leaves the
-// table (or its absence) as it was.  The first call creates the table with the shared data of every constraint in every row.
-int to_set_constraint_data(to_handle* h, int32_t con, const double* data) {
-    JOIN(h);
-    if (!h || !data) return TO_EINVAL;
+// The checks of `rows` rows data [rows][len] of constraint con, each row one `unit` ("instance", "problem") in the messages, which start with
+// `what`: to_set_constraint_data and to_solve_queue_tables
+static int constraint_data_rows(to_handle* h, int32_t con, const double* data, int rows, const char* what, const char* unit) {
+    const std::string pre = std::string(what) + ": ";
     if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance constraint data is not supported on hybrid problems");
-    if (con < 0 || con >= (int)h->h_cons.size()) return fail(h, TO_EINVAL, "to_set_constraint_data: no constraint " + std::to_string(con));
+    if (con < 0 || con >= (int)h->h_cons.size()) return fail(h, TO_EINVAL, pre + "no constraint " + std::to_string(con));
     const DevCon& c = h->h_cons[con];
-    if (c.kind == CON_GOAL) return fail(h, TO_EINVAL, "to_set_constraint_data: a Goal constraint's values are set with to_set_goal_values");
-    const int nm = h->P.n + h->P.m, len = con_data_len(c, nm), B = h->P.B;
-    if (len == 0) return fail(h, TO_EINVAL, "to_set_constraint_data: the data of QuatVecEq and recorded (expression) constraints stays shared");
-    auto where = [](int b, int j) { return "instance " + std::to_string(b) + ", entry " + std::to_string(j); };
-    for (int b = 0; b < B; b++) {
+    if (c.kind == CON_GOAL) return fail(h, TO_EINVAL, pre + "a Goal constraint's values are set with to_set_goal_values");
+    const int nm = h->P.n + h->P.m, len = con_data_len(c, nm);
+    if (len == 0) return fail(h, TO_EINVAL, pre + "the data of QuatVecEq and recorded (expression) constraints stays shared");
+    auto where = [&](int b, int j) { return pre + unit + " " + std::to_string(b) + ", entry " + std::to_string(j); };
+    for (int b = 0; b < rows; b++) {
         const double* row = data + (size_t)b * len;
         if (c.kind == CON_BOUND) {   // the rows, and so p and the multiplier layout, stay those of the shared bound
             for (int j = 0; j < 2 * nm; j++) {
                 const double v = row[j], s = j < nm ? c.a[j] : c.b[j - nm];
                 if (std::isfinite(s) ? !std::isfinite(v) : !(v == s))
-                    return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, j) + ": BoundConstraint entries must be finite exactly where the shared "
-                                              "bound is, with the same infinities");
+                    return fail(h, TO_EINVAL, where(b, j) + ": BoundConstraint entries must be finite exactly where the shared bound is, with the same infinities");
             }
             for (int j = 0; j < nm; j++)
                 if (!(row[j] >= row[nm + j]))
-                    return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, j) + ": Upper bounds must be greater than or equal to lower bounds");   // src/constraints.jl:712
+                    return fail(h, TO_EINVAL, where(b, j) + ": Upper bounds must be greater than or equal to lower bounds");   // src/constraints.jl:712
         } else {
             for (int j = 0; j < len; j++)
-                if (!std::isfinite(row[j])) return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, j) + " is not finite");
+                if (!std::isfinite(row[j])) return fail(h, TO_EINVAL, where(b, j) + " is not finite");
             if (c.kind == CON_NORM && !(row[0] >= 0))
-                return fail(h, TO_EINVAL, "to_set_constraint_data: " + where(b, 0) + ": NormConstraint value must be non-negative");   // src/constraints.jl:451
+                return fail(h, TO_EINVAL, where(b, 0) + ": NormConstraint value must be non-negative");   // src/constraints.jl:451
         }
     }
+    return TO_OK;
+}
+// data [B][len] of constraint con (the layout of con_shared_row).  The whole batch is checked before anything changes: a refused call leaves the
+// table (or its absence) as it was.  The first call creates the table with the shared data of every constraint in every row.
+int to_set_constraint_data(to_handle* h, int32_t con, const double* data) {
+    JOIN(h);
+    if (!h || !data) return TO_EINVAL;
+    const int B = h->P.B;
+    int rc = constraint_data_rows(h, con, data, B, "to_set_constraint_data", "instance"); if (rc) return rc;
+    const DevCon& c = h->h_cons[con];
+    const int len = con_data_len(c, h->P.n + h->P.m);
     stage_cdata(h);
     for (int b = 0; b < B; b++) std::memcpy(h->stage.data() + cd_off(h, b, c), data + (size_t)b * len, sizeof(double) * len);
-    int rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
+    rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1269,30 +1287,40 @@ int to_cost_weights_len(const to_handle* h, int32_t cost, int32_t* len) {
     *len = cost_weights_len(h->h_costs[cost], h->P.n, h->P.m);
     return TO_OK;
 }
+// The checks of `rows` rows w [rows][len] of cost `cost`, each row one `unit` ("instance", "problem") in the messages, which start with `what`:
+// to_set_cost_weights and to_solve_queue_tables
+static int cost_weight_rows(to_handle* h, int32_t cost, const double* w, int rows, const char* what, const char* unit) {
+    const std::string pre = std::string(what) + ": ";
+    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance cost weights are not supported on hybrid problems");
+    if (cost < 0 || cost >= (int)h->h_costs.size()) return fail(h, TO_EINVAL, pre + "no cost " + std::to_string(cost));
+    const DevCost& c = h->h_costs[cost];
+    if (c.expr) return fail(h, TO_EINVAL, pre + "the constants of a recorded (expression) cost stay shared");
+    const int n = h->P.n, m = h->P.m, len = cost_weights_len(c, n, m);
+    const int h0 = n * n + m * m;   // QUADRATIC: H sits at [h0, h0 + m n)
+    auto where = [&](int b, int j) { return pre + unit + " " + std::to_string(b) + ", entry " + std::to_string(j); };
+    for (int b = 0; b < rows; b++) {
+        const double* row = w + (size_t)b * len;
+        for (int j = 0; j < len; j++) {
+            if (!std::isfinite(row[j])) return fail(h, TO_EINVAL, where(b, j) + " is not finite");
+            if (!c.diag && c.zeroH && j >= h0 && j < h0 + m * n && row[j] != 0.0)
+                return fail(h, TO_EINVAL, where(b, j) + ": H must stay zero where the shared H is zero (it selects kernel code)");
+        }
+    }
+    return TO_OK;
+}
 // w [B][len] of cost `cost` (the layout of cost_shared_row).  The whole batch is checked before anything changes: a refused call leaves the
 // table (or its absence) as it was.  The first call creates the table with the shared weights of every cost in every row.  The linear terms
 // stay as they are (mutating cost.Q leaves cost.q alone); the goal setters derive them from each instance's weights from then on.
 int to_set_cost_weights(to_handle* h, int32_t cost, const double* w) {
     JOIN(h);
     if (!h || !w) return TO_EINVAL;
-    if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance cost weights are not supported on hybrid problems");
-    if (cost < 0 || cost >= (int)h->h_costs.size()) return fail(h, TO_EINVAL, "to_set_cost_weights: no cost " + std::to_string(cost));
+    const int B = h->P.B;
+    int rc = cost_weight_rows(h, cost, w, B, "to_set_cost_weights", "instance"); if (rc) return rc;
     const DevCost& c = h->h_costs[cost];
-    if (c.expr) return fail(h, TO_EINVAL, "to_set_cost_weights: the constants of a recorded (expression) cost stay shared");
-    const int n = h->P.n, m = h->P.m, len = cost_weights_len(c, n, m), B = h->P.B;
-    const int h0 = n * n + m * m;   // QUADRATIC: H sits at [h0, h0 + m n)
-    auto where = [](int b, int j) { return "instance " + std::to_string(b) + ", entry " + std::to_string(j); };
-    for (int b = 0; b < B; b++) {
-        const double* row = w + (size_t)b * len;
-        for (int j = 0; j < len; j++) {
-            if (!std::isfinite(row[j])) return fail(h, TO_EINVAL, "to_set_cost_weights: " + where(b, j) + " is not finite");
-            if (!c.diag && c.zeroH && j >= h0 && j < h0 + m * n && row[j] != 0.0)
-                return fail(h, TO_EINVAL, "to_set_cost_weights: " + where(b, j) + ": H must stay zero where the shared H is zero (it selects kernel code)");
-        }
-    }
+    const int len = cost_weights_len(c, h->P.n, h->P.m);
     stage_cw(h);
     for (int b = 0; b < B; b++) std::memcpy(h->stage.data() + cw_off(h, b, c), w + (size_t)b * len, sizeof(double) * len);
-    int rc = commit_rows(h, h->h_cw, h->P.cw); if (rc) return rc;
+    rc = commit_rows(h, h->h_cw, h->P.cw); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1316,19 +1344,27 @@ int to_get_cost_weights(to_handle* h, int32_t cost, double* w) {
 // Problem(model, obj, x0_b, tf_b; t0 = t0_b, dt = dt_b) holds.  The whole batch is checked before anything changes: a refused call leaves the
 // table (or its absence) and the clocks as they were.  The first call starts every clock at the shared t0 unless t0 is given.  The closed-form
 // Jacobian columns are rewritten from the new steps; X is not rolled out again.
-int to_set_time_steps(to_handle* h, const double* dt, const double* t0) {
-    JOIN(h);
-    if (!h || !dt) return TO_EINVAL;
+// The checks of `rows` rows dt [rows][N-1], each row one `unit` ("instance", "problem") in the messages, which start with `what`:
+// to_set_time_steps and to_solve_queue_tables
+static int time_step_rows(to_handle* h, const double* dt, int rows, const char* what, const char* unit) {
     if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance time steps are not supported on hybrid problems");
-    const int B = h->P.B, K = h->P.N - 1;
-    for (int b = 0; b < B; b++) {
+    const int K = h->P.N - 1;
+    for (int b = 0; b < rows; b++)
         for (int k = 0; k < K; k++) {
             const double v = dt[(size_t)b * K + k];
             if (!(std::isfinite(v) && v > 0))
-                return fail(h, TO_EINVAL, "to_set_time_steps: instance " + std::to_string(b) + ", knot " + std::to_string(k) + ": a time step must be finite and positive");
+                return fail(h, TO_EINVAL, std::string(what) + ": " + unit + " " + std::to_string(b) + ", knot " + std::to_string(k) +
+                                              ": a time step must be finite and positive");
         }
+    return TO_OK;
+}
+int to_set_time_steps(to_handle* h, const double* dt, const double* t0) {
+    JOIN(h);
+    if (!h || !dt) return TO_EINVAL;
+    const int B = h->P.B, K = h->P.N - 1;
+    int rc0 = time_step_rows(h, dt, B, "to_set_time_steps", "instance"); if (rc0) return rc0;
+    for (int b = 0; b < B; b++)
         if (t0 && !std::isfinite(t0[b])) return fail(h, TO_EINVAL, "to_set_time_steps: instance " + std::to_string(b) + ": the initial time must be finite");
-    }
     h->stage.assign(dt, dt + (size_t)B * K);
     int rc = commit_rows(h, h->h_dtb, h->P.dtb); if (rc) return rc;
     if (t0) h->t0b.assign(t0, t0 + B);
@@ -1371,7 +1407,7 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
     JOIN(h);
     if (!h || !Xref || !Uref) return TO_EINVAL;
     const int n = h->P.n, m = h->P.m, N = h->P.N;
-    if (start < 1 || start - 1 + N > nref) return fail(h, TO_EDIM, "update_trajectory!: the reference is shorter than start + N - 1");
+    if (reference_window(h, nref, start)) return TO_EDIM;
     for (int i = 0; i < N; i++) {                       // set_LQR_goal!(obj[i], state(Z[k]), control(Z[k]))
         DevCost& c = h->h_costs[h->h_cost_index[i]];
         lqr_linear_term(c.Q, n, Xref + (size_t)(start - 1 + i) * n, c.q);
@@ -1886,6 +1922,12 @@ static int queue_refill(to_handle* h, const QueueDev& q, int half, int mode, cud
     CU(h, launch_queue_harvest(h->P, h->solve, q, half, mode, st));
     CU(h, launch_cost(M, q.cost_slot, nullptr, st));
     CU(h, launch_queue_refill(h->P, h->solve, q, half, mode, st));
+    if (q.dtb && h->P.model == MODEL_QUADROTOR && !(h->P.lie && h->P.frag)) {
+        // the closed-form Jacobian columns of the refilled slots, from their problems' time steps: no expansion kernel writes them, so a slot
+        // would keep its previous problem's (write_closed_form_columns; the record path writes them into every block itself)
+        CU(h, h->P.lie ? launch_trivial_columns(M, st, true) : launch_trivial_columns_full(M, st, true));
+        h->launches++;
+    }
     CU(h, launch_rollout(M, st, true));
     CU(h, launch_merit(M, M.J, h->d_viol, st));
     CU(h, launch_queue_begin(h->P, h->solve, q, half, st));
@@ -1921,11 +1963,25 @@ static int uniform_rows(to_handle* h, const std::vector<double>& rows, size_t w,
                                               "), so a problem's result would depend on its slot; the queue needs them equal in every row");
     return TO_OK;
 }
+// The checks of `rows` penalties mu [rows] of one constraint, each one `unit` ("instance", "problem") in the messages, which start with `what`:
+// to_set_penalties and to_solve_queue_tables
+static int penalty_rows(to_handle* h, const double* mu, int rows, const std::string& what, const char* unit) {
+    for (int b = 0; b < rows; b++)
+        if (!(std::isfinite(mu[b]) && mu[b] > 0))
+            return fail(h, TO_EINVAL, what + ": " + unit + " " + std::to_string(b) + ": a penalty must be finite and positive");
+    return TO_OK;
+}
 int to_solve_queue(to_handle* h, const to_queue_spec* qs, const to_solve_options* o, int32_t* status, int32_t* iterations, int32_t* iterations_outer,
                    double* cost, double* dJ, double* gradient, double* c_max, double* X, double* U) {
+    return to_solve_queue_tables(h, qs, nullptr, 0, o, status, iterations, iterations_outer, cost, dJ, gradient, c_max, X, U);
+}
+int to_solve_queue_tables(to_handle* h, const to_queue_spec* qs, const to_queue_table* tables, int32_t ntables, const to_solve_options* o,
+                          int32_t* status, int32_t* iterations, int32_t* iterations_outer, double* cost, double* dJ, double* gradient, double* c_max,
+                          double* X, double* U) {
     JOIN(h);
-    if (!h || !qs || !o) return TO_EINVAL;
-    const int B = h->P.B, n = h->P.n, m = h->P.m, N = h->P.N, M = qs->M, ncost = h->P.ncost, ncd = h->P.ncdata, nc = h->P.ncon;
+    if (!h || !qs || !o || ntables < 0 || (ntables > 0 && !tables)) return TO_EINVAL;
+    const int B = h->P.B, n = h->P.n, m = h->P.m, N = h->P.N, K = N - 1, M = qs->M, ncost = h->P.ncost, ncd = h->P.ncdata, nc = h->P.ncon;
+    const int ncw = h->P.ncw;
     // ---- every check before any device work
     if (M < 1) return fail(h, TO_EINVAL, "to_solve_queue: M must be >= 1");
     if (!qs->x0 || !qs->U0) return fail(h, TO_EINVAL, "to_solve_queue: x0 and U0 are required");
@@ -1952,48 +2008,151 @@ int to_solve_queue(to_handle* h, const to_queue_spec* qs, const to_solve_options
     std::vector<double> mp_rows;
     if (qs->params) { rc = model_param_rows(h, qs->params, qs->nparams, "to_solve_queue", mp_rows, M); if (rc) return rc; }
     const bool objective = qs->xf && qs->goal_objective, goal_con = qs->xf && qs->goal_constraint && ncd > 0;
-    // the tables the queue keeps must not depend on the slot
-    if (h->P.cw) { rc = uniform_rows(h, h->h_cw, h->P.ncw, {}, "cost weights"); if (rc) return rc; }
-    if (h->P.dtb) { rc = uniform_rows(h, h->h_dtb, N - 1, {}, "time steps"); if (rc) return rc; }
+    // each table, with its setter's checks; at most one of each kind (and of each cost, each constraint)
+    const char* qt = "to_solve_queue_tables";
+    const to_queue_table *t_dt = nullptr, *t_ref = nullptr;
+    std::vector<const to_queue_table*> t_cw(ncost, nullptr), t_cd(nc, nullptr), t_mu(nc, nullptr);
+    bool any_cw = false, any_cd = false, any_mu = false;
+    for (int t = 0; t < ntables; t++) {
+        const to_queue_table& T = tables[t];
+        const std::string pre = std::string(qt) + ": table " + std::to_string(t) + ": ";
+        auto len_is = [&](int want) {
+            return T.len == want ? TO_OK : fail(h, TO_EDIM, pre + "len is " + std::to_string(T.len) + ", the table takes " + std::to_string(want) + " doubles per problem");
+        };
+        auto index_zero = [&]() { return T.index == 0 ? TO_OK : fail(h, TO_EINVAL, pre + "index must be 0 for this kind"); };
+        auto twice = [&]() { return fail(h, TO_EINVAL, pre + "the same table is given twice"); };
+        if (!T.rows || (T.kind == TO_QT_REFERENCE) != (T.rows2 != nullptr))
+            return fail(h, TO_EINVAL, pre + "rows are required, and rows2 (Uref) with a reference alone");
+        switch (T.kind) {
+        case TO_QT_TIME_STEPS:
+            if (t_dt) return twice();
+            if ((rc = index_zero()) || (rc = len_is(K)) || (rc = time_step_rows(h, T.rows, M, qt, "problem"))) return rc;
+            t_dt = &T;
+            break;
+        case TO_QT_COST_WEIGHTS:
+            if ((rc = cost_weight_rows(h, T.index, T.rows, 0, qt, "problem"))) return rc;   // the cost alone: the rows are read once len is known
+            if (t_cw[T.index]) return twice();
+            if ((rc = len_is(cost_weights_len(h->h_costs[T.index], n, m))) || (rc = cost_weight_rows(h, T.index, T.rows, M, qt, "problem"))) return rc;
+            t_cw[T.index] = &T; any_cw = true;
+            break;
+        case TO_QT_CONSTRAINT_DATA:
+            if ((rc = constraint_data_rows(h, T.index, T.rows, 0, qt, "problem"))) return rc;
+            if (t_cd[T.index]) return twice();
+            if ((rc = len_is(con_data_len(h->h_cons[T.index], n + m))) || (rc = constraint_data_rows(h, T.index, T.rows, M, qt, "problem"))) return rc;
+            t_cd[T.index] = &T; any_cd = true;
+            break;
+        case TO_QT_PENALTIES:
+            if (T.index < 0 || T.index >= nc) return fail(h, TO_EINVAL, pre + "no constraint " + std::to_string(T.index));
+            if (t_mu[T.index]) return twice();
+            if ((rc = len_is(1)) || (rc = penalty_rows(h, T.rows, M, std::string(qt) + ": constraint " + std::to_string(T.index), "problem"))) return rc;
+            t_mu[T.index] = &T; any_mu = true;
+            break;
+        case TO_QT_REFERENCE:
+            if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
+            if (t_ref) return twice();
+            if ((rc = reference_window(h, T.len, T.index))) return rc;
+            {
+                auto finite_ref = [&](const double* a, int w, const char* what) {   // a [M][nref][w]
+                    for (size_t i = 0; i < (size_t)M * T.len * w; i++)
+                        if (!std::isfinite(a[i]))
+                            return fail(h, TO_EINVAL, std::string(qt) + ": problem " + std::to_string(i / ((size_t)T.len * w)) + ", row " +
+                                                          std::to_string(i / w % T.len) + ", entry " + std::to_string(i % w) + ": " + what + " is not finite");
+                    return TO_OK;
+                };
+                if ((rc = finite_ref(T.rows, n, "Xref")) || (rc = finite_ref(T.rows2, m, "Uref"))) return rc;
+            }
+            t_ref = &T;
+            break;
+        default:
+            return fail(h, TO_EINVAL, pre + "unknown kind " + std::to_string(T.kind));
+        }
+    }
+    if (t_ref && objective)
+        return fail(h, TO_EINVAL, std::string(qt) + ": a reference and xf with goal_objective = 1 would both set the linear cost terms");
+    // the tables the queue keeps must not depend on the slot; the entries it replaces need not agree
+    if (h->P.cw) {
+        std::vector<char> keep(ncw, 1);
+        for (int ci = 0; ci < ncost; ci++)
+            if (t_cw[ci]) std::fill(keep.begin() + h->h_costs[ci].cwoff, keep.begin() + h->h_costs[ci].cwoff + t_cw[ci]->len, 0);
+        rc = uniform_rows(h, h->h_cw, ncw, keep, "cost weights"); if (rc) return rc;
+    }
+    if (h->P.dtb && !t_dt) { rc = uniform_rows(h, h->h_dtb, K, {}, "time steps"); if (rc) return rc; }
     if (h->P.mparams && !qs->params) { rc = uniform_rows(h, h->h_mparams, TO_NPARAM, {}, "model parameters"); if (rc) return rc; }
     if (h->P.cdata) {
-        std::vector<char> keep(ncd, 1);     // the Goal values xf replaces need not agree
-        if (goal_con) for (const auto& c : h->h_cons) if (c.kind == CON_GOAL) std::fill(keep.begin() + c.cdoff, keep.begin() + c.cdoff + c.p, 0);
+        std::vector<char> keep(ncd, 1);     // the Goal values xf replaces, the data of the constraints given
+        for (size_t ci = 0; ci < h->h_cons.size(); ci++) {
+            const DevCon& c = h->h_cons[ci];
+            if (goal_con && c.kind == CON_GOAL) std::fill(keep.begin() + c.cdoff, keep.begin() + c.cdoff + c.p, 0);
+            if (t_cd[ci]) std::fill(keep.begin() + c.cdoff, keep.begin() + c.cdoff + t_cd[ci]->len, 0);
+        }
         rc = uniform_rows(h, h->h_cdata, ncd, keep, "constraint data"); if (rc) return rc;
     }
     const size_t wq = (size_t)ncost * (n + m);
     if (h->P.qr) {
         rc = refresh_qr(h); if (rc) return rc;
-        std::vector<char> keep(wq, 1);      // the q that xf replaces need not agree
+        std::vector<char> keep(wq, 1);      // the q that xf replaces, the q | r of every knot's cost a reference replaces
         if (objective) for (int ci = 0; ci < ncost; ci++) std::fill(keep.begin() + ci * (n + m), keep.begin() + ci * (n + m) + n, 0);
+        if (t_ref) for (int i = 0; i < N; i++) { const int ci = h->h_cost_index[i]; std::fill(keep.begin() + ci * (n + m), keep.begin() + (ci + 1) * (n + m), 0); }
         rc = uniform_rows(h, h->h_qr, wq, keep, "linear cost terms"); if (rc) return rc;
     }
-    // ---- each problem's rows, built as the setters build them (to_set_goal_states, to_set_model_params)
-    std::vector<double> qr_rows, cd_rows;
-    if (objective) {
+    // ---- each problem's rows, built as the setters build them, in their order: to_set_cost_weights, to_set_constraint_data,
+    // to_update_trajectories, to_set_goal_states, to_set_model_params (the time steps and penalties are the tables' rows as given)
+    std::vector<double> cw_rows, qr_rows, cd_rows;
+    if (any_cw) {
+        stage_cw(h);
+        cw_rows.resize((size_t)M * ncw);
+        for (int p = 0; p < M; p++) {
+            double* row = cw_rows.data() + (size_t)p * ncw;
+            std::memcpy(row, h->stage.data(), sizeof(double) * ncw);
+            for (int ci = 0; ci < ncost; ci++)
+                if (t_cw[ci]) std::memcpy(row + h->h_costs[ci].cwoff, t_cw[ci]->rows + (size_t)p * t_cw[ci]->len, sizeof(double) * t_cw[ci]->len);
+        }
+    }
+    if (objective || t_ref) {
         rc = stage_qr(h); if (rc) return rc;
         qr_rows.resize((size_t)M * wq);
         for (int p = 0; p < M; p++) {
             double* row = qr_rows.data() + (size_t)p * wq;
             std::memcpy(row, h->stage.data(), sizeof(double) * wq);
-            for (int ci = 0; ci < ncost; ci++) instance_linear_term(h, 0, ci, qs->xf + (size_t)p * n, nullptr, row + (size_t)ci * (n + m));
+            // the problem's own weights: its row once given, else the handle's (the same in every instance), else the shared ones
+            const double* w = any_cw ? cw_rows.data() + (size_t)p * ncw : h->P.cw ? h->h_cw.data() : nullptr;
+            if (t_ref) {
+                const size_t nref = t_ref->len, k0 = (size_t)p * nref + t_ref->index - 1;
+                for (int i = 0; i < N; i++) {
+                    const int ci = h->h_cost_index[i];
+                    weights_linear_term(h, w, ci, t_ref->rows + (k0 + i) * n, t_ref->rows2 + (k0 + i) * m, row + (size_t)ci * (n + m));
+                }
+            } else {
+                for (int ci = 0; ci < ncost; ci++) weights_linear_term(h, w, ci, qs->xf + (size_t)p * n, nullptr, row + (size_t)ci * (n + m));
+            }
         }
     }
-    if (goal_con) {
+    if (any_cd || goal_con) {
         stage_cdata(h);
         cd_rows.resize((size_t)M * ncd);
         for (int p = 0; p < M; p++) {
             double* row = cd_rows.data() + (size_t)p * ncd;
             std::memcpy(row, h->stage.data(), sizeof(double) * ncd);
-            for (const auto& c : h->h_cons)
-                if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) row[c.cdoff + i] = qs->xf[(size_t)p * n + c.inds[i]];
+            for (size_t ci = 0; ci < h->h_cons.size(); ci++) {
+                const DevCon& c = h->h_cons[ci];
+                if (t_cd[ci]) std::memcpy(row + c.cdoff, t_cd[ci]->rows + (size_t)p * t_cd[ci]->len, sizeof(double) * t_cd[ci]->len);
+                if (goal_con && c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) row[c.cdoff + i] = qs->xf[(size_t)p * n + c.inds[i]];
+            }
         }
     }
+    std::vector<double> mu_rows;            // the shared penalties, the given constraints' replaced (to_set_penalties after the refill's)
+    if (any_mu) {
+        mu_rows.resize((size_t)M * nc);
+        for (int p = 0; p < M; p++)
+            for (int i = 0; i < nc; i++) mu_rows[(size_t)p * nc + i] = t_mu[i] ? t_mu[i]->rows[p] : h->h_mu[i];
+    }
+    const size_t ndt = t_dt ? (size_t)M * K : 0, nmu = mu_rows.size();
     // ---- one allocation: the staged problems, the slot tables, the outputs and the handle's state the refills overwrite
     const bool traj = X || U;
     const size_t nX = (size_t)N * n, ll = (size_t)h->P.lambda_len;
-    const size_t d_in = (size_t)M * n + mu0 * wu + qr_rows.size() + cd_rows.size() + mp_rows.size();
-    const size_t d_slot = (objective ? B * wq : 0) + (goal_con ? (size_t)B * ncd : 0) + (qs->params ? (size_t)B * TO_NPARAM : 0) + (size_t)B * nc + B;
+    const size_t d_in = (size_t)M * n + mu0 * wu + qr_rows.size() + cd_rows.size() + mp_rows.size() + cw_rows.size() + ndt + nmu;
+    const size_t d_slot = (qr_rows.empty() ? 0 : B * wq) + (cd_rows.empty() ? 0 : (size_t)B * ncd) + (qs->params ? (size_t)B * TO_NPARAM : 0) +
+                          (cw_rows.empty() ? 0 : (size_t)B * ncw) + (t_dt ? (size_t)B * K : 0) + (size_t)B * nc + B;
     const size_t d_out = 4 * (size_t)M + (traj ? (size_t)M * (nX + wu) : 0);
     const size_t d_save = (size_t)B * n + (size_t)B * ll;
     const size_t n_int = 3 * (size_t)M + 1 + 3 * (size_t)B + 2 * (size_t)B;
@@ -2013,8 +2172,10 @@ int to_solve_queue(to_handle* h, const to_queue_spec* qs, const to_solve_options
     q.M = M; q.U0_shared = qs->U0_shared ? 1 : 0;
     double* x0_in = take((size_t)M * n); double* U0_in = take(mu0 * wu);
     double* qr_in = take(qr_rows.size()); double* cd_in = take(cd_rows.size()); double* mp_in = take(mp_rows.size());
-    q.x0 = x0_in; q.U0 = U0_in; q.qr_src = qr_in; q.cd_src = cd_in; q.mp_src = mp_in;
-    q.qr = take(objective ? B * wq : 0); q.cd = take(goal_con ? (size_t)B * ncd : 0); q.mp = take(qs->params ? (size_t)B * TO_NPARAM : 0);
+    double* cw_in = take(cw_rows.size()); double* dt_in = take(ndt); double* mu_in = take(nmu);
+    q.x0 = x0_in; q.U0 = U0_in; q.qr_src = qr_in; q.cd_src = cd_in; q.mp_src = mp_in; q.cw_src = cw_in; q.dt_src = dt_in; q.mu_src = mu_in;
+    q.qr = take(qr_rows.empty() ? 0 : B * wq); q.cd = take(cd_rows.empty() ? 0 : (size_t)B * ncd); q.mp = take(qs->params ? (size_t)B * TO_NPARAM : 0);
+    q.cw = take(cw_rows.empty() ? 0 : (size_t)B * ncw); q.dtb = take(t_dt ? (size_t)B * K : 0);
     q.mub = take((size_t)B * nc); q.cost_slot = take(B);
     q.cost = take(M); q.dJ = take(M); q.grad = take(M); q.cmax = take(M);
     q.X = traj ? take((size_t)M * nX) : nullptr; q.U = traj ? take((size_t)M * wu) : nullptr;
@@ -2031,6 +2192,9 @@ int to_solve_queue(to_handle* h, const to_queue_spec* qs, const to_solve_options
     if (e == cudaSuccess) e = up(qr_in, qr_rows.data(), qr_rows.size());
     if (e == cudaSuccess) e = up(cd_in, cd_rows.data(), cd_rows.size());
     if (e == cudaSuccess) e = up(mp_in, mp_rows.data(), mp_rows.size());
+    if (e == cudaSuccess) e = up(cw_in, cw_rows.data(), cw_rows.size());
+    if (e == cudaSuccess && t_dt) e = up(dt_in, t_dt->rows, ndt);
+    if (e == cudaSuccess) e = up(mu_in, mu_rows.data(), nmu);
     // the handle's state the refills overwrite: x0, the live trajectories (in the get / set staging buffers), the multipliers
     if (e == cudaSuccess) e = cudaMemcpyAsync(save_x0, h->P.x0, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, h->stream);
     if (e == cudaSuccess && ll) e = cudaMemcpyAsync(save_lam, h->P.lambda, (size_t)B * ll * sizeof(double), cudaMemcpyDeviceToDevice, h->stream);
@@ -2043,6 +2207,8 @@ int to_solve_queue(to_handle* h, const to_queue_spec* qs, const to_solve_options
     if (q.qr) h->P.qr = q.qr;
     if (q.cd) h->P.cdata = q.cd;
     if (q.mp) h->P.mparams = q.mp;
+    if (q.cw) h->P.cw = q.cw;
+    if (q.dtb) h->P.dtb = q.dtb;
     h->P.mub = q.mub;                          // (nullptr without constraints)
     prepare_solve(h, o);
     S.go = nc > 0 ? go : nullptr;              // a constrained problem takes every outer step on the device
@@ -2050,7 +2216,7 @@ int to_solve_queue(to_handle* h, const to_queue_spec* qs, const to_solve_options
     rc = queue_run(h, q);
     const int jrc = join_side(h);
     h->P.active = nullptr;
-    h->P.qr = saved.qr; h->P.cdata = saved.cdata; h->P.mparams = saved.mparams; h->P.mub = saved.mub;
+    h->P.qr = saved.qr; h->P.cdata = saved.cdata; h->P.mparams = saved.mparams; h->P.mub = saved.mub; h->P.cw = saved.cw; h->P.dtb = saved.dtb;
     S.go = h->P.mub ? h->d_go : nullptr;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     if (!rc) rc = jrc;
@@ -2075,6 +2241,12 @@ int to_solve_queue(to_handle* h, const to_queue_spec* qs, const to_solve_options
     if (e == cudaSuccess) { e = launch_scatter_traj(h->P, h->d_stageX, h->d_stageU, h->stream); h->launches++; }
     const cudaError_t se = cudaStreamSynchronize(h->stream);
     cudaFree(buf);
+    if (t_dt) {    // the handle's own closed-form columns, which the refills overwrote, on every way out (a failure keeps the first message)
+        const std::string err = h->err;
+        const int crc = write_closed_form_columns(h);
+        if (rc || e != cudaSuccess || se != cudaSuccess) h->err = err;
+        else if (crc) return crc;
+    }
     if (rc) return rc;
     if (e != cudaSuccess) return cuda_fail(h, e, "to_solve_queue: results");
     if (se != cudaSuccess) return cuda_fail(h, se, "to_solve_queue");
@@ -2401,11 +2573,8 @@ int to_set_penalties(to_handle* h, int32_t con, const double* mu) {
     if (!h || !mu) return TO_EINVAL;
     if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance penalties are not supported on hybrid problems");
     if (con < 0 || con >= (int)h->h_cons.size()) return fail(h, TO_EINVAL, "to_set_penalties: no constraint " + std::to_string(con));
-    const int B = h->P.B;
-    for (int b = 0; b < B; b++)
-        if (!(std::isfinite(mu[b]) && mu[b] > 0))
-            return fail(h, TO_EINVAL, "to_set_penalties: instance " + std::to_string(b) + ": a penalty must be finite and positive");
-    int rc = ensure_penalty_table(h); if (rc) return rc;
+    int rc = penalty_rows(h, mu, h->P.B, "to_set_penalties", "instance"); if (rc) return rc;
+    rc = ensure_penalty_table(h); if (rc) return rc;
     rc = penalty_column(h, con, const_cast<double*>(mu), false); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;

@@ -95,8 +95,9 @@ cudaError_t launch_expand_lie(const DevProblem& P, cudaStream_t s, int mode = 0)
 // register-resident Riccati pass of the error-state Quadrotor + its record producers   (riccati_frag.cu)
 cudaError_t launch_expansion_rec(const DevProblem& P, cudaStream_t s);                 // compact expansion -> REC[192..240) of every knot
 cudaError_t launch_expansion_rec16(const DevProblem& P, cudaStream_t s, int mode);               // ... 16-knot blocks per 16-lane group, from the host-built term table (rollout.cu)
-cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s);          // ... of the full-state [A B]
-cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s);               // closed-form position / velocity columns of [A_e B_e], once per problem
+// masked (to_solve_queue_tables' refill, with per-slot time steps): only the instances P.active marks ACTIVE
+cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s, bool masked = false);   // ... of the full-state [A B]
+cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s, bool masked = false);        // closed-form position / velocity columns of [A_e B_e], once per problem
 cudaError_t launch_export_abe(const DevProblem& P, cudaStream_t s);                    // REC fragments -> ABe (col-major 12 x 16)
 size_t frag_queue_ints(int B);
 size_t frag_pool_doubles(int B, int N);                                                 // doubles of the speculative candidates' gain pool                                                         // ints of the kernel's work queue (allocated by the handle)
@@ -151,7 +152,12 @@ struct QueueDev {
     double* cd;
     const double* mp_src;    // w = TO_NPARAM: DevProblem::mparams
     double* mp;
-    double* mub;             // [B][ncon] or nullptr: DevProblem::mub, refilled with the shared penalties
+    const double* cw_src;    // w = ncw: DevProblem::cw
+    double* cw;
+    const double* dt_src;    // w = N-1: DevProblem::dtb
+    double* dtb;
+    double* mub;             // [B][ncon] or nullptr: DevProblem::mub, refilled with the shared penalties, or with the problem's row of mu_src
+    const double* mu_src;    // [M][ncon] or nullptr
     // outputs [M]: to_solve's statistics, and X [M][N][n], U [M][N-1][m] or nullptr
     int *status, *iter, *outer;
     double *cost, *dJ, *grad, *cmax, *X, *U;

@@ -197,8 +197,9 @@ __global__ void __launch_bounds__(128) k_expand(const DevProblem P, int mode) {
 
 #if TO_RULE == 4
 // the closed-form columns of [A B] (SeedList<MODEL>::trivial): thread = (instance, knot, one of them); run when the problem is created and
-// whenever its time steps change (INST: each instance's own, DevProblem::dtb)
-template <int MODEL, bool INST>
+// whenever its time steps change (INST: each instance's own, DevProblem::dtb).  MASK (to_solve_queue_tables' refill): only the instances
+// P.active marks ACTIVE
+template <int MODEL, bool INST, bool MASK = false>
 __global__ void __launch_bounds__(128) k_trivial_columns_full(const DevProblem P) {
     constexpr int n = ModelDims<MODEL>::n, NT = SeedList<MODEL>::ntrivial();
     if constexpr (NT > 0) {
@@ -207,16 +208,19 @@ __global__ void __launch_bounds__(128) k_trivial_columns_full(const DevProblem P
         const int jt = SeedList<MODEL>::trivial((int)(t % NT));
         const long long bk = t / NT;
         const int k = (int)(bk % (P.N - 1));
+        if constexpr (MASK) { if (retired(P, (int)(bk / (P.N - 1)))) return; }
         double* AB = P.AB + (size_t)bk * n * P.ldab;
         const double h = time_step<INST>(P, (int)(bk / (P.N - 1)), k);
         // x = [r(0..2); q(3..6); v(7..9); omega(10..12)]: d r+/d r = I, d r+/d v = h I, d v+/d v = I
         for (int i = 0; i < n; i++) AB[i * P.ldab + jt] = (i == jt) ? 1.0 : ((jt >= 7 && i == jt - 7) ? h : 0.0);
     }
 }
-cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s) {
+// (a masked launch comes with per-slot time steps, so it has INST instantiations only)
+cudaError_t launch_trivial_columns_full(const DevProblem& P, cudaStream_t s, bool masked) {
     if (P.model == MODEL_QUADROTOR) {
         const long long total = (long long)P.B * (P.N - 1) * SeedList<MODEL_QUADROTOR>::ntrivial();
-        if (inst_dynamics(P)) k_trivial_columns_full<MODEL_QUADROTOR, true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+        if (masked) k_trivial_columns_full<MODEL_QUADROTOR, true, true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+        else if (inst_dynamics(P)) k_trivial_columns_full<MODEL_QUADROTOR, true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
         else k_trivial_columns_full<MODEL_QUADROTOR, false><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
     }
     return cudaGetLastError();
@@ -430,8 +434,9 @@ __global__ void __launch_bounds__(EXPB_T, TO_EXPAND_LIE_MINB * 128 / EXPB_T) k_e
 }
 
 #if TO_RULE == 4
-// the closed-form columns of [A_e B_e] (positions, velocities): thread = (instance, knot, one of the six); INST: each instance's time steps
-template <bool INST>
+// the closed-form columns of [A_e B_e] (positions, velocities): thread = (instance, knot, one of the six); INST: each instance's time steps;
+// MASK as k_trivial_columns_full
+template <bool INST, bool MASK = false>
 __global__ void __launch_bounds__(128) k_trivial_columns(const DevProblem P) {
     constexpr int ne = 12, nme = 16;
     const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -439,14 +444,16 @@ __global__ void __launch_bounds__(128) k_trivial_columns(const DevProblem P) {
     const int sd = (int)(t % 6);
     const long long bk = t / 6;
     const int k = (int)(bk % (P.N - 1));
+    if constexpr (MASK) { if (retired(P, (int)(bk / (P.N - 1)))) return; }
     const int jt = lie_trivial(sd);
     const double h = time_step<INST>(P, (int)(bk / (P.N - 1)), k);
     for (int e = 0; e < ne; e++) P.ABe[((size_t)bk * nme + jt) * ne + e] = (e == jt) ? 1.0 : ((jt >= 6 && e == jt - 6) ? h : 0.0);
 }
-cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s) {
+cudaError_t launch_trivial_columns(const DevProblem& P, cudaStream_t s, bool masked) {
     const long long total = (long long)P.B * (P.N - 1) * 6;
     if (P.frag) return cudaSuccess;       // k_expand_lie_rec writes the whole block, closed-form columns included, every time
-    if (inst_dynamics(P)) k_trivial_columns<true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+    if (masked) k_trivial_columns<true, true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
+    else if (inst_dynamics(P)) k_trivial_columns<true><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
     else k_trivial_columns<false><<<(unsigned)((total + 127) / 128), 128, 0, s>>>(P);
     return cudaGetLastError();
 }

@@ -149,8 +149,8 @@ __global__ void k_queue_harvest(const DevProblem P, SolveDev S, QueueDev Q, int 
 
 // The harvested slots hand their statistics, objective and trajectory to their problem's row of the outputs; then every DONE slot of the half
 // claims the next problem.  A claimed problem starts as to_solve starts an instance that holds it: x0, U0 in the live buffer, lambda = 0, the
-// shared penalties, its rows of the slot tables, k_solve_init's state.  The mask then marks the refilled slots, for their rollout, merit and
-// k_queue_begin.
+// shared penalties or its own, its rows of the slot tables, k_solve_init's state.  The mask then marks the refilled slots, for their closed-form
+// Jacobian columns (with time-step rows), rollout, merit and k_queue_begin.
 __global__ void k_queue_refill(const DevProblem P, SolveDev S, QueueDev Q, int half, int mode) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= P.B || !in_half(P, b, mode)) return;
@@ -174,13 +174,15 @@ __global__ void k_queue_refill(const DevProblem P, SolveDev S, QueueDev Q, int h
     double* U = traj_Uw(P, P.cur[b], b);
     for (int i = 0; i < (N - 1) * m; i++) U[i] = U0[i];
     for (int i = 0; i < P.lambda_len; i++) P.lambda[(size_t)b * P.lambda_len + i] = 0.0;
-    if (Q.mub) for (int i = 0; i < P.ncon; i++) Q.mub[(size_t)b * P.ncon + i] = P.mu[i];
+    if (Q.mub) for (int i = 0; i < P.ncon; i++) Q.mub[(size_t)b * P.ncon + i] = Q.mu_src ? Q.mu_src[(size_t)p * P.ncon + i] : P.mu[i];
     auto rows = [&](const double* src, double* dst, int w) {
         if (dst) for (int i = 0; i < w; i++) dst[(size_t)b * w + i] = src[(size_t)p * w + i];
     };
     rows(Q.qr_src, Q.qr, P.ncost * (n + m));
     rows(Q.cd_src, Q.cd, P.ncdata);
     rows(Q.mp_src, Q.mp, TO_NPARAM);
+    rows(Q.cw_src, Q.cw, P.ncw);
+    rows(Q.dt_src, Q.dtb, N - 1);
     solve_init_instance(P, S, b);
     *mask = SOLVE_ACTIVE;
     __threadfence();

@@ -483,7 +483,16 @@ struct ToQueueSpec
     params::Ptr{Float64}
     nparams::Int32; pad::Int32
 end
-function solve_queue!(p::BatchedProblem, x0s, U0s; xf = nothing, params = nothing, objective::Bool = true, constraint::Bool = true, kw...)
+# Per-problem tables (to_solve_queue_tables, DESIGN.md 5p), each as its setter takes it with M columns: dt (N-1, M); cost_weights and
+# constraint_data Dicts of the (1-based) distinct cost / constraint => (len, M); penalties a Dict of the (1-based) constraint => mu (M),
+# the others keeping the shared penalty; Xref (n, nref, M) with Uref (m, nref, M) and start.  Problem p's rows are those the setters write in the order of the C header.
+struct ToQueueTable
+    kind::Int32; index::Int32; len::Int32; pad::Int32
+    rows::Ptr{Float64}; rows2::Ptr{Float64}
+end
+function solve_queue!(p::BatchedProblem, x0s, U0s; xf = nothing, params = nothing, objective::Bool = true, constraint::Bool = true,
+                      dt = nothing, cost_weights = Dict(), constraint_data = Dict(), penalties = Dict(), Xref = nothing, Uref = nothing,
+                      start::Integer = 1, kw...)
     X0 = Matrix{Float64}(x0s); M = size(X0, 2)
     U0 = Array{Float64}(U0s); shared = ndims(U0) == 2
     (shared || size(U0, 3) == M) || throw(DimensionMismatch("U0s must be (m, N-1, M) or (m, N-1)"))
@@ -491,18 +500,49 @@ function solve_queue!(p::BatchedProblem, x0s, U0s; xf = nothing, params = nothin
     XF === nothing || size(XF, 2) == M || throw(DimensionMismatch("xf must be (n, M)"))
     P = params === nothing ? nothing : Matrix{Float64}(params)
     P === nothing || size(P, 2) == M || throw(DimensionMismatch("params must be (nparams, M)"))
+    (Xref === nothing) == (Uref === nothing) || throw(ArgumentError("Xref and Uref come together"))
     o = solve_options(kw)
     n, N = size(X0, 1), size(U0, 2) + 1; m = size(U0, 1)
+    keep = Any[]      # the arrays the tables point into
+    tables = ToQueueTable[]
+    if dt !== nothing
+        D = Matrix{Float64}(dt); size(D) == (N - 1, M) || throw(DimensionMismatch("dt must be (N-1, M)"))
+        push!(keep, D); push!(tables, ToQueueTable(0, 0, N - 1, 0, pointer(D), C_NULL))
+    end
+    for (c, W) in cost_weights
+        A = Matrix{Float64}(W); size(A, 2) == M || throw(DimensionMismatch("cost weights must be (len, M)"))
+        push!(keep, A); push!(tables, ToQueueTable(1, c - 1, size(A, 1), 0, pointer(A), C_NULL))
+    end
+    for (c, W) in constraint_data
+        A = Matrix{Float64}(W); size(A, 2) == M || throw(DimensionMismatch("constraint data must be (len, M)"))
+        push!(keep, A); push!(tables, ToQueueTable(2, c - 1, size(A, 1), 0, pointer(A), C_NULL))
+    end
+    for (c, mu) in penalties
+        A = Vector{Float64}(mu); length(A) == M || throw(DimensionMismatch("penalties must have length M"))
+        push!(keep, A); push!(tables, ToQueueTable(3, c - 1, 1, 0, pointer(A), C_NULL))
+    end
+    if Xref !== nothing
+        XR, UR = Array{Float64,3}(Xref), Array{Float64,3}(Uref)
+        (size(XR, 3) == M && size(UR, 3) == M && size(XR, 2) == size(UR, 2)) || throw(DimensionMismatch("Xref must be (n, nref, M) and Uref (m, nref, M)"))
+        push!(keep, XR, UR); push!(tables, ToQueueTable(4, start, size(XR, 2), 0, pointer(XR), pointer(UR)))
+    end
     status, iters, outer = Vector{Int32}(undef, M), Vector{Int32}(undef, M), Vector{Int32}(undef, M)
     cost, dJ, grad, cmax = (Vector{Float64}(undef, M) for _ in 1:4)
     X, U = Array{Float64,3}(undef, n, N, M), Array{Float64,3}(undef, m, N - 1, M)
-    GC.@preserve X0 U0 XF P begin
+    GC.@preserve X0 U0 XF P keep begin
         spec = Ref(ToQueueSpec(M, shared, pointer(X0), pointer(U0), XF === nothing ? C_NULL : pointer(XF), objective, constraint,
                                P === nothing ? C_NULL : pointer(P), P === nothing ? 0 : size(P, 1), 0))
-        check(p.h, ccall((:to_solve_queue, libb200), Cint,
-                         (Ptr{Cvoid}, Ref{ToQueueSpec}, Ref{ToSolveOptions}, Ptr{Int32}, Ptr{Int32}, Ptr{Int32}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
-                          Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
-                         p.h, spec, o, status, iters, outer, cost, dJ, grad, cmax, X, U))
+        if isempty(tables)
+            check(p.h, ccall((:to_solve_queue, libb200), Cint,
+                             (Ptr{Cvoid}, Ref{ToQueueSpec}, Ref{ToSolveOptions}, Ptr{Int32}, Ptr{Int32}, Ptr{Int32}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64},
+                              Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                             p.h, spec, o, status, iters, outer, cost, dJ, grad, cmax, X, U))
+        else
+            check(p.h, ccall((:to_solve_queue_tables, libb200), Cint,
+                             (Ptr{Cvoid}, Ref{ToQueueSpec}, Ptr{ToQueueTable}, Int32, Ref{ToSolveOptions}, Ptr{Int32}, Ptr{Int32}, Ptr{Int32},
+                              Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}, Ptr{Float64}),
+                             p.h, spec, tables, length(tables), o, status, iters, outer, cost, dJ, grad, cmax, X, U))
+        end
     end
     (status = [SOLVE_STATUS[s + 1] for s in status], iterations = iters, iterations_outer = outer, cost = cost, dJ = dJ, gradient = grad,
      c_max = cmax, X = X, U = U)
