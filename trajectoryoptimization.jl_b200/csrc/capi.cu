@@ -165,43 +165,6 @@ void lqr_linear_term(const double* M, int dim, const double* xf, double* out) {
     for (int i = 0; i < dim; i++) { double t = 0; for (int j = 0; j < dim; j++) t += M[j * dim + i] * xf[j]; out[i] = -t; }
 }
 
-// Commits the complete rows staged in h->stage as the per-instance table whose host copy is `host` and whose device pointer is `dev`
-// (DevProblem::qr / mparams / cdata): the device buffer is allocated on first use, the rows are copied, and only once the device holds them
-// do they become the host copy and is the pointer published.  A failed call leaves the table, or its absence, as it was: no kernel reads
-// rows the device lacks and no getter reports them.
-int commit_rows(to_handle* h, std::vector<double>& host, const double*& dev) {
-    std::vector<double>& rows = h->stage;
-    double* d = const_cast<double*>(dev);
-    if (!d) { int rc = dalloc(h, &d, rows.size()); if (rc) return rc; }
-    CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));   // the staged rows are the source of the copy
-    host.swap(rows);
-    dev = d;
-    return TO_OK;
-}
-
-// Every row of the penalty table `d` ([B][ncon] on the device) = the shared penalties
-int fill_penalty_rows(to_handle* h, double* d) {
-    const int B = h->P.B, nc = (int)h->h_mu.size();
-    std::vector<double>& rows = h->stage;
-    rows.resize((size_t)B * nc);
-    for (int b = 0; b < B; b++) std::memcpy(rows.data() + (size_t)b * nc, h->h_mu.data(), sizeof(double) * nc);
-    CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));   // the staged rows are the source of the copy
-    return TO_OK;
-}
-// The per-instance penalty table (DevProblem::mub) and SolveDev::go, created once with the shared penalties in every row: by the first
-// to_set_penalties, and by the first to_mpc_solve of a constrained problem
-int ensure_penalty_table(to_handle* h) {
-    if (h->P.mub) return TO_OK;
-    double* d = nullptr;
-    int rc = dalloc(h, &d, (size_t)h->P.B * h->h_mu.size()); if (rc) return rc;
-    if (!h->d_go) { rc = dalloc(h, &h->d_go, 2 * (size_t)h->P.B); if (rc) return rc; }
-    rc = fill_penalty_rows(h, d); if (rc) return rc;
-    h->P.mub = d;   // published once the device holds every row
-    return TO_OK;
-}
-
 // The closed-form columns of [A B] (full-state Quadrotor) and of the materialised [A_e B_e] (error state outside the record path): functions of
 // the time steps alone, so no expansion kernel writes them.  Written when the problem is created and whenever its time steps change, through
 // the same view as the expansion kernels (each instance's own steps once DevProblem::dtb exists).
@@ -397,6 +360,103 @@ void con_shared_row(const DevCon& c, int nm, double* row) {
         }
         case CON_NORM: case CON_COLLISION: row[0] = c.val; break;
     }
+}
+
+// ---- the per-instance tables of DevProblem: the one place that lists them ------------------------------------------------------------
+// Each is nullptr until the first per-instance call creates it from the shared values.  The order is the one in which to_solve_queue_tables
+// checks that the tables it keeps agree between instances.
+enum Table { T_CW, T_DTB, T_MPARAMS, T_CDATA, T_QR, T_MUB, T_COUNT };
+static_assert((int)T_COUNT == (int)QUEUE_TABLES, "QueueDev holds one entry per table");
+struct TableRef {
+    const char* name;            // in the messages
+    size_t width;                // doubles of an instance's row
+    const double*& dev;          // the DevProblem field, [B][width] on the device
+    std::vector<double>* host;   // the host copy, [B][width] while the table exists; nullptr for mub, whose rows the device scales
+};
+TableRef table(to_handle* h, Table t) {
+    DevProblem& P = h->P;
+    switch (t) {
+        case T_CW: return {"cost weights", (size_t)P.ncw, P.cw, &h->h_cw};
+        case T_DTB: return {"time steps", (size_t)P.N - 1, P.dtb, &h->h_dtb};
+        case T_MPARAMS: return {"model parameters", TO_NPARAM, P.mparams, &h->h_mparams};
+        case T_CDATA: return {"constraint data", (size_t)P.ncdata, P.cdata, &h->h_cdata};
+        case T_QR: return {"linear cost terms", (size_t)P.ncost * (P.n + P.m), P.qr, &h->h_qr};
+        default: return {"penalties", (size_t)P.ncon, const_cast<const double*&>(P.mub), nullptr};
+    }
+}
+// row := the shared values in the layout of an instance's row: q | r of every cost, the data of every constraint (a Goal's values
+// included), the parameter vector, the weights of every cost, the time steps, the penalties
+void shared_row(const to_handle* h, Table t, double* row) {
+    const int n = h->P.n, m = h->P.m;
+    switch (t) {
+        case T_CW:
+            for (const auto& c : h->h_costs)
+                if (c.cwoff >= 0) cost_shared_row(c, n, m, row + c.cwoff);
+            break;
+        case T_DTB: std::memcpy(row, h->h_dt.data(), sizeof(double) * (h->P.N - 1)); break;
+        case T_MPARAMS: std::memcpy(row, h->P.params, sizeof(double) * TO_NPARAM); break;
+        case T_CDATA:
+            for (const auto& c : h->h_cons)
+                if (c.cdoff >= 0) con_shared_row(c, n + m, row + c.cdoff);
+            break;
+        case T_QR:
+            for (int ci = 0; ci < h->P.ncost; ci++) {
+                std::memcpy(row + (size_t)ci * (n + m), h->h_costs[ci].q, sizeof(double) * n);
+                std::memcpy(row + (size_t)ci * (n + m) + n, h->h_costs[ci].r, sizeof(double) * m);
+            }
+            break;
+        default: std::memcpy(row, h->h_mu.data(), sizeof(double) * h->h_mu.size());
+    }
+}
+
+// h->h_qr := the device's rows when to_mpc_run has written them since the host copy was last current.  The only way h_qr is brought up to
+// date: every reader of it (to_get_cost_terms, stage, to_solve_queue_tables) calls this first.
+int refresh_qr(to_handle* h) {
+    if (!h->qr_stale) return TO_OK;
+    CU(h, cudaMemcpyAsync(h->h_qr.data(), h->P.qr, sizeof(double) * h->h_qr.size(), cudaMemcpyDeviceToHost, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));
+    h->qr_stale = false;
+    return TO_OK;
+}
+// h->stage := the rows of table t, or the shared row in every instance's row when the table does not exist yet (always, for mub)
+int stage(to_handle* h, Table t) {
+    if (t == T_QR) { int rc = refresh_qr(h); if (rc) return rc; }
+    const TableRef T = table(h, t);
+    if (T.host && T.dev) { h->stage = *T.host; return TO_OK; }
+    h->stage.resize((size_t)h->P.B * T.width);
+    for (int b = 0; b < h->P.B; b++) shared_row(h, t, h->stage.data() + (size_t)b * T.width);
+    return TO_OK;
+}
+// Commits the complete rows staged in h->stage as table t: the device buffer is allocated on first use, the rows are copied, and only once
+// the device holds them do they become the host copy and is the pointer published.  A failed call leaves the table, or its absence, as it
+// was: no kernel reads rows the device lacks and no getter reports them.
+int commit_rows(to_handle* h, Table t) {
+    std::vector<double>& rows = h->stage;
+    const TableRef T = table(h, t);
+    double* d = const_cast<double*>(T.dev);
+    if (!d) { int rc = dalloc(h, &d, rows.size()); if (rc) return rc; }
+    CU(h, cudaMemcpyAsync(d, rows.data(), sizeof(double) * rows.size(), cudaMemcpyHostToDevice, h->stream));
+    CU(h, cudaStreamSynchronize(h->stream));   // the staged rows are the source of the copy
+    if (T.host) T.host->swap(rows);
+    T.dev = d;
+    return TO_OK;
+}
+// out[b * stride + j] := entry off + j of instance b's row of table t (not mub), j < len, for every instance: the host copy's, or the shared
+// row's while the table does not exist (what the getters report)
+void read_rows(to_handle* h, Table t, size_t off, size_t len, double* out, size_t stride) {
+    const TableRef T = table(h, t);
+    std::vector<double> shared(T.width);
+    if (!T.dev) shared_row(h, t, shared.data());
+    for (int b = 0; b < h->P.B; b++)
+        std::memcpy(out + b * stride, (T.dev ? T.host->data() + (size_t)b * T.width : shared.data()) + off, sizeof(double) * len);
+}
+// The per-instance penalty table (DevProblem::mub) and SolveDev::go, created once with the shared penalties in every row: by the first
+// to_set_penalties, and by the first to_mpc_solve of a constrained problem
+int ensure_penalty_table(to_handle* h) {
+    if (h->P.mub) return TO_OK;
+    if (!h->d_go) { int rc = dalloc(h, &h->d_go, 2 * (size_t)h->P.B); if (rc) return rc; }
+    const int rc = stage(h, T_MUB);
+    return rc ? rc : commit_rows(h, T_MUB);
 }
 
 int build_con(to_handle* h, const to_constraint_spec& tc, int n, int m, int N, DevCon& c) {
@@ -842,7 +902,7 @@ int to_set_options(to_handle* h, const to_options* o) {
     d.penalty_initial = o->penalty_initial; d.penalty_scaling = o->penalty_scaling; d.penalty_max = o->penalty_max; d.dual_max = o->dual_max;
     if (reset_mu) {
         for (auto& mu : h->h_mu) mu = d.penalty_initial;
-        if (h->P.mub) { int rc = fill_penalty_rows(h, h->P.mub); if (rc) return rc; }   // every instance restarts with them
+        if (h->P.mub) { int rc = stage(h, T_MUB); if (!rc) rc = commit_rows(h, T_MUB); if (rc) return rc; }   // every instance restarts with them
     }
     if (reset_rho) {
         std::vector<double> r(h->P.B, d.bp_reg_initial);
@@ -972,31 +1032,6 @@ int to_set_initial_time(to_handle* h, double t0, double* tf_out) {
 static int hybrid_goals(to_handle* h) { return fail(h, TO_EINVAL, "per-instance goals are not supported on hybrid problems"); }
 static size_t q_off(const to_handle* h, int b, int cid) { return ((size_t)b * h->P.ncost + cid) * (h->P.n + h->P.m); }
 static size_t cd_off(const to_handle* h, int b, const DevCon& c) { return (size_t)b * h->P.ncdata + c.cdoff; }
-// h->h_qr := the device's rows when to_mpc_run has written them since the host copy was last current.  The only way h_qr is brought up to
-// date: every reader of it (to_get_cost_terms, stage_qr) calls this first.
-static int refresh_qr(to_handle* h) {
-    if (!h->qr_stale) return TO_OK;
-    CU(h, cudaMemcpyAsync(h->h_qr.data(), h->P.qr, sizeof(double) * h->h_qr.size(), cudaMemcpyDeviceToHost, h->stream));
-    CU(h, cudaStreamSynchronize(h->stream));
-    h->qr_stale = false;
-    return TO_OK;
-}
-// h->stage := the rows of the cost-term table, or every instance's shared terms when it does not exist yet
-static int stage_qr(to_handle* h) {
-    if (h->P.qr) {
-        int rc = refresh_qr(h); if (rc) return rc;
-        h->stage = h->h_qr;
-        return TO_OK;
-    }
-    const int B = h->P.B, ncost = h->P.ncost, n = h->P.n, m = h->P.m;
-    h->stage.resize((size_t)B * ncost * (n + m));
-    for (int b = 0; b < B; b++)
-        for (int ci = 0; ci < ncost; ci++) {
-            std::memcpy(h->stage.data() + q_off(h, b, ci), h->h_costs[ci].q, sizeof(double) * n);
-            std::memcpy(h->stage.data() + q_off(h, b, ci) + n, h->h_costs[ci].r, sizeof(double) * m);
-        }
-    return TO_OK;
-}
 static size_t cw_off(const to_handle* h, int b, const DevCost& c) { return (size_t)b * h->P.ncw + c.cwoff; }
 // q | r of cost ci from the goal xf and, when uf is given, the control reference uf: with the Q and R of the weights row w (one row of
 // DevProblem::cw, [ncw]) when it is given, else with the shared ones (the bits every instance had before)
@@ -1013,23 +1048,6 @@ static void weights_linear_term(const to_handle* h, const double* w, int ci, con
 static void instance_linear_term(const to_handle* h, int b, int ci, const double* xf, const double* uf, double* row) {
     weights_linear_term(h, h->P.cw ? h->h_cw.data() + (size_t)b * h->P.ncw : nullptr, ci, xf, uf, row);
 }
-// h->stage := the rows of the cost-weight table, or every instance's shared weights of every cost when it does not exist yet
-static void stage_cw(to_handle* h) {
-    if (h->P.cw) { h->stage = h->h_cw; return; }
-    h->stage.resize((size_t)h->P.B * h->P.ncw);
-    for (int b = 0; b < h->P.B; b++)
-        for (const auto& c : h->h_costs)
-            if (c.cwoff >= 0) cost_shared_row(c, h->P.n, h->P.m, h->stage.data() + cw_off(h, b, c));
-}
-// h->stage := the rows of the constraint-data table, or every instance's shared data of every constraint when it does not exist yet
-static void stage_cdata(to_handle* h) {
-    if (h->P.cdata) { h->stage = h->h_cdata; return; }
-    const int nm = h->P.n + h->P.m;
-    h->stage.resize((size_t)h->P.B * h->P.ncdata);
-    for (int b = 0; b < h->P.B; b++)
-        for (const auto& c : h->h_cons)
-            if (c.cdoff >= 0) con_shared_row(c, nm, h->stage.data() + cd_off(h, b, c));
-}
 
 // set_goal_state! src/problem.jl:294-310 with set_LQR_goal! (q = -Q xf; c untouched) src/cost_functions.jl:245-248
 int to_set_goal_state(to_handle* h, const double* xf, int objective, int constraint) {
@@ -1045,21 +1063,21 @@ int to_set_goal_state(to_handle* h, const double* xf, int objective, int constra
     int rc = upload_tables(h); if (rc) return rc;
     // the later call wins: every instance takes the shared goal, through its own weights once they are per instance
     if (objective && (h->P.qr || h->P.cw)) {
-        rc = stage_qr(h); if (rc) return rc;
+        rc = stage(h, T_QR); if (rc) return rc;
         for (int b = 0; b < h->P.B; b++)
             for (int ci = 0; ci < h->P.ncost; ci++) {
                 double* row = h->stage.data() + q_off(h, b, ci);
                 if (h->P.cw) instance_linear_term(h, b, ci, xf, nullptr, row);
                 else std::memcpy(row, h->h_costs[ci].q, sizeof(double) * n);
             }
-        rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
+        rc = commit_rows(h, T_QR); if (rc) return rc;
     }
     if (constraint && h->P.cdata) {
-        stage_cdata(h);
+        rc = stage(h, T_CDATA); if (rc) return rc;
         for (int b = 0; b < h->P.B; b++)
             for (const auto& c : h->h_cons)
                 if (c.kind == CON_GOAL) std::memcpy(h->stage.data() + cd_off(h, b, c), c.a, sizeof(double) * c.p);
-        rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
+        rc = commit_rows(h, T_CDATA); if (rc) return rc;
     }
     return TO_OK;
 }
@@ -1070,18 +1088,18 @@ int to_set_goal_states(to_handle* h, const double* xf, int objective, int constr
     if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
     const int n = h->P.n;
     if (objective) {
-        int rc = stage_qr(h); if (rc) return rc;
+        int rc = stage(h, T_QR); if (rc) return rc;
         for (int b = 0; b < h->P.B; b++)
             for (int ci = 0; ci < h->P.ncost; ci++) instance_linear_term(h, b, ci, xf + (size_t)b * n, nullptr, h->stage.data() + q_off(h, b, ci));
-        rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
+        rc = commit_rows(h, T_QR); if (rc) return rc;
         h->J_valid = false;
     }
     if (constraint) {
-        stage_cdata(h);
+        int rc = stage(h, T_CDATA); if (rc) return rc;
         for (int b = 0; b < h->P.B; b++)
             for (const auto& c : h->h_cons)
                 if (c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) h->stage[cd_off(h, b, c) + i] = xf[(size_t)b * n + c.inds[i]];
-        int rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
+        rc = commit_rows(h, T_CDATA); if (rc) return rc;
         h->J_valid = false;
     }
     return TO_OK;
@@ -1098,14 +1116,14 @@ int to_update_trajectories(to_handle* h, const double* Xref, const double* Uref,
     const int n = h->P.n, m = h->P.m, N = h->P.N;
     if (reference_window(h, nref, start)) return TO_EDIM;
     if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
-    int rc = stage_qr(h); if (rc) return rc;
+    int rc = stage(h, T_QR); if (rc) return rc;
     for (int b = 0; b < h->P.B; b++)
         for (int i = 0; i < N; i++) {                   // set_LQR_goal!(obj[i], state(Z[k]), control(Z[k])) of instance b
             const int cid = h->h_cost_index[i];
             instance_linear_term(h, b, cid, Xref + ((size_t)b * nref + start - 1 + i) * n, Uref + ((size_t)b * nref + start - 1 + i) * m,
                                  h->stage.data() + q_off(h, b, cid));
         }
-    rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
+    rc = commit_rows(h, T_QR); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1115,13 +1133,10 @@ int to_get_cost_terms(to_handle* h, double* q, double* r) {
     if (!h || !q || !r) return TO_EINVAL;
     int rc = refresh_qr(h); if (rc) return rc;
     const int n = h->P.n, m = h->P.m, ncost = h->P.ncost;
-    for (int b = 0; b < h->P.B; b++)
-        for (int ci = 0; ci < ncost; ci++) {
-            const double* sq = h->P.qr ? h->h_qr.data() + q_off(h, b, ci) : h->h_costs[ci].q;
-            const double* sr = h->P.qr ? h->h_qr.data() + q_off(h, b, ci) + n : h->h_costs[ci].r;
-            std::memcpy(q + ((size_t)b * ncost + ci) * n, sq, sizeof(double) * n);
-            std::memcpy(r + ((size_t)b * ncost + ci) * m, sr, sizeof(double) * m);
-        }
+    for (int ci = 0; ci < ncost; ci++) {
+        read_rows(h, T_QR, (size_t)ci * (n + m), n, q + (size_t)ci * n, (size_t)ncost * n);
+        read_rows(h, T_QR, (size_t)ci * (n + m) + n, m, r + (size_t)ci * m, (size_t)ncost * m);
+    }
     return TO_OK;
 }
 // the values of Goal constraint con of every instance: vals [B][p] (the shared ones broadcast when none are set)
@@ -1130,8 +1145,7 @@ int to_get_goal_values(to_handle* h, int32_t con, double* vals) {
     if (!h || !vals) return TO_EINVAL;
     if (con < 0 || con >= (int)h->h_cons.size() || h->h_cons[con].kind != CON_GOAL) return fail(h, TO_EINVAL, "to_get_goal_values: not a Goal constraint");
     const DevCon& c = h->h_cons[con];
-    for (int b = 0; b < h->P.B; b++)
-        std::memcpy(vals + (size_t)b * c.p, h->P.cdata ? h->h_cdata.data() + cd_off(h, b, c) : c.a, sizeof(double) * c.p);
+    read_rows(h, T_CDATA, c.cdoff, c.p, vals, c.p);
     return TO_OK;
 }
 int to_set_goal_values(to_handle* h, int32_t con, const double* vals) {
@@ -1140,9 +1154,9 @@ int to_set_goal_values(to_handle* h, int32_t con, const double* vals) {
     if (con < 0 || con >= (int)h->h_cons.size() || h->h_cons[con].kind != CON_GOAL) return fail(h, TO_EINVAL, "to_set_goal_values: not a Goal constraint");
     if (h->P.model == MODEL_EXPR) return hybrid_goals(h);
     const DevCon& c = h->h_cons[con];
-    stage_cdata(h);
+    int rc = stage(h, T_CDATA); if (rc) return rc;
     for (int b = 0; b < h->P.B; b++) std::memcpy(h->stage.data() + cd_off(h, b, c), vals + (size_t)b * c.p, sizeof(double) * c.p);
-    int rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
+    rc = commit_rows(h, T_CDATA); if (rc) return rc;
     h->J_valid = false;
     return TO_OK;
 }
@@ -1158,7 +1172,7 @@ int to_set_cost_terms(to_handle* h, const double* q, const double* r) {
             std::memcpy(h->stage.data() + q_off(h, b, ci), q + ((size_t)b * ncost + ci) * n, sizeof(double) * n);
             std::memcpy(h->stage.data() + q_off(h, b, ci) + n, r + ((size_t)b * ncost + ci) * m, sizeof(double) * m);
         }
-    int rc = commit_rows(h, h->h_qr, h->P.qr); if (rc) return rc;
+    int rc = commit_rows(h, T_QR); if (rc) return rc;
     h->qr_stale = false;                                  // every row was written
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
@@ -1197,7 +1211,7 @@ int to_set_model_params(to_handle* h, const double* params, int32_t nparams) {
     if (!h || !params) return TO_EINVAL;
     if (h->P.model == MODEL_EXPR) return fail(h, TO_EINVAL, "per-instance model parameters are not supported on hybrid problems (their constants live in the recorded programs)");
     int rc = model_param_rows(h, params, nparams, "to_set_model_params", h->stage); if (rc) return rc;
-    rc = commit_rows(h, h->h_mparams, h->P.mparams); if (rc) return rc;
+    rc = commit_rows(h, T_MPARAMS); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1207,8 +1221,7 @@ int to_get_model_params(to_handle* h, double* params) {
     if (!h || !params) return TO_EINVAL;
     const int np = model_nparams(h->P.model);
     if (np == 0) return fail(h, TO_EINVAL, "hybrid problems have no model parameter vector");
-    for (int b = 0; b < h->P.B; b++)
-        std::memcpy(params + (size_t)b * np, h->P.mparams ? h->h_mparams.data() + (size_t)b * TO_NPARAM : h->P.params, sizeof(double) * np);
+    read_rows(h, T_MPARAMS, 0, np, params, np);
     return TO_OK;
 }
 
@@ -1259,9 +1272,9 @@ int to_set_constraint_data(to_handle* h, int32_t con, const double* data) {
     int rc = constraint_data_rows(h, con, data, B, "to_set_constraint_data", "instance"); if (rc) return rc;
     const DevCon& c = h->h_cons[con];
     const int len = con_data_len(c, h->P.n + h->P.m);
-    stage_cdata(h);
+    rc = stage(h, T_CDATA); if (rc) return rc;
     for (int b = 0; b < B; b++) std::memcpy(h->stage.data() + cd_off(h, b, c), data + (size_t)b * len, sizeof(double) * len);
-    rc = commit_rows(h, h->h_cdata, h->P.cdata); if (rc) return rc;
+    rc = commit_rows(h, T_CDATA); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1273,10 +1286,7 @@ int to_get_constraint_data(to_handle* h, int32_t con, double* data) {
     const DevCon& c = h->h_cons[con];
     const int nm = h->P.n + h->P.m, len = con_data_len(c, nm);
     if (len == 0) return fail(h, TO_EINVAL, "to_get_constraint_data: the constraint has no per-instance data here (Goal: to_get_goal_values)");
-    std::vector<double> shared(len);
-    con_shared_row(c, nm, shared.data());
-    for (int b = 0; b < h->P.B; b++)
-        std::memcpy(data + (size_t)b * len, h->P.cdata ? h->h_cdata.data() + cd_off(h, b, c) : shared.data(), sizeof(double) * len);
+    read_rows(h, T_CDATA, c.cdoff, len, data, len);
     return TO_OK;
 }
 
@@ -1318,9 +1328,9 @@ int to_set_cost_weights(to_handle* h, int32_t cost, const double* w) {
     int rc = cost_weight_rows(h, cost, w, B, "to_set_cost_weights", "instance"); if (rc) return rc;
     const DevCost& c = h->h_costs[cost];
     const int len = cost_weights_len(c, h->P.n, h->P.m);
-    stage_cw(h);
+    rc = stage(h, T_CW); if (rc) return rc;
     for (int b = 0; b < B; b++) std::memcpy(h->stage.data() + cw_off(h, b, c), w + (size_t)b * len, sizeof(double) * len);
-    rc = commit_rows(h, h->h_cw, h->P.cw); if (rc) return rc;
+    rc = commit_rows(h, T_CW); if (rc) return rc;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     return TO_OK;
 }
@@ -1332,10 +1342,7 @@ int to_get_cost_weights(to_handle* h, int32_t cost, double* w) {
     const DevCost& c = h->h_costs[cost];
     const int n = h->P.n, m = h->P.m, len = cost_weights_len(c, n, m);
     if (len == 0) return fail(h, TO_EINVAL, "to_get_cost_weights: a recorded (expression) cost has no weights");
-    std::vector<double> shared(len);
-    cost_shared_row(c, n, m, shared.data());
-    for (int b = 0; b < h->P.B; b++)
-        std::memcpy(w + (size_t)b * len, h->P.cw ? h->h_cw.data() + cw_off(h, b, c) : shared.data(), sizeof(double) * len);
+    read_rows(h, T_CW, c.cwoff, len, w, len);
     return TO_OK;
 }
 
@@ -1366,7 +1373,7 @@ int to_set_time_steps(to_handle* h, const double* dt, const double* t0) {
     for (int b = 0; b < B; b++)
         if (t0 && !std::isfinite(t0[b])) return fail(h, TO_EINVAL, "to_set_time_steps: instance " + std::to_string(b) + ": the initial time must be finite");
     h->stage.assign(dt, dt + (size_t)B * K);
-    int rc = commit_rows(h, h->h_dtb, h->P.dtb); if (rc) return rc;
+    int rc = commit_rows(h, T_DTB); if (rc) return rc;
     if (t0) h->t0b.assign(t0, t0 + B);
     else if (h->t0b.empty()) h->t0b.assign(B, h->t0);
     h->J_valid = false; h->expanded = false; h->backward_done = false;
@@ -1376,11 +1383,9 @@ int to_set_time_steps(to_handle* h, const double* dt, const double* t0) {
 int to_get_time_steps(to_handle* h, double* dt, double* t0) {
     JOIN(h);
     if (!h || !dt) return TO_EINVAL;
-    const int B = h->P.B, K = h->P.N - 1;
-    for (int b = 0; b < B; b++) {
-        std::memcpy(dt + (size_t)b * K, h->P.dtb ? h->h_dtb.data() + (size_t)b * K : h->h_dt.data(), sizeof(double) * K);
-        if (t0) t0[b] = h->P.dtb ? h->t0b[b] : h->t0;
-    }
+    const int K = h->P.N - 1;
+    read_rows(h, T_DTB, 0, K, dt, K);
+    if (t0) for (int b = 0; b < h->P.B; b++) t0[b] = h->P.dtb ? h->t0b[b] : h->t0;
     return TO_OK;
 }
 
@@ -1416,7 +1421,7 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     int rc = upload_tables(h); if (rc) return rc;
     if (!h->P.qr && !h->P.cw) return TO_OK;
-    rc = stage_qr(h); if (rc) return rc;
+    rc = stage(h, T_QR); if (rc) return rc;
     for (int b = 0; b < h->P.B; b++)                    // the later call wins: every instance takes the shared reference, through its own weights
         for (int i = 0; i < N; i++) {
             const int cid = h->h_cost_index[i];
@@ -1427,7 +1432,7 @@ int to_update_trajectory(to_handle* h, const double* Xref, const double* Uref, i
                 std::memcpy(row + n, h->h_costs[cid].r, sizeof(double) * m);
             }
         }
-    return commit_rows(h, h->h_qr, h->P.qr);
+    return commit_rows(h, T_QR);
 }
 // the host's clocks after a shift by `steps` knots (to_shift_trajectory, each step of to_mpc_run): the shared one by the shared steps, each
 // instance's by its own skipped steps, in the same order (the rows stay)
@@ -1922,7 +1927,7 @@ static int queue_refill(to_handle* h, const QueueDev& q, int half, int mode, cud
     CU(h, launch_queue_harvest(h->P, h->solve, q, half, mode, st));
     CU(h, launch_cost(M, q.cost_slot, nullptr, st));
     CU(h, launch_queue_refill(h->P, h->solve, q, half, mode, st));
-    if (q.dtb && h->P.model == MODEL_QUADROTOR && !(h->P.lie && h->P.frag)) {
+    if (q.tables[T_DTB].slot && h->P.model == MODEL_QUADROTOR && !(h->P.lie && h->P.frag)) {
         // the closed-form Jacobian columns of the refilled slots, from their problems' time steps: no expansion kernel writes them, so a slot
         // would keep its previous problem's (write_closed_form_columns; the record path writes them into every block itself)
         CU(h, h->P.lie ? launch_trivial_columns(M, st, true) : launch_trivial_columns_full(M, st, true));
@@ -1954,12 +1959,14 @@ static int queue_run(to_handle* h, const QueueDev& q) {
     }
     return join_side(h);
 }
-// TO_EINVAL when the rows [B][w] of a per-instance table differ between instances (in the entries keep[j] != 0, all when keep is empty)
-static int uniform_rows(to_handle* h, const std::vector<double>& rows, size_t w, const std::vector<char>& keep, const char* what) {
+// TO_EINVAL when the host copy [B][w] of table t differs between instances in the entries keep[j] != 0 (keep [w])
+static int uniform_rows(to_handle* h, Table t, const std::vector<char>& keep) {
+    const std::vector<double>& rows = *table(h, t).host;
+    const size_t w = keep.size();
     for (int b = 1; b < h->P.B; b++)
         for (size_t j = 0; j < w; j++)
-            if ((keep.empty() || keep[j]) && std::memcmp(&rows[j], &rows[(size_t)b * w + j], sizeof(double)) != 0)
-                return fail(h, TO_EINVAL, std::string("to_solve_queue: the per-instance ") + what + " differ between instances (instance " + std::to_string(b) +
+            if (keep[j] && std::memcmp(&rows[j], &rows[(size_t)b * w + j], sizeof(double)) != 0)
+                return fail(h, TO_EINVAL, std::string("to_solve_queue: the per-instance ") + table(h, t).name + " differ between instances (instance " + std::to_string(b) +
                                               "), so a problem's result would depend on its slot; the queue needs them equal in every row");
     return TO_OK;
 }
@@ -2005,8 +2012,9 @@ int to_solve_queue_tables(to_handle* h, const to_queue_spec* qs, const to_queue_
     rc = finite(qs->x0, M, n, "x0"); if (rc) return rc;
     rc = finite(qs->U0, mu0, wu, "U0"); if (rc) return rc;
     if (qs->xf) { rc = finite(qs->xf, M, n, "xf"); if (rc) return rc; }
-    std::vector<double> mp_rows;
-    if (qs->params) { rc = model_param_rows(h, qs->params, qs->nparams, "to_solve_queue", mp_rows, M); if (rc) return rc; }
+    // each problem's rows of the tables the queue replaces, [M][width] (empty: the slots keep the handle's table)
+    std::vector<double> rows[T_COUNT];
+    if (qs->params) { rc = model_param_rows(h, qs->params, qs->nparams, "to_solve_queue", rows[T_MPARAMS], M); if (rc) return rc; }
     const bool objective = qs->xf && qs->goal_objective, goal_con = qs->xf && qs->goal_constraint && ncd > 0;
     // each table, with its setter's checks; at most one of each kind (and of each cost, each constraint)
     const char* qt = "to_solve_queue_tables";
@@ -2069,94 +2077,85 @@ int to_solve_queue_tables(to_handle* h, const to_queue_spec* qs, const to_queue_
     }
     if (t_ref && objective)
         return fail(h, TO_EINVAL, std::string(qt) + ": a reference and xf with goal_objective = 1 would both set the linear cost terms");
-    // the tables the queue keeps must not depend on the slot; the entries it replaces need not agree
-    if (h->P.cw) {
-        std::vector<char> keep(ncw, 1);
+    // ---- each problem's rows, built as the setters build them, in their order (DESIGN.md 5p): to_set_time_steps, to_set_cost_weights,
+    // to_set_constraint_data, to_update_trajectories or to_set_goal_states, to_set_model_params, to_set_penalties.  A row starts as the
+    // handle's row of instance 0 (or the shared values); keep[t] loses the entries the rows replace, and the handle's instances must agree on
+    // the others, or a problem's result would depend on its slot.
+    std::vector<char> keep[T_COUNT];
+    for (int t = 0; t < T_COUNT; t++) keep[t].assign(table(h, Table(t)).width, 1);
+    auto replaced = [&](Table t, size_t off, size_t len) { std::fill(keep[t].begin() + off, keep[t].begin() + off + len, 0); };
+    auto from_handle = [&](Table t) {
+        const int rc2 = stage(h, t); if (rc2) return rc2;
+        const size_t w = table(h, t).width;
+        rows[t].resize((size_t)M * w);
+        for (int p = 0; p < M; p++) std::memcpy(rows[t].data() + (size_t)p * w, h->stage.data(), sizeof(double) * w);
+        return TO_OK;
+    };
+    auto given = [&](Table t, size_t off, const to_queue_table* T) {   // entries [off, off + len) := the table's row p, in problem p's row
+        replaced(t, off, T->len);
+        const size_t w = table(h, t).width;
+        for (int p = 0; p < M; p++) std::memcpy(rows[t].data() + (size_t)p * w + off, T->rows + (size_t)p * T->len, sizeof(double) * T->len);
+    };
+    if (t_dt) { rows[T_DTB].resize((size_t)M * K); given(T_DTB, 0, t_dt); }
+    if (any_cw) {
+        rc = from_handle(T_CW); if (rc) return rc;
         for (int ci = 0; ci < ncost; ci++)
-            if (t_cw[ci]) std::fill(keep.begin() + h->h_costs[ci].cwoff, keep.begin() + h->h_costs[ci].cwoff + t_cw[ci]->len, 0);
-        rc = uniform_rows(h, h->h_cw, ncw, keep, "cost weights"); if (rc) return rc;
+            if (t_cw[ci]) given(T_CW, h->h_costs[ci].cwoff, t_cw[ci]);
     }
-    if (h->P.dtb && !t_dt) { rc = uniform_rows(h, h->h_dtb, K, {}, "time steps"); if (rc) return rc; }
-    if (h->P.mparams && !qs->params) { rc = uniform_rows(h, h->h_mparams, TO_NPARAM, {}, "model parameters"); if (rc) return rc; }
-    if (h->P.cdata) {
-        std::vector<char> keep(ncd, 1);     // the Goal values xf replaces, the data of the constraints given
+    if (any_cd || goal_con) {
+        rc = from_handle(T_CDATA); if (rc) return rc;
         for (size_t ci = 0; ci < h->h_cons.size(); ci++) {
             const DevCon& c = h->h_cons[ci];
-            if (goal_con && c.kind == CON_GOAL) std::fill(keep.begin() + c.cdoff, keep.begin() + c.cdoff + c.p, 0);
-            if (t_cd[ci]) std::fill(keep.begin() + c.cdoff, keep.begin() + c.cdoff + t_cd[ci]->len, 0);
+            if (t_cd[ci]) given(T_CDATA, c.cdoff, t_cd[ci]);
+            if (goal_con && c.kind == CON_GOAL) {       // the Goal values from xf
+                replaced(T_CDATA, c.cdoff, c.p);
+                for (int p = 0; p < M; p++)
+                    for (int i = 0; i < c.p; i++) rows[T_CDATA][(size_t)p * ncd + c.cdoff + i] = qs->xf[(size_t)p * n + c.inds[i]];
+            }
         }
-        rc = uniform_rows(h, h->h_cdata, ncd, keep, "constraint data"); if (rc) return rc;
     }
     const size_t wq = (size_t)ncost * (n + m);
-    if (h->P.qr) {
-        rc = refresh_qr(h); if (rc) return rc;
-        std::vector<char> keep(wq, 1);      // the q that xf replaces, the q | r of every knot's cost a reference replaces
-        if (objective) for (int ci = 0; ci < ncost; ci++) std::fill(keep.begin() + ci * (n + m), keep.begin() + ci * (n + m) + n, 0);
-        if (t_ref) for (int i = 0; i < N; i++) { const int ci = h->h_cost_index[i]; std::fill(keep.begin() + ci * (n + m), keep.begin() + (ci + 1) * (n + m), 0); }
-        rc = uniform_rows(h, h->h_qr, wq, keep, "linear cost terms"); if (rc) return rc;
-    }
-    // ---- each problem's rows, built as the setters build them, in their order: to_set_cost_weights, to_set_constraint_data,
-    // to_update_trajectories, to_set_goal_states, to_set_model_params (the time steps and penalties are the tables' rows as given)
-    std::vector<double> cw_rows, qr_rows, cd_rows;
-    if (any_cw) {
-        stage_cw(h);
-        cw_rows.resize((size_t)M * ncw);
-        for (int p = 0; p < M; p++) {
-            double* row = cw_rows.data() + (size_t)p * ncw;
-            std::memcpy(row, h->stage.data(), sizeof(double) * ncw);
-            for (int ci = 0; ci < ncost; ci++)
-                if (t_cw[ci]) std::memcpy(row + h->h_costs[ci].cwoff, t_cw[ci]->rows + (size_t)p * t_cw[ci]->len, sizeof(double) * t_cw[ci]->len);
-        }
-    }
     if (objective || t_ref) {
-        rc = stage_qr(h); if (rc) return rc;
-        qr_rows.resize((size_t)M * wq);
+        rc = from_handle(T_QR); if (rc) return rc;
         for (int p = 0; p < M; p++) {
-            double* row = qr_rows.data() + (size_t)p * wq;
-            std::memcpy(row, h->stage.data(), sizeof(double) * wq);
+            double* row = rows[T_QR].data() + (size_t)p * wq;
             // the problem's own weights: its row once given, else the handle's (the same in every instance), else the shared ones
-            const double* w = any_cw ? cw_rows.data() + (size_t)p * ncw : h->P.cw ? h->h_cw.data() : nullptr;
-            if (t_ref) {
+            const double* w = any_cw ? rows[T_CW].data() + (size_t)p * ncw : h->P.cw ? h->h_cw.data() : nullptr;
+            if (t_ref) {                                // q | r of every knot's cost
                 const size_t nref = t_ref->len, k0 = (size_t)p * nref + t_ref->index - 1;
                 for (int i = 0; i < N; i++) {
                     const int ci = h->h_cost_index[i];
+                    replaced(T_QR, (size_t)ci * (n + m), n + m);
                     weights_linear_term(h, w, ci, t_ref->rows + (k0 + i) * n, t_ref->rows2 + (k0 + i) * m, row + (size_t)ci * (n + m));
                 }
-            } else {
-                for (int ci = 0; ci < ncost; ci++) weights_linear_term(h, w, ci, qs->xf + (size_t)p * n, nullptr, row + (size_t)ci * (n + m));
+            } else {                                    // q of every cost
+                for (int ci = 0; ci < ncost; ci++) {
+                    replaced(T_QR, (size_t)ci * (n + m), n);
+                    weights_linear_term(h, w, ci, qs->xf + (size_t)p * n, nullptr, row + (size_t)ci * (n + m));
+                }
             }
         }
     }
-    if (any_cd || goal_con) {
-        stage_cdata(h);
-        cd_rows.resize((size_t)M * ncd);
-        for (int p = 0; p < M; p++) {
-            double* row = cd_rows.data() + (size_t)p * ncd;
-            std::memcpy(row, h->stage.data(), sizeof(double) * ncd);
-            for (size_t ci = 0; ci < h->h_cons.size(); ci++) {
-                const DevCon& c = h->h_cons[ci];
-                if (t_cd[ci]) std::memcpy(row + c.cdoff, t_cd[ci]->rows + (size_t)p * t_cd[ci]->len, sizeof(double) * t_cd[ci]->len);
-                if (goal_con && c.kind == CON_GOAL) for (int i = 0; i < c.p; i++) row[c.cdoff + i] = qs->xf[(size_t)p * n + c.inds[i]];
-            }
-        }
+    if (qs->params) replaced(T_MPARAMS, 0, TO_NPARAM);
+    if (any_mu) {     // the shared penalties, the given constraints' replaced (to_set_penalties after the refill's)
+        rc = from_handle(T_MUB); if (rc) return rc;
+        for (int i = 0; i < nc; i++)
+            if (t_mu[i]) given(T_MUB, i, t_mu[i]);
     }
-    std::vector<double> mu_rows;            // the shared penalties, the given constraints' replaced (to_set_penalties after the refill's)
-    if (any_mu) {
-        mu_rows.resize((size_t)M * nc);
-        for (int p = 0; p < M; p++)
-            for (int i = 0; i < nc; i++) mu_rows[(size_t)p * nc + i] = t_mu[i] ? t_mu[i]->rows[p] : h->h_mu[i];
-    }
-    const size_t ndt = t_dt ? (size_t)M * K : 0, nmu = mu_rows.size();
-    // ---- one allocation: the staged problems, the slot tables, the outputs and the handle's state the refills overwrite
+    rc = refresh_qr(h); if (rc) return rc;
+    for (int t = 0; t < T_COUNT; t++)
+        if (table(h, Table(t)).host && table(h, Table(t)).dev) { rc = uniform_rows(h, Table(t), keep[t]); if (rc) return rc; }
+    // ---- one allocation: the staged problems, the slot tables, the outputs and the handle's state the refills overwrite.  A table with rows
+    // gets a slot table, and so do the penalties of a constrained problem: every refill writes them (without rows, the shared ones, P.mu).
+    auto slotted = [&](int t) { return !rows[t].empty() || (t == T_MUB && nc > 0); };
     const bool traj = X || U;
     const size_t nX = (size_t)N * n, ll = (size_t)h->P.lambda_len;
-    const size_t d_in = (size_t)M * n + mu0 * wu + qr_rows.size() + cd_rows.size() + mp_rows.size() + cw_rows.size() + ndt + nmu;
-    const size_t d_slot = (qr_rows.empty() ? 0 : B * wq) + (cd_rows.empty() ? 0 : (size_t)B * ncd) + (qs->params ? (size_t)B * TO_NPARAM : 0) +
-                          (cw_rows.empty() ? 0 : (size_t)B * ncw) + (t_dt ? (size_t)B * K : 0) + (size_t)B * nc + B;
+    size_t d_in = (size_t)M * n + mu0 * wu + B;     // x0, U0, the tables' rows and slot tables, cost_slot
+    for (int t = 0; t < T_COUNT; t++) d_in += rows[t].size() + (slotted(t) ? (size_t)B * table(h, Table(t)).width : 0);
     const size_t d_out = 4 * (size_t)M + (traj ? (size_t)M * (nX + wu) : 0);
     const size_t d_save = (size_t)B * n + (size_t)B * ll;
     const size_t n_int = 3 * (size_t)M + 1 + 3 * (size_t)B + 2 * (size_t)B;
-    const size_t bytes = (d_in + d_slot + d_out + d_save) * sizeof(double) + n_int * sizeof(int);
+    const size_t bytes = (d_in + d_out + d_save) * sizeof(double) + n_int * sizeof(int);
     void* buf = nullptr;
     cudaError_t e = cudaMalloc(&buf, bytes);
     if (e != cudaSuccess) {
@@ -2168,15 +2167,26 @@ int to_solve_queue_tables(to_handle* h, const to_queue_spec* qs, const to_queue_
     }
     double* d = static_cast<double*>(buf);
     auto take = [&](size_t cnt) { double* p = cnt ? d : nullptr; d += cnt; return p; };
+    auto up = [&](double* dst, const double* src, size_t cnt) {
+        return cnt ? cudaMemcpyAsync(dst, src, cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream) : cudaSuccess;
+    };
     QueueDev q{};
     q.M = M; q.U0_shared = qs->U0_shared ? 1 : 0;
     double* x0_in = take((size_t)M * n); double* U0_in = take(mu0 * wu);
-    double* qr_in = take(qr_rows.size()); double* cd_in = take(cd_rows.size()); double* mp_in = take(mp_rows.size());
-    double* cw_in = take(cw_rows.size()); double* dt_in = take(ndt); double* mu_in = take(nmu);
-    q.x0 = x0_in; q.U0 = U0_in; q.qr_src = qr_in; q.cd_src = cd_in; q.mp_src = mp_in; q.cw_src = cw_in; q.dt_src = dt_in; q.mu_src = mu_in;
-    q.qr = take(qr_rows.empty() ? 0 : B * wq); q.cd = take(cd_rows.empty() ? 0 : (size_t)B * ncd); q.mp = take(qs->params ? (size_t)B * TO_NPARAM : 0);
-    q.cw = take(cw_rows.empty() ? 0 : (size_t)B * ncw); q.dtb = take(t_dt ? (size_t)B * K : 0);
-    q.mub = take((size_t)B * nc); q.cost_slot = take(B);
+    q.x0 = x0_in; q.U0 = U0_in;
+    e = up(x0_in, qs->x0, (size_t)M * n);
+    if (e == cudaSuccess) e = up(U0_in, qs->U0, mu0 * wu);
+    for (int t = 0; t < T_COUNT; t++) {
+        if (!slotted(t)) continue;
+        QueueTable& T = q.tables[t];
+        T.w = (int)table(h, Table(t)).width;
+        T.slot = take((size_t)B * T.w);
+        double* src = take(rows[t].size());
+        if (e == cudaSuccess) e = up(src, rows[t].data(), rows[t].size());
+        T.src = src ? src : h->P.mu;
+        T.stride = src ? T.w : 0;
+    }
+    q.cost_slot = take(B);
     q.cost = take(M); q.dJ = take(M); q.grad = take(M); q.cmax = take(M);
     q.X = traj ? take((size_t)M * nX) : nullptr; q.U = traj ? take((size_t)M * wu) : nullptr;
     double* save_x0 = take((size_t)B * n); double* save_lam = take((size_t)B * ll);
@@ -2184,17 +2194,6 @@ int to_solve_queue_tables(to_handle* h, const to_queue_spec* qs, const to_queue_
     q.status = ip; q.iter = ip + M; q.outer = ip + 2 * (size_t)M; ip += 3 * (size_t)M;
     q.next = ip++; q.slot = ip; ip += B; q.mask = ip; ip += 2 * (size_t)B;
     int* go = ip;
-    auto up = [&](double* dst, const double* src, size_t cnt) {
-        return cnt ? cudaMemcpyAsync(dst, src, cnt * sizeof(double), cudaMemcpyHostToDevice, h->stream) : cudaSuccess;
-    };
-    e = up(x0_in, qs->x0, (size_t)M * n);
-    if (e == cudaSuccess) e = up(U0_in, qs->U0, mu0 * wu);
-    if (e == cudaSuccess) e = up(qr_in, qr_rows.data(), qr_rows.size());
-    if (e == cudaSuccess) e = up(cd_in, cd_rows.data(), cd_rows.size());
-    if (e == cudaSuccess) e = up(mp_in, mp_rows.data(), mp_rows.size());
-    if (e == cudaSuccess) e = up(cw_in, cw_rows.data(), cw_rows.size());
-    if (e == cudaSuccess && t_dt) e = up(dt_in, t_dt->rows, ndt);
-    if (e == cudaSuccess) e = up(mu_in, mu_rows.data(), nmu);
     // the handle's state the refills overwrite: x0, the live trajectories (in the get / set staging buffers), the multipliers
     if (e == cudaSuccess) e = cudaMemcpyAsync(save_x0, h->P.x0, (size_t)B * n * sizeof(double), cudaMemcpyDeviceToDevice, h->stream);
     if (e == cudaSuccess && ll) e = cudaMemcpyAsync(save_lam, h->P.lambda, (size_t)B * ll * sizeof(double), cudaMemcpyDeviceToDevice, h->stream);
@@ -2202,21 +2201,20 @@ int to_solve_queue_tables(to_handle* h, const to_queue_spec* qs, const to_queue_
     if (e != cudaSuccess) { cudaStreamSynchronize(h->stream); cudaFree(buf); return cuda_fail(h, e, "to_solve_queue: upload"); }
     h->launches++;
     // ---- the run, on the slot tables; the handle's own tables (or their absence) come back afterwards
-    const DevProblem saved = h->P;
     SolveDev& S = h->solve;
-    if (q.qr) h->P.qr = q.qr;
-    if (q.cd) h->P.cdata = q.cd;
-    if (q.mp) h->P.mparams = q.mp;
-    if (q.cw) h->P.cw = q.cw;
-    if (q.dtb) h->P.dtb = q.dtb;
-    h->P.mub = q.mub;                          // (nullptr without constraints)
+    const double* own[T_COUNT];
+    for (int t = 0; t < T_COUNT; t++) {
+        const double*& dev = table(h, Table(t)).dev;
+        own[t] = dev;
+        if (q.tables[t].slot) dev = q.tables[t].slot;
+    }
     prepare_solve(h, o);
     S.go = nc > 0 ? go : nullptr;              // a constrained problem takes every outer step on the device
     h->P.active = S.state;
     rc = queue_run(h, q);
     const int jrc = join_side(h);
     h->P.active = nullptr;
-    h->P.qr = saved.qr; h->P.cdata = saved.cdata; h->P.mparams = saved.mparams; h->P.mub = saved.mub; h->P.cw = saved.cw; h->P.dtb = saved.dtb;
+    for (int t = 0; t < T_COUNT; t++) table(h, Table(t)).dev = own[t];
     S.go = h->P.mub ? h->d_go : nullptr;
     h->J_valid = false; h->expanded = false; h->backward_done = false;
     if (!rc) rc = jrc;
@@ -2321,8 +2319,8 @@ int to_mpc_setup(to_handle* h, const to_mpc_spec* s) {
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);     // the host arrays are the sources of the copies
     if (e != cudaSuccess) { cudaFree(buf); return cuda_fail(h, e, "to_mpc_setup: upload"); }
     if (ref && !h->P.qr) {   // the per-instance linear terms the window writes: created as to_update_trajectories creates them
-        rc = stage_qr(h);
-        if (!rc) rc = commit_rows(h, h->h_qr, h->P.qr);
+        rc = stage(h, T_QR);
+        if (!rc) rc = commit_rows(h, T_QR);
         if (rc) { cudaFree(buf); return rc; }
     }
     if (h->mpc_buf) cudaFree(h->mpc_buf);     // (the stream was synchronised above: no kernel of an earlier run reads it)

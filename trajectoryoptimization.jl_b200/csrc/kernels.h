@@ -137,6 +137,14 @@ cudaError_t launch_solve_restart(const DevProblem& P, const SolveDev& S, int hal
 cudaError_t launch_mpc_solve_record(const DevProblem& P, const SolveDev& S, const MpcDev& M, int j, cudaStream_t s);   // row j of the statistics
 // to_solve_queue (capi.cu, DESIGN.md 5n): M problems through the B slots of the batch.  A slot whose instance is DONE hands its results to row p
 // of the outputs (harvest) and takes the next problem (refill), in the half of the iteration whose check stopped it.
+enum { QUEUE_TABLES = 6 };   // the per-instance tables of DevProblem (capi.cu Table)
+// One of them as the refill replaces it: problem p's row src + p * stride (stride 0: every problem takes the same row) goes to row b of the
+// slot table, [B][w] (nullptr: the slots keep the handle's table)
+struct QueueTable {
+    const double* src;
+    double* slot;
+    int stride, w;
+};
 struct QueueDev {
     int M, U0_shared;
     int* next;               // [1] the next problem to claim
@@ -145,19 +153,7 @@ struct QueueDev {
     double* cost_slot;       // [B] the objective of the harvested slots (k_cost)
     const double* x0;        // [M][n]
     const double* U0;        // [M][N-1][m], or [N-1][m] when U0_shared
-    // each problem's rows, src [M][w], and the slot tables the refill writes them into, [B][w] (nullptr: the table is not replaced)
-    const double* qr_src;    // w = ncost (n + m): DevProblem::qr
-    double* qr;
-    const double* cd_src;    // w = ncdata: DevProblem::cdata
-    double* cd;
-    const double* mp_src;    // w = TO_NPARAM: DevProblem::mparams
-    double* mp;
-    const double* cw_src;    // w = ncw: DevProblem::cw
-    double* cw;
-    const double* dt_src;    // w = N-1: DevProblem::dtb
-    double* dtb;
-    double* mub;             // [B][ncon] or nullptr: DevProblem::mub, refilled with the shared penalties, or with the problem's row of mu_src
-    const double* mu_src;    // [M][ncon] or nullptr
+    QueueTable tables[QUEUE_TABLES];
     // outputs [M]: to_solve's statistics, and X [M][N][n], U [M][N-1][m] or nullptr
     int *status, *iter, *outer;
     double *cost, *dJ, *grad, *cmax, *X, *U;

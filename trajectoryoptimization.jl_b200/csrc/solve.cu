@@ -174,15 +174,11 @@ __global__ void k_queue_refill(const DevProblem P, SolveDev S, QueueDev Q, int h
     double* U = traj_Uw(P, P.cur[b], b);
     for (int i = 0; i < (N - 1) * m; i++) U[i] = U0[i];
     for (int i = 0; i < P.lambda_len; i++) P.lambda[(size_t)b * P.lambda_len + i] = 0.0;
-    if (Q.mub) for (int i = 0; i < P.ncon; i++) Q.mub[(size_t)b * P.ncon + i] = Q.mu_src ? Q.mu_src[(size_t)p * P.ncon + i] : P.mu[i];
-    auto rows = [&](const double* src, double* dst, int w) {
-        if (dst) for (int i = 0; i < w; i++) dst[(size_t)b * w + i] = src[(size_t)p * w + i];
-    };
-    rows(Q.qr_src, Q.qr, P.ncost * (n + m));
-    rows(Q.cd_src, Q.cd, P.ncdata);
-    rows(Q.mp_src, Q.mp, TO_NPARAM);
-    rows(Q.cw_src, Q.cw, P.ncw);
-    rows(Q.dt_src, Q.dtb, N - 1);
+#pragma unroll
+    for (int t = 0; t < QUEUE_TABLES; t++) {
+        const QueueTable& T = Q.tables[t];
+        if (T.slot) for (int i = 0; i < T.w; i++) T.slot[(size_t)b * T.w + i] = T.src[(size_t)p * T.stride + i];
+    }
     solve_init_instance(P, S, b);
     *mask = SOLVE_ACTIVE;
     __threadfence();
