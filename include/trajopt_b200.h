@@ -46,7 +46,12 @@ enum to_model_id {
     TO_MODEL_QUADROTOR = 2,         /* examples/Quadrotor.ipynb cells 4,8 ; params = mass, J1..3, g1..3, motor_dist, kf, km */
     TO_MODEL_ACROBOT = 3,           /* RobotZoo.Acrobot ; params = l1,l2,m1,m2,J1,J2,friction,g */
     TO_MODEL_EXPR = 4               /* user dynamics recorded as programs, one per knot allowed (hybrid / variable-dimension models, src/dynamics.jl:15-31,
-                                       test/hybrid_dynamics_model.jl): to_spec.dyn, dyn_index, nx, nu */
+                                       test/hybrid_dynamics_model.jl): to_spec.dyn, dyn_index, nx, nu.  Costs are given on the padded
+                                       class layout, a knot's own entries first: TO_COST_DIAGONAL, TO_COST_QUADRATIC (dense Q, R, H) and
+                                       TO_COST_EXPR (the Python Problem refuses TO_COST_DIAGONAL_QUAT
+                                       on user models: quaternion costs are for the built-in rigid body).  Pad controls need a positive
+                                       curvature of their own (unit R diagonal, or 0.5 u_j^2 in a program) so that Quu stays positive
+                                       definite; they stay zero. */
 };
 
 /* The explicit rule that discretises the dynamics (RobotDynamics' Euler, RK2, RK3, RK4 with zero-order hold on u; `Problem(...; integration)`,

@@ -1079,6 +1079,54 @@ def _integration_code(rule):
     return cls.code
 
 
+def _padded_cost_spec(c, k, nk, mk, n, m, last):
+    """The spec of cost ``c`` of knot ``k`` (0-based; ``last``: the terminal knot), whose own dimensions are ``(nk, mk)``, on the padded
+    layout ``(n, m)`` of a recorded-program problem, with the knot's own entries first.  The pad states carry no cost.  The pad controls
+    get unit curvature, so that Quu stays positive definite; they stay exactly zero, so that the cost, its gradient and the merit are
+    those of ``c``."""
+    if isinstance(c, DiagonalQuatCost):
+        raise ArgumentError(f"knot {k + 1}: quaternion costs (DiagonalQuatCost / QuatLQRCost) need a built-in rigid body (Quadrotor); "
+                            "user dynamics models take DiagonalCost, QuadraticCost and AutodiffCost")
+    if not isinstance(c, (QuadraticCostFunction, AutodiffCost)):
+        raise ArgumentError(f"knot {k + 1}: user dynamics models take DiagonalCost, QuadraticCost and AutodiffCost, not {type(c).__name__}")
+    if (nk, mk) == (n, m):
+        return c._spec()
+    if isinstance(c, DiagonalCost):
+        Qd, Rd, q, r = np.zeros(n), np.ones(m), np.zeros(n), np.zeros(m)
+        Qd[:nk], Rd[:mk], q[:nk], r[:mk] = np.diag(c.Q), np.diag(c.R), c.q, c.r
+        return DiagonalCost(Qd, Rd, q=q, r=r, c=c.c, terminal=c.terminal, checks=False)._spec()
+    if isinstance(c, QuadraticCostFunction):
+        Q, R, H, q, r = np.zeros((n, n)), np.eye(m), np.zeros((m, n)), np.zeros(n), np.zeros(m)
+        Q[:nk, :nk], R[:mk, :mk], H[:mk, :nk], q[:nk], r[:mk] = c.Q, c.R, c.H, c.q, c.r
+        return QuadraticCost(Q, R, H=H, q=q, r=r, c=c.c, terminal=c.terminal, checks=False)._spec()
+    # AutodiffCost: the program loads x[0 .. nk) and u[0 .. mk), which keep their places; on a non-terminal knot it gains
+    # 0.5 (u_mk^2 + ... + u_{m-1}^2) as its new result
+    spec = c._spec()
+    if last or mk == m:
+        return spec
+    prog, consts = [tuple(int(v) for v in ins) for ins in spec["prog"]], [float(v) for v in spec["consts"]]
+    result, total = len(prog) - 1, None
+    for j in range(mk, m):
+        prog.append((K.OP_U, j, 0))
+        prog.append((K.OP_MUL, len(prog) - 1, len(prog) - 1))
+        if total is not None:
+            prog.append((K.OP_ADD, total, len(prog) - 1))
+        total = len(prog) - 1
+    half = next((i for i, v in enumerate(consts) if v == 0.5), None)
+    if half is None:
+        consts.append(0.5)
+        half = len(consts) - 1
+    prog.append((K.OP_MULC, total, half))
+    prog.append((K.OP_ADD, result, len(prog) - 1))
+    if len(prog) > K.EXPR_MAXLEN:
+        raise ArgumentError(f"knot {k + 1}: the AutodiffCost padded to {m} controls needs {len(prog)} instructions, past the limit of "
+                            f"{K.EXPR_MAXLEN} (TO_EXPR_MAXLEN)")
+    if len(consts) > K.EXPR_MAXCONST:
+        raise ArgumentError(f"knot {k + 1}: the AutodiffCost padded to {m} controls needs {len(consts)} constants, past the limit of "
+                            f"{K.EXPR_MAXCONST} (TO_EXPR_MAXCONST)")
+    return dict(spec, prog=np.asarray(prog, dtype=np.int32), consts=np.asarray(consts, dtype=float))
+
+
 class Problem:
     """``Problem(model, obj, x0, tf; xf, constraints, t0, X0, U0, dt, integration)`` (src/problem.jl:79-123) for a batch.
 
@@ -1199,23 +1247,15 @@ class Problem:
             return K.Spec(self.model.model_id, self.n, self.m, self.N, self.B, dtv, [c._spec() for c in uniq], index, con_specs,
                           params=self.model.params, t0=t0, device=self._device, error_state=self.error_state)
         # hybrid: every cost / constraint is re-expressed on the padded [x(n); u(m)] layout (change_dimension, src/cost_functions.jl:391-401,
-        # src/constraints.jl:934-936); the unused controls get a unit weight so that Quu stays positive definite -- they stay exactly zero
+        # src/constraints.jl:934-936)
         n, m = self.n, self.m
-        padded, uniq, index, seen = {}, [], [], {}
+        uniq, index, seen = [], [], {}
         self._cost_objs = []
         for k, c in enumerate(self.obj.cost):
             key = (id(c), self.nx[k], self.nu[k])
-            if key not in padded:
-                if not isinstance(c, DiagonalCost) or isinstance(c, DiagonalQuatCost):
-                    raise ArgumentError("hybrid problems take DiagonalCost / LQRCost stage costs")
-                pc = c
-                if (self.nx[k], self.nu[k]) != (n, m):
-                    nk, mk = self.nx[k], self.nu[k]
-                    Qd, Rd, q, r = np.zeros(n), np.ones(m), np.zeros(n), np.zeros(m)
-                    Qd[:nk], Rd[:mk], q[:nk], r[:mk] = np.diag(c.Q), np.diag(c.R), c.q, c.r
-                    pc = DiagonalCost(Qd, Rd, q=q, r=r, c=c.c, terminal=c.terminal, checks=False)
-                padded[key] = pc
-                seen[key] = len(uniq); uniq.append(pc); self._cost_objs.append(c)
+            if key not in seen:
+                seen[key] = len(uniq); uniq.append(_padded_cost_spec(c, k, self.nx[k], self.nu[k], n, m, k == self.N - 1))
+                self._cost_objs.append(c)
             index.append(seen[key])
         con_specs = []
         for (f, l), c in zip(cons.inds, cons.constraints):
@@ -1227,7 +1267,7 @@ class Problem:
             if id(mdl) not in mseen:
                 mseen[id(mdl)] = len(mods); mods.append(mdl._spec())
             dyn_index.append(mseen[id(mdl)])
-        return K.Spec(K.MODEL_EXPR, n, m, self.N, self.B, dtv, [c._spec() for c in uniq], index, con_specs, t0=t0, device=self._device,
+        return K.Spec(K.MODEL_EXPR, n, m, self.N, self.B, dtv, uniq, index, con_specs, t0=t0, device=self._device,
                       dyn=mods, dyn_index=dyn_index, nx=self.nx, nu=self.nu)
 
     def _open(self):
@@ -1516,6 +1556,8 @@ def set_goal_state(prob, xf, objective=True, constraint=True):   # set_goal_stat
     if constraint:   # every instance takes the shared Goal values
         goals = {id(c) for c in prob.constraints if isinstance(c, GoalConstraint)}
         prob._con_snap = {cid: v for cid, v in getattr(prob, "_con_snap", {}).items() if cid not in goals}
+    # the library reads n entries: a padded problem's xf (the terminal knot's own dimension) gets zeros in the pad states
+    xf = np.concatenate([xf.ravel(), np.zeros(max(0, prob.n - xf.size))])
     prob._call("to_set_goal_state", K._dp(xf), int(objective), int(constraint))
 
 

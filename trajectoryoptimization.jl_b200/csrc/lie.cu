@@ -518,9 +518,8 @@ cudaError_t launch_dense_mma(const DevProblem& P, bool compact, cudaStream_t s) 
     return cudaGetLastError();
 }
 
-template <int NR, int M>
+template <int NR, int M, int WARPS = 4>
 cudaError_t launch_dense_t(const DevProblem& P, cudaStream_t s) {
-    constexpr int WARPS = 4;
     static_assert(sizeof(DenseSmem<NR, M>) * WARPS <= 48 * 1024, "static shared memory");
     k_riccati_dense<NR, M, WARPS><<<(P.B + WARPS - 1) / WARPS, 32 * WARPS, 0, s>>>(P);
     return cudaGetLastError();
@@ -552,5 +551,9 @@ cudaError_t launch_backward_dense(const DevProblem& P, const BackwardPlan& plan,
     if (P.ne == 4 && P.m == 1) return launch_dense_t<4, 1>(P, s);
     if (P.ne == 4 && P.m == 2) return launch_dense_t<4, 2>(P, s);
     if (P.ne == 2 && P.m == 1) return launch_dense_t<2, 1>(P, s);
+    // the recorded-program size classes (8, 4) and (16, 8) with a user cost.  (16, 8) takes 220 registers and 15 KB of shared memory per
+    // warp: the register file holds 9 such warps per SM, which one-warp CTAs reach and two- or four-warp CTAs do not (8)
+    if (P.ne == 8 && P.m == 4) return launch_dense_t<8, 4>(P, s);
+    if (P.ne == 16 && P.m == 8) return launch_dense_t<16, 8, 1>(P, s);
     return cudaErrorNotSupported;
 }
